@@ -1,6 +1,6 @@
-"""astroz_b200 -- B200-native batch SGP4/SDP4 propagation behind the astroz interface.
+"""astroz_b200 -- H100-native batch SGP4/SDP4 propagation behind the astroz interface.
 
-Only the propagation hot path of ATTron/astroz lives here (SURVEY.md section 8): hand-written sm_100a
+Only the propagation hot path of ATTron/astroz lives here (SURVEY.md section 8): hand-written sm_90a
 CUDA kernels behind a C ABI (include/astroz_b200.h), plus host-side mirrors of the reference's
 `Constellation` and python-sgp4-compatible `Satrec` / `SatrecArray`.  There is no CPU fallback.
 """

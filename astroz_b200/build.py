@@ -1,8 +1,8 @@
-"""Build the CUDA library in-tree: astroz_b200/libastroz_b200.so (sm_100a only).
+"""Build the CUDA library in-tree: astroz_b200/libastroz_b200.so (sm_90a only).
 
     python -m astroz_b200.build [--force]
 
-nvcc cross-compiles without a GPU; the built .so travels with the source tree to the GPU box.
+nvcc cross-compiles without a GPU; the built .so sits next to the sources it was built from.
 """
 from __future__ import annotations
 
@@ -17,7 +17,8 @@ LIB = os.path.join(HERE, "libastroz_b200.so")
 SOURCES = ["az_kernels.cu", "az_ingest.cu", "az_capi.cu"]
 HEADERS = ["az_math.cuh", "az_device.cuh", "az_kernels.cuh", "az_ingest.cuh", "az_elements.hpp", "az_tables.hpp",
            os.path.join("..", "..", "include", "astroz_b200.h")]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = [*GENCODE, "-O3", "-std=c++17", "-lineinfo",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr"]
 
 
@@ -47,7 +48,7 @@ def build_variant(out: str, defines: list[str]) -> str:
         if r.returncode != 0:
             raise RuntimeError(f"nvcc failed for {src}:\n{r.stdout}\n{r.stderr}")
         objs.append(obj)
-    r = subprocess.run([nvcc, "-shared", "-o", out, *objs, "-gencode", "arch=compute_100a,code=sm_100a", "-cudart", "static"],
+    r = subprocess.run([nvcc, "-shared", "-o", out, *objs, *GENCODE, "-cudart", "static"],
                        capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")
@@ -70,7 +71,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         if verbose:
             print(r.stderr)
         objs.append(obj)
-    cmd = [nvcc, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a", "-cudart", "static"]
+    cmd = [nvcc, "-shared", "-o", LIB, *objs, *GENCODE, "-cudart", "static"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")
@@ -78,7 +79,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
 
 
 if __name__ == "__main__":
-    if "--variant" in sys.argv:   # python -m astroz_b200.build --variant /tmp/lib_x.so AZ_K2_LANES=1 AZ_DEFAULT_K2_BLOCKS=5
+    if "--variant" in sys.argv:   # python -m astroz_b200.build --variant lib_x.so AZ_K2_LANES=1 AZ_DEFAULT_K2_BLOCKS=5
         i = sys.argv.index("--variant")
         print(build_variant(sys.argv[i + 1], sys.argv[i + 2:]))
     else:

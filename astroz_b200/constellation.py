@@ -33,7 +33,7 @@ def _c_lines(tles):
 
 
 class Constellation:
-    """Mixed SGP4/SDP4 constellation resident on one B200.
+    """Mixed SGP4/SDP4 constellation resident on one GPU.
 
     Parameters
     ----------
@@ -273,7 +273,7 @@ class Constellation:
         check(lib().astroz_cuda_constellation_synchronize(self._h))
 
     def set_timing(self, enabled: bool = True) -> None:
-        """Record CUDA events around the kernels of every later call (off by default: ~12 us of stream time per call)."""
+        """Record CUDA events around the kernels of every later call (off by default: the events cost stream time)."""
         check(lib().astroz_cuda_constellation_set_timing(self._h, 1 if enabled else 0))
 
     def last_kernel_ms(self):

@@ -228,8 +228,7 @@ struct DevBuf {  // grow-only device buffer
 };
 
 // Worker threads of a multi-device handle: one per shard after the first (the caller's thread serves shard 0), parked on
-// a condition variable between calls.  Creating eight std::threads per call instead put the last shard's first launch
-// ~0.2 ms behind the first one's -- 6 % of a 3.3 ms call at eight GPUs.
+// a condition variable between calls, so a call does not wait for thread creation before its last shard's first launch.
 struct ShardWorkers {
     std::mutex m;
     std::condition_variable wake, done;
@@ -303,8 +302,8 @@ struct Constellation {
     cudaEvent_t ev[6] = {};  // K1 start/end, K2 start/end, whole call start/end
     cudaEvent_t chunkDone[64] = {};
     bool timed = false, spanTimed = false;
-    bool timing = false;  // kernel-time events are recorded only on request (astroz_cuda_constellation_set_timing): six
-                          // timed event records per call cost ~12 us of stream time, 20 % of a 1/8-catalog step
+    bool timing = false;  // kernel-time events are recorded only on request (astroz_cuda_constellation_set_timing): the
+                          // six timed event records per call cost stream time, which is not work
     int variant = -1;  // -1 = shipped default; >= 0 selects a tuning variant (ASTROZ_SGP4_VARIANT)
     int chunks = 8;
     // Multi-device handle (device = -1 at creation): the catalog is cut into contiguous satellite ranges, one
@@ -1346,8 +1345,7 @@ static int32_t propagate_host_wait(Constellation *c) {
 }
 
 // Run `work(k)` (queue + wait of shard k) for every shard of a multi-device handle, one host thread per shard: the
-// launches and copies of the devices are issued side by side instead of one device after the other (for 8 GPUs the
-// serial issue of ~40 launches and ~130 copies was ~0.4 ms of a 3 ms call).
+// launches and copies of the devices are issued side by side instead of one device after the other.
 void ShardWorkers::start(size_t nShards) {
     rc.assign(nShards, ASTROZ_OK);
     err.assign(nShards, std::string());
@@ -2059,8 +2057,7 @@ int32_t astroz_cuda_sgp4_propagate(astroz_sgp4_t h, double tsince, double pos[3]
 // ---- result blocks placed next to the GPUs that fill them ---------------------------------------------------------
 // A multi-device handle writes one host block from several GPUs at once.  A plain pinned allocation sits on the NUMA
 // node of the thread that made it, so half the GPUs of a two-socket box write across the socket interconnect and all of
-// them into one node's memory controllers (measured: 93 GB/s for 8 GPUs against 315 GB/s when every GPU writes node-local
-// memory).  astroz_cuda_constellation_host_block maps the block anonymously, binds each device's slice of a
+// them into one node's memory controllers.  astroz_cuda_constellation_host_block maps the block anonymously, binds each device's slice of a
 // satellite-major block to the NUMA node of that device (mbind), touches it, and page-locks the whole range.
 static int device_numa_node(int device) {
     char bus[32] = {};
@@ -2157,7 +2154,7 @@ int32_t astroz_cuda_constellation_devices(astroz_constellation_t h, int32_t *n_d
 }
 
 // Peer mappings between every pair of distinct devices of the handle (cudaMalloc memory of one is then directly
-// addressable from kernels on the other: NVLink 5 loads/stores).  Idempotent.
+// addressable from kernels on the other: NVLink loads/stores).  Idempotent.
 static int32_t enable_peers(Constellation *c) {
     for (Constellation *a : c->shards)
         for (Constellation *b : c->shards) {

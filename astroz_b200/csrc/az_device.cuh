@@ -1,4 +1,4 @@
-// az_device.cuh -- device-side data layout and the per-cell propagation cores (sm_100a, fp64).
+// az_device.cuh -- device-side data layout and the per-cell propagation cores (sm_90a, fp64).
 //
 // Replaces src/Sgp4Batch.zig (BatchElements :15-75, propagateBatchDirect :113-157) and the shared
 // src/Sgp4.zig keplerAndPosVel (:646-750) of the reference.  One *cell* = one (satellite, epoch) pair.
@@ -228,8 +228,7 @@ AZ_HD void kepler_posvel(const double (&am)[kN], const double (&em)[kN], const d
         const double yb = rsqrt_nr1(omel2);  // 2^-46: betal is Heron-corrected, 1/pl scales J2-sized terms only
         const double betal = sqrt_from_rsqrt(omel2, yb);
         // a / r = 1 / (1 - e cos E).  (Starting this reciprocal from the solver's last 1 / (1 - e cos E), one Newton step
-        // instead of four FMAs, measured the same 0.373 ms on its own and 0.408 ms together with the carried
-        // e sin E / e cos E above: profiles/r02r_kepler_handoff.jsonl.)
+        // instead of four FMAs, gained nothing on its own and lost time together with the carried e sin E / e cos E above.)
         const double omec = 1.0 - ecose;
         const double rl = am[k] * omec;
         const double aor = rcp(omec);
@@ -368,8 +367,8 @@ AZ_HD void sgp4_cell(ColFn col, const double (&t)[kN], const GravConsts &g, Cell
 // Angle of the unit vector (s, c) = (sin a, cos a), a in (-pi, pi].  An fp32 arctangent (idle FMA/XU pipes) is snapped
 // to the lattice a0 = k / 128 rad, whose sines and cosines sit in a 13 KB table (L1-resident; az_angle_table.inc,
 // tools/gen_angle_table.py); d = sin(a - a0) = s cos a0 - c sin a0 with |d| <= 2^-8 + 2e-5, and the three-term arcsine
-// finishes it: the x^7 term is below 7e-19.  8 fp64 instructions against ~54 for libdevice's atan2 (round 1's version
-// ran the full range-reducing sincos on the seed: 28).  A common scale error eps of (s, c) moves the result by eps d <
+// finishes it: the x^7 term is below 7e-19.  8 fp64 instructions, where libdevice's atan2 takes several times as many.
+// A common scale error eps of (s, c) moves the result by eps d <
 // 4e-3 eps.  The sign of a zero s survives the conversion, so the branch cut at +-pi falls where atan2 puts it.
 struct AnglePair { double s, c; };
 static __device__ const AnglePair __align__(16) kAngleTabDev[807] = {

@@ -1,4 +1,4 @@
-// az_kernels.cu -- hand-written sm_100a kernels of the batch SGP4/SDP4 path.
+// az_kernels.cu -- hand-written sm_90a kernels of the batch SGP4/SDP4 path.
 //
 //   K1  sgp4_grid_kernel    near-earth (n_sats x n_times) grid   -- replaces sgp4Batch8 + the
 //                           Constellation hot loop (src/simdKernels.zig:9-13, src/Constellation.zig:405-434,478-509)
@@ -58,7 +58,7 @@ __device__ __forceinline__ void tma_bulk_g2s(void *dst, const void *src, uint32_
 //     L2 merges the column stores of a warp-run into full lines before they reach HBM);
 //   * fused all-gather (satellite-major): a warp's 32 consecutive epochs form one contiguous 768-byte
 //     run; the 32 x (x,y,z) records are transposed through shared memory and leave as 128-bit stores to
-//     each peer mapping over NVLink 5, or as one multimem.st to the NVLS multicast address.
+//     each peer mapping over NVLink, or as one multimem.st to the NVLS multicast address.
 // ---------------------------------------------------------------------------------------------------
 template <int kMode, bool kVel>
 __device__ __forceinline__ void to_output_frame(const GridArgs &a, uint32_t t, CellOut &o) {
@@ -70,8 +70,8 @@ __device__ __forceinline__ void to_output_frame(const GridArgs &a, uint32_t t, C
     }
 }
 
-// direct 24-byte record stores; idx in doubles.  For the local satellite-major block this measured ~4 %
-// faster than staging through shared memory (the L2 merges the three 8-byte column stores of a warp-run),
+// direct 24-byte record stores; idx in doubles.  For the local satellite-major block this needs no staging through
+// shared memory (the L2 merges the three 8-byte column stores of a warp-run),
 // so the staged 128-bit path is used only where every byte crosses NVLink (fused all-gather).
 template <int kLayout, bool kVel>
 __device__ __forceinline__ void store_direct(const GridArgs &a, uint32_t row, uint32_t t, const CellOut &o) {
@@ -192,8 +192,8 @@ __global__ void __launch_bounds__(kWarps * 32, kMinBlocks) sgp4_grid_kernel(cons
         // their output rows are consecutive, i.e. an all-near-earth catalog).  Each warp takes PAIRS of adjacent
         // satellites: a pair's two records are 48 contiguous, 16-byte aligned bytes per epoch, so the warp can
         // transpose its own 64 epochs x 2 satellites through a private shared-memory patch and emit 128-bit
-        // stores without any CTA-wide barrier (per-lane 24-byte stores at a stride of n_sats*24 B measured 2.6x
-        // slower with velocities on; a CTA-wide 192-byte-row transpose with two barriers per run 11 % slower).
+        // stores without any CTA-wide barrier (per-lane 24-byte stores at a stride of n_sats*24 B touch a different row's
+        // sector with every word; a CTA-wide 192-byte-row transpose costs two barriers per run).
         // The L2 merges the neighbouring pairs' halves of each 32-byte sector before it is written back.
         constexpr int kRun = 32 * kLanes;
         // The patch IS the pair's slice of the output: 48 contiguous bytes per epoch, epochs back to back.  Lanes write
@@ -421,10 +421,10 @@ const char *sgp4_variant_name(int) { return "?"; }
 static int k1_resident_slots() {
     static int cached[64] = {};
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148 * 3;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132 * 3;
     if (cached[dev] == 0) {
         int sms = 0;
-        if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 148;
+        if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
         cached[dev] = sms * 3;
     }
     return cached[dev];
@@ -481,14 +481,13 @@ static cudaError_t launch_k1(const GridArgs &a0, cudaStream_t stream) {
     return cudaGetLastError();
 }
 
-// Shipped launch shapes (warps per CTA, epochs per stripe, resident CTAs per SM, epochs per thread), from the
-// on-device sweeps in profiles/.  The plain satellite-major TEME/ECEF grid: three epochs per thread (nine independent
-// fp64 chains per scheduler), 3 resident CTAs / SM (164 registers).  History on the headline grid: two epochs per thread
-// (4, 256, 3, 2) 0.476 ms -> three epochs -2.2 % -> with the table-reduced sincos (az_math.cuh: 14 instead of 18 fp64
-// instructions, no quadrant selects) 0.347 ms at 3 CTAs / SM; the same code at 2 CTAs / SM (184 registers) 0.392 ms,
-// two epochs x 4 CTAs 0.355 ms, stripes of 256 0.389 ms, of 768 0.347 ms (profiles/r02w_sincos_table.jsonl,
-// r02x_k1_shapes.jsonl).  The time-major grids take the same three epochs per thread; only the satellite-major geodetic
-// grid, whose epilogue needs the registers itself, is faster with two (profiles/r02y_layout_modes.jsonl, r02z3 for TEME).
+// Shipped launch shapes (warps per CTA, epochs per stripe, resident CTAs per SM, epochs per thread).  The plain
+// satellite-major TEME/ECEF grid: three epochs per thread (nine independent fp64 chains per scheduler), 3 resident CTAs / SM
+// (164 registers).  On one H100 80GB HBM3 SXM (power limit 700 W, maximum SM clock 1980 MHz) the 23 shapes of the
+// AZ_TUNING sweep (tools/sweep_variants.py: 20 steps per shape from a card not yet at its power cap) put this one first on
+// the headline grid: 0.386 ms per step, against 0.392 ms for two epochs per thread (4, 256, 3, 2) and 0.441 ms for three
+// epochs at 2 CTAs / SM; two passes agreed to 0.3 %.  The time-major grids take the same three epochs
+// per thread; only the satellite-major geodetic grid, whose epilogue needs the registers itself, keeps two.
 #ifndef AZ_K1_STRIPE
 #define AZ_K1_STRIPE 384
 #endif
@@ -504,7 +503,7 @@ static cudaError_t launch_k1(const GridArgs &a0, cudaStream_t stream) {
 #define AZ_COMPACT_K1 4, 256, 3, 2
 // epochs per thread of the time-major and geodetic specialisations (2: the compact shape, 3: stripe 384 x 3 CTAs / SM)
 #ifndef AZ_TM_LANES
-#define AZ_TM_LANES 3   // TEME time-major: 0.422 ms against 0.459 ms with two epochs per thread (final build)
+#define AZ_TM_LANES 3
 #endif
 #ifndef AZ_GEO_LANES
 #define AZ_GEO_LANES 2
@@ -515,7 +514,7 @@ static cudaError_t launch_k1(const GridArgs &a0, cudaStream_t stream) {
 #define AZ_TIME_MAJOR_K1 AZ_COMPACT_K1
 #endif
 #ifndef AZ_TM_ECEF_LANES
-#define AZ_TM_ECEF_LANES 3   // with the table-reduced sincos the registers are there: 0.489 -> 0.451 ms (profiles/r02y_layout_modes.jsonl)
+#define AZ_TM_ECEF_LANES 3   // with the table-reduced sincos the registers are there
 #endif
 #if AZ_TM_ECEF_LANES == 3
 #define AZ_TM_ECEF_K1 4, 384, 3, 3
@@ -1015,8 +1014,8 @@ cudaError_t launch_sgp4_grid_f32(const GridArgs &a, int phase64, cudaStream_t st
 //   * the pipe's arithmetic peak: SMs x 64 DFMA lanes x 2 FLOP x the maximum SM clock;
 //   * a live DFMA microbenchmark: 8 independent chains per thread, each x = fma(x, a, 0.5) -- the multiplier sits in one
 //     register every instruction re-reads from the operand-reuse cache and the addend is an immediate, so the register
-//     file serves one fresh 64-bit pair per DFMA (the pattern tools/fp64_probe.cu measured at the pipe's full rate;
-//     fma(x, ra, rb) with two live register operands reads 8 % lower), run long enough for the clocks to settle
+//     file serves one fresh 64-bit pair per DFMA (tools/fp64_probe.cu compares it with patterns that read more pairs),
+//     run long enough for the clocks to settle
 //     (~0.2 s of warm-up), best of 10.
 // bench.py reports the roofline against the larger of the two.
 // ---------------------------------------------------------------------------------------------------
@@ -1046,7 +1045,7 @@ cudaError_t fp64_pipe_peak(double *flops) {
     if (rc != cudaSuccess) return rc;
     rc = cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, dev);
     if (rc != cudaSuccess) return rc;
-    *flops = (double)sms * 64.0 * 2.0 * (double)khz * 1e3;  // sm_100: 64 fp64 FMA lanes per SM
+    *flops = (double)sms * 64.0 * 2.0 * (double)khz * 1e3;  // sm_90: 64 fp64 FMA lanes per SM
     return cudaSuccess;
 }
 
@@ -1059,7 +1058,7 @@ cudaError_t measure_fp64_peak(double *flops) {
     double *d = nullptr;
     rc = cudaMalloc(&d, 8);
     if (rc != cudaSuccess) return rc;
-    const int blocks = sms * 8, threads = 256, iters = 4096;  // ~4.3 ms per launch at the pipe's peak
+    const int blocks = sms * 8, threads = 256, iters = 4096;  // 2^27 FLOP per block: ~4.2 ms per launch at an H100's peak
     cudaEvent_t e0, e1;
     cudaEventCreate(&e0);
     cudaEventCreate(&e1);

@@ -1,4 +1,4 @@
-// az_math.cuh -- fp64 device math for the SGP4/SDP4 grid kernels (sm_100a).
+// az_math.cuh -- fp64 device math for the SGP4/SDP4 grid kernels (sm_90a).
 //
 // Replaces src/simdMath.zig (sincosN :29-97, modTwoPiN :110-122, atan2N :124-177, pow15N :180-182,
 // pow23N :201-212) of the reference.  Design differences, all deliberate:
@@ -53,8 +53,8 @@ AZ_HD double dbl_with_hi(double x, uint32_t hi) {
 }
 
 // Magnitude tests that only steer control flow (which series to use, whether to iterate again) are done on the
-// HIGH WORD of the double with integer instructions: a DSETP occupies the half-rate fp64 pipe like a DFMA does
-// (ncu: 16 of 313 fp64-pipe instructions per cell were compares), the integer pipe has idle issue slots.  Ignoring
+// HIGH WORD of the double with integer instructions: a DSETP occupies the half-rate fp64 pipe like a DFMA does,
+// the integer pipe has idle issue slots.  Ignoring
 // the low word moves a threshold by at most 2^-20 relative, far inside the margin of every series it selects.
 // NaN compares as larger than any limit, so a poisoned lane takes the general path.
 constexpr uint32_t kHiTiny = 0x3fa99999u;     // 0.05
@@ -89,13 +89,13 @@ constexpr double kTwoPi = 6.28318530717958647692528676655900577;
 
 // Every fp64 literal whose low 32 bits are non-zero lives in __constant__ memory: fp64 instructions take
 // constant-bank operands (c[bank][offset]) for free, whereas an immediate costs two UMOV / IMAD.MOV issue
-// slots each time it is materialised -- ncu showed ~230 of 739 instructions per cell were exactly that
-// (profiles/r01_sgp4_grid_notes.md), making the kernel issue-bound instead of fp64-pipe-bound.
+// slots each time it is materialised -- in the first build that was about a third of the instructions per cell,
+// making the kernel issue-bound instead of fp64-pipe-bound.
 // sin / cos kernels on |r| <= pi/4 (tools/fit_sincos_imm.py): sin r = r + r^3 (s1 + s2 z + ... + s6 z^5),
 // cos r = 1 - z/2 + z^2 (c1 + ... + c5 z^4), z = r^2.  s6, s4 and c5 are fp64 numbers whose low 32 bits are zero --
-// sm_100 encodes such an operand in the instruction, so the Horner step that multiplies by it reads two register pairs
-// instead of three (a DFMA with three fresh register-pair sources holds the fp64 pipe 3 cycles instead of 2,
-// tools/fp64_probe.cu) -- and the other coefficients were re-solved with those fixed.  Max error in exact arithmetic
+// the instruction encodes such an operand as an immediate, so the Horner step that multiplies by it reads two register
+// pairs instead of three (a DFMA with three fresh register-pair sources can hold the fp64 pipe longer; tools/fp64_probe.cu
+// measures it) -- and the other coefficients were re-solved with those fixed.  Max error in exact arithmetic
 // 3.4e-17 (sin), 8.4e-17 (cos): on this interval a sixth cosine coefficient buys nothing, so the cosine kernel is one
 // FMA shorter than fdlibm's, whose unconstrained minimax set reads 6e-18 / 5e-19 before the ~1e-16 of rounding all carry.
 #define AZ_S4 0x1.71de3p-19

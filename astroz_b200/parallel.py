@@ -1,6 +1,6 @@
 """Satellite-axis sharding across the GPUs of one box (SURVEY.md section 8e).
 
-One process per GPU (torch.distributed, NCCL over NVLink 5 on the GPU box, gloo in CPU tests).  Cells are
+One process per GPU (torch.distributed, NCCL over NVLink between GPUs, gloo in CPU tests).  Cells are
 independent and SDP4 couples only along time *within* a satellite, so the satellite axis shards with no
 data-path collective.  The one collective the north star names -- an all-gather of the satellite-major
 position/velocity block so every rank holds the whole result -- is `ShardedPropagator.all_gather`.

@@ -2,6 +2,7 @@
 """bench.py -- headline benchmark of the batch SGP4/SDP4 path (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload config2|config3|config4]
+                    [--dump-outputs DIR]
 
 A "step" is one pass of the hot path over the synthetic grid (BASELINE config 2 by default: 13,478
 near-earth satellites x 1,440 epochs, fp64, velocities on, TEME).  One JSON line is printed by rank 0.
@@ -24,6 +25,14 @@ near-earth satellites x 1,440 epochs, fp64, velocities on, TEME).  One JSON line
   config3 / config4   sub-records for the other BASELINE grids (mixed SGP4/SDP4 at N = 1; the week-long grid
                sharded + gathered at N > 1).
   --impl reference  times only that CPU path and prints the same line shape with "impl": "reference".
+  --dump-outputs DIR  after the timed steps, DIR/pos.npy and DIR/vel.npy (float64, satellite-major (rows, n_times, 3)):
+               what the last timed step computed, for a fixed seeded sample of catalog rows (at most 64 MB in all).  The
+               sample depends only on the workload, so runs of either --impl and at any --gpus N (the ranks' shards are
+               gathered to rank 0) can be compared output for output on identical inputs.
+
+--steps K is the number of timed steps of `value` and of the config3 sub-record.  Records with step counts of their own:
+the e2e legs, the fused screen and the all-gather legs time max(3, min(K, 10)) calls, config4 times 5 steps (its gather
+legs 3), the bracketed kernel time averages 10 calls, and cpu_baseline repeats the CPU pass for a fixed wall time.
 """
 from __future__ import annotations
 
@@ -54,11 +63,11 @@ def _peaks():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return json.load(f), "measured"
     except Exception:
-        return {"hbm_gbs": 6650.0}, "fallback"
+        return {"hbm_gbs": 3350.0}, "fallback"   # H100 SXM data sheet, not a measurement
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -110,6 +119,24 @@ class ClockSampler:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["no samples"]}
         return {"sm_mhz": float(np.median(sm)), "sm_max_mhz": float(max(mx)), "power_w_max": max(pw) if pw else None,
                 "samples": len(sm), "reasons": sorted(reasons)}
+
+
+DUMP_BYTES = 64_000_000
+
+
+def dump_rows(n_sats: int, n_times: int, n_blocks: int = 2) -> np.ndarray:
+    """Catalog rows --dump-outputs writes: a fixed seeded sample of as many satellites as fit DUMP_BYTES over n_blocks
+    float64 (n_sats, n_times, 3) blocks, in ascending order."""
+    keep = min(n_sats, DUMP_BYTES // (n_blocks * n_times * 3 * 8))
+    if keep >= n_sats:
+        return np.arange(n_sats)
+    return np.sort(np.random.default_rng(0).choice(n_sats, keep, replace=False))
+
+
+def write_dump(out_dir: str, arrays: dict) -> None:
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), np.ascontiguousarray(a, dtype=np.float64))
 
 
 def workload(name: str):
@@ -169,7 +196,7 @@ def cpu_reference_pass(tles, jd, fr, min_seconds: float, min_reps: int, max_reps
         t0 = time.perf_counter()
         sim.propagate(jd, fr, layout=1, threads=threads, out=(pos, vel), sdp4_threads=sdp4_threads)
         times.append(time.perf_counter() - t0)
-    return times, threads, orc.simd_isa(), sim.numSdp4
+    return times, threads, orc.simd_isa(), sim.numSdp4, (pos, vel)
 
 
 def cpu_baseline_record(tles, jd, fr, seconds: float, min_reps: int, max_reps: int) -> dict:
@@ -177,7 +204,7 @@ def cpu_baseline_record(tles, jd, fr, seconds: float, min_reps: int, max_reps: i
     the SDP4 phase -- the reference's own (the phase gets the threads the SGP4 phase left over, i.e. one,
     src/Constellation.zig:358-364) and an even split -- and the FASTER one is the baseline."""
     cells = len(tles) * len(jd)
-    times, threads, isa, nd = cpu_reference_pass(tles, jd, fr, seconds, min_reps, max_reps, 0)
+    times, threads, isa, nd, _ = cpu_reference_pass(tles, jd, fr, seconds, min_reps, max_reps, 0)
     rec = {"value": cells * len(times) / sum(times), "unit": "props/s", "cores": threads, "kind": "port", "isa": isa,
            "host": usable_cpus(),
            "sample": f"full grid ({cells} cells) x {len(times)} passes over ~{sum(times):.0f} s, sustained mean, "
@@ -185,7 +212,7 @@ def cpu_baseline_record(tles, jd, fr, seconds: float, min_reps: int, max_reps: i
            "best_pass_value": cells / min(times),
            "published_reference": "303 M props/s (16 thr) / 37.7 M (1 thr) on Ryzen 7 7840U, README.md:39 (near-earth only)"}
     if nd:
-        t2, _, _, _ = cpu_reference_pass(tles, jd, fr, seconds, min_reps, max_reps, max(1, threads // 2))
+        t2, _, _, _, _ = cpu_reference_pass(tles, jd, fr, seconds, min_reps, max_reps, max(1, threads // 2))
         even = cells * len(t2) / sum(t2)
         rec["sdp4_thread_policy"] = {"reference_rule_value": rec["value"], "even_split_value": even,
                                      "note": "src/Constellation.zig:358-364 gives the deep-space phase only the threads "
@@ -202,13 +229,16 @@ def run_reference(args, rank: int, world: int) -> None:
     tles, jd, fr, desc = workload(args.workload)
     cells = len(tles) * len(jd)
     reps = args.warmup + args.steps
-    times, threads, isa, nd = cpu_reference_pass(tles, jd, fr, 0.0, reps, reps, 0)
+    times, threads, isa, nd, out = cpu_reference_pass(tles, jd, fr, 0.0, reps, reps, 0)
     policy = "reference rule"
     if nd:   # mixed catalog: also the even split of threads for the deep-space phase; keep the faster
-        t2, _, _, _ = cpu_reference_pass(tles, jd, fr, 0.0, reps, reps, max(1, threads // 2))
+        t2, _, _, _, out = cpu_reference_pass(tles, jd, fr, 0.0, reps, reps, max(1, threads // 2))
         if sum(t2[args.warmup:]) < sum(times[args.warmup:]):
             times, policy = t2, "even split of threads between the SGP4 and SDP4 phases"
     timed = times[args.warmup:]
+    if args.dump_outputs:   # the CPU pass writes time-major (n_times, n_sats, 3) blocks
+        rows = dump_rows(len(tles), len(jd))
+        write_dump(args.dump_outputs, {name: a[:, rows].transpose(1, 0, 2) for name, a in zip(("pos", "vel"), out)})
     total = float(sum(timed))
     value = cells * len(timed) / total
     out = {
@@ -414,6 +444,17 @@ def run_ours(args, rank: int, local_rank: int, world: int) -> None:
     # ---- timed region: exactly K steps, CUDA events on the launching stream, max over ranks ----------------------
     ms_per_step = h.time_steps(step, args.steps)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs:
+        # this rank's share of the catalog-wide row sample; the ranks hold contiguous ascending catalog ranges
+        sample = dump_rows(n, nt)
+        mine = torch.as_tensor(sample[(sample >= sp.begin) & (sample < sp.end)] - sp.begin, device=dev)
+        part = {"pos": pos.index_select(0, mine).cpu().numpy(), "vel": vel.index_select(0, mine).cpu().numpy()}
+        if dist is not None:
+            parts = [None] * world
+            dist.all_gather_object(parts, part)
+            part = {k: np.concatenate([p[k] for p in parts]) for k in part}
+        if rank == 0:
+            write_dump(args.dump_outputs, part)
     if clocks is not None:
         clocks["soak_steps_before_timed_region"] = soak_steps
     value = cells / (ms_per_step * 1e-3)
@@ -435,7 +476,7 @@ def run_ours(args, rank: int, local_rank: int, world: int) -> None:
         c.set_timing(False)
     # One kernel per step (near-earth catalog): its average launch duration over the timed region IS ms_per_step -- K
     # back-to-back launches between two events -- which is the figure the roofline uses; the per-launch bracketing
-    # events of the library add their own ~4 us each and are reported beside it.  A mixed catalog has two overlapping
+    # events of the library add their own stream time and are reported beside it.  A mixed catalog has two overlapping
     # kernels per step: there the bracketed span of the call is the kernel time.
     kernel_ms = ms_per_step if (kernels_per_step == 1 and world == 1) else kernel_ms_bracketed
 
@@ -525,15 +566,6 @@ def run_ours(args, rank: int, local_rank: int, world: int) -> None:
     cells_rank0 = n_local * nt
     ach_tflops = FLOP_PER_CELL * cells_rank0 / (kernel_ms * 1e-3) / 1e12 if kernel_ms else None
     ach_gbs = BYTES_PER_CELL * cells_rank0 / (kernel_ms * 1e-3) / 1e9 if kernel_ms else None
-    traffic = None
-    tfile = os.path.join(ROOT, "profiles", "traffic.json")   # DRAM bytes per launch from the committed ncu capture
-    if os.path.exists(tfile) and world == 1:
-        try:
-            traffic = json.load(open(tfile)).get(args.workload)
-            if isinstance(traffic, dict):
-                traffic = traffic.get("total")
-        except Exception:
-            traffic = None
     roofline = {
         "bound": "fp64", "kernel": "sgp4_grid_kernel" + (" (+ sdp4_grid_kernel side by side)" if n_sdp4_local else ""),
         "achieved": ach_tflops, "peak": pipe_peak, "unit": "TFLOP/s",
@@ -548,7 +580,6 @@ def run_ours(args, rank: int, local_rank: int, world: int) -> None:
         "hbm": {"bound": "hbm", "achieved": ach_gbs, "peak": peaks.get("hbm_gbs"), "unit": "GB/s",
                 "frac": ach_gbs / peaks["hbm_gbs"] if (peaks.get("hbm_gbs") and ach_gbs) else None,
                 "peak_source": peaks_kind, "bytes_per_cell": BYTES_PER_CELL},
-        "traffic": traffic,
     }
     if n_sdp4_local:
         roofline["note"] = ("mixed catalog: 578 FLOP/cell is the near-earth figure applied to every cell; the deep-space "
@@ -571,8 +602,8 @@ def run_ours(args, rank: int, local_rank: int, world: int) -> None:
                    "cells_total": cells, "cells_per_gpu": cells_rank0, "n_sats_total": n, "rows_per_rank": rows,
                    "output_bytes_per_step_total": 2 * cells * 24,
                    "l2": f"{2 * cells_rank0 * 24 / 1e6:.1f} MB written per step per GPU"
-                         + (" >> 126 MB L2 (nothing re-read between steps)" if 2 * cells_rank0 * 24 > 2 * 126e6 else
-                            " (comparable to the 126 MB L2: a step's stores may still be draining while the next runs; "
+                         + (" >> 50 MB L2 (nothing re-read between steps)" if 2 * cells_rank0 * 24 > 2 * 50e6 else
+                            " (comparable to the 50 MB L2: a step's stores may still be draining while the next runs; "
                             "outputs are write-only, nothing is re-read)")
                          + "; the element table is L2-resident by design",
                    "parallelism": par},
@@ -598,7 +629,7 @@ def run_ours(args, rank: int, local_rank: int, world: int) -> None:
 
 def gather_legs(h: Harness, sp, jd, fr, full, step, ms_per_step: float, cells: int, reps: int) -> dict:
     """(a) baseline: shard-local kernel, then ONE in-place ncclAllGather of the [pos|vel] blocks;
-    (b) product: the same kernel writes every 768-byte run straight into all GPUs' copies of the block over NVLink 5
+    (b) product: the same kernel writes every 768-byte run straight into all GPUs' copies of the block over NVLink
         (peer stores into a symmetric allocation), so the transfer overlaps the compute.
     The two gathered blocks are compared over EVERY element (torch.equal), not sampled."""
     from astroz_b200.parallel import SymmetricBlock
@@ -644,7 +675,7 @@ def gather_legs(h: Harness, sp, jd, fr, full, step, ms_per_step: float, cells: i
                         "identical_to_nccl": h.all_true(same), "compared": "every element of both gathered blocks (torch.equal)",
                         "multicast_available": sym.has_multicast,
                         "what": "one kernel per GPU: propagate + 128-bit stores of each run into every GPU's copy "
-                                "of the block (NVLink 5 peer mappings of a symmetric allocation), then a "
+                                "of the block (NVLink peer mappings of a symmetric allocation), then a "
                                 "symmetric-memory barrier"}
         del sym
     except Exception as exc:  # symmetric memory unavailable on this box: report, do not hide
@@ -701,7 +732,7 @@ def config3_record(h: Harness, pipe_peak: float, args) -> dict:
 
     for _ in range(max(args.warmup, 3)):
         step()
-    ms = h.time_steps(step, max(args.steps, 20))
+    ms = h.time_steps(step, args.steps)
     kms, k1, k2 = [], [], []
     c.set_timing(True)
     for _ in range(10):
@@ -744,12 +775,14 @@ def config3_record(h: Harness, pipe_peak: float, args) -> dict:
 def main() -> None:
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=2000)     # ~0.9 s of device time at 0.45 ms per step
+    ap.add_argument("--steps", type=int, default=2000)     # timed steps: about a second of device time on the headline grid
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--impl", choices=["ours", "reference"], default="ours")
     ap.add_argument("--workload", default="config2")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-subrecords", action="store_true", help="skip the config3 sub-record of the default N=1 run")
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="write pos.npy / vel.npy: seeded catalog rows of the last timed step (either --impl, any --gpus)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     rank = int(os.environ.get("RANK", "0"))

@@ -1,5 +1,5 @@
 /*
- * astroz_b200.h -- C ABI of the B200-native batch SGP4/SDP4 propagator.
+ * astroz_b200.h -- C ABI of the H100-native batch SGP4/SDP4 propagator.
  *
  * Drop-in boundary for the propagation path of ATTron/astroz (reference paths relative to the
  * reference repo root).  Every entry point names the reference interface it replaces.
@@ -172,7 +172,7 @@ int32_t astroz_cuda_constellation_propagate_gather(astroz_constellation_t h, con
 /* A page-locked result block of n * n_times * 3 doubles placed for the handle that will fill it: on a multi-device
  * handle each device's satellite range of a satellite-major block is bound to the NUMA node that device hangs off
  * (mbind), so every GPU writes node-local host memory over its own PCIe link -- a plain pinned allocation lives on one
- * node and was measured at 93 GB/s for 8 GPUs against 315 GB/s node-local.  Free with astroz_cuda_host_free. */
+ * node, and every GPU's writes then share that node's memory controllers.  Free with astroz_cuda_host_free. */
 int32_t astroz_cuda_constellation_host_block(astroz_constellation_t h, uint32_t n_times, int32_t layout, double **out);
 
 /* Devices behind a handle: *n_devices (1 for a single-device handle); device_ids[n_devices] (nullable) their CUDA

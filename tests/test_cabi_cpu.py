@@ -34,12 +34,12 @@ def test_header_and_exports_match(built):
     assert L.astroz_cuda_version() == 0x000100
 
 
-def test_library_is_sm100a_with_tma(built):
-    """The shipped kernels are sm_100a SASS and the element tile is staged by a TMA bulk copy (UBLKCP)."""
+def test_library_is_sm90a_with_tma(built):
+    """The shipped kernels are sm_90a SASS and the element tile is staged by a TMA bulk copy (UBLKCP)."""
     sass = subprocess.run(["cuobjdump", "-sass", built], capture_output=True, text=True).stdout
     if not sass:
         pytest.skip("cuobjdump unavailable")
-    assert "sm_100a" in sass
+    assert "sm_90a" in sass and "sm_100" not in sass
     assert "UBLKCP" in sass and "DFMA" in sass and "MUFU.RCP64H" in sass
 
 

@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """Design of the sin/cos kernels whose high-order coefficients are fp64 numbers with a zero low word (CPU tool).
 
-On sm_100 a DFMA that reads three fresh 64-bit register pairs occupies the fp64 pipe for 3 cycles instead of 2
-(tools/fp64_probe.cu), and ptxas keeps polynomial coefficients in registers, so a Horner step fma(p, z, c) with c in a
+A DFMA that reads three fresh 64-bit register pairs can occupy the fp64 pipe longer than one that reads two
+(tools/fp64_probe.cu measures it), and ptxas keeps polynomial coefficients in registers, so a Horner step fma(p, z, c) with c in a
 register is such an instruction.  An fp64 operand whose low 32 bits are zero is encoded in the instruction as an
 immediate and costs no register read.  This script re-fits the |r| <= pi/4 kernels
     sin r = r + r^3 (s1 + s2 z + ... + s6 z^5),   cos r = 1 - z/2 + z^2 (c1 + c2 z + ... + c6 z^5),   z = r^2
