@@ -78,6 +78,8 @@ def lib() -> C.CDLL:
         "astroz_cuda_constellation_propagate_gather": (i32, [vp, dp, dp, u32, C.POINTER(vp), C.POINTER(vp), u32, vp, vp,
                                                              u32, u32, vp]),
         "astroz_cuda_constellation_propagate_device_f32": (i32, [vp, dp, dp, u32, vp, vp, i32, vp]),
+        "astroz_cuda_constellation_propagate_pairs": (i32, [vp, vp, dp, dp, u32, i32, dp, dp, vp]),
+        "astroz_cuda_constellation_propagate_pairs_device": (i32, [vp, vp, vp, vp, u32, i32, vp, vp, vp, vp]),
         "astroz_cuda_constellation_reset_carry": (i32, [vp]),
         "astroz_cuda_constellation_synchronize": (i32, [vp]),
         "astroz_cuda_constellation_last_kernel_ms": (i32, [vp, C.POINTER(C.c_float)]),
@@ -132,6 +134,7 @@ EXPORTS = [
     "astroz_cuda_fp64_peak", "astroz_cuda_fp64_pipe_peak", "astroz_cuda_constellation_devices",
     "astroz_cuda_constellation_propagate_replicated", "astroz_cuda_host_register", "astroz_cuda_host_unregister",
     "astroz_cuda_constellation_set_timing", "astroz_cuda_constellation_host_block",
+    "astroz_cuda_constellation_propagate_pairs", "astroz_cuda_constellation_propagate_pairs_device",
 ]
 
 

@@ -245,6 +245,58 @@ class Constellation:
             C.c_void_p(status.data_ptr()) if status is not None else None,
             int(outputMode), int(layout), rows, int(out_sat_offset), C.c_void_p(stream) if stream else None))
 
+    # ---- arbitrary (satellite, time) pairs -----------------------------------------------------------
+    def propagate_pairs(self, sat, jd, fr, outputMode: int = OutputMode.teme, velocities: bool = True):
+        """Propagate n queries (sat[i], jd[i] + fr[i]) in one call -- the batched form of
+        `for s, jd, fr in obs: sats[s].sgp4(jd, fr)`.  sat[i] is a catalog row (the row numbering of `propagate`).
+        Returns (pos[n, 3], vel[n, 3] or None, status[n] uint8) in the frame of `outputMode`, with the grid's time
+        model, epilogues and failed-cell rules; a row outside the catalog raises (valueError), nothing is computed.
+        Single-device handles only."""
+        sat = np.ascontiguousarray(np.atleast_1d(np.asarray(sat)))
+        jd, fr = as_f64(jd), as_f64(fr)
+        if not (sat.ndim == jd.ndim == fr.ndim == 1) or not (sat.shape[0] == jd.shape[0] == fr.shape[0]):
+            raise ValueError("sat, jd and fr must be 1-D arrays of the same length")
+        if sat.size and not np.issubdtype(sat.dtype, np.integer):
+            raise ValueError("sat must hold integer catalog rows")
+        if sat.size and (sat.min() < 0 or sat.max() > 0xFFFFFFFF):
+            raise ValueError("sat holds a negative or too large row index")
+        sat = sat.astype(np.uint32, copy=False)
+        n = sat.shape[0]
+        pos = _lib.pinned_empty((n, 3))
+        vel = _lib.pinned_empty((n, 3)) if velocities else None
+        status = _lib.pinned_empty((n,), np.uint8)
+        check(lib().astroz_cuda_constellation_propagate_pairs(
+            self._h, C.c_void_p(sat.ctypes.data), dptr(jd), dptr(fr), n, int(outputMode), dptr(pos),
+            dptr(vel) if vel is not None else None, C.c_void_p(status.ctypes.data)))
+        return pos, vel, status
+
+    def propagate_pairs_device(self, sat, jd, fr, pos, vel=None, status=None, outputMode: int = OutputMode.teme,
+                               stream: int = 0) -> None:
+        """`propagate_pairs` with torch CUDA tensors on this constellation's device: sat (int32 / uint32), jd, fr
+        (float64) of n queries; pos / vel (n, 3) float64 and status (n,) uint8 receive the results (vel / status
+        optional).  A row outside the catalog gets zeros and status 3 (ASTROZ_CELL_BAD_SATELLITE).  Asynchronous on
+        `stream` (a raw cudaStream_t value, 0 = the handle's own stream), except that a catalog with deep-space members
+        reads the queries' time range back first."""
+        import torch
+
+        n = int(sat.numel())
+        if int(jd.numel()) != n or int(fr.numel()) != n:
+            raise ValueError("sat, jd and fr must have the same length")
+        if sat.dtype not in (torch.int32, getattr(torch, "uint32", torch.int32)) or jd.dtype != torch.float64 or \
+                fr.dtype != torch.float64:
+            raise ValueError("sat must be int32 / uint32, jd and fr float64")
+        for name, t, per, dt in (("pos", pos, 3, torch.float64), ("vel", vel, 3, torch.float64),
+                                 ("status", status, 1, torch.uint8)):
+            if t is not None and (t.dtype != dt or not t.is_contiguous() or int(t.numel()) < n * per):
+                raise ValueError(f"{name} must be a contiguous {dt} tensor with at least {n * per} elements")
+        for t in (sat, jd, fr):
+            if not t.is_contiguous():
+                raise ValueError("sat, jd and fr must be contiguous")
+        check(lib().astroz_cuda_constellation_propagate_pairs_device(
+            self._h, C.c_void_p(sat.data_ptr()), C.c_void_p(jd.data_ptr()), C.c_void_p(fr.data_ptr()), n,
+            int(outputMode), C.c_void_p(pos.data_ptr()), C.c_void_p(vel.data_ptr()) if vel is not None else None,
+            C.c_void_p(status.data_ptr()) if status is not None else None, C.c_void_p(stream) if stream else None))
+
     def propagate_gather(self, jd, fr, peer_pos=None, peer_vel=None, mc_pos: int = 0, mc_vel: int = 0,
                          out_num_sats: int | None = None, out_sat_offset: int = 0, stream: int = 0) -> None:
         """Fused propagate + all-gather (TEME, satellite-major): this constellation's rows are written into

@@ -295,6 +295,12 @@ struct Constellation {
     int latticeNodes = 0;
     // staging for the host-buffer API
     DevBuf<double> dPos, dVel;
+    // (satellite, time) pairs (K6): catalog row -> table key (built on first use), sort keys / indices and segment
+    // bounds, the sort's temporary storage, the jd-range reduction, and the host call's two slots of queries / results
+    DevBuf<uint32_t> dRowKey, dPairsKeys;
+    DevBuf<char> dPairsSort;
+    DevBuf<double> dPairsRange, dPairsIn, dPairsOut;
+    uint32_t pairsChunk = 1u << 21;  // queries per chunk of the host call (ASTROZ_PAIRS_CHUNK)
     // coarse-screen scratch: hash heads / chains for one batch of epochs, hit buffers, counter
     DevBuf<uint32_t> dHead, dNext, dPairs, dTIdx;
     DevBuf<unsigned long long> dCount;
@@ -331,6 +337,8 @@ struct Constellation {
         dSdp4.release(); dTime.release(); dToffCall.release(); dMask.release(); dLattice.release(); dPos.release(); dVel.release();
         dHead.release(); dNext.release(); dPairs.release(); dTIdx.release(); dCount.release();
         dFullPos.release(); dFullVel.release();
+        dRowKey.release(); dPairsKeys.release(); dPairsSort.release(); dPairsRange.release(); dPairsIn.release();
+        dPairsOut.release();
         if (ring) cudaFreeHost(ring);
         for (auto &e : ringEv) if (e) cudaEventDestroy(e);
         for (auto &h : hTimeSlot) if (h) cudaFreeHost(h);
@@ -387,6 +395,7 @@ int32_t open_device(Constellation *c, int device) {
     if (const char *v = std::getenv("ASTROZ_TIMING")) c->timing = std::atoi(v) != 0;
     if (const char *v = std::getenv("ASTROZ_K1_STRIPE")) az::set_sgp4_stripe((uint32_t)std::max(0, std::atoi(v)));
     if (const char *v = std::getenv("ASTROZ_D2H_CHUNKS")) c->chunks = std::max(1, std::min(64, std::atoi(v)));
+    if (const char *v = std::getenv("ASTROZ_PAIRS_CHUNK")) c->pairsChunk = (uint32_t)std::max(1024, std::min(1 << 26, std::atoi(v)));
     return ASTROZ_OK;
 }
 
@@ -1419,6 +1428,206 @@ int32_t astroz_cuda_constellation_propagate(astroz_constellation_t h, const doub
         const int32_t w = propagate_host_wait(sh);   // also drains what was queued before a failure
         return q != ASTROZ_OK ? q : w;
     });
+}
+
+// ---- (satellite, time) pairs (K6, az_pairs.cu) ----------------------------------------------------------------------
+// Catalog row -> sort key: its near-earth table index, or nSgp4 + its deep-space index (the catalog's, built once).
+static int32_t pairs_row_keys(Constellation *c, cudaStream_t s) {
+    const az::CatalogTables &t = c->cat;
+    if (c->dRowKey.cap >= t.n) return ASTROZ_OK;
+    std::vector<uint32_t> key(t.n, 0);
+    for (uint32_t i = 0; i < t.nSgp4; ++i) key[t.sgp4Orig[i]] = i;
+    for (uint32_t d = 0; d < t.nSdp4; ++d) key[t.sdp4Orig[d]] = t.nSgp4 + d;
+    AZ_CUDA(c->dRowKey.reserve(t.n));
+    AZ_CUDA(cudaMemcpyAsync(c->dRowKey.p, key.data(), (size_t)t.n * 4, cudaMemcpyHostToDevice, s));  // staged: returns
+    return ASTROZ_OK;                                                                                 // after the copy-out
+}
+
+// Queue key / sort / split / K6 for n device-resident queries on s.  The lattice must already reach every query.
+static int32_t pairs_queue(Constellation *c, const uint32_t *dSat, const double *dJd, const double *dFr, uint32_t n,
+                           int mode, double *dPos, double *dVel, uint8_t *dStatus, cudaStream_t s) {
+    const az::CatalogTables &t = c->cat;
+    int32_t rc = pairs_row_keys(c, s);
+    if (rc != ASTROZ_OK) return rc;
+    size_t sortBytes = 0;
+    AZ_CUDA(az::pairs_sort_scratch_bytes(n, t.n, &sortBytes));
+    AZ_CUDA(c->dPairsKeys.reserve((size_t)n * 4 + 2));
+    AZ_CUDA(c->dPairsSort.reserve(std::max<size_t>(sortBytes, 16)));
+    az::PairsArgs a;
+    a.sgp4Tiles = c->dTiles.p;
+    a.toff = c->dToff.p;
+    a.sdp4 = c->dSdp4.p;
+    a.lattice = c->dLattice.p;
+    a.latticeNodes = c->latticeNodes;
+    a.rowKey = c->dRowKey.p;
+    a.nRows = t.n;
+    a.nSgp4 = t.nSgp4;
+    a.refJd = t.referenceEpochJd;
+    a.sat = dSat;
+    a.jd = dJd;
+    a.fr = dFr;
+    a.n = n;
+    uint32_t *k = c->dPairsKeys.p;
+    a.keys = k;
+    a.idx = k + n;
+    a.keysSorted = k + 2 * (size_t)n;
+    a.idxSorted = k + 3 * (size_t)n;
+    a.split = k + 4 * (size_t)n;
+    a.sortScratch = c->dPairsSort.p;
+    a.sortScratchBytes = c->dPairsSort.cap;
+    a.pos = dPos;
+    a.vel = dVel;
+    a.status = dStatus;
+    a.g = c->g;
+    AZ_CUDA(az::launch_pairs(a, mode, s));
+    c->timed = false;
+    return ASTROZ_OK;
+}
+
+static int32_t pairs_check(Constellation *c, int32_t mode) {
+    if (!c) return ASTROZ_NULL_POINTER;
+    if (c->multi()) {
+        g_lastError = "pairs propagation needs a single-device handle (create it with device >= 0)";
+        return ASTROZ_VALUE_ERROR;
+    }
+    if (mode < 0 || mode > 2) {
+        g_lastError = "invalid output mode";
+        return ASTROZ_VALUE_ERROR;
+    }
+    return ASTROZ_OK;
+}
+
+int32_t astroz_cuda_constellation_propagate_pairs_device(astroz_constellation_t h, const uint32_t *d_sat,
+                                                         const double *d_jd, const double *d_fr, uint32_t n,
+                                                         int32_t mode, double *d_pos, double *d_vel,
+                                                         uint8_t *d_status, void *stream) {
+    Constellation *c = static_cast<Constellation *>(h);
+    int32_t rc = pairs_check(c, mode);
+    if (rc != ASTROZ_OK) return rc;
+    if (n == 0) return ASTROZ_OK;
+    if (!d_sat || !d_jd || !d_fr || !d_pos) return ASTROZ_NULL_POINTER;
+    AZ_CUDA(cudaSetDevice(c->device));
+    cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
+    if (c->cat.nSdp4) {
+        // the resonance lattice is grown to the furthest query: min / max of jd + fr on the device, 16 bytes back
+        // (this call's one synchronisation point)
+        AZ_CUDA(c->dPairsRange.reserve(az::pairs_range_scratch_doubles()));
+        AZ_CUDA(az::launch_pairs_range(d_jd, d_fr, n, c->dPairsRange.p, s));
+        double range[2];
+        AZ_CUDA(cudaMemcpyAsync(range, c->dPairsRange.p, 16, cudaMemcpyDeviceToHost, s));
+        AZ_CUDA(cudaStreamSynchronize(s));
+        rc = prepare_deep_space(c, range[0], range[1], s);
+        if (rc != ASTROZ_OK) return rc;
+    }
+    return pairs_queue(c, d_sat, d_jd, d_fr, n, mode, d_pos, d_vel, d_status, s);
+}
+
+// Host buffers: chunks of pairsChunk queries on two device slots.  Chunk k's queries go up and its kernels run on the
+// compute stream while chunk k-1's results come back on the copy stream (pinned / registered destinations) or through
+// the pinned ring and the copy pool (pageable ones); pageable queries are staged through the same ring.
+int32_t astroz_cuda_constellation_propagate_pairs(astroz_constellation_t h, const uint32_t *sat, const double *jd,
+                                                  const double *fr, uint32_t n, int32_t mode, double *pos, double *vel,
+                                                  uint8_t *status) {
+    Constellation *c = static_cast<Constellation *>(h);
+    int32_t rc = pairs_check(c, mode);
+    if (rc != ASTROZ_OK) return rc;
+    if (n == 0) return ASTROZ_OK;
+    if (!sat || !jd || !fr || !pos) return ASTROZ_NULL_POINTER;
+    const az::CatalogTables &t = c->cat;
+    for (uint32_t i = 0; i < n; ++i)
+        if (sat[i] >= t.n) {
+            g_lastError = "query " + std::to_string(i) + ": satellite row " + std::to_string(sat[i]) + " is not in the " +
+                          std::to_string(t.n) + "-row catalog";
+            return ASTROZ_VALUE_ERROR;
+        }
+    AZ_CUDA(cudaSetDevice(c->device));
+    cudaStream_t st = c->stream;
+    if (t.nSdp4) {
+        double lo = INFINITY, hi = -INFINITY;
+        for (uint32_t i = 0; i < n; ++i) {
+            const double j = jd[i] + fr[i];
+            lo = std::min(lo, j);
+            hi = std::max(hi, j);
+        }
+        rc = prepare_deep_space(c, lo, hi, st);
+        if (rc != ASTROZ_OK) return rc;
+    }
+    const uint32_t chunk = std::min(n, c->pairsChunk);
+    const uint32_t nChunks = (uint32_t)(((uint64_t)n + chunk - 1) / chunk);
+    const uint32_t slots = nChunks > 1 ? 2 : 1;
+    // slot layout, in doubles: queries [jd | fr | sat], results [pos | vel | status]
+    const size_t inD = (size_t)chunk * 2 + (chunk + 1) / 2;
+    const size_t outD = (size_t)chunk * (vel ? 6 : 3) + (status ? (chunk + 7) / 8 : 0);
+    AZ_CUDA(c->dPairsIn.reserve(inD * slots));
+    AZ_CUDA(c->dPairsOut.reserve(outD * slots));
+    const bool inPageable = is_pageable(sat) || is_pageable(jd) || is_pageable(fr);
+    const bool posPg = is_pageable(pos), velPg = vel && is_pageable(vel), stPg = status && is_pageable(status);
+    const bool outPageable = posPg || velPg || stPg;
+    if ((inPageable || outPageable) && !c->ring) {
+        AZ_CUDA(cudaMallocHost(&c->ring, kPieceBytes * kRingSlots));
+        for (auto &e : c->ringEv) AZ_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    }
+    CopyPool &pool = CopyPool::get();
+    const cudaEvent_t kdone[2] = {c->chunkDone[0], c->chunkDone[1]}, ddone[2] = {c->chunkDone[2], c->chunkDone[3]};
+    const cudaEvent_t inDone = c->chunkDone[4];
+    const uint32_t granule = std::min<uint32_t>(chunk, (uint32_t)(kPieceBytes / 20));  // queries per ring slot
+    c->plan.clear();
+    uint32_t g = 0;
+    for (uint32_t k = 0; k < nChunks; ++k) {
+        const uint32_t slot = k % slots;
+        const uint32_t q0 = k * chunk, m = std::min(chunk, n - q0);
+        double *dJd = c->dPairsIn.p + slot * inD, *dFr = dJd + chunk;
+        uint32_t *dSat = reinterpret_cast<uint32_t *>(dFr + chunk);
+        double *dPos = c->dPairsOut.p + slot * outD, *dVel = vel ? dPos + (size_t)chunk * 3 : nullptr;
+        uint8_t *dSt = status ? reinterpret_cast<uint8_t *>(dPos + (size_t)chunk * (vel ? 6 : 3)) : nullptr;
+        if (k >= slots) AZ_CUDA(cudaEventSynchronize(ddone[slot]));  // chunk k-2's results have left this slot
+        if (inPageable) {
+            for (uint32_t g0 = 0; g0 < m; g0 += granule, ++g) {
+                const uint32_t gn = std::min(granule, m - g0);
+                const int ri = (int)(g % kRingSlots);
+                char *stage = c->ring + (size_t)ri * kPieceBytes;
+                AZ_CUDA(cudaEventSynchronize(c->ringEv[ri]));  // the slot's last transfer is done
+                pool.copy(stage, reinterpret_cast<const char *>(jd + q0 + g0), 1, (size_t)gn * 8, (size_t)gn * 8);
+                pool.copy(stage + (size_t)gn * 8, reinterpret_cast<const char *>(fr + q0 + g0), 1, (size_t)gn * 8,
+                          (size_t)gn * 8);
+                pool.copy(stage + (size_t)gn * 16, reinterpret_cast<const char *>(sat + q0 + g0), 1, (size_t)gn * 4,
+                          (size_t)gn * 4);
+                AZ_CUDA(cudaMemcpyAsync(dJd + g0, stage, (size_t)gn * 8, cudaMemcpyHostToDevice, st));
+                AZ_CUDA(cudaMemcpyAsync(dFr + g0, stage + (size_t)gn * 8, (size_t)gn * 8, cudaMemcpyHostToDevice, st));
+                AZ_CUDA(cudaMemcpyAsync(dSat + g0, stage + (size_t)gn * 16, (size_t)gn * 4, cudaMemcpyHostToDevice, st));
+                AZ_CUDA(cudaEventRecord(c->ringEv[ri], st));
+            }
+        } else {
+            AZ_CUDA(cudaMemcpyAsync(dJd, jd + q0, (size_t)m * 8, cudaMemcpyHostToDevice, st));
+            AZ_CUDA(cudaMemcpyAsync(dFr, fr + q0, (size_t)m * 8, cudaMemcpyHostToDevice, st));
+            AZ_CUDA(cudaMemcpyAsync(dSat, sat + q0, (size_t)m * 4, cudaMemcpyHostToDevice, st));
+        }
+        AZ_CUDA(cudaEventRecord(inDone, st));
+        rc = pairs_queue(c, dSat, dJd, dFr, m, mode, dPos, dVel, dSt, st);
+        if (rc != ASTROZ_OK) return rc;
+        AZ_CUDA(cudaEventRecord(kdone[slot], st));
+        if (outPageable) {
+            // chunk k-1's pageable results go through the ring while chunk k computes; the ring is free once this
+            // chunk's queries have left it
+            AZ_CUDA(cudaEventSynchronize(inDone));
+            rc = run_ring(c);
+            if (rc != ASTROZ_OK) return rc;
+        }
+        AZ_CUDA(cudaStreamWaitEvent(c->copyStream, kdone[slot], 0));
+        rc = deliver(c, posPg, (int)slot, dPos, pos + (size_t)q0 * 3, 1, (size_t)m * 24, (size_t)m * 24);
+        if (rc == ASTROZ_OK && vel)
+            rc = deliver(c, velPg, (int)slot, dVel, vel + (size_t)q0 * 3, 1, (size_t)m * 24, (size_t)m * 24);
+        if (rc == ASTROZ_OK && status)
+            rc = deliver(c, stPg, (int)slot, reinterpret_cast<const double *>(dSt),
+                         reinterpret_cast<double *>(status + q0), 1, m, m);
+        if (rc != ASTROZ_OK) return rc;
+        AZ_CUDA(cudaEventRecord(ddone[slot], c->copyStream));
+    }
+    rc = run_ring(c);
+    if (rc != ASTROZ_OK) return rc;
+    AZ_CUDA(cudaStreamSynchronize(c->copyStream));
+    AZ_CUDA(cudaStreamSynchronize(st));
+    return ASTROZ_OK;
 }
 
 int32_t astroz_cuda_constellation_reset_carry(astroz_constellation_t h) { return h ? ASTROZ_OK : ASTROZ_NULL_POINTER; }

@@ -96,6 +96,38 @@ cudaError_t launch_coarse_screen(const CoarseArgs &a, cudaStream_t stream);
 // arithmetic in fp32; phase64 != 0 forms the secular angles in fp64 first.
 cudaError_t launch_sgp4_grid_f32(const GridArgs &a, int phase64, cudaStream_t stream);
 
+// K6: n (satellite, time) queries in one call (az_pairs.cu).  All pointers are device pointers.
+struct PairsArgs {
+    // the handle's tables
+    const double *sgp4Tiles = nullptr;   // [tiles][kSgp4Cols][8]
+    const double *toff = nullptr;        // per near-earth table index: (referenceEpochJd - epoch) * 1440
+    const Sdp4Sat *sdp4 = nullptr;
+    const double2 *lattice = nullptr;    // [nSdp4][2][latticeNodes]
+    int latticeNodes = 0;
+    const uint32_t *rowKey = nullptr;    // per catalog row: near-earth table index, or nSgp4 + deep-space index
+    uint32_t nRows = 0, nSgp4 = 0;
+    double refJd = 0.0;
+    // queries
+    const uint32_t *sat = nullptr;
+    const double *jd = nullptr, *fr = nullptr;
+    uint32_t n = 0;
+    // scratch: keys / indices before and after the sort, the segment bounds, the sort's temporary storage
+    uint32_t *keys = nullptr, *idx = nullptr, *keysSorted = nullptr, *idxSorted = nullptr, *split = nullptr;
+    void *sortScratch = nullptr;
+    size_t sortScratchBytes = 0;
+    // outputs, indexed by query
+    double *pos = nullptr;
+    double *vel = nullptr;               // nullable
+    uint8_t *status = nullptr;           // nullable
+    GravConsts g{};
+};
+cudaError_t launch_pairs(const PairsArgs &a, int mode, cudaStream_t stream);
+// temporary storage the sort of n queries over nRows catalog rows needs
+cudaError_t pairs_sort_scratch_bytes(uint32_t n, uint32_t nRows, size_t *bytes);
+// min / max of jd + fr over n queries into scratch[0..1] (scratch: pairs_range_scratch_doubles() doubles)
+cudaError_t launch_pairs_range(const double *jd, const double *fr, uint32_t n, double *scratch, cudaStream_t stream);
+size_t pairs_range_scratch_doubles();
+
 // DFMA throughput microbenchmark: returns achieved fp64 FLOP/s (FMA = 2).
 cudaError_t measure_fp64_peak(double *flops);
 // Arithmetic peak of the fp64 pipe: SMs x 64 lanes x 2 FLOP x the maximum SM clock.

@@ -49,6 +49,7 @@ extern "C" {
 #define ASTROZ_CELL_OK           0
 #define ASTROZ_CELL_DECAYED      1
 #define ASTROZ_CELL_INVALID_ECC  2
+#define ASTROZ_CELL_BAD_SATELLITE 3   /* pairs calls: the query's satellite row is not in the catalog */
 
 /* gravity model selector: src/c_api/sgp4.zig:17-20 (0 = WGS84, 1 = WGS72) */
 #define ASTROZ_WGS84 0
@@ -153,6 +154,35 @@ int32_t astroz_cuda_constellation_propagate_device(astroz_constellation_t h, con
                                                    uint32_t n_times, double *d_pos, double *d_vel, uint8_t *d_status,
                                                    int32_t mode, int32_t layout, uint32_t out_num_sats,
                                                    uint32_t out_sat_offset, void *stream);
+
+/* Arbitrary (satellite, time) pairs: replaces a loop of Satrec.sgp4(jd, fr) calls, one per observation
+ * (bindings/python/src/satrec.zig:169-201); the reference has no batched counterpart.  For catalogue workloads that are
+ * not grids: correlating observations, orbit-determination residuals, sensor tasking, "where was object k at t_k".
+ * Query i propagates catalog row sat[i] (the row numbering of propagate's output block) to jd[i] + fr[i]; pos[i] /
+ * vel[i] / status[i] are what propagate would store in that row at that epoch, in the same frame and units:
+ *   near earth: tsince = ((jd + fr) - referenceEpochJd) * 1440 + (referenceEpochJd - epoch) * 1440, the grid's
+ *               expression to the bit (set_reference_epoch applies); deep space: ((jd + fr) - epoch) * 1440;
+ *   ECEF / geodetic: the GMST of the query's own jd + fr, the grid's rotation and geodetic epilogue;
+ *   failed cells: a deep-space cell failing the scalar checks is zero-filled with its ASTROZ_CELL_* code; a near-earth
+ *   cell is always stored, its status byte flags ASTROZ_CELL_DECAYED only.
+ * A query's result depends on (sat, jd, fr) alone: any permutation or duplication of the query list gives the same bits
+ * per query.  (Propagation runs one query per thread, so results equal the grid's cells to 1e-10 km, not to the bit:
+ * the grid picks some small-angle series per thread over 2-3 epochs.)
+ * Host buffers: pos[n][3], vel[n][3] (nullable), status[n] (nullable).  sat[i] >= n_satellites: ASTROZ_VALUE_ERROR,
+ * nothing written.  Device memory stays bounded: the queries are processed in chunks, upload / kernels / download
+ * overlapped like astroz_cuda_sgp4_array; pageable buffers go through the handle's pinned ring and copy pool.
+ * n = 0 is a no-op.  Multi-device handles (device = -1) return ASTROZ_VALUE_ERROR. */
+int32_t astroz_cuda_constellation_propagate_pairs(astroz_constellation_t h, const uint32_t *sat, const double *jd,
+                                                  const double *fr, uint32_t n, int32_t mode,
+                                                  double *pos, double *vel, uint8_t *status);
+/* Same with DEVICE pointers on the handle's device.  A query whose sat is out of range gets zeros and
+ * ASTROZ_CELL_BAD_SATELLITE; nothing is read for it.  Asynchronous on `stream` (NULL = the handle's stream) except when
+ * the catalog has deep-space members: the min / max of jd + fr is then reduced on the device and read back (16 bytes,
+ * a synchronisation point) to grow the resonance lattice.  Multi-device handles return ASTROZ_VALUE_ERROR. */
+int32_t astroz_cuda_constellation_propagate_pairs_device(astroz_constellation_t h, const uint32_t *d_sat,
+                                                         const double *d_jd, const double *d_fr, uint32_t n,
+                                                         int32_t mode, double *d_pos, double *d_vel,
+                                                         uint8_t *d_status, void *stream);
 
 /* Fused propagate + all-gather for satellite-sharded multi-GPU runs (SURVEY.md section 8e; no reference
  * counterpart -- the reference is single-process).  TEME, satellite-major.  This handle's rows

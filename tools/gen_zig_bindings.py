@@ -33,6 +33,7 @@ def zig_type(ctype: str, name: str) -> str:
         "double **": "?[*]?[*]f64",
         "const uint8_t *": "?[*]const u8",
         "uint8_t *": "?[*]u8",
+        "const uint32_t *": "?[*]const u32",
         "uint32_t *": "?[*]u32",
         "int32_t *": "?[*]i32",
         "uint64_t *": "*u64",

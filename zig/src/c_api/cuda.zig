@@ -25,6 +25,8 @@ pub extern fn astroz_cuda_constellation_get_reference_epoch(h: Handle, jd: ?[*]f
 pub extern fn astroz_cuda_constellation_set_reference_epoch(h: Handle, jd: f64) i32;
 pub extern fn astroz_cuda_constellation_propagate(h: Handle, jd: ?[*]const f64, fr: ?[*]const f64, n_times: u32, pos: ?[*]f64, vel: ?[*]f64, mode: i32, layout: i32) i32;
 pub extern fn astroz_cuda_constellation_propagate_device(h: Handle, jd: ?[*]const f64, fr: ?[*]const f64, n_times: u32, d_pos: ?[*]f64, d_vel: ?[*]f64, d_status: ?[*]u8, mode: i32, layout: i32, out_num_sats: u32, out_sat_offset: u32, stream: ?*anyopaque) i32;
+pub extern fn astroz_cuda_constellation_propagate_pairs(h: Handle, sat: ?[*]const u32, jd: ?[*]const f64, fr: ?[*]const f64, n: u32, mode: i32, pos: ?[*]f64, vel: ?[*]f64, status: ?[*]u8) i32;
+pub extern fn astroz_cuda_constellation_propagate_pairs_device(h: Handle, d_sat: ?[*]const u32, d_jd: ?[*]const f64, d_fr: ?[*]const f64, n: u32, mode: i32, d_pos: ?[*]f64, d_vel: ?[*]f64, d_status: ?[*]u8, stream: ?*anyopaque) i32;
 pub extern fn astroz_cuda_constellation_propagate_gather(h: Handle, jd: ?[*]const f64, fr: ?[*]const f64, n_times: u32, peer_pos: ?[*]const ?*anyopaque, peer_vel: ?[*]const ?*anyopaque, n_peers: u32, mc_pos: ?*anyopaque, mc_vel: ?*anyopaque, out_num_sats: u32, out_sat_offset: u32, stream: ?*anyopaque) i32;
 pub extern fn astroz_cuda_constellation_host_block(h: Handle, n_times: u32, layout: i32, out: ?[*]?[*]f64) i32;
 pub extern fn astroz_cuda_constellation_devices(h: Handle, n_devices: ?[*]i32, device_ids: ?[*]i32, first_rows: ?[*]u32) i32;
