@@ -20,6 +20,10 @@ HEADERS = ["az_math.cuh", "az_device.cuh", "az_kernels.cuh", "az_ingest.cuh", "a
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = [*GENCODE, "-O3", "-std=c++17", "-lineinfo",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr"]
+# Device element initialisation (K5) runs the host builders' arithmetic (az_elements.hpp) without FMA contraction, as the
+# host compiler does: the 12-hour resonance polynomials for e > 0.65 cancel terms of 1e5 down to 1e2, so a contracted
+# evaluation moved their coefficients by ~1e-12 and a device-initialised Molniya orbit by 4e-4 km after 30 years.
+SOURCE_FLAGS = {"az_ingest.cu": ["-fmad=false"]}
 
 
 def _nvcc() -> str:
@@ -43,7 +47,8 @@ def build_variant(out: str, defines: list[str]) -> str:
     objs = []
     for src in SOURCES:
         obj = out + "." + src.replace(".cu", ".o")
-        cmd = [nvcc, *NVCC_FLAGS, *[f"-D{d}" for d in defines], "-c", os.path.join(CSRC, src), "-o", obj]
+        cmd = [nvcc, *NVCC_FLAGS, *SOURCE_FLAGS.get(src, []), *[f"-D{d}" for d in defines], "-c", os.path.join(CSRC, src),
+               "-o", obj]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"nvcc failed for {src}:\n{r.stdout}\n{r.stderr}")
@@ -62,7 +67,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     objs = []
     for src in SOURCES:
         obj = os.path.join(CSRC, src.replace(".cu", ".o"))
-        cmd = [nvcc, *NVCC_FLAGS, "-c", os.path.join(CSRC, src), "-o", obj]
+        cmd = [nvcc, *NVCC_FLAGS, *SOURCE_FLAGS.get(src, []), "-c", os.path.join(CSRC, src), "-o", obj]
         if verbose:
             cmd.insert(1, "-Xptxas=-v")
         r = subprocess.run(cmd, capture_output=True, text=True)

@@ -95,11 +95,11 @@ AZ_HD void kepler_posvel(const double (&am)[kN], const double (&em)[kN], const d
                          const GravConsts &g, CellOut (&o)[kN]) {
     double ya[kN], inv_am[kN], axnl[kN], aynl[kN], s[kN], c[kN], eps[kN];
     AZ_LANES {
-        // am^-1/2 to 2^-46: it scales only J2/J3-sized terms (1/am, am^-3/2, 1/pl), and sqrt(am) below comes out of a
+        // am^-1/2 to 1.5e-12 (one Newton step on the device seed): it scales only J2/J3-sized terms (1/am, am^-3/2, 1/pl), and sqrt(am) below comes out of a
         // Heron correction that squares the error
         ya[k] = rsqrt_nr1(am[k]);
         inv_am[k] = ya[k] * ya[k];
-        // 1 / (am (1 - em^2)); only scales the 1e-3-sized J3 terms, so the 2^-46 reciprocal is ample
+        // 1 / (am (1 - em^2)); only scales the 1e-3-sized J3 terms, so the 1e-12 reciprocal is ample
         const double temp = inv_am[k] * rcp_fast(fma(-em[k], em[k], 1.0));
         double sw, cw;
         sincos_full(argpm[k], sw, cw);
@@ -225,14 +225,14 @@ AZ_HD void kepler_posvel(const double (&am)[kN], const double (&em)[kN], const d
     AZ_LANES {
         const double ecose = ecoseF[k], esine = esineF[k];
         const double omel2 = 1.0 - fma(axnl[k], axnl[k], aynl[k] * aynl[k]);
-        const double yb = rsqrt_nr1(omel2);  // 2^-46: betal is Heron-corrected, 1/pl scales J2-sized terms only
+        const double yb = rsqrt_nr1(omel2);  // 1.5e-12: betal is Heron-corrected, 1/pl scales J2-sized terms only
         const double betal = sqrt_from_rsqrt(omel2, yb);
         // a / r = 1 / (1 - e cos E).  (Starting this reciprocal from the solver's last 1 / (1 - e cos E), one Newton step
         // instead of four FMAs, gained nothing on its own and lost time together with the carried e sin E / e cos E above.)
         const double omec = 1.0 - ecose;
         const double rl = am[k] * omec;
         const double aor = rcp(omec);
-        // sqrt(am) / rl = (a / r) am^-1/2; the 2^-46 of ya is 1e-13 km/s on the velocity
+        // sqrt(am) / rl = (a / r) am^-1/2; the 1.5e-12 of ya is 1e-11 km/s on the velocity
         const double q = aor * ya[k];
         const double rdotl = esine * q;
         const double rvdotl = betal * q;  // sqrt(pl) / rl
@@ -493,7 +493,7 @@ AZ_HD int resonance_node(double t) {
     const double a = fabs(t);
     int n = (int)(a * (1.0 / kStepp));  // a first guess (a division costs ~20 instructions); the two lines below settle it
     if ((double)n * kStepp > a) --n;
-    if (a - (double)n * kStepp >= kStepp) ++n;
+    if (a - (double)n * kStepp >= kStepp) ++n;  // a guard: 1.0 / kStepp rounds up, so the guess is never one short
     return n;
 }
 
@@ -727,7 +727,7 @@ AZ_HD void ecef_to_geodetic(double &x, double &y, double &z) {
         z = az - b;
         return;
     }
-    // Reciprocal square roots carry one Newton step (2^-46) where that is provably enough: the Heron correction in
+    // Reciprocal square roots carry one Newton step (1.5e-12) where that is provably enough: the Heron correction in
     // sqrt_from_rsqrt squares the error; angle_of_unit sees a common scale error of its arguments 4e-3 times smaller;
     // the height-corrected start needs its 0.7 % term to a few digits.
     const double ip = rsqrt_nr1(p2);

@@ -71,7 +71,8 @@ AZ_HD double floor_at(double x, uint32_t hiFloor, double floorValue) {
     return ((int)dbl_hi(x) < (int)hiFloor) ? floorValue : x;
 }
 // x >= 1.0, exactly (1.0 has a zero low word): any double >= 1 has a high word >= 0x3ff00000 as a signed integer,
-// any smaller or negative one does not; NaN compares as >= 1 and is flagged by the callers
+// any smaller or negative one does not; a NaN with the sign bit clear (the device's canonical NaN) compares as >= 1
+// and is flagged by the callers, one with the sign bit set compares as negative
 AZ_HD bool ge_one(double x) { return (int)dbl_hi(x) >= 0x3ff00000; }
 // clamp to +-limit (limit given by its high word and value), sign preserved
 AZ_HD double clamp_abs(double x, uint32_t hiLimit, double limit) {
@@ -142,13 +143,14 @@ static const MathTable kMathHost = AZ_MATH_TABLE_INIT;
 AZ_HD double rcp_seed(double x) {
 #ifdef __CUDA_ARCH__
     double y;
-    asm("rcp.approx.ftz.f64 %0, %1;" : "=d"(y) : "d"(x));
+    asm("rcp.approx.ftz.f64 %0, %1;" : "=d"(y) : "d"(x));  // 1e-6 relative (2^-20.0 measured on an H100)
     return y;
 #else
-    return (double)(1.0f / (float)x);  // ~2^-23, like the MUFU seed
+    return (double)(1.0f / (float)x);  // ~2^-23
 #endif
 }
-// ~2^-46 relative: enough for Newton correction steps (the fixed point does not depend on it)
+// the seed's error squared, from below: 1e-12 relative on the device, 2^-46 with the host's fp32 seed.  Enough for
+// Newton correction steps (the fixed point does not depend on it) and for factors of J3- and e-sized terms
 AZ_HD double rcp_fast(double x) {
     double y = rcp_seed(x);
     double e = fma(-x, y, 1.0);
@@ -174,7 +176,7 @@ AZ_HD double div_nr(double a, double b) {
 AZ_HD double rsqrt_seed(double x) {
 #ifdef __CUDA_ARCH__
     double y;
-    asm("rsqrt.approx.ftz.f64 %0, %1;" : "=d"(y) : "d"(x));
+    asm("rsqrt.approx.ftz.f64 %0, %1;" : "=d"(y) : "d"(x));  // 1e-6 relative (2^-20.1 measured on an H100)
     return y;
 #else
     return (double)(1.0f / sqrtf((float)x));
@@ -189,7 +191,8 @@ AZ_HD double rsqrt_nr(double x) {
     y = fma(half_of(y), r, y);
     return y;
 }
-// 1/sqrt(x) to ~2^-46 (one Newton step): enough wherever a Heron correction (sqrt_from_rsqrt squares the error), a
+// 1/sqrt(x) to 1.5e-12 on the device, 1.5 * 2^-46 on the host (one Newton step leaves 3/2 the square of the seed's
+// error, from below): enough wherever a Heron correction (sqrt_from_rsqrt squares the error), a
 // scale-invariant angle extraction, or a later iteration of the caller's own fixed point follows
 AZ_HD double rsqrt_nr1(double x) {
     double y = rsqrt_seed(x);
@@ -301,10 +304,10 @@ AZ_HD void sincos_tiny(double x, double &s, double &c) {
     c = fma(x2, q, 1.0);
 }
 
-// |x| <= 2e-3 (the J2 short-period angles of any orbit above the surface are < 1e-3): abs error < 3e-16 |x|
+// |x| <= 2e-3 (the J2 short-period angles of any orbit above the surface are < 1e-3): abs error < 3e-16 (sin: 4e-8 |x|^3)
 AZ_HD void sincos_micro(double x, double &s, double &c) {
     // -1/6 and 1/24 rounded to 21 significant bits (immediate operands): the rounding moves sin by |x|^3 * 4e-8 <= 3e-16
-    // and cos by x^4 * 1e-8 <= 2e-19 on this range
+    // (the omitted x^5 / 120 has the other sign and cancels part of it) and cos by x^4 * 1e-8 <= 2e-19 on this range
     double x2 = x * x;
     s = fma(x * x2, -0x1.55555p-3, x);
     c = fma(x2, fma(x2, AZK(tc4), -0.5), 1.0);

@@ -107,6 +107,74 @@ extern "C" int emul_constellation_propagate(const char *const *l1, const char *c
     return 0;
 }
 
+// The quantities that pick a core's series path, per (satellite, epoch), from the product's host tables: lets a fixture
+// prove which path it reaches.  Near-earth rows: [0] tho, the drag angle sgp4_cell rotates by (0 when isimp is set);
+// [1] ecco - tempe before the 1e-6 floor; [2] the Newton loop's first step (e sin E) / (1 - e cos E) before the +-0.95
+// clamp; [3] -1.  Deep-space rows: [0..2] 0, [3] irez.  ecco[n] and inclo[n] (rad) per satellite.
+extern "C" int emul_regimes(const char *const *l1, const char *const *l2, uint32_t n, int grav, const double *jd,
+                            const double *fr, uint32_t nt, double *out, double *ecco, double *inclo) {
+    CatalogTables cat;
+    int rc = build_catalog(l1, l2, n, grav, cat);
+    if (rc != kOk) return rc;
+    for (uint32_t s = 0; s < cat.nSgp4; ++s) {
+        const double *tile = cat.sgp4Tiles.data() + (size_t)(s / kTileSats) * kSgp4TileDoubles;
+        const int sl = s % kTileSats;
+        auto col = [&](int i) { return tile[i * kTileSats + sl]; };
+        const uint32_t orig = cat.sgp4Orig[s];
+        ecco[orig] = col(kEcco);
+        inclo[orig] = std::atan2(col(kSinio), col(kCosio));
+        for (uint32_t k = 0; k < nt; ++k) {
+            // sgp4_cell's secular and drag update, one lane
+            const double t = ((jd[k] + fr[k]) - cat.referenceEpochJd) * 1440.0 +
+                             (cat.referenceEpochJd - cat.sgp4Epoch[s]) * 1440.0;
+            const double t2 = t * t, t3 = t2 * t, t4 = t3 * t;
+            const double xmdf = fma(col(kMdot), t, col(kMo));
+            double argpm = fma(col(kArgpdot), t, col(kArgpo)), mm = xmdf, tho = 0.0;
+            double tempa = fma(-col(kCc1), t, 1.0), tempe = col(kBc4) * t, templ = col(kT2cof) * t2;
+            if (col(kIsimp) == 0.0) {
+                double sm, cm, sd, cd;
+                sincos_full(xmdf, sm, cm);
+                const double dm = fma(col(kEta), cm, 1.0);
+                tho = fma(col(kOmgcof), t, col(kXmcof) * (dm * dm * dm - col(kDelmo)));
+                mm = xmdf + tho;
+                argpm -= tho;
+                sincos_full(tho, sd, cd);
+                tempa = tempa - col(kD2) * t2 - col(kD3) * t3 - col(kD4) * t4;
+                tempe = fma(col(kBc5), fma(sm, cd, cm * sd) - col(kSinmao), tempe);
+                templ = templ + col(kT3cof) * t3 + t4 * fma(t, col(kT5cof), col(kT4cof));
+            }
+            const double am = col(kAbase) * tempa * tempa;
+            const double emRaw = col(kEcco) - tempe;
+            const double em = floor_at(emRaw, kHiEmFloor, AZK(emFloor));
+            mm = fma(col(kNo), templ, mm);
+            // kepler_posvel's prologue and the general loop's first step
+            const double ya = rsqrt_nr1(am), temp = ya * ya * rcp_fast(fma(-em, em, 1.0));
+            double sw, cw, su, cu;
+            sincos_full(argpm, sw, cw);
+            const double axnl = em * cw, aynl = fma(em, sw, temp * col(kAycof));
+            sincos_full(mm + argpm + temp * col(kXlcof) * axnl, su, cu);
+            const double esine = fma(axnl, su, -(aynl * cu)), ecose = fma(axnl, cu, aynl * su);
+            double *o = out + ((size_t)orig * nt + k) * 4;
+            o[0] = tho;
+            o[1] = emRaw;
+            o[2] = esine * rcp_fast(1.0 - ecose);
+            o[3] = -1.0;
+        }
+    }
+    for (uint32_t s = 0; s < cat.nSdp4; ++s) {
+        const Sdp4Sat &e = cat.sdp4[s];
+        const uint32_t orig = cat.sdp4Orig[s];
+        ecco[orig] = e.ecco;
+        inclo[orig] = e.inclo;
+        for (uint32_t k = 0; k < nt; ++k) {
+            double *o = out + ((size_t)orig * nt + k) * 4;
+            o[0] = o[1] = o[2] = 0.0;
+            o[3] = (double)e.irez;
+        }
+    }
+    return 0;
+}
+
 extern "C" void emul_sincos(const double *x, int n, double *s, double *c) {
     for (int i = 0; i < n; ++i) sincos_full(x[i], s[i], c[i]);
 }
