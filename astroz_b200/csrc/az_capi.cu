@@ -13,17 +13,17 @@
 #include <sys/syscall.h>
 #include <unistd.h>
 
-#include <atomic>
-#include <map>
 #include <condition_variable>
-#include <deque>
 #include <functional>
+#include <map>
+#include <memory>
 #include <mutex>
 #include <new>
 #include <string>
 #include <thread>
 #include <vector>
 
+#include "az_hostcopy.cuh"
 #include "az_ingest.cuh"
 #include "az_kernels.cuh"
 #include "az_tables.hpp"
@@ -44,15 +44,6 @@ int32_t cuda_fail(cudaError_t e, const char *what) {
         if (_e != cudaSuccess) return cuda_fail(_e, #expr);  \
     } while (0)
 
-#define AZ_SINGLE(c)                                                                                        \
-    do {                                                                                                    \
-        if ((c) && (c)->multi()) {                                                                          \
-            g_lastError = "this entry point works on device pointers of ONE GPU: create the handle with "  \
-                          "device >= 0 (a device = -1 handle spans several GPUs)";                          \
-            return ASTROZ_VALUE_ERROR;                                                                      \
-        }                                                                                                   \
-    } while (0)
-
 int32_t status_to_code(int st) {  // kernel-level code -> C API code (src/c_api/sgp4.zig:22-28)
     switch (st) {
         case az::kOk: return ASTROZ_OK;
@@ -65,167 +56,28 @@ int32_t status_to_code(int st) {  // kernel-level code -> C API code (src/c_api/
     }
 }
 
-// ---- delivery into caller-owned PAGEABLE host memory --------------------------------------------------------------
-// The reference writes into whatever slices the caller hands in (src/Constellation.zig:245-258; the Python layer
-// passes plain numpy buffers, bindings/python/src/satrec.zig:917-942).  A device->host DMA into pageable memory is
-// staged by the driver through a small internal buffer, synchronously, at a fraction of the PCIe rate.  Instead the
-// result leaves the GPU in pieces into a ring of pinned slots owned by the handle (full-rate DMA), and a small pool of
-// host threads copies each landed piece to its final place while the next pieces are in flight.
-// Piece size: large enough that (a) the wake-up of the copy threads is amortised and (b) each thread's share (a few MB)
-// is above libc's non-temporal threshold, so the destination lines are streamed instead of read for ownership first.
-constexpr size_t kPieceBytes = 32u << 20;
-constexpr int kRingSlots = 3;
-
-// Streaming copy for the landed pieces: the destination is written once and not read again by this library, so the
-// stores bypass the cache (no read-for-ownership of the destination lines, no eviction of the caller's working set):
-// a third less memory traffic per byte than a cached copy.  AVX2 hosts; anything else uses memcpy.
-#if defined(__x86_64__) && defined(__GNUC__)
-#include <immintrin.h>
-__attribute__((target("avx2"))) static void stream_copy_avx2(char *dst, const char *src, size_t n) {
-    const size_t head = (32 - (reinterpret_cast<uintptr_t>(dst) & 31)) & 31;
-    if (head) {
-        const size_t h = std::min(head, n);
-        std::memcpy(dst, src, h);
-        dst += h; src += h; n -= h;
+// ASTROZ_NO_DEVICE when no CUDA device is visible (`message` becomes the last error); *count = the device count
+int32_t check_device_present(int *count, const char *message) {
+    if (cudaGetDeviceCount(count) != cudaSuccess || *count == 0) {
+        g_lastError = message;
+        return ASTROZ_NO_DEVICE;
     }
-    size_t i = 0;
-    for (; i + 128 <= n; i += 128) {
-        const __m256i a = _mm256_loadu_si256(reinterpret_cast<const __m256i *>(src + i));
-        const __m256i b = _mm256_loadu_si256(reinterpret_cast<const __m256i *>(src + i + 32));
-        const __m256i c = _mm256_loadu_si256(reinterpret_cast<const __m256i *>(src + i + 64));
-        const __m256i d = _mm256_loadu_si256(reinterpret_cast<const __m256i *>(src + i + 96));
-        _mm256_stream_si256(reinterpret_cast<__m256i *>(dst + i), a);
-        _mm256_stream_si256(reinterpret_cast<__m256i *>(dst + i + 32), b);
-        _mm256_stream_si256(reinterpret_cast<__m256i *>(dst + i + 64), c);
-        _mm256_stream_si256(reinterpret_cast<__m256i *>(dst + i + 96), d);
-    }
-    _mm_sfence();
-    if (i < n) std::memcpy(dst + i, src + i, n - i);
-}
-static void stream_copy(char *dst, const char *src, size_t n) {
-    static const bool avx2 = __builtin_cpu_supports("avx2");
-    if (avx2 && n >= (64u << 10)) stream_copy_avx2(dst, src, n);
-    else std::memcpy(dst, src, n);
-}
-#else
-static void stream_copy(char *dst, const char *src, size_t n) { std::memcpy(dst, src, n); }
-#endif
-
-class CopyPool {  // process-wide, created on first use, never destroyed (workers sleep on the condition variable)
-public:
-    static CopyPool &get() {
-        static CopyPool *p = new CopyPool();
-        return *p;
-    }
-    int threads() const { return (int)workers_.size(); }
-    // copy `rows` rows of rowBytes from a contiguous source to a destination with pitch hpitch, split over the pool
-    void copy(char *dst, const char *src, size_t rows, size_t rowBytes, size_t hpitch) {
-        const size_t total = rows * rowBytes;
-        const int parts = (int)std::max<size_t>(1, std::min<size_t>(workers_.size(), total / (1u << 20)));
-        if (parts <= 1 || workers_.empty()) {
-            run(dst, src, 0, rows, rowBytes, hpitch, 0, total);
-            return;
-        }
-        std::atomic<int> left(parts);
-        std::mutex dm;
-        std::condition_variable dcv;
-        for (int k = 0; k < parts; ++k) {
-            const size_t b0 = total * k / parts, b1 = total * (k + 1) / parts;
-            push([=, &left, &dm, &dcv] {
-                run(dst, src, 0, rows, rowBytes, hpitch, b0, b1);
-                if (left.fetch_sub(1) == 1) {
-                    std::lock_guard<std::mutex> g(dm);
-                    dcv.notify_one();
-                }
-            });
-        }
-        std::unique_lock<std::mutex> g(dm);
-        dcv.wait(g, [&] { return left.load() == 0; });
-    }
-
-private:
-    CopyPool() {
-        int n = 12;
-        if (const char *v = std::getenv("ASTROZ_COPY_THREADS")) n = std::max(0, std::min(64, std::atoi(v)));
-        const unsigned hw = std::thread::hardware_concurrency();
-        if (hw && (unsigned)n > hw) n = (int)hw;
-        for (int i = 0; i < n; ++i) workers_.emplace_back([this] { loop(); });
-        for (auto &t : workers_) t.detach();
-    }
-    // bytes [b0, b1) of the logical contiguous source, scattered to rows of the destination
-    static void run(char *dst, const char *src, size_t, size_t, size_t rowBytes, size_t hpitch, size_t b0, size_t b1) {
-        if (hpitch == rowBytes) {
-            stream_copy(dst + b0, src + b0, b1 - b0);
-            return;
-        }
-        size_t b = b0;
-        while (b < b1) {
-            const size_t r = b / rowBytes, o = b % rowBytes;
-            const size_t len = std::min(rowBytes - o, b1 - b);
-            stream_copy(dst + r * hpitch + o, src + b, len);
-            b += len;
-        }
-    }
-    void push(std::function<void()> f) {
-        {
-            std::lock_guard<std::mutex> g(m_);
-            q_.push_back(std::move(f));
-        }
-        cv_.notify_one();
-    }
-    void loop() {
-        for (;;) {
-            std::function<void()> f;
-            {
-                std::unique_lock<std::mutex> g(m_);
-                cv_.wait(g, [&] { return !q_.empty(); });
-                f = std::move(q_.front());
-                q_.pop_front();
-            }
-            f();
-        }
-    }
-    std::vector<std::thread> workers_;
-    std::mutex m_;
-    std::condition_variable cv_;
-    std::deque<std::function<void()>> q_;
-};
-
-struct Piece {  // one ring-sized piece of a deferred delivery: rows x rowBytes, contiguous on the device
-    const char *dsrc;
-    char *hdst;
-    size_t rows, rowBytes, hpitch;
-    int chunk;  // the grid chunk whose kernels produce it (chunkDone[chunk])
-};
-
-bool is_pageable(const void *p) {
-    cudaPointerAttributes a{};
-    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
-        (void)cudaGetLastError();
-        return true;
-    }
-    return a.type == cudaMemoryTypeUnregistered;
+    return ASTROZ_OK;
 }
 
-template <typename T>
-struct DevBuf {  // grow-only device buffer
-    T *p = nullptr;
-    size_t cap = 0;
-    cudaError_t reserve(size_t n) {
-        if (n <= cap) return cudaSuccess;
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
-        cudaError_t e = cudaMalloc(&p, n * sizeof(T));
-        if (e == cudaSuccess) cap = n;
-        return e;
+// check_device_present, then ASTROZ_VALUE_ERROR unless `device` is one of the visible ordinals
+int32_t check_device_ordinal(int device) {
+    int count = 0;
+    const int32_t rc = check_device_present(&count, "no CUDA device available (this library has no CPU propagation path)");
+    if (rc != ASTROZ_OK) return rc;
+    if (device < 0 || device >= count) {
+        g_lastError = "device index out of range";
+        return ASTROZ_VALUE_ERROR;
     }
-    void release() {
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
-    }
-};
+    return ASTROZ_OK;
+}
+
+using az::DevBuf;
 
 // Worker threads of a multi-device handle: one per shard after the first (the caller's thread serves shard 0), parked on
 // a condition variable between calls, so a call does not wait for thread creation before its last shard's first launch.
@@ -268,14 +120,10 @@ struct Constellation {
     // without stalling on the previous call's asynchronous upload
     static constexpr int kSlots = 4;
     DevBuf<double> dTime;
-    double *hTimeSlot[kSlots] = {};
-    size_t hTimeSlotCap[kSlots] = {};
+    az::PinnedBuf<double> hTimeSlot[kSlots];
     cudaEvent_t slotCopied[kSlots] = {};
-    bool slotPending[kSlots] = {};
-    int slot = 0;
-    double *hTime = nullptr;          // the slot in use by the current call
-    cudaEvent_t timeCopied = nullptr;  // its event
-    bool timePending = false;          // kept for call sites: set after recording timeCopied
+    bool slotPending[kSlots] = {};  // slotCopied[k] was recorded after an upload from slot k
+    int slot = 0;                   // the slot of the current call
     // the time axis last uploaded by upload_time_axis: a repeated call with the same jd/fr (a propagation loop over a
     // fixed grid) reuses the device copy instead of re-uploading it
     std::vector<double> cachedJd, cachedFr;
@@ -286,8 +134,7 @@ struct Constellation {
     // stateless-path epoch offsets
     DevBuf<double> dToffCall;
     DevBuf<uint8_t> dMask;
-    double *hToffCall = nullptr;
-    size_t hToffCap = 0;
+    az::PinnedBuf<double> hToffCall;
     cudaEvent_t toffCopied = nullptr;
     bool toffPending = false;
     // resonance lattice (depends on the elements only; grown when a call reaches further in time)
@@ -304,12 +151,16 @@ struct Constellation {
     // coarse-screen scratch: hash heads / chains for one batch of epochs, hit buffers, counter
     DevBuf<uint32_t> dHead, dNext, dPairs, dTIdx;
     DevBuf<unsigned long long> dCount;
-    // kernel timing
-    cudaEvent_t ev[6] = {};  // K1 start/end, K2 start/end, whole call start/end
-    cudaEvent_t chunkDone[64] = {};
-    bool timed = false, spanTimed = false;
+    // kernel timing: start / end events of K1, K2 and the call's span (TimedSpan), and the set of them the last timed
+    // call recorded (bit k = ev[k])
+    cudaEvent_t ev[3][2] = {};
+    unsigned timedSet = 0;
     bool timing = false;  // kernel-time events are recorded only on request (astroz_cuda_constellation_set_timing): the
-                          // six timed event records per call cost stream time, which is not work
+                          // timed event records cost stream time, which is not work
+    cudaEvent_t chunkDone[64] = {};  // grid chunk k of a host-buffer propagate has finished
+    // the two-slot pipelines of the pairs call and sgp4_array: slot k's kernels / result copy have finished, and the
+    // current chunk's inputs are on the device
+    cudaEvent_t kernelDone[2] = {}, copyDone[2] = {}, inputsDone = nullptr;
     int variant = -1;  // -1 = shipped default; >= 0 selects a tuning variant (ASTROZ_SGP4_VARIANT)
     int chunks = 8;
     // Multi-device handle (device = -1 at creation): the catalog is cut into contiguous satellite ranges, one
@@ -322,32 +173,23 @@ struct Constellation {
     DevBuf<double> dFullPos, dFullVel; // per shard: the WHOLE block, for the replicated (all-gather) propagate
     ShardWorkers *workers = nullptr;   // multi-device handle: parked host threads, one per shard after the first
     bool multi() const { return !shards.empty(); }
-    // deferred delivery into pageable host memory (see CopyPool)
-    std::vector<Piece> plan;
-    char *ring = nullptr;
-    cudaEvent_t ringEv[kRingSlots] = {};
+    az::HostRing ring;  // pinned transfers from / to pageable caller memory
 
+    // The members are destroyed after this body, on the device it makes current.
     ~Constellation() {
         delete workers;  // joins them: no shard is in use after this line
         for (Constellation *sh : shards) delete sh;
         shards.clear();
         if (!stream) return;  // never opened on a device (a Satrec that was only inspected): nothing to release
         cudaSetDevice(device);
-        dTiles.release(); dToff.release(); dSgp4Orig.release(); dSdp4Orig.release(); dIdentity.release(); dSdp4Identity.release();
-        dSdp4.release(); dTime.release(); dToffCall.release(); dMask.release(); dLattice.release(); dPos.release(); dVel.release();
-        dHead.release(); dNext.release(); dPairs.release(); dTIdx.release(); dCount.release();
-        dFullPos.release(); dFullVel.release();
-        dRowKey.release(); dPairsKeys.release(); dPairsSort.release(); dPairsRange.release(); dPairsIn.release();
-        dPairsOut.release();
-        if (ring) cudaFreeHost(ring);
-        for (auto &e : ringEv) if (e) cudaEventDestroy(e);
-        for (auto &h : hTimeSlot) if (h) cudaFreeHost(h);
-        if (hToffCall) cudaFreeHost(hToffCall);
         for (auto &e : slotCopied) if (e) cudaEventDestroy(e);
         if (toffCopied) cudaEventDestroy(toffCopied);
         if (axisReady) cudaEventDestroy(axisReady);
-        for (auto &e : ev) if (e) cudaEventDestroy(e);
+        for (auto &pair : ev) for (auto &e : pair) if (e) cudaEventDestroy(e);
         for (auto &e : chunkDone) if (e) cudaEventDestroy(e);
+        for (auto &e : kernelDone) if (e) cudaEventDestroy(e);
+        for (auto &e : copyDone) if (e) cudaEventDestroy(e);
+        if (inputsDone) cudaEventDestroy(inputsDone);
         if (stream) cudaStreamDestroy(stream);
         if (copyStream) cudaStreamDestroy(copyStream);
         if (auxStream) cudaStreamDestroy(auxStream);
@@ -367,16 +209,8 @@ int32_t upload_toff(Constellation *c) {  // src/Constellation.zig:153
 }
 
 int32_t open_device(Constellation *c, int device) {
-    int count = 0;
-    cudaError_t e = cudaGetDeviceCount(&count);
-    if (e != cudaSuccess || count == 0) {
-        g_lastError = "no CUDA device available (this library has no CPU propagation path)";
-        return ASTROZ_NO_DEVICE;
-    }
-    if (device < 0 || device >= count) {
-        g_lastError = "device index out of range";
-        return ASTROZ_VALUE_ERROR;
-    }
+    const int32_t rc = check_device_ordinal(device);
+    if (rc != ASTROZ_OK) return rc;
     c->device = device;
     AZ_CUDA(cudaSetDevice(device));
     AZ_CUDA(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
@@ -387,9 +221,12 @@ int32_t open_device(Constellation *c, int device) {
     for (auto &e : c->slotCopied) AZ_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
     AZ_CUDA(cudaEventCreateWithFlags(&c->toffCopied, cudaEventDisableTiming));
     AZ_CUDA(cudaEventCreateWithFlags(&c->axisReady, cudaEventDisableTiming));
-    c->timeCopied = c->slotCopied[0];
-    for (auto &ev : c->ev) AZ_CUDA(cudaEventCreate(&ev));
+    for (auto &pair : c->ev)
+        for (auto &ev : pair) AZ_CUDA(cudaEventCreate(&ev));
     for (auto &ev : c->chunkDone) AZ_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+    for (auto &ev : c->kernelDone) AZ_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+    for (auto &ev : c->copyDone) AZ_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+    AZ_CUDA(cudaEventCreateWithFlags(&c->inputsDone, cudaEventDisableTiming));
     if (const char *v = std::getenv("ASTROZ_SGP4_VARIANT")) c->variant = std::atoi(v);
     if (const char *v = std::getenv("ASTROZ_SDP4_VARIANT")) az::set_sdp4_variant(std::atoi(v));
     if (const char *v = std::getenv("ASTROZ_TIMING")) c->timing = std::atoi(v) != 0;
@@ -514,10 +351,6 @@ int32_t ingest_on_device(Constellation *c, az::IngestArgs a, int grav) {
     DevBuf<uint32_t> counts;   // blockNear | blockDeep | totals[2]
     DevBuf<unsigned long long> fail;
     DevBuf<int32_t> classes;
-    struct Release {
-        DevBuf<uint8_t> &a; DevBuf<uint32_t> &b; DevBuf<unsigned long long> &c; DevBuf<int32_t> &d;
-        ~Release() { a.release(); b.release(); c.release(); d.release(); }
-    } release{flags, counts, fail, classes};
     AZ_CUDA(flags.reserve(a.n));
     AZ_CUDA(counts.reserve((size_t)blocks * 2 + 2));
     AZ_CUDA(fail.reserve(1));
@@ -581,29 +414,76 @@ int32_t ingest_on_device(Constellation *c, az::IngestArgs a, int grav) {
     return upload_toff(c);
 }
 
-// host staging for the time axis; waits for the previous call's async upload before reuse
-int32_t reserve_time(Constellation *c, size_t nt) {
-    c->cacheValid = false;  // every writer of dTime comes through here (or says so itself)
-    // the call that last used the current slot recorded slotCopied[slot] (timePending tells us so)
-    if (c->timePending) c->slotPending[c->slot] = true;
-    c->timePending = false;
+cudaStream_t call_stream(const Constellation *c, void *stream) {
+    return stream ? static_cast<cudaStream_t>(stream) : c->stream;
+}
+
+// ASTROZ_VALUE_ERROR for a multi-device handle at an entry point that works on one GPU
+int32_t refuse_multi(const Constellation *c) {
+    if (c && c->multi()) {
+        g_lastError = "this entry point works on ONE GPU: create the handle with device >= 0 (a device = -1 handle "
+                      "spans several GPUs)";
+        return ASTROZ_VALUE_ERROR;
+    }
+    return ASTROZ_OK;
+}
+
+// Column k of the device time axis dTime: tbase | jdFull | gsin | gcos
+double *time_col(Constellation *c, int k) { return c->dTime.p + (size_t)k * (c->dTime.cap / 4); }
+
+// Host staging for an nt-epoch time axis: the next pinned slot of the rotation, column k at *h + k * nt, once the
+// upload that last used it has finished.  Every writer of dTime comes through here (or says so itself).
+int32_t time_slot(Constellation *c, size_t nt, double **h) {
+    c->cacheValid = false;
     c->slot = (c->slot + 1) % Constellation::kSlots;
     const int k = c->slot;
     if (c->slotPending[k]) {  // kSlots calls ago: almost always long finished
         AZ_CUDA(cudaEventSynchronize(c->slotCopied[k]));
         c->slotPending[k] = false;
     }
-    if (nt * 4 > c->hTimeSlotCap[k]) {
-        if (c->hTimeSlot[k]) cudaFreeHost(c->hTimeSlot[k]);
-        c->hTimeSlot[k] = nullptr;
-        c->hTimeSlotCap[k] = 0;
-        AZ_CUDA(cudaMallocHost(&c->hTimeSlot[k], nt * 4 * 8));
-        c->hTimeSlotCap[k] = nt * 4;
-    }
-    c->hTime = c->hTimeSlot[k];
-    c->timeCopied = c->slotCopied[k];
+    AZ_CUDA(c->hTimeSlot[k].reserve(nt * 4));
     AZ_CUDA(c->dTime.reserve(nt * 4));
+    *h = c->hTimeSlot[k].p;
     return ASTROZ_OK;
+}
+
+// Queue the upload of the staged columns `cols` (bit k = column k) of the current slot and mark the slot in flight.
+int32_t upload_time_slot(Constellation *c, size_t nt, unsigned cols, cudaStream_t s) {
+    const double *h = c->hTimeSlot[c->slot].p;
+    for (int k = 0; k < 4; ++k)
+        if (cols & (1u << k))
+            AZ_CUDA(cudaMemcpyAsync(time_col(c, k), h + k * nt, nt * 8, cudaMemcpyHostToDevice, s));
+    AZ_CUDA(cudaEventRecord(c->slotCopied[c->slot], s));
+    c->slotPending[c->slot] = true;
+    return ASTROZ_OK;
+}
+
+// Per-call epoch offsets of the stateless near-earth path, padded to whole tiles, into dToffCall on s.
+int32_t stage_epoch_offsets(Constellation *c, const double *offsets, cudaStream_t s) {
+    const uint32_t ns = c->cat.nSgp4, padded = c->cat.sgp4Padded();
+    if (c->toffPending) {  // the previous call's upload of the offsets must have left the staging buffer
+        AZ_CUDA(cudaEventSynchronize(c->toffCopied));
+        c->toffPending = false;
+    }
+    AZ_CUDA(c->hToffCall.reserve(padded));
+    for (uint32_t i = 0; i < padded; ++i) c->hToffCall.p[i] = offsets[std::min(i, ns - 1)];
+    AZ_CUDA(c->dToffCall.reserve(padded));
+    AZ_CUDA(cudaMemcpyAsync(c->dToffCall.p, c->hToffCall.p, (size_t)padded * 8, cudaMemcpyHostToDevice, s));
+    AZ_CUDA(cudaEventRecord(c->toffCopied, s));
+    c->toffPending = true;
+    return ASTROZ_OK;
+}
+
+// Kernel timing (astroz_cuda_constellation_last_kernel_ms).  A timed call starts a new record with time_begin, then
+// marks the start and end of each span it times; events are recorded only while timing is on.
+enum TimedSpan { kTimeK1 = 0, kTimeK2 = 1, kTimeSpan = 2 };
+
+void time_begin(Constellation *c) { c->timedSet = 0; }
+
+cudaError_t time_mark(Constellation *c, TimedSpan k, bool end, cudaStream_t s) {
+    if (!c->timing) return cudaSuccess;
+    if (end) c->timedSet |= 1u << k;
+    return cudaEventRecord(c->ev[k][end], s);
 }
 
 int32_t ensure_lattice(Constellation *c, int nodes, cudaStream_t s) {
@@ -635,15 +515,14 @@ int32_t queue_grid(Constellation *c, const Launch &L, uint32_t ntTotal, double *
                    int mode, int layout, uint32_t outNumSats, uint32_t outSatOffset, cudaStream_t s, bool timeIt,
                    const GatherTargets *gt = nullptr) {
     const az::CatalogTables &t = c->cat;
-    const size_t tcap = c->dTime.cap / 4;
     az::GridArgs a;
     a.g = c->g;
     a.nTimes = (layout == 0) ? ntTotal : L.nt;  // satellite-major rows are ntTotal long
     a.outNumSats = outNumSats;
-    a.tbase = c->dTime.p + L.t0;
-    a.jdFull = c->dTime.p + tcap + L.t0;
-    a.gsin = c->dTime.p + 2 * tcap + L.t0;
-    a.gcos = c->dTime.p + 3 * tcap + L.t0;
+    a.tbase = time_col(c, 0) + L.t0;
+    a.jdFull = time_col(c, 1) + L.t0;
+    a.gsin = time_col(c, 2) + L.t0;
+    a.gcos = time_col(c, 3) + L.t0;
     // outputs: rows are shifted by outSatOffset, epochs by t0
     size_t shift;
     if (layout == 0) shift = ((size_t)outSatOffset * ntTotal + L.t0) * 3;
@@ -665,37 +544,32 @@ int32_t queue_grid(Constellation *c, const Launch &L, uint32_t ntTotal, double *
         g_lastError = "internal: satellite-major launches cover the whole time axis";
         return ASTROZ_UNKNOWN;
     }
-    timeIt = timeIt && c->timing;
     const bool doK1 = L.tileCount && t.nSgp4, doK2 = L.deepSpace && t.nSdp4;
     // A mixed call runs its two grids side by side: the deep-space grid is small (a few waves of CTAs at lower
     // fp64-pipe utilisation) and goes first, on the auxiliary stream, so the near-earth CTAs fill the SMs as it drains.
     const bool fork = doK1 && doK2;
     cudaStream_t s2 = fork ? c->auxStream : s;
     if (timeIt) {
-        if (c->timing) AZ_CUDA(cudaEventRecord(c->ev[4], s));
-        c->spanTimed = true;
+        time_begin(c);
+        AZ_CUDA(time_mark(c, kTimeSpan, false, s));
     }
     if (fork) {
         AZ_CUDA(cudaEventRecord(c->forkEv, s));
         AZ_CUDA(cudaStreamWaitEvent(s2, c->forkEv, 0));
     }
-    if (!fork && timeIt) AZ_CUDA(cudaEventRecord(c->ev[0], s));
-    if (fork || !doK1) {
-        if (timeIt && !fork) AZ_CUDA(cudaEventRecord(c->ev[1], s));
-        if (timeIt) AZ_CUDA(cudaEventRecord(c->ev[2], s2));
-        if (doK2) {
-            az::GridArgs k2 = a;
-            k2.sdp4 = c->dSdp4.p;
-            k2.orig = c->dSdp4Orig.p;
-            k2.nSats = t.nSdp4;
-            k2.lattice = c->dLattice.p;
-            k2.latticeNodes = c->latticeNodes;
-            AZ_CUDA(az::launch_sdp4_grid(k2, mode, layout, s2));
-        }
-        if (timeIt) AZ_CUDA(cudaEventRecord(c->ev[3], s2));
+    if (doK2) {
+        if (timeIt) AZ_CUDA(time_mark(c, kTimeK2, false, s2));
+        az::GridArgs k2 = a;
+        k2.sdp4 = c->dSdp4.p;
+        k2.orig = c->dSdp4Orig.p;
+        k2.nSats = t.nSdp4;
+        k2.lattice = c->dLattice.p;
+        k2.latticeNodes = c->latticeNodes;
+        AZ_CUDA(az::launch_sdp4_grid(k2, mode, layout, s2));
+        if (timeIt) AZ_CUDA(time_mark(c, kTimeK2, true, s2));
     }
     if (doK1) {
-        if (fork && timeIt) AZ_CUDA(cudaEventRecord(c->ev[0], s));
+        if (timeIt) AZ_CUDA(time_mark(c, kTimeK1, false, s));
         az::GridArgs k1 = a;
         k1.sgp4Tiles = c->dTiles.p + (size_t)L.tile0 * az::kSgp4TileDoubles;
         k1.toff = c->dToff.p + (size_t)L.tile0 * az::kTileSats;
@@ -703,17 +577,13 @@ int32_t queue_grid(Constellation *c, const Launch &L, uint32_t ntTotal, double *
         const uint32_t first = L.tile0 * az::kTileSats;
         k1.nSats = std::min<uint32_t>(t.nSgp4 - first, L.tileCount * az::kTileSats);
         AZ_CUDA(az::launch_sgp4_grid(k1, mode, layout, s, c->variant));
-        if (timeIt) AZ_CUDA(cudaEventRecord(c->ev[1], s));
-        if (!fork && timeIt) {
-            if (c->timing) AZ_CUDA(cudaEventRecord(c->ev[2], s));
-            if (c->timing) AZ_CUDA(cudaEventRecord(c->ev[3], s));
-        }
+        if (timeIt) AZ_CUDA(time_mark(c, kTimeK1, true, s));
     }
     if (fork) {
         AZ_CUDA(cudaEventRecord(c->joinEv, s2));
         AZ_CUDA(cudaStreamWaitEvent(s, c->joinEv, 0));
     }
-    if (timeIt) AZ_CUDA(cudaEventRecord(c->ev[5], s));
+    if (timeIt) AZ_CUDA(time_mark(c, kTimeSpan, true, s));
     return ASTROZ_OK;
 }
 
@@ -729,11 +599,10 @@ int32_t upload_time_axis(Constellation *c, const double *jd, const double *fr, u
         if (s != c->axisStream) AZ_CUDA(cudaStreamWaitEvent(s, c->axisReady, 0));
         return ASTROZ_OK;
     }
-    c->cacheValid = false;
-    int32_t rc = reserve_time(c, nt);
+    double *tb;
+    int32_t rc = time_slot(c, nt, &tb);
     if (rc != ASTROZ_OK) return rc;
-    const size_t cap = c->dTime.cap / 4;
-    double *tb = c->hTime, *jf = c->hTime + nt, *gs = c->hTime + 2 * (size_t)nt, *gc = c->hTime + 3 * (size_t)nt;
+    double *jf = tb + nt, *gs = tb + 2 * (size_t)nt, *gc = tb + 3 * (size_t)nt;
     double lo = INFINITY, hi = -INFINITY;
     for (uint32_t t = 0; t < nt; ++t) {
         const double j = jd[t] + fr[t];
@@ -749,11 +618,8 @@ int32_t upload_time_axis(Constellation *c, const double *jd, const double *fr, u
     }
     *jdMin = lo;
     *jdMax = hi;
-    const int arrays = (mode != 0) ? 4 : 2;
-    for (int k = 0; k < arrays; ++k)
-        AZ_CUDA(cudaMemcpyAsync(c->dTime.p + k * cap, c->hTime + (size_t)k * nt, (size_t)nt * 8, cudaMemcpyHostToDevice, s));
-    AZ_CUDA(cudaEventRecord(c->timeCopied, s));
-    c->timePending = true;
+    rc = upload_time_slot(c, nt, (mode != 0) ? 0xFu : 0x3u, s);
+    if (rc != ASTROZ_OK) return rc;
     AZ_CUDA(cudaEventRecord(c->axisReady, s));
     c->axisStream = s;
     c->cachedJd.assign(jd, jd + nt);
@@ -782,8 +648,16 @@ int32_t check_args(Constellation *c, const void *jd, const void *fr, const void 
     return ASTROZ_OK;
 }
 
+// Open a freshly built handle on `device` (finish_create_any) and hand it to the caller; freed on failure.
+int32_t publish(std::unique_ptr<Constellation> c, int device, astroz_constellation_t *out) {
+    const int32_t rc = finish_create_any(c.get(), device);
+    if (rc != ASTROZ_OK) return rc;
+    *out = c.release();
+    return ASTROZ_OK;
+}
+
 struct Sgp4Single {
-    Constellation *c = nullptr;
+    std::unique_ptr<Constellation> c;
     int device = 0;
     bool opened = false;  // streams, events and the device tables are created by the first propagation call
     double epochJd = 0;
@@ -835,20 +709,11 @@ int32_t astroz_cuda_constellation_create(const char *const *line1, const char *c
                                          int32_t device, astroz_constellation_t *out) {
     if (!out || (n && (!line1 || !line2))) return ASTROZ_NULL_POINTER;
     *out = nullptr;
-    Constellation *c = new (std::nothrow) Constellation();
+    std::unique_ptr<Constellation> c(new (std::nothrow) Constellation());
     if (!c) return ASTROZ_ALLOC_FAILED;
-    int rc = az::build_catalog(line1, line2, n, grav, c->cat);
-    if (rc != az::kOk) {
-        delete c;
-        return status_to_code(rc);
-    }
-    int32_t e = finish_create_any(c, device);
-    if (e != ASTROZ_OK) {
-        delete c;
-        return e;
-    }
-    *out = c;
-    return ASTROZ_OK;
+    const int rc = az::build_catalog(line1, line2, n, grav, c->cat);
+    if (rc != az::kOk) return status_to_code(rc);
+    return publish(std::move(c), device, out);
 }
 
 int32_t astroz_cuda_constellation_create_from_text(const char *text, size_t len, int32_t grav, int32_t device,
@@ -885,20 +750,11 @@ int32_t astroz_cuda_constellation_create_from_elements(const double *epoch_jd, c
         t.maDeg = ma_deg[i];
         t.bstar = bstar[i];
     }
-    Constellation *c = new (std::nothrow) Constellation();
+    std::unique_ptr<Constellation> c(new (std::nothrow) Constellation());
     if (!c) return ASTROZ_ALLOC_FAILED;
-    int rc = az::build_catalog_records(recs.data(), n, grav, c->cat);
-    if (rc != az::kOk) {
-        delete c;
-        return status_to_code(rc);
-    }
-    int32_t e = finish_create_any(c, device);
-    if (e != ASTROZ_OK) {
-        delete c;
-        return e;
-    }
-    *out = c;
-    return ASTROZ_OK;
+    const int rc = az::build_catalog_records(recs.data(), n, grav, c->cat);
+    if (rc != az::kOk) return status_to_code(rc);
+    return publish(std::move(c), device, out);
 }
 
 int32_t astroz_cuda_constellation_create_from_elements_device(
@@ -909,27 +765,23 @@ int32_t astroz_cuda_constellation_create_from_elements_device(
                        !d_ma_deg || !d_bstar)))
         return ASTROZ_NULL_POINTER;
     *out = nullptr;
-    Constellation *c = new (std::nothrow) Constellation();
+    std::unique_ptr<Constellation> c(new (std::nothrow) Constellation());
     if (!c) return ASTROZ_ALLOC_FAILED;
-    int32_t e = open_device(c, device);
-    if (e == ASTROZ_OK) {
-        az::IngestArgs a;
-        a.epochJd = d_epoch_jd;
-        a.revPerDay = d_mean_motion_rev_day;
-        a.ecc = d_ecc;
-        a.inclDeg = d_incl_deg;
-        a.raanDeg = d_raan_deg;
-        a.argpDeg = d_argp_deg;
-        a.maDeg = d_ma_deg;
-        a.bstar = d_bstar;
-        a.n = n;
-        e = ingest_on_device(c, a, grav);
-    }
-    if (e != ASTROZ_OK) {
-        delete c;
-        return e;
-    }
-    *out = c;
+    int32_t e = open_device(c.get(), device);
+    if (e != ASTROZ_OK) return e;
+    az::IngestArgs a;
+    a.epochJd = d_epoch_jd;
+    a.revPerDay = d_mean_motion_rev_day;
+    a.ecc = d_ecc;
+    a.inclDeg = d_incl_deg;
+    a.raanDeg = d_raan_deg;
+    a.argpDeg = d_argp_deg;
+    a.maDeg = d_ma_deg;
+    a.bstar = d_bstar;
+    a.n = n;
+    e = ingest_on_device(c.get(), a, grav);
+    if (e != ASTROZ_OK) return e;
+    *out = c.release();
     return ASTROZ_OK;
 }
 
@@ -989,8 +841,8 @@ int32_t astroz_cuda_constellation_propagate_device(astroz_constellation_t h, con
                                                    int32_t mode, int32_t layout, uint32_t out_num_sats,
                                                    uint32_t out_sat_offset, void *stream) {
     Constellation *c = static_cast<Constellation *>(h);
-    AZ_SINGLE(c);
-    int32_t rc = check_args(c, jd, fr, d_pos, mode, layout);
+    int32_t rc = refuse_multi(c);
+    if (rc == ASTROZ_OK) rc = check_args(c, jd, fr, d_pos, mode, layout);
     if (rc != ASTROZ_OK) return rc;
     if (n_times == 0 || c->cat.n == 0) return ASTROZ_OK;
     if (out_num_sats < out_sat_offset + c->cat.n) {  // src/Constellation.zig:255-257 reports a short buffer this way
@@ -998,7 +850,7 @@ int32_t astroz_cuda_constellation_propagate_device(astroz_constellation_t h, con
         return ASTROZ_DECAYED;
     }
     AZ_CUDA(cudaSetDevice(c->device));
-    cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
+    cudaStream_t s = call_stream(c, stream);
     double jdMin, jdMax;
     rc = upload_time_axis(c, jd, fr, n_times, mode, s, &jdMin, &jdMax);
     if (rc != ASTROZ_OK) return rc;
@@ -1007,9 +859,7 @@ int32_t astroz_cuda_constellation_propagate_device(astroz_constellation_t h, con
     Launch L;
     L.tileCount = c->cat.sgp4Tiles_count();
     L.nt = n_times;
-    rc = queue_grid(c, L, n_times, d_pos, d_vel, d_status, mode, layout, out_num_sats, out_sat_offset, s, true);
-    c->timed = (rc == ASTROZ_OK) && c->timing;
-    return rc;
+    return queue_grid(c, L, n_times, d_pos, d_vel, d_status, mode, layout, out_num_sats, out_sat_offset, s, true);
 }
 
 // ---- deep-space members only (Constellation.propagateSdp4Constellation, src/Constellation.zig:611-674) --------
@@ -1028,14 +878,13 @@ static int32_t sdp4_into_common(Constellation *c, const double *jd, const double
     if (rc != ASTROZ_OK) return rc;
     rc = prepare_deep_space(c, jdMin, jdMax, s);
     if (rc != ASTROZ_OK) return rc;
-    const size_t tcap = c->dTime.cap / 4;
     az::GridArgs a;
     a.g = c->g;
     a.nTimes = nt;
     a.outNumSats = outNumSats;
-    a.jdFull = c->dTime.p + tcap;
-    a.gsin = c->dTime.p + 2 * tcap;
-    a.gcos = c->dTime.p + 3 * tcap;
+    a.jdFull = time_col(c, 1);
+    a.gsin = time_col(c, 2);
+    a.gcos = time_col(c, 3);
     const size_t shift = (layout == 0) ? (size_t)satOffset * nt * 3 : (size_t)satOffset * 3;
     a.pos = dPos + shift;
     a.vel = dVel ? dVel + shift : nullptr;
@@ -1044,13 +893,10 @@ static int32_t sdp4_into_common(Constellation *c, const double *jd, const double
     a.nSats = nd;
     a.lattice = c->dLattice.p;
     a.latticeNodes = c->latticeNodes;
-    if (c->timing) AZ_CUDA(cudaEventRecord(c->ev[0], s));
-    if (c->timing) AZ_CUDA(cudaEventRecord(c->ev[1], s));
-    if (c->timing) AZ_CUDA(cudaEventRecord(c->ev[2], s));
+    time_begin(c);
+    AZ_CUDA(time_mark(c, kTimeK2, false, s));
     AZ_CUDA(az::launch_sdp4_grid(a, mode, layout, s));
-    if (c->timing) AZ_CUDA(cudaEventRecord(c->ev[3], s));
-    c->timed = c->timing;
-    c->spanTimed = false;
+    AZ_CUDA(time_mark(c, kTimeK2, true, s));
     return ASTROZ_OK;
 }
 
@@ -1067,15 +913,15 @@ int32_t astroz_cuda_sdp4_propagate_into_device(astroz_constellation_t h, const d
                                                uint32_t n_times, double *d_pos, double *d_vel, int32_t mode,
                                                int32_t layout, uint32_t out_num_sats, uint32_t sat_offset, void *stream) {
     Constellation *c = static_cast<Constellation *>(h);
-    AZ_SINGLE(c);
-    int32_t rc = check_args(c, jd, fr, d_pos, mode, layout);
+    int32_t rc = refuse_multi(c);
+    if (rc == ASTROZ_OK) rc = check_args(c, jd, fr, d_pos, mode, layout);
     if (rc != ASTROZ_OK) return rc;
     if (n_times == 0 || c->cat.nSdp4 == 0) return ASTROZ_OK;
     uint32_t rows;
     rc = sdp4_into_check(c, out_num_sats, sat_offset, &rows);
     if (rc != ASTROZ_OK) return rc;
     AZ_CUDA(cudaSetDevice(c->device));
-    cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
+    cudaStream_t s = call_stream(c, stream);
     return sdp4_into_common(c, jd, fr, n_times, d_pos, d_vel, mode, layout, rows, sat_offset, s);
 }
 
@@ -1083,8 +929,8 @@ int32_t astroz_cuda_sdp4_propagate_into(astroz_constellation_t h, const double *
                                         double *pos, double *vel, int32_t mode, int32_t layout, uint32_t out_num_sats,
                                         uint32_t sat_offset) {
     Constellation *c = static_cast<Constellation *>(h);
-    AZ_SINGLE(c);
-    int32_t rc = check_args(c, jd, fr, pos, mode, layout);
+    int32_t rc = refuse_multi(c);
+    if (rc == ASTROZ_OK) rc = check_args(c, jd, fr, pos, mode, layout);
     if (rc != ASTROZ_OK) return rc;
     const uint32_t nd = c->cat.nSdp4;
     if (n_times == 0 || nd == 0) return ASTROZ_OK;
@@ -1118,11 +964,11 @@ int32_t astroz_cuda_constellation_propagate_device_f32(astroz_constellation_t h,
                                                        uint32_t n_times, double *d_pos, double *d_vel, int32_t phase64,
                                                        void *stream) {
     Constellation *c = static_cast<Constellation *>(h);
-    AZ_SINGLE(c);
+    if (const int32_t rc = refuse_multi(c); rc != ASTROZ_OK) return rc;
     if (!c || !jd || !fr || !d_pos || !d_vel) return ASTROZ_NULL_POINTER;
     if (n_times == 0 || c->cat.nSgp4 == 0) return ASTROZ_OK;
     AZ_CUDA(cudaSetDevice(c->device));
-    cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
+    cudaStream_t s = call_stream(c, stream);
     double jdMin, jdMax;
     int32_t rc = upload_time_axis(c, jd, fr, n_times, ASTROZ_MODE_TEME, s, &jdMin, &jdMax);
     if (rc != ASTROZ_OK) return rc;
@@ -1132,18 +978,15 @@ int32_t astroz_cuda_constellation_propagate_device_f32(astroz_constellation_t h,
     a.toff = c->dToff.p;
     a.orig = c->dSgp4Orig.p;
     a.nSats = c->cat.nSgp4;
-    a.tbase = c->dTime.p;
+    a.tbase = time_col(c, 0);
     a.nTimes = n_times;
     a.pos = d_pos;
     a.vel = d_vel;
     a.outNumSats = c->cat.n;
-    if (c->timing) AZ_CUDA(cudaEventRecord(c->ev[0], s));
+    time_begin(c);
+    AZ_CUDA(time_mark(c, kTimeK1, false, s));
     AZ_CUDA(az::launch_sgp4_grid_f32(a, phase64, s));
-    if (c->timing) AZ_CUDA(cudaEventRecord(c->ev[1], s));
-    if (c->timing) AZ_CUDA(cudaEventRecord(c->ev[2], s));
-    if (c->timing) AZ_CUDA(cudaEventRecord(c->ev[3], s));
-    c->timed = c->timing;
-    c->spanTimed = false;
+    AZ_CUDA(time_mark(c, kTimeK1, true, s));
     return ASTROZ_OK;
 }
 
@@ -1152,7 +995,7 @@ int32_t astroz_cuda_constellation_propagate_gather(astroz_constellation_t h, con
                                                    uint32_t n_peers, void *mc_pos, void *mc_vel, uint32_t out_num_sats,
                                                    uint32_t out_sat_offset, void *stream) {
     Constellation *c = static_cast<Constellation *>(h);
-    AZ_SINGLE(c);
+    if (const int32_t rc = refuse_multi(c); rc != ASTROZ_OK) return rc;
     if (!c || !jd || !fr) return ASTROZ_NULL_POINTER;
     if (!mc_pos && (!peer_pos || n_peers == 0)) return ASTROZ_NULL_POINTER;
     if (n_peers > (uint32_t)az::kMaxPeers) {
@@ -1175,7 +1018,7 @@ int32_t astroz_cuda_constellation_propagate_gather(astroz_constellation_t h, con
         if (!gt.peerPos[p]) return ASTROZ_NULL_POINTER;
     }
     AZ_CUDA(cudaSetDevice(c->device));
-    cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
+    cudaStream_t s = call_stream(c, stream);
     double jdMin, jdMax;
     int32_t rc = upload_time_axis(c, jd, fr, n_times, ASTROZ_MODE_TEME, s, &jdMin, &jdMax);
     if (rc != ASTROZ_OK) return rc;
@@ -1184,77 +1027,8 @@ int32_t astroz_cuda_constellation_propagate_gather(astroz_constellation_t h, con
     Launch L;
     L.tileCount = c->cat.sgp4Tiles_count();
     L.nt = n_times;
-    rc = queue_grid(c, L, n_times, nullptr, nullptr, nullptr, ASTROZ_MODE_TEME, ASTROZ_LAYOUT_SATELLITE_MAJOR,
-                    out_num_sats, out_sat_offset, s, true, &gt);
-    c->timed = (rc == ASTROZ_OK) && c->timing;
-    return rc;
-}
-
-// Send `rows` rows of rowBytes (contiguous on the device at dsrc) to the host at hdst with pitch hpitch, after the
-// kernels of grid chunk `chunk`.  Pinned / registered destinations get the copy queued on the copy stream right away;
-// pageable ones are recorded as ring-sized pieces and delivered by run_ring() in the wait half of the call.
-static int32_t deliver(Constellation *c, bool pageable, int chunk, const double *dsrc, double *hdst, size_t rows,
-                       size_t rowBytes, size_t hpitch) {
-    if (!pageable) {
-        if (rows == 1 || hpitch == rowBytes)
-            AZ_CUDA(cudaMemcpyAsync(hdst, dsrc, rows * rowBytes, cudaMemcpyDeviceToHost, c->copyStream));
-        else
-            AZ_CUDA(cudaMemcpy2DAsync(hdst, hpitch, dsrc, rowBytes, rowBytes, rows, cudaMemcpyDeviceToHost, c->copyStream));
-        return ASTROZ_OK;
-    }
-    const char *src = reinterpret_cast<const char *>(dsrc);
-    char *dst = reinterpret_cast<char *>(hdst);
-    if (rows == 1 || hpitch == rowBytes) {  // one contiguous run: cut by bytes
-        const size_t total = rows * rowBytes;
-        for (size_t b = 0; b < total; b += kPieceBytes)
-            c->plan.push_back(Piece{src + b, dst + b, 1, std::min(kPieceBytes, total - b), std::min(kPieceBytes, total - b), chunk});
-    } else if (rowBytes > kPieceBytes) {     // very wide rows: each row cut by bytes
-        for (size_t r = 0; r < rows; ++r)
-            for (size_t b = 0; b < rowBytes; b += kPieceBytes)
-                c->plan.push_back(Piece{src + r * rowBytes + b, dst + r * hpitch + b, 1, std::min(kPieceBytes, rowBytes - b),
-                                        std::min(kPieceBytes, rowBytes - b), chunk});
-    } else {                                // whole rows per piece
-        const size_t per = std::max<size_t>(1, kPieceBytes / rowBytes);
-        for (size_t r = 0; r < rows; r += per)
-            c->plan.push_back(Piece{src + r * rowBytes, dst + r * hpitch, std::min(per, rows - r), rowBytes, hpitch, chunk});
-    }
-    return ASTROZ_OK;
-}
-
-// Drain the deferred deliveries of one handle: up to kRingSlots pieces in flight over PCIe while the pool copies the
-// landed one to its final place.
-static int32_t run_ring(Constellation *c) {
-    if (c->plan.empty()) return ASTROZ_OK;
-    AZ_CUDA(cudaSetDevice(c->device));
-    if (!c->ring) {
-        AZ_CUDA(cudaMallocHost(&c->ring, kPieceBytes * kRingSlots));
-        for (auto &e : c->ringEv) AZ_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    }
-    CopyPool &pool = CopyPool::get();
-    const size_t n = c->plan.size();
-    auto issue = [&](size_t i) -> cudaError_t {
-        const Piece &p = c->plan[i];
-        const int slot = (int)(i % kRingSlots);
-        cudaError_t e = cudaStreamWaitEvent(c->copyStream, c->chunkDone[p.chunk], 0);
-        if (e == cudaSuccess)
-            e = cudaMemcpyAsync(c->ring + (size_t)slot * kPieceBytes, p.dsrc, p.rows * p.rowBytes, cudaMemcpyDeviceToHost,
-                                c->copyStream);
-        if (e == cudaSuccess) e = cudaEventRecord(c->ringEv[slot], c->copyStream);
-        return e;
-    };
-    cudaError_t e = cudaSuccess;
-    for (size_t i = 0; i < std::min<size_t>(kRingSlots, n) && e == cudaSuccess; ++i) e = issue(i);
-    for (size_t i = 0; i < n && e == cudaSuccess; ++i) {
-        const int slot = (int)(i % kRingSlots);
-        e = cudaEventSynchronize(c->ringEv[slot]);
-        if (e != cudaSuccess) break;
-        const Piece &p = c->plan[i];
-        pool.copy(p.hdst, c->ring + (size_t)slot * kPieceBytes, p.rows, p.rowBytes, p.hpitch);
-        if (i + kRingSlots < n) e = issue(i + kRingSlots);
-    }
-    c->plan.clear();
-    if (e != cudaSuccess) return cuda_fail(e, "pageable delivery ring");
-    return ASTROZ_OK;
+    return queue_grid(c, L, n_times, nullptr, nullptr, nullptr, ASTROZ_MODE_TEME, ASTROZ_LAYOUT_SATELLITE_MAJOR,
+                      out_num_sats, out_sat_offset, s, true, &gt);
 }
 
 // Host-buffer propagate, in a queue half and a wait half (deliveries to pageable memory are drained in the latter):
@@ -1290,9 +1064,12 @@ static int32_t propagate_host_queue(Constellation *c, const double *jd, const do
     // launch: time chunks that start on multiples of 192 keep every thread's set of epochs -- and with it the series each
     // cell takes, i.e. every result bit -- the same however the call is chunked (one device or many, any chunk count)
     if (byTime && nChunks > 1) per = (per + 191) / 192 * 192;
-    const bool posPageable = is_pageable(pos), velPageable = vel && is_pageable(vel);
-    c->plan.clear();
-    if (c->timing) AZ_CUDA(cudaEventRecord(c->ev[4], s));  // whole-call span: first kernel of the first chunk ...
+    const bool posPageable = az::is_pageable(pos), velPageable = vel && az::is_pageable(vel);
+    c->ring.discard();
+    // last_kernel_ms after a host-buffer call: the span from the first kernel of the first chunk to the last kernel of
+    // the last chunk (copies overlapping) in all three slots
+    time_begin(c);
+    AZ_CUDA(time_mark(c, kTimeSpan, false, s));
     for (uint32_t k = 0; k < nChunks; ++k) {
         const uint32_t u0 = k * per, u1 = std::min(units, u0 + per);
         if (u0 >= u1) break;
@@ -1320,34 +1097,26 @@ static int32_t propagate_host_queue(Constellation *c, const double *jd, const do
             double *hdst = which ? vel : pos;
             const double *dsrc = (which ? dVel : dPos) + off;
             const bool pg = which ? velPageable : posPageable;
+            const cudaEvent_t ready = c->chunkDone[k];
             if (layout == 0) {  // this handle's rows are one contiguous run of the (possibly wider) host block
-                rc = deliver(c, pg, (int)k, dsrc, hdst + (size_t)rowOffset * n_times * 3 + off, 1, cnt * 8, cnt * 8);
+                AZ_CUDA(c->ring.deliver(pg, ready, dsrc, hdst + (size_t)rowOffset * n_times * 3 + off, 1, cnt * 8, cnt * 8,
+                                        c->copyStream));
             } else if (totalRows == n) {
-                rc = deliver(c, pg, (int)k, dsrc, hdst + off, 1, cnt * 8, cnt * 8);
+                AZ_CUDA(c->ring.deliver(pg, ready, dsrc, hdst + off, 1, cnt * 8, cnt * 8, c->copyStream));
             } else {            // time-major into a wider block: n*24 bytes per epoch at a pitch of totalRows*24
-                rc = deliver(c, pg, (int)k, dsrc, hdst + ((size_t)u0 * totalRows + rowOffset) * 3, u1 - u0, (size_t)n * 24,
-                             (size_t)totalRows * 24);
+                AZ_CUDA(c->ring.deliver(pg, ready, dsrc, hdst + ((size_t)u0 * totalRows + rowOffset) * 3, u1 - u0,
+                                        (size_t)n * 24, (size_t)totalRows * 24, c->copyStream));
             }
-            if (rc != ASTROZ_OK) return rc;
         }
     }
-    if (c->timing) AZ_CUDA(cudaEventRecord(c->ev[5], s));  // ... to the last kernel of the last chunk
-    // last_kernel_ms after a host-buffer call: ms[1] = the span above (all chunks, copies overlapping); the per-kernel
-    // slots repeat it
-    if (c->timing) AZ_CUDA(cudaEventRecord(c->ev[0], s));
-    if (c->timing) AZ_CUDA(cudaEventRecord(c->ev[1], s));
-    if (c->timing) AZ_CUDA(cudaEventRecord(c->ev[2], s));
-    if (c->timing) AZ_CUDA(cudaEventRecord(c->ev[3], s));
-    c->timed = c->timing;
-    c->spanTimed = true;
+    AZ_CUDA(time_mark(c, kTimeSpan, true, s));
     return ASTROZ_OK;
 }
 
 static int32_t propagate_host_wait(Constellation *c) {
     if (!c->stream) return ASTROZ_OK;
     AZ_CUDA(cudaSetDevice(c->device));
-    const int32_t rr = run_ring(c);
-    if (rr != ASTROZ_OK) return rr;
+    AZ_CUDA(c->ring.drain(c->copyStream));
     AZ_CUDA(cudaStreamSynchronize(c->copyStream));
     AZ_CUDA(cudaStreamSynchronize(c->stream));
     return ASTROZ_OK;
@@ -1480,16 +1249,13 @@ static int32_t pairs_queue(Constellation *c, const uint32_t *dSat, const double 
     a.status = dStatus;
     a.g = c->g;
     AZ_CUDA(az::launch_pairs(a, mode, s));
-    c->timed = false;
+    time_begin(c);  // the pairs kernels are not timed
     return ASTROZ_OK;
 }
 
 static int32_t pairs_check(Constellation *c, int32_t mode) {
     if (!c) return ASTROZ_NULL_POINTER;
-    if (c->multi()) {
-        g_lastError = "pairs propagation needs a single-device handle (create it with device >= 0)";
-        return ASTROZ_VALUE_ERROR;
-    }
+    if (const int32_t rc = refuse_multi(c); rc != ASTROZ_OK) return rc;
     if (mode < 0 || mode > 2) {
         g_lastError = "invalid output mode";
         return ASTROZ_VALUE_ERROR;
@@ -1507,7 +1273,7 @@ int32_t astroz_cuda_constellation_propagate_pairs_device(astroz_constellation_t 
     if (n == 0) return ASTROZ_OK;
     if (!d_sat || !d_jd || !d_fr || !d_pos) return ASTROZ_NULL_POINTER;
     AZ_CUDA(cudaSetDevice(c->device));
-    cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
+    cudaStream_t s = call_stream(c, stream);
     if (c->cat.nSdp4) {
         // the resonance lattice is grown to the furthest query: min / max of jd + fr on the device, 16 bytes back
         // (this call's one synchronisation point)
@@ -1560,19 +1326,12 @@ int32_t astroz_cuda_constellation_propagate_pairs(astroz_constellation_t h, cons
     const size_t outD = (size_t)chunk * (vel ? 6 : 3) + (status ? (chunk + 7) / 8 : 0);
     AZ_CUDA(c->dPairsIn.reserve(inD * slots));
     AZ_CUDA(c->dPairsOut.reserve(outD * slots));
-    const bool inPageable = is_pageable(sat) || is_pageable(jd) || is_pageable(fr);
-    const bool posPg = is_pageable(pos), velPg = vel && is_pageable(vel), stPg = status && is_pageable(status);
+    const bool inPageable = az::is_pageable(sat) || az::is_pageable(jd) || az::is_pageable(fr);
+    const bool posPg = az::is_pageable(pos), velPg = vel && az::is_pageable(vel);
+    const bool stPg = status && az::is_pageable(status);
     const bool outPageable = posPg || velPg || stPg;
-    if ((inPageable || outPageable) && !c->ring) {
-        AZ_CUDA(cudaMallocHost(&c->ring, kPieceBytes * kRingSlots));
-        for (auto &e : c->ringEv) AZ_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    }
-    CopyPool &pool = CopyPool::get();
-    const cudaEvent_t kdone[2] = {c->chunkDone[0], c->chunkDone[1]}, ddone[2] = {c->chunkDone[2], c->chunkDone[3]};
-    const cudaEvent_t inDone = c->chunkDone[4];
-    const uint32_t granule = std::min<uint32_t>(chunk, (uint32_t)(kPieceBytes / 20));  // queries per ring slot
-    c->plan.clear();
-    uint32_t g = 0;
+    const size_t inBytes[3] = {8, 8, 4};
+    c->ring.discard();
     for (uint32_t k = 0; k < nChunks; ++k) {
         const uint32_t slot = k % slots;
         const uint32_t q0 = k * chunk, m = std::min(chunk, n - q0);
@@ -1580,51 +1339,31 @@ int32_t astroz_cuda_constellation_propagate_pairs(astroz_constellation_t h, cons
         uint32_t *dSat = reinterpret_cast<uint32_t *>(dFr + chunk);
         double *dPos = c->dPairsOut.p + slot * outD, *dVel = vel ? dPos + (size_t)chunk * 3 : nullptr;
         uint8_t *dSt = status ? reinterpret_cast<uint8_t *>(dPos + (size_t)chunk * (vel ? 6 : 3)) : nullptr;
-        if (k >= slots) AZ_CUDA(cudaEventSynchronize(ddone[slot]));  // chunk k-2's results have left this slot
-        if (inPageable) {
-            for (uint32_t g0 = 0; g0 < m; g0 += granule, ++g) {
-                const uint32_t gn = std::min(granule, m - g0);
-                const int ri = (int)(g % kRingSlots);
-                char *stage = c->ring + (size_t)ri * kPieceBytes;
-                AZ_CUDA(cudaEventSynchronize(c->ringEv[ri]));  // the slot's last transfer is done
-                pool.copy(stage, reinterpret_cast<const char *>(jd + q0 + g0), 1, (size_t)gn * 8, (size_t)gn * 8);
-                pool.copy(stage + (size_t)gn * 8, reinterpret_cast<const char *>(fr + q0 + g0), 1, (size_t)gn * 8,
-                          (size_t)gn * 8);
-                pool.copy(stage + (size_t)gn * 16, reinterpret_cast<const char *>(sat + q0 + g0), 1, (size_t)gn * 4,
-                          (size_t)gn * 4);
-                AZ_CUDA(cudaMemcpyAsync(dJd + g0, stage, (size_t)gn * 8, cudaMemcpyHostToDevice, st));
-                AZ_CUDA(cudaMemcpyAsync(dFr + g0, stage + (size_t)gn * 8, (size_t)gn * 8, cudaMemcpyHostToDevice, st));
-                AZ_CUDA(cudaMemcpyAsync(dSat + g0, stage + (size_t)gn * 16, (size_t)gn * 4, cudaMemcpyHostToDevice, st));
-                AZ_CUDA(cudaEventRecord(c->ringEv[ri], st));
-            }
-        } else {
-            AZ_CUDA(cudaMemcpyAsync(dJd, jd + q0, (size_t)m * 8, cudaMemcpyHostToDevice, st));
-            AZ_CUDA(cudaMemcpyAsync(dFr, fr + q0, (size_t)m * 8, cudaMemcpyHostToDevice, st));
-            AZ_CUDA(cudaMemcpyAsync(dSat, sat + q0, (size_t)m * 4, cudaMemcpyHostToDevice, st));
-        }
-        AZ_CUDA(cudaEventRecord(inDone, st));
+        if (k >= slots) AZ_CUDA(cudaEventSynchronize(c->copyDone[slot]));  // chunk k-2's results have left this slot
+        const void *src[3] = {jd + q0, fr + q0, sat + q0};
+        void *const dst[3] = {dJd, dFr, dSat};
+        AZ_CUDA(c->ring.upload(inPageable, 3, src, dst, inBytes, m, st));
+        AZ_CUDA(cudaEventRecord(c->inputsDone, st));
         rc = pairs_queue(c, dSat, dJd, dFr, m, mode, dPos, dVel, dSt, st);
         if (rc != ASTROZ_OK) return rc;
-        AZ_CUDA(cudaEventRecord(kdone[slot], st));
+        const cudaEvent_t ready = c->kernelDone[slot];
+        AZ_CUDA(cudaEventRecord(ready, st));
         if (outPageable) {
             // chunk k-1's pageable results go through the ring while chunk k computes; the ring is free once this
             // chunk's queries have left it
-            AZ_CUDA(cudaEventSynchronize(inDone));
-            rc = run_ring(c);
-            if (rc != ASTROZ_OK) return rc;
+            AZ_CUDA(cudaEventSynchronize(c->inputsDone));
+            AZ_CUDA(c->ring.drain(c->copyStream));
         }
-        AZ_CUDA(cudaStreamWaitEvent(c->copyStream, kdone[slot], 0));
-        rc = deliver(c, posPg, (int)slot, dPos, pos + (size_t)q0 * 3, 1, (size_t)m * 24, (size_t)m * 24);
-        if (rc == ASTROZ_OK && vel)
-            rc = deliver(c, velPg, (int)slot, dVel, vel + (size_t)q0 * 3, 1, (size_t)m * 24, (size_t)m * 24);
-        if (rc == ASTROZ_OK && status)
-            rc = deliver(c, stPg, (int)slot, reinterpret_cast<const double *>(dSt),
-                         reinterpret_cast<double *>(status + q0), 1, m, m);
-        if (rc != ASTROZ_OK) return rc;
-        AZ_CUDA(cudaEventRecord(ddone[slot], c->copyStream));
+        AZ_CUDA(cudaStreamWaitEvent(c->copyStream, ready, 0));
+        AZ_CUDA(c->ring.deliver(posPg, ready, dPos, pos + (size_t)q0 * 3, 1, (size_t)m * 24, (size_t)m * 24,
+                                c->copyStream));
+        if (vel)
+            AZ_CUDA(c->ring.deliver(velPg, ready, dVel, vel + (size_t)q0 * 3, 1, (size_t)m * 24, (size_t)m * 24,
+                                    c->copyStream));
+        if (status) AZ_CUDA(c->ring.deliver(stPg, ready, dSt, status + q0, 1, m, m, c->copyStream));
+        AZ_CUDA(cudaEventRecord(c->copyDone[slot], c->copyStream));
     }
-    rc = run_ring(c);
-    if (rc != ASTROZ_OK) return rc;
+    AZ_CUDA(c->ring.drain(c->copyStream));
     AZ_CUDA(cudaStreamSynchronize(c->copyStream));
     AZ_CUDA(cudaStreamSynchronize(st));
     return ASTROZ_OK;
@@ -1653,10 +1392,10 @@ int32_t astroz_cuda_constellation_set_timing(astroz_constellation_t h, int32_t e
     if (!h) return ASTROZ_NULL_POINTER;
     Constellation *c = static_cast<Constellation *>(h);
     c->timing = enabled != 0;
-    c->timed = false;
+    time_begin(c);
     for (Constellation *sh : c->shards) {
         sh->timing = c->timing;
-        sh->timed = false;
+        time_begin(sh);
     }
     return ASTROZ_OK;
 }
@@ -1674,18 +1413,19 @@ int32_t astroz_cuda_constellation_last_kernel_ms(astroz_constellation_t h, float
         }
         return ASTROZ_OK;
     }
-    if (!c->timed) return ASTROZ_NOT_INITIALIZED;
+    if (!c->timedSet) return ASTROZ_NOT_INITIALIZED;
     AZ_CUDA(cudaSetDevice(c->device));
-    AZ_CUDA(cudaEventSynchronize(c->ev[1]));
-    AZ_CUDA(cudaEventSynchronize(c->ev[3]));
-    AZ_CUDA(cudaEventElapsedTime(&ms[0], c->ev[0], c->ev[1]));
-    AZ_CUDA(cudaEventElapsedTime(&ms[2], c->ev[2], c->ev[3]));
-    if (c->spanTimed) {  // the two grids of a mixed call overlap: ms[1] is the span of the whole call
-        AZ_CUDA(cudaEventSynchronize(c->ev[5]));
-        AZ_CUDA(cudaEventElapsedTime(&ms[1], c->ev[4], c->ev[5]));
-    } else {
-        ms[1] = ms[0] + ms[2];
-    }
+    float t[3] = {0.f, 0.f, 0.f};  // by TimedSpan; 0 for a span the call did not time
+    for (int k = 0; k < 3; ++k)
+        if (c->timedSet & (1u << k)) {
+            AZ_CUDA(cudaEventSynchronize(c->ev[k][1]));
+            AZ_CUDA(cudaEventElapsedTime(&t[k], c->ev[k][0], c->ev[k][1]));
+        }
+    ms[0] = t[kTimeK1];
+    ms[2] = t[kTimeK2];
+    // the two grids of a mixed call overlap: ms[1] is the span of the whole call where one was timed
+    ms[1] = (c->timedSet & (1u << kTimeSpan)) ? t[kTimeSpan] : ms[0] + ms[2];
+    if (c->timedSet == (1u << kTimeSpan)) ms[0] = ms[2] = ms[1];  // a host-buffer call times its span only
     return ASTROZ_OK;
 }
 
@@ -1694,11 +1434,10 @@ static int32_t sgp4_into_common(Constellation *c, const double *times, uint32_t 
                                 double *dPos, double *dVel, int mode, double reference_jd, int layout, cudaStream_t s,
                                 uint32_t recStride = 3, const uint8_t *mask = nullptr, uint32_t outNumSats = 0) {
     const uint32_t ns = c->cat.nSgp4;
-    const uint32_t padded = c->cat.sgp4Padded();
-    int32_t rc = reserve_time(c, nt);
+    double *tb;
+    int32_t rc = time_slot(c, nt, &tb);
     if (rc != ASTROZ_OK) return rc;
-    const size_t cap = c->dTime.cap / 4;
-    double *tb = c->hTime, *gs = c->hTime + 2 * (size_t)nt, *gc = c->hTime + 3 * (size_t)nt;
+    double *gs = tb + 2 * (size_t)nt, *gc = tb + 3 * (size_t)nt;
     for (uint32_t t = 0; t < nt; ++t) {
         tb[t] = times[t];
         if (mode != 0) {  // src/Constellation.zig:573-581
@@ -1707,28 +1446,9 @@ static int32_t sgp4_into_common(Constellation *c, const double *times, uint32_t 
             gc[t] = std::cos(gm);
         }
     }
-    AZ_CUDA(cudaMemcpyAsync(c->dTime.p, tb, (size_t)nt * 8, cudaMemcpyHostToDevice, s));
-    if (mode != 0) {
-        AZ_CUDA(cudaMemcpyAsync(c->dTime.p + 2 * cap, gs, (size_t)nt * 8, cudaMemcpyHostToDevice, s));
-        AZ_CUDA(cudaMemcpyAsync(c->dTime.p + 3 * cap, gc, (size_t)nt * 8, cudaMemcpyHostToDevice, s));
-    }
-    if (c->toffPending) {  // the previous call's upload of the offsets must have left the staging buffer
-        AZ_CUDA(cudaEventSynchronize(c->toffCopied));
-        c->toffPending = false;
-    }
-    if (padded > c->hToffCap) {
-        if (c->hToffCall) cudaFreeHost(c->hToffCall);
-        c->hToffCall = nullptr;
-        AZ_CUDA(cudaMallocHost(&c->hToffCall, (size_t)padded * 8));
-        c->hToffCap = padded;
-    }
-    for (uint32_t i = 0; i < padded; ++i) c->hToffCall[i] = epoch_offsets[std::min(i, ns - 1)];
-    AZ_CUDA(c->dToffCall.reserve(padded));
-    AZ_CUDA(cudaMemcpyAsync(c->dToffCall.p, c->hToffCall, (size_t)padded * 8, cudaMemcpyHostToDevice, s));
-    AZ_CUDA(cudaEventRecord(c->toffCopied, s));
-    c->toffPending = true;
-    AZ_CUDA(cudaEventRecord(c->timeCopied, s));
-    c->timePending = true;
+    rc = upload_time_slot(c, nt, (mode != 0) ? 0xDu : 0x1u, s);
+    if (rc == ASTROZ_OK) rc = stage_epoch_offsets(c, epoch_offsets, s);
+    if (rc != ASTROZ_OK) return rc;
 
     az::GridArgs a;
     a.g = c->g;
@@ -1736,9 +1456,9 @@ static int32_t sgp4_into_common(Constellation *c, const double *times, uint32_t 
     a.toff = c->dToffCall.p;
     a.orig = c->dIdentity.p;  // satellite i -> output row i (src/Constellation.zig:561-565)
     a.nSats = ns;
-    a.tbase = c->dTime.p;
-    a.gsin = c->dTime.p + 2 * cap;
-    a.gcos = c->dTime.p + 3 * cap;
+    a.tbase = time_col(c, 0);
+    a.gsin = time_col(c, 2);
+    a.gcos = time_col(c, 3);
     a.nTimes = nt;
     a.pos = dPos;
     a.vel = dVel;
@@ -1749,13 +1469,10 @@ static int32_t sgp4_into_common(Constellation *c, const double *times, uint32_t 
         AZ_CUDA(cudaMemcpyAsync(c->dMask.p, mask, ns, cudaMemcpyHostToDevice, s));
         a.mask = c->dMask.p;
     }
-    if (c->timing) AZ_CUDA(cudaEventRecord(c->ev[0], s));
+    time_begin(c);
+    AZ_CUDA(time_mark(c, kTimeK1, false, s));
     AZ_CUDA(az::launch_sgp4_grid(a, mode, layout, s, c->variant));
-    if (c->timing) AZ_CUDA(cudaEventRecord(c->ev[1], s));
-    if (c->timing) AZ_CUDA(cudaEventRecord(c->ev[2], s));
-    if (c->timing) AZ_CUDA(cudaEventRecord(c->ev[3], s));
-    c->timed = c->timing;
-    c->spanTimed = false;
+    AZ_CUDA(time_mark(c, kTimeK1, true, s));
     return ASTROZ_OK;
 }
 
@@ -1764,8 +1481,8 @@ int32_t astroz_cuda_sgp4_propagate_into_device(astroz_constellation_t h, const d
                                                double reference_jd, int32_t layout, const uint8_t *satellite_mask,
                                                uint32_t out_num_sats, void *stream) {
     Constellation *c = static_cast<Constellation *>(h);
-    AZ_SINGLE(c);
-    int32_t rc = check_args(c, times, epoch_offsets, d_pos, mode, layout);
+    int32_t rc = refuse_multi(c);
+    if (rc == ASTROZ_OK) rc = check_args(c, times, epoch_offsets, d_pos, mode, layout);
     if (rc != ASTROZ_OK) return rc;
     if (n_times == 0 || c->cat.nSgp4 == 0) return ASTROZ_OK;
     if (out_num_sats && out_num_sats < c->cat.nSgp4) {
@@ -1773,7 +1490,7 @@ int32_t astroz_cuda_sgp4_propagate_into_device(astroz_constellation_t h, const d
         return ASTROZ_VALUE_ERROR;
     }
     AZ_CUDA(cudaSetDevice(c->device));
-    cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
+    cudaStream_t s = call_stream(c, stream);
     return sgp4_into_common(c, times, n_times, epoch_offsets, d_pos, d_vel, mode, reference_jd, layout, s, 3,
                             satellite_mask, out_num_sats);
 }
@@ -1809,16 +1526,16 @@ static int32_t sgp4_into_host_queue(Constellation *c, const double *times, uint3
     int32_t rc = sgp4_into_common(c, times, n_times, epoch_offsets, c->dPos.p, vel ? c->dVel.p : nullptr, mode,
                                   reference_jd, layout, s, 3, mask, ns);
     if (rc != ASTROZ_OK) return rc;
-    c->plan.clear();
-    AZ_CUDA(cudaEventRecord(c->chunkDone[0], s));
-    AZ_CUDA(cudaStreamWaitEvent(c->copyStream, c->chunkDone[0], 0));
+    c->ring.discard();
+    const cudaEvent_t ready = c->chunkDone[0];
+    AZ_CUDA(cudaEventRecord(ready, s));
+    AZ_CUDA(cudaStreamWaitEvent(c->copyStream, ready, 0));
     for (int which = 0; which < (vel ? 2 : 1); ++which) {
         double *dst = host_at(which ? vel : pos);
         const double *src = which ? c->dVel.p : c->dPos.p;
-        const bool pg = is_pageable(which ? vel : pos);
-        if (!strided) rc = deliver(c, pg, 0, src, dst, 1, dense * 8, dense * 8);
-        else rc = deliver(c, pg, 0, src, dst, n_times, (size_t)ns * 24, (size_t)rows * 24);
-        if (rc != ASTROZ_OK) return rc;
+        const bool pg = az::is_pageable(which ? vel : pos);
+        if (!strided) AZ_CUDA(c->ring.deliver(pg, ready, src, dst, 1, dense * 8, dense * 8, c->copyStream));
+        else AZ_CUDA(c->ring.deliver(pg, ready, src, dst, n_times, (size_t)ns * 24, (size_t)rows * 24, c->copyStream));
     }
     return ASTROZ_OK;
 }
@@ -1858,7 +1575,7 @@ int32_t astroz_cuda_sgp4_screen(astroz_constellation_t h, const double *times, u
                                 double reference_jd, double *out_min_dists, uint32_t *out_min_t) {
     (void)reference_jd;
     Constellation *c = static_cast<Constellation *>(h);
-    AZ_SINGLE(c);
+    if (const int32_t rc = refuse_multi(c); rc != ASTROZ_OK) return rc;
     if (!c || !times || !epoch_offsets || !out_min_dists || !out_min_t) return ASTROZ_NULL_POINTER;
     const uint32_t ns = c->cat.nSgp4;
     if (ns == 0 || n_times == 0) return ASTROZ_OK;
@@ -1868,34 +1585,19 @@ int32_t astroz_cuda_sgp4_screen(astroz_constellation_t h, const double *times, u
     }
     AZ_CUDA(cudaSetDevice(c->device));
     cudaStream_t s = c->stream;
-    const uint32_t padded = c->cat.sgp4Padded();
-    int32_t rc = reserve_time(c, n_times);
+    double *tb;
+    int32_t rc = time_slot(c, n_times, &tb);
     if (rc != ASTROZ_OK) return rc;
-    for (uint32_t t = 0; t < n_times; ++t) c->hTime[t] = times[t];
-    AZ_CUDA(cudaMemcpyAsync(c->dTime.p, c->hTime, (size_t)n_times * 8, cudaMemcpyHostToDevice, s));
-    if (c->toffPending) {  // the previous call's upload of the offsets must have left the staging buffer
-        AZ_CUDA(cudaEventSynchronize(c->toffCopied));
-        c->toffPending = false;
-    }
-    if (padded > c->hToffCap) {
-        if (c->hToffCall) cudaFreeHost(c->hToffCall);
-        c->hToffCall = nullptr;
-        AZ_CUDA(cudaMallocHost(&c->hToffCall, (size_t)padded * 8));
-        c->hToffCap = padded;
-    }
-    for (uint32_t i = 0; i < padded; ++i) c->hToffCall[i] = epoch_offsets[std::min(i, ns - 1)];
-    AZ_CUDA(c->dToffCall.reserve(padded));
-    AZ_CUDA(cudaMemcpyAsync(c->dToffCall.p, c->hToffCall, (size_t)padded * 8, cudaMemcpyHostToDevice, s));
-    AZ_CUDA(cudaEventRecord(c->toffCopied, s));
-    c->toffPending = true;
-    AZ_CUDA(cudaEventRecord(c->timeCopied, s));
-    c->timePending = true;
+    std::memcpy(tb, times, (size_t)n_times * 8);
+    rc = upload_time_slot(c, n_times, 0x1u, s);
+    if (rc == ASTROZ_OK) rc = stage_epoch_offsets(c, epoch_offsets, s);
+    if (rc != ASTROZ_OK) return rc;
     // scratch: target track [nt][3] | minDist [ns] | minT [ns] (as doubles' worth of space)
     AZ_CUDA(c->dPos.reserve((size_t)n_times * 3 + 2 * (size_t)ns + 2));
     az::ScreenArgs a;
     a.sgp4Tiles = c->dTiles.p;
     a.toff = c->dToffCall.p;
-    a.tbase = c->dTime.p;
+    a.tbase = time_col(c, 0);
     a.nSats = ns;
     a.nTimes = n_times;
     a.targetIdx = target_idx;
@@ -1904,13 +1606,10 @@ int32_t astroz_cuda_sgp4_screen(astroz_constellation_t h, const double *times, u
     a.minDist = c->dPos.p + (size_t)n_times * 3;
     a.minT = reinterpret_cast<uint32_t *>(a.minDist + ns);
     a.g = c->g;
-    if (c->timing) AZ_CUDA(cudaEventRecord(c->ev[0], s));
+    time_begin(c);
+    AZ_CUDA(time_mark(c, kTimeK1, false, s));
     AZ_CUDA(az::launch_sgp4_screen(a, s));
-    if (c->timing) AZ_CUDA(cudaEventRecord(c->ev[1], s));
-    if (c->timing) AZ_CUDA(cudaEventRecord(c->ev[2], s));
-    if (c->timing) AZ_CUDA(cudaEventRecord(c->ev[3], s));
-    c->timed = c->timing;
-    c->spanTimed = false;
+    AZ_CUDA(time_mark(c, kTimeK1, true, s));
     AZ_CUDA(cudaMemcpyAsync(out_min_dists, a.minDist, (size_t)ns * 8, cudaMemcpyDeviceToHost, s));
     AZ_CUDA(cudaMemcpyAsync(out_min_t, a.minT, (size_t)ns * 4, cudaMemcpyDeviceToHost, s));
     AZ_CUDA(cudaStreamSynchronize(s));
@@ -1958,7 +1657,7 @@ int32_t astroz_cuda_constellation_coarse_screen_device(astroz_constellation_t h,
                                                        double threshold, const uint8_t *d_valid_mask, uint32_t *d_pairs,
                                                        uint32_t *d_t_indices, uint32_t max_results, uint64_t *count) {
     Constellation *c = static_cast<Constellation *>(h);
-    AZ_SINGLE(c);
+    if (const int32_t rc = refuse_multi(c); rc != ASTROZ_OK) return rc;
     if (!c || !d_positions || !count || (max_results && (!d_pairs || !d_t_indices))) return ASTROZ_NULL_POINTER;
     if (layout < 0 || layout > 1 || !(threshold > 0.0)) {
         g_lastError = "coarse screen: layout must be 0/1 and threshold positive";
@@ -1975,7 +1674,7 @@ int32_t astroz_cuda_sgp4_screen_all(astroz_constellation_t h, const double *time
                                     const double *epoch_offsets, double threshold, uint32_t *pairs, uint32_t *t_indices,
                                     uint32_t max_results, uint64_t *count) {
     Constellation *c = static_cast<Constellation *>(h);
-    AZ_SINGLE(c);
+    if (const int32_t rc = refuse_multi(c); rc != ASTROZ_OK) return rc;
     if (!c || !times || !epoch_offsets || !count || (max_results && (!pairs || !t_indices))) return ASTROZ_NULL_POINTER;
     if (!(threshold > 0.0)) return ASTROZ_VALUE_ERROR;
     *count = 0;
@@ -2008,31 +1707,15 @@ int32_t astroz_cuda_sgp4_init(const char *line1, const char *line2, int32_t grav
     *out = nullptr;
     // python-sgp4 style code builds thousands of Satrec objects only to hand them to a SatrecArray: parsing and
     // classification happen here, on the host; device resources come with the first propagation of THIS satellite.
-    {
-        int count = 0;
-        if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0) {
-            g_lastError = "no CUDA device available (this library has no CPU propagation path)";
-            return ASTROZ_NO_DEVICE;
-        }
-        if (device < 0 || device >= count) {
-            g_lastError = "device index out of range";
-            return ASTROZ_VALUE_ERROR;
-        }
-    }
-    Constellation *cc = new (std::nothrow) Constellation();
-    if (!cc) return ASTROZ_ALLOC_FAILED;
+    const int32_t drc = check_device_ordinal(device);
+    if (drc != ASTROZ_OK) return drc;
+    std::unique_ptr<Sgp4Single> s(new (std::nothrow) Sgp4Single());
+    if (!s) return ASTROZ_ALLOC_FAILED;
+    s->c.reset(new (std::nothrow) Constellation());
+    if (!s->c) return ASTROZ_ALLOC_FAILED;
     const char *l1[1] = {line1}, *l2[1] = {line2};
-    const int brc = az::build_catalog(l1, l2, 1, grav, cc->cat);
-    if (brc != az::kOk) {
-        delete cc;
-        return status_to_code(brc);
-    }
-    Sgp4Single *s = new (std::nothrow) Sgp4Single();
-    if (!s) {
-        delete cc;
-        return ASTROZ_ALLOC_FAILED;
-    }
-    s->c = cc;
+    const int brc = az::build_catalog(l1, l2, 1, grav, s->c->cat);
+    if (brc != az::kOk) return status_to_code(brc);
     s->device = device;
     s->epochJd = s->c->cat.epochs[0];
     s->deep = s->c->cat.nSdp4 == 1;
@@ -2046,13 +1729,13 @@ int32_t astroz_cuda_sgp4_init(const char *line1, const char *line2, int32_t grav
             std::memcpy(s->elements, e, sizeof e);
         }
     }
-    *out = s;
+    *out = s.release();
     return ASTROZ_OK;
 }
 
 static int32_t ensure_open(Sgp4Single *s) {
     if (s->opened) return ASTROZ_OK;
-    const int32_t rc = finish_create(s->c, s->device);
+    const int32_t rc = finish_create(s->c.get(), s->device);
     if (rc == ASTROZ_OK) s->opened = true;
     return rc;
 }
@@ -2063,12 +1746,7 @@ int32_t astroz_cuda_sgp4_elements(astroz_sgp4_t h, double *out10) {
     return ASTROZ_OK;
 }
 
-void astroz_cuda_sgp4_free(astroz_sgp4_t h) {
-    Sgp4Single *s = static_cast<Sgp4Single *>(h);
-    if (!s) return;
-    delete s->c;
-    delete s;
-}
+void astroz_cuda_sgp4_free(astroz_sgp4_t h) { delete static_cast<Sgp4Single *>(h); }
 
 int32_t astroz_cuda_sgp4_is_deep_space(astroz_sgp4_t h) { return h && static_cast<Sgp4Single *>(h)->deep ? 1 : 0; }
 
@@ -2086,7 +1764,7 @@ int32_t astroz_cuda_sgp4_propagate_batch(astroz_sgp4_t h, const double *times, d
         const int32_t orc = ensure_open(s);
         if (orc != ASTROZ_OK) return orc;
     }
-    Constellation *c = s->c;
+    Constellation *c = s->c.get();
     AZ_CUDA(cudaSetDevice(c->device));
     const bool fast = !s->deep && count >= 64;
     std::vector<double> pos(fast ? 0 : (size_t)count * 3), vel(fast ? 0 : (size_t)count * 3);
@@ -2109,17 +1787,17 @@ int32_t astroz_cuda_sgp4_propagate_batch(astroz_sgp4_t h, const double *times, d
         if (rc != ASTROZ_OK) return rc;
     } else {
         // deep space: minutes since epoch go to the kernel directly (no Julian-date round trip)
-        int32_t rt = reserve_time(c, count);
-        if (rt != ASTROZ_OK) return rt;
+        double *tb;
+        rc = time_slot(c, count, &tb);
+        if (rc != ASTROZ_OK) return rc;
         double reach = 0.0;
         for (uint32_t i = 0; i < count; ++i) {
-            c->hTime[i] = times[i];
+            tb[i] = times[i];
             reach = std::max(reach, std::fabs(times[i]));
         }
         cudaStream_t st = c->stream;
-        AZ_CUDA(cudaMemcpyAsync(c->dTime.p, c->hTime, (size_t)count * 8, cudaMemcpyHostToDevice, st));
-        AZ_CUDA(cudaEventRecord(c->timeCopied, st));
-        c->timePending = true;
+        rc = upload_time_slot(c, count, 0x1u, st);
+        if (rc != ASTROZ_OK) return rc;
         rc = ensure_lattice(c, (int)std::floor(reach / az::kStepp) + 2, st);
         if (rc != ASTROZ_OK) return rc;
         const size_t total = (size_t)count * 3;
@@ -2134,21 +1812,18 @@ int32_t astroz_cuda_sgp4_propagate_batch(astroz_sgp4_t h, const double *times, d
         a.nSats = 1;
         a.lattice = c->dLattice.p;
         a.latticeNodes = c->latticeNodes;
-        a.tsince = c->dTime.p;
+        a.tsince = time_col(c, 0);
         a.nTimes = count;
         a.pos = c->dPos.p;
         a.vel = c->dVel.p;
         a.status = dSt.p;
         a.outNumSats = 1;
         std::vector<uint8_t> cell(count);
-        cudaError_t e = az::launch_sdp4_grid(a, ASTROZ_MODE_TEME, ASTROZ_LAYOUT_SATELLITE_MAJOR, st);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(pos.data(), c->dPos.p, total * 8, cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(vel.data(), c->dVel.p, total * 8, cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(cell.data(), dSt.p, count, cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-        dSt.release();
-        if (e != cudaSuccess) return cuda_fail(e, "single-satellite deep-space propagate");
-        rc = ASTROZ_OK;
+        AZ_CUDA(az::launch_sdp4_grid(a, ASTROZ_MODE_TEME, ASTROZ_LAYOUT_SATELLITE_MAJOR, st));
+        AZ_CUDA(cudaMemcpyAsync(pos.data(), c->dPos.p, total * 8, cudaMemcpyDeviceToHost, st));
+        AZ_CUDA(cudaMemcpyAsync(vel.data(), c->dVel.p, total * 8, cudaMemcpyDeviceToHost, st));
+        AZ_CUDA(cudaMemcpyAsync(cell.data(), dSt.p, count, cudaMemcpyDeviceToHost, st));
+        AZ_CUDA(cudaStreamSynchronize(st));
         for (uint32_t i = 0; i < count; ++i)
             if (cell[i] != 0) rc = status_to_code(cell[i]);  // failing cells stay zero-filled; last failure reported
     }
@@ -2169,7 +1844,7 @@ int32_t astroz_cuda_sgp4_array(astroz_sgp4_t h, const double *jd, const double *
         const int32_t orc = ensure_open(s);
         if (orc != ASTROZ_OK) return orc;
     }
-    Constellation *c = s->c;
+    Constellation *c = s->c.get();
     if (s->deep || count < 64) {  // deep space / tiny: host-side tsince, then the batch entry point
         std::vector<double> ts(count);
         for (uint32_t i = 0; i < count; ++i) ts[i] = ((jd[i] + fr[i]) - epoch_jd) * 1440.0;
@@ -2177,7 +1852,7 @@ int32_t astroz_cuda_sgp4_array(astroz_sgp4_t h, const double *jd, const double *
     }
     AZ_CUDA(cudaSetDevice(c->device));
     cudaStream_t st = c->stream;
-    c->cacheValid = false;
+    c->cacheValid = false;  // dTime holds [jd | fr] slots here
     // A long axis ("1 year at one second" = 31.5 M epochs: 0.5 GB of jd/fr in, 1.5 GB of records out) is cut into
     // chunks on a two-slot pipeline: while chunk k is propagated, chunk k+1's epochs are staged and uploaded and chunk
     // k-1's records travel back, so the call runs at the PCIe rate of its 48 B/epoch result instead of the sum of three
@@ -2188,41 +1863,21 @@ int32_t astroz_cuda_sgp4_array(astroz_sgp4_t h, const double *jd, const double *
     const int slots = nChunks > 1 ? 2 : 1;
     AZ_CUDA(c->dTime.reserve((size_t)chunk * 2 * slots));
     AZ_CUDA(c->dPos.reserve((size_t)chunk * 6 * slots));
-    const bool inPageable = is_pageable(jd) || is_pageable(fr);
-    const bool outPageable = is_pageable(results);
-    if ((inPageable || outPageable) && !c->ring) {
-        AZ_CUDA(cudaMallocHost(&c->ring, kPieceBytes * kRingSlots));
-        for (auto &e : c->ringEv) AZ_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    }
-    // pinned staging inside the ring allocation (96 MB): two 16 MB input slots [jd | fr]; outputs of a pageable caller
-    // are not staged here (a 96 MB chunk does not fit) -- they go through cudaMemcpyAsync's own staging
-    CopyPool &pool = CopyPool::get();
-    cudaEvent_t kdone[2] = {c->chunkDone[0], c->chunkDone[1]}, ddone[2] = {c->chunkDone[2], c->chunkDone[3]};
-    const uint32_t inChunk = inPageable ? std::min<uint32_t>(chunk, (uint32_t)(kPieceBytes / 16)) : chunk;  // staging granule
-    if (c->timing) AZ_CUDA(cudaEventRecord(c->ev[0], st));
-    uint32_t granule = 0;
+    // pageable jd / fr are staged through the handle's pinned ring; pageable results are not (a 96 MB chunk does not
+    // fit a ring slot) -- they go through cudaMemcpyAsync's own staging
+    const bool inPageable = az::is_pageable(jd) || az::is_pageable(fr);
+    const size_t inBytes[2] = {8, 8};
+    time_begin(c);
+    AZ_CUDA(time_mark(c, kTimeK1, false, st));
     for (uint32_t k = 0; k < nChunks; ++k) {
         const int slot = (int)(k & 1u) % slots;
         const uint32_t t0 = k * chunk, n = std::min(chunk, count - t0);
         double *dJd = c->dTime.p + (size_t)slot * chunk * 2, *dFr = dJd + chunk;
         double *dOut = c->dPos.p + (size_t)slot * chunk * 6;
-        if (k >= (uint32_t)slots) AZ_CUDA(cudaEventSynchronize(ddone[slot]));  // chunk k-2 has left this slot
-        if (inPageable) {   // stage through pinned memory in granules of the ring slot size, copy pool does the memcpy
-            for (uint32_t g0 = 0; g0 < n; g0 += inChunk, ++granule) {
-                const uint32_t gn = std::min(inChunk, n - g0);
-                const int ri = (int)(granule % kRingSlots);
-                char *stage = c->ring + (size_t)ri * kPieceBytes;
-                if (granule >= (uint32_t)kRingSlots) AZ_CUDA(cudaEventSynchronize(c->ringEv[ri]));  // its last upload is done
-                pool.copy(stage, reinterpret_cast<const char *>(jd + t0 + g0), 1, (size_t)gn * 8, (size_t)gn * 8);
-                pool.copy(stage + (size_t)gn * 8, reinterpret_cast<const char *>(fr + t0 + g0), 1, (size_t)gn * 8, (size_t)gn * 8);
-                AZ_CUDA(cudaMemcpyAsync(dJd + g0, stage, (size_t)gn * 8, cudaMemcpyHostToDevice, st));
-                AZ_CUDA(cudaMemcpyAsync(dFr + g0, stage + (size_t)gn * 8, (size_t)gn * 8, cudaMemcpyHostToDevice, st));
-                AZ_CUDA(cudaEventRecord(c->ringEv[ri], st));
-            }
-        } else {
-            AZ_CUDA(cudaMemcpyAsync(dJd, jd + t0, (size_t)n * 8, cudaMemcpyHostToDevice, st));
-            AZ_CUDA(cudaMemcpyAsync(dFr, fr + t0, (size_t)n * 8, cudaMemcpyHostToDevice, st));
-        }
+        if (k >= (uint32_t)slots) AZ_CUDA(cudaEventSynchronize(c->copyDone[slot]));  // chunk k-2 has left this slot
+        const void *src[2] = {jd + t0, fr + t0};
+        void *const dst[2] = {dJd, dFr};
+        AZ_CUDA(c->ring.upload(inPageable, 2, src, dst, inBytes, n, st));
         az::GridArgs a;
         a.g = c->g;
         a.sgp4Tiles = c->dTiles.p;
@@ -2239,16 +1894,12 @@ int32_t astroz_cuda_sgp4_array(astroz_sgp4_t h, const double *jd, const double *
         a.outNumSats = 1;
         a.recStride = 6;
         AZ_CUDA(az::launch_sgp4_grid(a, ASTROZ_MODE_TEME, ASTROZ_LAYOUT_SATELLITE_MAJOR, st, c->variant));
-        AZ_CUDA(cudaEventRecord(kdone[slot], st));
-        AZ_CUDA(cudaStreamWaitEvent(c->copyStream, kdone[slot], 0));
+        AZ_CUDA(cudaEventRecord(c->kernelDone[slot], st));
+        AZ_CUDA(cudaStreamWaitEvent(c->copyStream, c->kernelDone[slot], 0));
         AZ_CUDA(cudaMemcpyAsync(results + (size_t)t0 * 6, dOut, (size_t)n * 48, cudaMemcpyDeviceToHost, c->copyStream));
-        AZ_CUDA(cudaEventRecord(ddone[slot], c->copyStream));
+        AZ_CUDA(cudaEventRecord(c->copyDone[slot], c->copyStream));
     }
-    if (c->timing) AZ_CUDA(cudaEventRecord(c->ev[1], st));
-    if (c->timing) AZ_CUDA(cudaEventRecord(c->ev[2], st));
-    if (c->timing) AZ_CUDA(cudaEventRecord(c->ev[3], st));
-    c->timed = c->timing;
-    c->spanTimed = false;
+    AZ_CUDA(time_mark(c, kTimeK1, true, st));
     AZ_CUDA(cudaStreamSynchronize(c->copyStream));
     AZ_CUDA(cudaStreamSynchronize(st));
     return ASTROZ_OK;
@@ -2441,10 +2092,8 @@ int32_t astroz_cuda_constellation_propagate_replicated(astroz_constellation_t h,
 int32_t astroz_cuda_fp64_peak(int32_t device, double *tflops) {
     if (!tflops) return ASTROZ_NULL_POINTER;
     int n = 0;
-    if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) {
-        g_lastError = "no CUDA device available";
-        return ASTROZ_NO_DEVICE;
-    }
+    const int32_t rc = check_device_present(&n, "no CUDA device available");
+    if (rc != ASTROZ_OK) return rc;
     AZ_CUDA(cudaSetDevice(device));
     double flops = 0;
     AZ_CUDA(az::measure_fp64_peak(&flops));
@@ -2455,10 +2104,8 @@ int32_t astroz_cuda_fp64_peak(int32_t device, double *tflops) {
 int32_t astroz_cuda_fp64_pipe_peak(int32_t device, double *tflops) {
     if (!tflops) return ASTROZ_NULL_POINTER;
     int n = 0;
-    if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) {
-        g_lastError = "no CUDA device available";
-        return ASTROZ_NO_DEVICE;
-    }
+    const int32_t rc = check_device_present(&n, "no CUDA device available");
+    if (rc != ASTROZ_OK) return rc;
     AZ_CUDA(cudaSetDevice(device));
     double flops = 0;
     AZ_CUDA(az::fp64_pipe_peak(&flops));
