@@ -104,6 +104,12 @@ def lib() -> C.CDLL:
         "astroz_cuda_sgp4_array": (i32, [vp, dp, dp, C.c_double, dp, u32]),
         "astroz_cuda_constellation_devices": (i32, [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(u32)]),
         "astroz_cuda_constellation_propagate_replicated": (i32, [vp, dp, dp, u32, i32, C.POINTER(vp), C.POINTER(vp)]),
+        "astroz_cuda_numerical_times": (i32, [C.c_double, C.c_double, C.c_double, vp, C.POINTER(C.c_uint64)]),
+        "astroz_cuda_propagate_numerical": (i32, [vp, u32, C.c_double, C.c_double, C.c_double, C.c_double, i32, dp, dp,
+                                                  vp, vp, vp, i32, C.c_double, C.c_double, i32, vp, vp, vp]),
+        "astroz_cuda_propagate_numerical_device": (i32, [vp, u32, C.c_double, C.c_double, C.c_double, C.c_double, i32,
+                                                         dp, dp, vp, vp, vp, i32, C.c_double, C.c_double, i32, vp, vp,
+                                                         vp, vp]),
         "astroz_cuda_fp64_peak": (i32, [i32, dp]),
         "astroz_cuda_fp64_pipe_peak": (i32, [i32, dp]),
     }
@@ -135,6 +141,7 @@ EXPORTS = [
     "astroz_cuda_constellation_propagate_replicated", "astroz_cuda_host_register", "astroz_cuda_host_unregister",
     "astroz_cuda_constellation_set_timing", "astroz_cuda_constellation_host_block",
     "astroz_cuda_constellation_propagate_pairs", "astroz_cuda_constellation_propagate_pairs_device",
+    "astroz_cuda_numerical_times", "astroz_cuda_propagate_numerical", "astroz_cuda_propagate_numerical_device",
 ]
 
 

@@ -26,6 +26,7 @@
 #include "az_hostcopy.cuh"
 #include "az_ingest.cuh"
 #include "az_kernels.cuh"
+#include "az_numerical.cuh"
 #include "az_tables.hpp"
 
 namespace {
@@ -2087,6 +2088,265 @@ int32_t astroz_cuda_constellation_propagate_replicated(astroz_constellation_t h,
         if (velocities) d_vel[k] = c->shards[k]->dFullVel.p;
     }
     return first;
+}
+
+// ---- numerical propagation (K7, az_numerical.cu) -------------------------------------------------------------------
+// The sampling rule of Propagator.propagate (src/propagators/Propagator.zig:32-45), stated here and nowhere else:
+//   t = t0; t_end = t0 + duration; while (t < t_end) { step = min(dt, t_end - t); ...; t += step; }
+// *count = samples (the initial state plus one per step); times (nullable) receives the sample times, table (nullable)
+// the step sizes K7 integrates over.  Nothing is allocated.  A loop that would not end (t + step == t) or run more than
+// kMaxNumSteps steps, and non-finite or non-positive inputs, are ASTROZ_VALUE_ERROR.
+static constexpr uint64_t kMaxNumSteps = 0xfffffffeull;  // K7 counts intervals in 32 bits
+static int32_t numerical_schedule(double t0, double duration, double dt, double *times, az::StepTable *table,
+                                  uint64_t *count) {
+    const double tEnd = t0 + duration;
+    if (!std::isfinite(t0) || !std::isfinite(duration) || !std::isfinite(dt) || !std::isfinite(tEnd) || !(dt > 0.0)) {
+        g_lastError = "t0, duration and dt must be finite and dt > 0";
+        return ASTROZ_VALUE_ERROR;
+    }
+    if (duration / dt > (double)kMaxNumSteps) {
+        g_lastError = "duration / dt exceeds the step limit";
+        return ASTROZ_VALUE_ERROR;
+    }
+    if (table) *table = az::StepTable{dt, 0, 0, {}};
+    double t = t0;
+    uint64_t k = 0;
+    if (times) times[0] = t;
+    while (t < tEnd) {
+        const double step = std::min(dt, tEnd - t);
+        if (t + step == t || ++k > kMaxNumSteps) {
+            g_lastError = "the sampling loop would not end: t0 + step rounds to t0";
+            return ASTROZ_VALUE_ERROR;
+        }
+        if (table && !az::step_table_push(*table, step)) {
+            g_lastError = "the sampling loop's steps do not fit the step table";
+            return ASTROZ_VALUE_ERROR;
+        }
+        t += step;
+        if (times) times[k] = t;
+    }
+    *count = k + 1;
+    return ASTROZ_OK;
+}
+
+// Argument checks shared by both batch calls, before anything is read, written or allocated.  *table receives the steps.
+static int32_t numerical_check(uint32_t n, double t0, double duration, double dt, double mu, int32_t forces,
+                               const double *j2, const double *r_eq, const double *cd, const double *area,
+                               const double *mass, int32_t integrator, double rtol, double atol, int32_t device,
+                               az::StepTable *table) {
+    auto bad = [](const char *why) {
+        g_lastError = why;
+        return ASTROZ_VALUE_ERROR;
+    };
+    if (device < 0) return bad("numerical propagation runs on one device: pass its ordinal");
+    if (integrator != az::kIntRk4 && integrator != az::kIntDp87) return bad("integrator must be RK4 (0) or DP87 (1)");
+    if (forces & ~(az::kForceJ2 | az::kForceDrag)) return bad("unknown force bit");
+    if (!std::isfinite(mu) || !std::isfinite(rtol) || !std::isfinite(atol)) return bad("mu, rtol and atol must be finite");
+    if ((forces & az::kForceJ2) && (!j2 || !std::isfinite(*j2))) return bad("J2 needs a finite j2");
+    if (forces && (!r_eq || !std::isfinite(*r_eq))) return bad("J2 and drag need a finite r_eq");
+    if ((forces & az::kForceDrag) && (!cd || !area || !mass)) return bad("drag needs drag_cd, drag_area and drag_mass");
+    uint64_t samples = 0;
+    const int32_t rc = numerical_schedule(t0, duration, dt, nullptr, table, &samples);
+    if (rc != ASTROZ_OK) return rc;
+    if ((uint64_t)n * samples > SIZE_MAX / 48) return bad("the output size overflows");
+    return ASTROZ_OK;
+}
+
+static az::NumArgs numerical_args(uint32_t n, const az::StepTable &table, double mu, int32_t forces, const double *j2,
+                                  const double *r_eq, double rtol, double atol) {
+    az::NumArgs a{};
+    a.n = n;
+    a.steps = table;
+    a.p.mu = mu;
+    a.p.j2 = (forces & az::kForceJ2) ? *j2 : 0.0;
+    a.p.rEq = forces ? *r_eq : 0.0;
+    a.p.rtol = rtol;
+    a.p.atol = atol;
+    return a;
+}
+
+// Per-device state of the host-buffer call: its two streams, the two-slot pipeline's events and the pinned ring (three
+// 32 MB pieces, allocated on the first pageable transfer).  Process-wide, created on first use and never destroyed, like
+// the host copy pool; a mutex serialises the calls that share it.  The device slots are not kept: each call allocates
+// them stream-ordered and returns them before it returns.
+struct NumericalContext {
+    std::mutex m;
+    cudaStream_t stream = nullptr, copyStream = nullptr;
+    cudaEvent_t kernelDone[2] = {}, copyDone[2] = {}, inputsDone = nullptr;
+    az::HostRing ring;
+};
+
+static int32_t numerical_context(int device, NumericalContext **out) {
+    static std::mutex created;
+    static std::map<int, NumericalContext *> contexts;
+    std::lock_guard<std::mutex> lk(created);
+    NumericalContext *&c = contexts[device];
+    if (!c) {
+        std::unique_ptr<NumericalContext> fresh(new (std::nothrow) NumericalContext());
+        if (!fresh) return ASTROZ_ALLOC_FAILED;
+        AZ_CUDA(cudaSetDevice(device));
+        AZ_CUDA(cudaStreamCreateWithFlags(&fresh->stream, cudaStreamNonBlocking));
+        AZ_CUDA(cudaStreamCreateWithFlags(&fresh->copyStream, cudaStreamNonBlocking));
+        for (auto &e : fresh->kernelDone) AZ_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+        for (auto &e : fresh->copyDone) AZ_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+        AZ_CUDA(cudaEventCreateWithFlags(&fresh->inputsDone, cudaEventDisableTiming));
+        c = fresh.release();
+    }
+    *out = c;
+    return ASTROZ_OK;
+}
+
+// A stream-ordered device allocation returned to the pool on `s` when it goes out of scope (also on an error return).
+struct StreamBuf {
+    void *p = nullptr;
+    cudaStream_t s = nullptr;
+    explicit StreamBuf(cudaStream_t stream) : s(stream) {}
+    StreamBuf(const StreamBuf &) = delete;
+    StreamBuf &operator=(const StreamBuf &) = delete;
+    ~StreamBuf() { release(); }
+    cudaError_t alloc(size_t bytes) { return cudaMallocAsync(&p, bytes, s); }
+    cudaError_t release() {
+        void *q = p;
+        p = nullptr;
+        return q ? cudaFreeAsync(q, s) : cudaSuccess;
+    }
+};
+
+int32_t astroz_cuda_numerical_times(double t0, double duration, double dt, double *times, uint64_t *count) {
+    if (!count) return ASTROZ_NULL_POINTER;
+    uint64_t k = 0;
+    int32_t rc = numerical_schedule(t0, duration, dt, nullptr, nullptr, &k);  // validate before writing anything
+    if (rc == ASTROZ_OK && times) rc = numerical_schedule(t0, duration, dt, times, nullptr, &k);
+    if (rc != ASTROZ_OK) return rc;
+    *count = k;
+    return ASTROZ_OK;
+}
+
+int32_t astroz_cuda_propagate_numerical_device(const double *d_states, uint32_t n, double t0, double duration,
+                                               double dt, double mu, int32_t forces, const double *j2,
+                                               const double *r_eq, const double *d_drag_cd,
+                                               const double *d_drag_area, const double *d_drag_mass,
+                                               int32_t integrator, double rtol, double atol, int32_t device,
+                                               double *d_out, uint8_t *d_status, uint64_t *d_steps, void *stream) {
+    az::StepTable table{};
+    int32_t rc = numerical_check(n, t0, duration, dt, mu, forces, j2, r_eq, d_drag_cd, d_drag_area, d_drag_mass,
+                                 integrator, rtol, atol, device, &table);
+    if (rc != ASTROZ_OK) return rc;
+    if (n == 0) return ASTROZ_OK;
+    if (!d_states || !d_out || !d_status) return ASTROZ_NULL_POINTER;
+    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
+    AZ_CUDA(cudaSetDevice(device));
+    az::NumArgs a = numerical_args(n, table, mu, forces, j2, r_eq, rtol, atol);
+    a.states = d_states;
+    a.cd = d_drag_cd;
+    a.area = d_drag_area;
+    a.mass = d_drag_mass;
+    a.out = d_out;
+    a.status = d_status;
+    a.counts = d_steps;
+    // the step table travels in the launch's parameters: nothing is uploaded, the call only queues the kernel
+    AZ_CUDA(az::launch_numerical(a, integrator, forces, static_cast<cudaStream_t>(stream)));
+    return ASTROZ_OK;
+}
+
+// Host buffers: chunks of states on two device slots, each chunk's trajectory block at most kNumChunkBytes (eight ring
+// pieces).  Chunk k's states go up and its kernel runs on the compute stream while chunk k-1's results come back on the
+// copy stream (pinned / registered destinations) or through the pinned ring and the copy pool (pageable ones);
+// pageable inputs are staged through the same ring.
+static constexpr size_t kNumChunkBytes = 256u << 20;
+int32_t astroz_cuda_propagate_numerical(const double *states, uint32_t n, double t0, double duration, double dt,
+                                        double mu, int32_t forces, const double *j2, const double *r_eq,
+                                        const double *drag_cd, const double *drag_area, const double *drag_mass,
+                                        int32_t integrator, double rtol, double atol, int32_t device, double *out,
+                                        uint8_t *status, uint64_t *steps) {
+    az::StepTable table{};
+    int32_t rc = numerical_check(n, t0, duration, dt, mu, forces, j2, r_eq, drag_cd, drag_area, drag_mass, integrator,
+                                 rtol, atol, device, &table);
+    if (rc != ASTROZ_OK) return rc;
+    if (n == 0) return ASTROZ_OK;
+    if (!states || !out || !status) return ASTROZ_NULL_POINTER;
+    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
+    NumericalContext *c = nullptr;
+    if ((rc = numerical_context(device, &c)) != ASTROZ_OK) return rc;
+    std::lock_guard<std::mutex> lk(c->m);
+    AZ_CUDA(cudaSetDevice(device));
+    cudaStream_t st = c->stream;
+    const bool drag = (forces & az::kForceDrag) != 0;
+    const size_t rowD = ((size_t)table.nFull + table.nTail + 1) * 6;  // doubles of one state's trajectory
+    const uint32_t chunk = (uint32_t)std::max<size_t>(1, std::min<size_t>(n, kNumChunkBytes / (rowD * 8)));
+    const uint32_t nChunks = (uint32_t)(((uint64_t)n + chunk - 1) / chunk);
+    const uint32_t slots = nChunks > 1 ? 2 : 1;
+    // slot layout, in doubles: inputs [states | cd | area | mass], results [trajectories | counts | status]
+    const size_t inD = (size_t)chunk * (drag ? 9 : 6);
+    const size_t outD = (size_t)chunk * rowD + (steps ? (size_t)chunk * 2 : 0) + (chunk + 7) / 8;
+    StreamBuf dIn(st), dOut(st);
+    // declared after the slots, so it runs before they are freed on any return: the ring's plan is forgotten and both
+    // streams have finished with the slots
+    struct Settle {
+        NumericalContext *c;
+        ~Settle() {
+            c->ring.discard();
+            cudaStreamSynchronize(c->copyStream);
+            cudaStreamSynchronize(c->stream);
+        }
+    } settle{c};
+    AZ_CUDA(dIn.alloc(inD * slots * 8));
+    AZ_CUDA(dOut.alloc(outD * slots * 8));
+    az::NumArgs a = numerical_args(n, table, mu, forces, j2, r_eq, rtol, atol);
+    const bool inPageable = az::is_pageable(states) ||
+                            (drag && (az::is_pageable(drag_cd) || az::is_pageable(drag_area) || az::is_pageable(drag_mass)));
+    const bool outPg = az::is_pageable(out), stPg = az::is_pageable(status), cntPg = steps && az::is_pageable(steps);
+    const bool outPageable = outPg || stPg || cntPg;
+    const size_t inBytes[4] = {48, 8, 8, 8};
+    c->ring.discard();
+    for (uint32_t k = 0; k < nChunks; ++k) {
+        const uint32_t slot = k % slots;
+        const uint32_t s0 = k * chunk, m = std::min(chunk, n - s0);
+        double *dStates = static_cast<double *>(dIn.p) + slot * inD;
+        double *dCd = dStates + (size_t)chunk * 6, *dArea = dCd + chunk, *dMass = dArea + chunk;
+        double *dTraj = static_cast<double *>(dOut.p) + slot * outD;
+        uint64_t *dCounts = steps ? reinterpret_cast<uint64_t *>(dTraj + (size_t)chunk * rowD) : nullptr;
+        uint8_t *dSt = reinterpret_cast<uint8_t *>(dTraj + (size_t)chunk * rowD + (steps ? (size_t)chunk * 2 : 0));
+        if (k >= slots) AZ_CUDA(cudaEventSynchronize(c->copyDone[slot]));  // chunk k-2's results have left this slot
+        const void *src[4] = {states + (size_t)s0 * 6, drag ? drag_cd + s0 : nullptr, drag ? drag_area + s0 : nullptr,
+                              drag ? drag_mass + s0 : nullptr};
+        void *const dst[4] = {dStates, dCd, dArea, dMass};
+        AZ_CUDA(c->ring.upload(inPageable, drag ? 4 : 1, src, dst, inBytes, m, st));
+        AZ_CUDA(cudaEventRecord(c->inputsDone, st));
+        a.n = m;
+        a.states = dStates;
+        a.cd = drag ? dCd : nullptr;
+        a.area = drag ? dArea : nullptr;
+        a.mass = drag ? dMass : nullptr;
+        a.out = dTraj;
+        a.status = dSt;
+        a.counts = dCounts;
+        AZ_CUDA(az::launch_numerical(a, integrator, forces, st));
+        const cudaEvent_t ready = c->kernelDone[slot];
+        AZ_CUDA(cudaEventRecord(ready, st));
+        if (outPageable) {
+            // chunk k-1's pageable results go through the ring while chunk k computes; the ring is free once this
+            // chunk's inputs have left it
+            AZ_CUDA(cudaEventSynchronize(c->inputsDone));
+            AZ_CUDA(c->ring.drain(c->copyStream));
+        }
+        AZ_CUDA(cudaStreamWaitEvent(c->copyStream, ready, 0));
+        AZ_CUDA(c->ring.deliver(outPg, ready, dTraj, out + (size_t)s0 * rowD, 1, (size_t)m * rowD * 8,
+                                (size_t)m * rowD * 8, c->copyStream));
+        AZ_CUDA(c->ring.deliver(stPg, ready, dSt, status + s0, 1, m, m, c->copyStream));
+        if (steps)
+            AZ_CUDA(c->ring.deliver(cntPg, ready, dCounts, steps + (size_t)s0 * 2, 1, (size_t)m * 16, (size_t)m * 16,
+                                    c->copyStream));
+        AZ_CUDA(cudaEventRecord(c->copyDone[slot], c->copyStream));
+    }
+    AZ_CUDA(c->ring.drain(c->copyStream));
+    AZ_CUDA(cudaStreamSynchronize(c->copyStream));
+    AZ_CUDA(cudaStreamSynchronize(st));
+    // give the slots back before returning (the default pool keeps nothing across a synchronisation)
+    AZ_CUDA(dIn.release());
+    AZ_CUDA(dOut.release());
+    AZ_CUDA(cudaStreamSynchronize(st));
+    return ASTROZ_OK;
 }
 
 int32_t astroz_cuda_fp64_peak(int32_t device, double *tflops) {

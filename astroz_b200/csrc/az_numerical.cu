@@ -1,0 +1,56 @@
+// az_numerical.cu -- K7: numerical propagation of a batch of initial states (RK4 / Dormand-Prince 8(7), two-body with
+// optional J2 and drag), one state per thread.  The per-state cores are in az_numerical.cuh.
+//
+// A state's whole trajectory is one thread's sequential loop; its state, its DP87 step size and the stages of the
+// current attempt live in registers (tools/numerical_timing.py and DESIGN.md section 3 "K7 numerical" give the register
+// counts of the eight specialisations).  The states of a batch are independent, so the batch is the parallel axis, and
+// a state's bits depend on its own inputs alone.
+#include "az_numerical.cuh"
+
+namespace az {
+namespace {
+
+constexpr int kNumThreads = 64;
+
+template <int kInt, int kForces>
+__global__ void __launch_bounds__(kNumThreads) numerical_kernel(NumArgs a) {
+    const uint32_t i = blockIdx.x * kNumThreads + threadIdx.x;
+    if (i >= a.n) return;
+    double y0[6];
+#pragma unroll
+    for (int c = 0; c < 6; ++c) y0[c] = a.states[(size_t)i * 6 + c];
+    DragBody d{0.0, 0.0, 0.0};
+    if (kForces & kForceDrag) d = DragBody{a.cd[i], a.area[i], a.mass[i]};
+    uint64_t counts[2];
+    const size_t samples = (size_t)a.steps.nFull + a.steps.nTail + 1;
+    const uint8_t st = propagate_state<kInt, kForces>(y0, d, a.p, a.steps, a.out + (size_t)i * samples * 6, counts);
+    a.status[i] = st;
+    if (a.counts) {
+        a.counts[(size_t)i * 2] = counts[0];
+        a.counts[(size_t)i * 2 + 1] = counts[1];
+    }
+}
+
+template <int kInt>
+cudaError_t launch_forces(const NumArgs &a, int forces, dim3 grid, cudaStream_t s) {
+    switch (forces) {
+        case 0: numerical_kernel<kInt, 0><<<grid, kNumThreads, 0, s>>>(a); break;
+        case kForceJ2: numerical_kernel<kInt, kForceJ2><<<grid, kNumThreads, 0, s>>>(a); break;
+        case kForceDrag: numerical_kernel<kInt, kForceDrag><<<grid, kNumThreads, 0, s>>>(a); break;
+        case kForceJ2 | kForceDrag: numerical_kernel<kInt, kForceJ2 | kForceDrag><<<grid, kNumThreads, 0, s>>>(a); break;
+        default: return cudaErrorInvalidValue;
+    }
+    return cudaGetLastError();
+}
+
+}  // namespace
+
+cudaError_t launch_numerical(const NumArgs &a, int integrator, int forces, cudaStream_t s) {
+    if (a.n == 0) return cudaSuccess;
+    const dim3 grid((a.n + kNumThreads - 1) / kNumThreads);
+    if (integrator == kIntRk4) return launch_forces<kIntRk4>(a, forces, grid, s);
+    if (integrator == kIntDp87) return launch_forces<kIntDp87>(a, forces, grid, s);
+    return cudaErrorInvalidValue;
+}
+
+}  // namespace az

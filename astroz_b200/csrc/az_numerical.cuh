@@ -1,0 +1,351 @@
+// az_numerical.cuh -- per-state cores of K7, numerical propagation of a batch of initial states: what
+// propagate_numerical(state, t0, duration, dt, mu, ...) computes for one state (bindings/python/src/propagator.zig:13-193),
+// one state per thread.  __host__ __device__, so tests/host_emul runs the same arithmetic on the CPU.
+//
+// The integrator (RK4 / Dormand-Prince 8(7)) and the force set (two-body, + J2, + drag, + J2 + drag) are template
+// parameters: each of the eight specialisations carries only its own stages and force terms.  Every operation follows
+// the reference's order (the file is compiled without FMA contraction), so a two-body or J2 trajectory equals the
+// scalar restatement bit for bit; the step-growth factor (errNorm^-1/8, three square roots here, pow in the reference)
+// and exp (drag) round differently.
+#pragma once
+
+#include "az_math.cuh"
+
+namespace az {
+
+// force-set bits (ASTROZ_FORCE_*); two-body is always on
+constexpr int kForceJ2 = 1, kForceDrag = 2;
+// integrators (ASTROZ_INTEGRATOR_*)
+constexpr int kIntRk4 = 0, kIntDp87 = 1;
+// per-state status bytes (ASTROZ_NUMERICAL_*)
+constexpr uint8_t kNumOk = 0, kNumStopped = 1, kNumSubstepLimit = 2, kNumNonFinite = 3;
+
+// Exponential atmosphere of the binding: earth's sea-level density and scale height (src/constants.zig:163-164) and the
+// 1500 km cutoff (bindings/python/src/propagator.zig:11)
+constexpr double kDragRho0 = 1.225, kDragScaleHeight = 7.249, kDragMaxAltitude = 1500.0;
+// DormandPrince87 step control (src/propagators/Integrator.zig:62-69)
+constexpr double kDpHMin = 0.001, kDpHMax = 3600.0, kDpSafety = 0.9, kDpHStart = 60.0;
+constexpr uint32_t kDpMaxSubsteps = 10000;
+
+// Prince & Dormand (1981), RK8(7)13M: nodes c, stage weights a (row i uses stages j < i), the 8th-order weights b8
+// (the propagated solution) and the 7th-order weights b7 (the error estimate).
+struct Dp87Tableau {
+    double c[13];
+    double a[13][12];
+    double b8[13];
+    double b7[13];
+};
+// clang-format off
+#define AZ_DP87_TABLEAU {                                                                                              \
+    {0.0, 1.0 / 18.0, 1.0 / 12.0, 1.0 / 8.0, 5.0 / 16.0, 3.0 / 8.0, 59.0 / 400.0, 93.0 / 200.0,                        \
+     5490023248.0 / 9719169821.0, 13.0 / 20.0, 1201146811.0 / 1299019798.0, 1.0, 1.0},                                 \
+    {{0},                                                                                                              \
+     {1.0 / 18.0},                                                                                                     \
+     {1.0 / 48.0, 1.0 / 16.0},                                                                                         \
+     {1.0 / 32.0, 0, 3.0 / 32.0},                                                                                      \
+     {5.0 / 16.0, 0, -75.0 / 64.0, 75.0 / 64.0},                                                                       \
+     {3.0 / 80.0, 0, 0, 3.0 / 16.0, 3.0 / 20.0},                                                                       \
+     {29443841.0 / 614563906.0, 0, 0, 77736538.0 / 692538347.0, -28693883.0 / 1125000000.0,                           \
+      23124283.0 / 1800000000.0},                                                                                      \
+     {16016141.0 / 946692911.0, 0, 0, 61564180.0 / 158732637.0, 22789713.0 / 633445777.0,                             \
+      545815736.0 / 2771057229.0, -180193667.0 / 1043307555.0},                                                        \
+     {39632708.0 / 573591083.0, 0, 0, -433636366.0 / 683701615.0, -421739975.0 / 2616292301.0,                        \
+      100302831.0 / 723423059.0, 790204164.0 / 839813087.0, 800635310.0 / 3783071287.0},                               \
+     {246121993.0 / 1340847787.0, 0, 0, -37695042795.0 / 15268766246.0, -309121744.0 / 1061227803.0,                  \
+      -12992083.0 / 490766935.0, 6005943493.0 / 2108947869.0, 393006217.0 / 1396673457.0,                              \
+      123872331.0 / 1001029789.0},                                                                                     \
+     {-1028468189.0 / 846180014.0, 0, 0, 8478235783.0 / 508512852.0, 1311729495.0 / 1432422823.0,                     \
+      -10304129995.0 / 1701304382.0, -48777925059.0 / 3047939560.0, 15336726248.0 / 1032824649.0,                      \
+      -45442868181.0 / 3398467696.0, 3065993473.0 / 597172653.0},                                                      \
+     {185892177.0 / 718116043.0, 0, 0, -3185094517.0 / 667107341.0, -477755414.0 / 1098053517.0,                      \
+      -703635378.0 / 230739211.0, 5731566787.0 / 1027545527.0, 5232866602.0 / 850066563.0,                             \
+      -4093664535.0 / 808688257.0, 3962137247.0 / 1805957418.0, 65686358.0 / 487910083.0},                             \
+     {403863854.0 / 491063109.0, 0, 0, -5068492393.0 / 434740067.0, -411421997.0 / 543043805.0,                       \
+      652783627.0 / 914296604.0, 11173962825.0 / 925320556.0, -13158990841.0 / 6184727034.0,                           \
+      3936647629.0 / 1978049680.0, -160528059.0 / 685178525.0, 248638103.0 / 1413531060.0, 0}},                        \
+    {14005451.0 / 335480064.0, 0, 0, 0, 0, -59238493.0 / 1068277825.0, 181606767.0 / 758867731.0,                      \
+     561292985.0 / 797845732.0, -1041891430.0 / 1371343529.0, 760417239.0 / 1151165299.0,                              \
+     118820643.0 / 751138087.0, -528747749.0 / 2220607170.0, 1.0 / 4.0},                                               \
+    {13451932.0 / 455176623.0, 0, 0, 0, 0, -808719846.0 / 976000145.0, 1757004468.0 / 5645159321.0,                    \
+     656045339.0 / 265891186.0, -3867574721.0 / 1518517206.0, 465885868.0 / 322736535.0,                               \
+     53011238.0 / 667516719.0, 2.0 / 45.0, 0}}
+// clang-format on
+// Almost every weight has a non-zero low word: they are read from constant memory, warp-uniform broadcasts that the
+// DFMA / DMUL takes as a c[bank][offset] operand (the K1 rule, az_math.cuh).
+static __constant__ Dp87Tableau kDp87Dev = AZ_DP87_TABLEAU;
+static const Dp87Tableau kDp87Host = AZ_DP87_TABLEAU;
+#ifdef __CUDA_ARCH__
+#define AZ_DP87(field) (::az::kDp87Dev.field)
+#else
+#define AZ_DP87(field) (::az::kDp87Host.field)
+#endif
+
+// The tableau's zero pattern, as compile-time facts for the unrolled stage loops (a zero weight is skipped, as the
+// reference skips it): stages 1 and 2 feed only rows 2-4, a[12][11] = 0, b8 and b7 have no weight on stages 1-4, b7
+// none on stage 12.  tests/test_numerical_host_emulation.py checks these against the table.
+AZ_HD constexpr bool dp87_a_nz(int i, int j) {
+    return j < i && !(j == 1 && i != 2) && !(j == 2 && i != 3 && i != 4) && !(i == 3 && j == 1) &&
+           !(i == 12 && j == 11);
+}
+AZ_HD constexpr bool dp87_b8_nz(int i) { return i == 0 || i >= 5; }
+AZ_HD constexpr bool dp87_b7_nz(int i) { return i == 0 || (i >= 5 && i <= 11); }
+
+struct NumParams {
+    double mu, j2, rEq;  // km^3/s^2, -, km
+    double rtol, atol;   // DP87 tolerances
+};
+struct DragBody {
+    double cd, area, mass;  // -, m^2, kg
+};
+
+// Accelerations in the order of the binding's force list (propagator.zig:119-146): TwoBody (ForceModel.zig:49-55), J2
+// (:67-79), Drag (:95-110).  Several models are summed by Composite (:365-374) into a total that starts at zero;
+// a single model is returned as it is.
+template <int kForces>
+AZ_HD void accel(const double s[6], const NumParams &p, const DragBody &d, double acc[3]) {
+    const double x = s[0], y = s[1], z = s[2];
+    const double r = sqrt(x * x + y * y + z * z);
+    const double f = -p.mu / (r * r * r);
+    if (kForces == 0) {
+        acc[0] = f * x;
+        acc[1] = f * y;
+        acc[2] = f * z;
+        return;
+    }
+    acc[0] = 0.0 + f * x;
+    acc[1] = 0.0 + f * y;
+    acc[2] = 0.0 + f * z;
+    if (kForces & kForceJ2) {
+        const double r2 = x * x + y * y + z * z;
+        const double rj = sqrt(r2);
+        const double fj = -1.5 * p.j2 * p.mu * p.rEq * p.rEq / (r2 * r2 * rj);
+        const double z2r2 = (z * z) / r2;
+        acc[0] += fj * x * (5.0 * z2r2 - 1.0);
+        acc[1] += fj * y * (5.0 * z2r2 - 1.0);
+        acc[2] += fj * z * (5.0 * z2r2 - 3.0);
+    }
+    if (kForces & kForceDrag) {
+        // a model returning zeros adds nothing to a total that is never -0
+        const double alt = r - p.rEq;
+        if (!(alt > kDragMaxAltitude)) {
+            const double vx = s[3], vy = s[4], vz = s[5];
+            const double v = sqrt(vx * vx + vy * vy + vz * vz);
+            if (!(v < 1e-10)) {
+                const double rho = kDragRho0 * exp(-alt / kDragScaleHeight);
+                const double fd = -0.5 * d.cd * d.area * rho * v * 1e3 / d.mass;
+                acc[0] += fd * vx / v;
+                acc[1] += fd * vy / v;
+                acc[2] += fd * vz / v;
+            }
+        }
+    }
+}
+
+// derivative of Integrator.zig:47-50 / :261-264: (velocity, acceleration)
+template <int kForces>
+AZ_HD void deriv(const double s[6], const NumParams &p, const DragBody &d, double k[6]) {
+    double a[3];
+    accel<kForces>(s, p, d, a);
+    k[0] = s[3];
+    k[1] = s[4];
+    k[2] = s[5];
+    k[3] = a[0];
+    k[4] = a[1];
+    k[5] = a[2];
+}
+
+// Rk4.step (Integrator.zig:28-45); y is replaced by the state after dt
+template <int kForces>
+AZ_HD void rk4_step(double y[6], double dt, const NumParams &p, const DragBody &d) {
+    double k1[6], k2[6], k3[6], k4[6], s[6];
+    const double half = 0.5 * dt;
+    deriv<kForces>(y, p, d, k1);
+#pragma unroll
+    for (int c = 0; c < 6; ++c) s[c] = y[c] + k1[c] * half;
+    deriv<kForces>(s, p, d, k2);
+#pragma unroll
+    for (int c = 0; c < 6; ++c) s[c] = y[c] + k2[c] * half;
+    deriv<kForces>(s, p, d, k3);
+#pragma unroll
+    for (int c = 0; c < 6; ++c) s[c] = y[c] + k3[c] * dt;
+    deriv<kForces>(s, p, d, k4);
+    const double factor = dt / 6.0;
+#pragma unroll
+    for (int c = 0; c < 6; ++c) y[c] = y[c] + factor * (k1[c] + 2.0 * k2[c] + 2.0 * k3[c] + k4[c]);
+}
+
+// One attempt of DormandPrince87.adaptiveStep (Integrator.zig:190-259) from y with step h: y8 receives the 8th-order
+// solution, the return value is errNorm.  The 8th- and 7th-order sums are accumulated as each stage is formed; that is
+// the reference's order of additions (stage by stage, zero weights skipped), so only stages still read by later rows
+// stay live.
+template <int kForces>
+AZ_HD double dp87_attempt(const double y[6], double h, const NumParams &p, const DragBody &d, double y8[6]) {
+    double k[13][6];
+    double y7[6];
+#pragma unroll
+    for (int c = 0; c < 6; ++c) y8[c] = y7[c] = y[c];
+#pragma unroll
+    for (int i = 0; i < 13; ++i) {
+        double ys[6];
+#pragma unroll
+        for (int c = 0; c < 6; ++c) ys[c] = y[c];
+#pragma unroll
+        for (int j = 0; j < 12; ++j) {
+            if (dp87_a_nz(i, j)) {
+                const double ah = AZ_DP87(a[i][j]) * h;
+#pragma unroll
+                for (int c = 0; c < 6; ++c) ys[c] = ys[c] + ah * k[j][c];
+            }
+        }
+        deriv<kForces>(ys, p, d, k[i]);
+        if (dp87_b8_nz(i)) {
+            const double bh = AZ_DP87(b8[i]) * h;
+#pragma unroll
+            for (int c = 0; c < 6; ++c) y8[c] = y8[c] + bh * k[i][c];
+        }
+        if (dp87_b7_nz(i)) {
+            const double bh = AZ_DP87(b7[i]) * h;
+#pragma unroll
+            for (int c = 0; c < 6; ++c) y7[c] = y7[c] + bh * k[i][c];
+        }
+    }
+    double e = 0.0;
+#pragma unroll
+    for (int c = 0; c < 6; ++c) {
+        const double scale = p.atol + p.rtol * fmax(fabs(y[c]), fabs(y8[c]));
+        const double se = (y8[c] - y7[c]) / scale;
+        e += se * se;
+    }
+    return sqrt(e / 6.0);
+}
+
+// hNew of adaptiveStep (Integrator.zig:244-252).  errNorm^(-1/8) is formed as three correctly rounded square roots
+// (the same bits on host and device; the reference's pow differs from it in the last place).  fmin / fmax return the
+// non-NaN operand, as Zig's @min / @max do, so a NaN errNorm shrinks the step tenfold.
+AZ_HD double dp87_next_h(double h, double errNorm) {
+    double hNew;
+    if (errNorm < 1e-10) {
+        hNew = h * 5.0;
+    } else {
+        const double factor = kDpSafety * sqrt(sqrt(sqrt(1.0 / errNorm)));
+        hNew = h * fmin(5.0, fmax(0.1, factor));
+    }
+    hNew = fmin(hNew, kDpHMax);
+    return fmax(hNew, kDpHMin);
+}
+
+// DormandPrince87.step (Integrator.zig:154-182) over one output interval of length dt, carrying hCur from interval to
+// interval.  Returns kNumOk, kNumSubstepLimit (10,000 accepted substeps and the interval not finished: y is where the
+// reference leaves it) or kNumStopped: an attempt rejected at h == hMin, which the reference retries with the same y
+// and h forever (this is also where a non-finite errNorm ends).  counts[0] / counts[1] add accepted / rejected attempts.
+template <int kForces>
+AZ_HD uint8_t dp87_interval(double y[6], double &hCur, double dt, const NumParams &p, const DragBody &d,
+                            uint64_t counts[2]) {
+    double remaining = dt;
+    uint32_t substeps = 0;
+    double h = fmin(hCur, remaining);
+    while (remaining > 1e-14 && substeps < kDpMaxSubsteps) {
+        h = fmin(h, remaining);
+        h = fmax(h, kDpHMin);
+        double y8[6];
+        const double errNorm = dp87_attempt<kForces>(y, h, p, d, y8);
+        const double hNew = dp87_next_h(h, errNorm);
+        if (errNorm <= 1.0) {
+#pragma unroll
+            for (int c = 0; c < 6; ++c) y[c] = y8[c];
+            remaining -= h;
+            ++substeps;
+            ++counts[0];
+        } else {
+            ++counts[1];
+            if (h == kDpHMin) {
+                hCur = hNew;
+                return kNumStopped;
+            }
+        }
+        h = hNew;
+    }
+    hCur = h;
+    return (remaining > 1e-14) ? kNumSubstepLimit : kNumOk;
+}
+
+AZ_HD bool all_finite(const double y[6]) {
+    bool ok = true;
+#pragma unroll
+    for (int c = 0; c < 6; ++c) ok = ok && isfinite(y[c]);
+    return ok;
+}
+
+// The step sizes of the sampling loop `while (t < t_end) { step = min(dt, t_end - t); ...; t += step; }`
+// (src/propagators/Propagator.zig:39-45), as the host's loop produced them: every step is dt until t_end - t < dt, then a
+// tail of short steps.  The tail is one step, or two when t_end - t was rounded (after one short step t is within an ulp
+// of t_end, and the next difference is exact); kMaxTail leaves room.  Small enough to travel as a kernel parameter, so no
+// table has to be uploaded before a launch.
+constexpr uint32_t kMaxTail = 4;
+struct StepTable {
+    double dt;
+    uint32_t nFull, nTail;    // K = nFull + nTail steps
+    double tail[kMaxTail];
+    AZ_HD double step(uint32_t k) const { return k < nFull ? dt : tail[k - nFull]; }
+};
+// Append the loop's next step to t (start from StepTable{dt, 0, 0, {}}); false when the steps do not have the shape above.
+inline bool step_table_push(StepTable &t, double step) {
+    if (step == t.dt && t.nTail == 0) return ++t.nFull != 0;  // 32-bit wrap: more steps than K7 counts
+    if (t.nTail == kMaxTail) return false;
+    t.tail[t.nTail++] = step;
+    return true;
+}
+
+// One state's trajectory (Propagator.propagate, src/propagators/Propagator.zig:22-48): y0 at out[0..6), then the state
+// after each of the K intervals of `steps` (the sampling loop's step sizes, built once on the host) at out[6 (k + 1)).
+// A stopped state's later samples are zero-filled.  Returns the status byte; counts[2] receives accepted / rejected
+// steps (RK4: one accepted step per interval).
+template <int kInt, int kForces>
+AZ_HD uint8_t propagate_state(const double y0[6], const DragBody &d, const NumParams &p, const StepTable &steps,
+                              double *out, uint64_t counts[2]) {
+    const uint32_t K = steps.nFull + steps.nTail;
+    double y[6];
+#pragma unroll
+    for (int c = 0; c < 6; ++c) out[c] = y[c] = y0[c];
+    counts[0] = counts[1] = 0;
+    uint8_t status = kNumOk;
+    double hCur = kDpHStart;
+    for (uint32_t k = 0; k < K; ++k) {
+        const double dt = steps.step(k);
+        if (kInt == kIntRk4) {
+            rk4_step<kForces>(y, dt, p, d);
+            ++counts[0];
+            if (status == kNumOk && !all_finite(y)) status = kNumNonFinite;
+        } else {
+            const uint8_t st = dp87_interval<kForces>(y, hCur, dt, p, d, counts);
+            if (st == kNumStopped) {
+                for (size_t w = (size_t)(k + 1) * 6; w < (size_t)(K + 1) * 6; ++w) out[w] = 0.0;
+                return kNumStopped;
+            }
+            if (st == kNumSubstepLimit) status = kNumSubstepLimit;
+        }
+        double *o = out + (size_t)(k + 1) * 6;
+#pragma unroll
+        for (int c = 0; c < 6; ++c) o[c] = y[c];
+    }
+    return status;
+}
+
+}  // namespace az
+
+#ifndef AZ_NUMERICAL_CORES_ONLY
+namespace az {
+struct NumArgs {
+    const double *states;            // [n][6]
+    const double *cd, *area, *mass;  // [n] each (drag force sets only)
+    StepTable steps;                 // the sampling loop's step sizes
+    uint32_t n;
+    NumParams p;
+    double *out;        // [n][K + 1][6]
+    uint8_t *status;    // [n]
+    uint64_t *counts;   // [n][2] or nullptr
+};
+// Queue K7 for `integrator` / `forces` on s.
+cudaError_t launch_numerical(const NumArgs &a, int integrator, int forces, cudaStream_t s);
+}  // namespace az
+#endif

@@ -193,4 +193,47 @@ def screen(source, times, threshold=10.0, *, target=None, start_time=None, norad
     return dev.coarse_screen_device(block, float(threshold))
 
 
-__all__ = ["Constellation", "propagate", "screen", "parse_tle_pairs", "omm_to_tle_pairs"]
+# WGS-84 (src/constants.zig:55-58), the values the reference exports as EARTH_MU / EARTH_R_EQ / EARTH_J2
+EARTH_MU = 398600.5
+EARTH_R_EQ = 6378.137
+EARTH_J2 = 0.00108262998905
+
+
+def propagate_numerical(state, t0, duration, dt, mu, j2=None, r_eq=None, drag_cd=None, drag_area=None, drag_mass=None,
+                        integrator=None, rtol=None, atol=None):
+    """`astroz.propagate_numerical(state, t0, duration, dt, mu, ...)` (bindings/python/src/propagator.zig:13-193): the
+    trajectory of one state as (list of times, list of (x, y, z, vx, vy, vz) tuples), integrated on the device as a batch
+    of one.  Every argument after mu is positional-or-keyword and None selects its default, as the reference's parser
+    does (:28-52, :76-79).  Raises the reference's ValueErrors; where the reference would never return it raises instead:
+    ValueError for dt <= 0 with a loop to run, RuntimeError when a Dormand-Prince step is rejected at its minimum size
+    (the reference retries that step forever)."""
+    from . import numerical
+
+    if len(state) != 6:
+        raise ValueError("state must have exactly 6 elements [x, y, z, vx, vy, vz]")
+    initial = [float(x) for x in state]
+    t0, duration, dt, mu = float(t0), float(duration), float(dt), float(mu)
+    if (j2 is not None or drag_cd is not None) and r_eq is None:
+        raise ValueError("r_eq is required when j2 or drag_cd is specified")
+    if drag_cd is not None and (drag_area is None or drag_mass is None):
+        raise ValueError("drag_area and drag_mass are required when drag_cd is specified")
+    if integrator is None:
+        integrator = "dp87"
+    if integrator not in ("rk4", "dp87"):
+        raise ValueError("integrator must be 'rk4' or 'dp87'")
+    if not t0 < t0 + duration:
+        return [t0], [tuple(initial)]   # the loop does not run, whatever dt is (Propagator.zig:36-40)
+    if not dt > 0.0:
+        raise ValueError("dt must be positive (the reference's sampling loop would not end)")
+    times, traj, status, _ = numerical.propagate_numerical_batch(
+        np.array([initial]), t0, duration, dt, mu, j2=j2, r_eq=r_eq, drag_cd=drag_cd, drag_area=drag_area,
+        drag_mass=drag_mass, integrator=integrator, rtol=1e-9 if rtol is None else float(rtol),
+        atol=1e-12 if atol is None else float(atol))
+    if status[0] == numerical.STOPPED:
+        raise RuntimeError("propagation stopped: a Dormand-Prince step was rejected at the minimum step size "
+                           "(the reference retries it forever)")
+    return [float(t) for t in times], [tuple(float(x) for x in row) for row in traj[0]]
+
+
+__all__ = ["Constellation", "propagate", "screen", "parse_tle_pairs", "omm_to_tle_pairs", "propagate_numerical",
+           "EARTH_MU", "EARTH_R_EQ", "EARTH_J2"]

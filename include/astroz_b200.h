@@ -339,6 +339,63 @@ int32_t astroz_cuda_constellation_propagate_device_f32(astroz_constellation_t h,
                                                        uint32_t n_times, double *d_pos, double *d_vel, int32_t phase64,
                                                        void *stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Numerical propagation of a batch of initial states: replaces propagate_numerical (bindings/python/src/propagator.zig:
+ * 13-193), which integrates ONE state per call on one CPU thread, with n independent states in one device call.
+ * State i's trajectory is what propagate_numerical(states[i], t0, duration, dt, mu, ...) returns for it:
+ *   samples: Propagator.propagate (src/propagators/Propagator.zig:22-48) -- the state at t0, then after each step of
+ *            while (t < t_end) { step = min(dt, t_end - t); ...; t += step; }, t_end = t0 + duration; every state shares
+ *            this sequence, given by astroz_cuda_numerical_times;
+ *   forces:  two-body, then J2 (forces & ASTROZ_FORCE_J2), then exponential-atmosphere drag (forces & ASTROZ_FORCE_DRAG:
+ *            rho0 1.225 kg/m^3, H 7.249 km, none above 1500 km), ForceModel.zig:42-111 and :351-375; drag takes cd,
+ *            area [m^2] and mass [kg] per state;
+ *   integrator: ASTROZ_INTEGRATOR_RK4 (Integrator.zig:21-58) or ASTROZ_INTEGRATOR_DP87 (Dormand-Prince 8(7),
+ *            Integrator.zig:60-269: hMin 0.001 s, hMax 3600 s, h starting at 60 s and carried from interval to interval,
+ *            10,000 accepted substeps per interval at most) with tolerances rtol / atol.
+ * Units: km, km/s, s, km^3/s^2.  Outputs: out[n][samples][6] (x y z vx vy vz), status[n] (ASTROZ_NUMERICAL_*),
+ * steps[n][2] (nullable): accepted and rejected steps (RK4: one accepted step per interval).
+ * Where the reference never returns -- a DP87 step rejected at hMin is retried with the same state and step forever
+ * (e.g. a state whose error norm is not finite at any step size, such as one at the centre; a re-entry under drag does
+ * not stop, its stiff drag term only shrinks the steps) -- the state stops: status ASTROZ_NUMERICAL_STOPPED and its
+ * remaining samples zero-filled, like the library's failed cells.
+ * ASTROZ_VALUE_ERROR, nothing written: dt <= 0; t0, duration, dt, mu, rtol, atol (or j2 / r_eq when used) not finite;
+ * j2 missing with J2 on; r_eq missing with J2 or drag on; drag arrays missing with drag on; an unknown integrator or
+ * force bit; a sampling loop that would not end or more than 2^32 - 2 steps; an output size that overflows;
+ * device = -1 (these calls run on one device). */
+#define ASTROZ_FORCE_J2        1
+#define ASTROZ_FORCE_DRAG      2
+#define ASTROZ_INTEGRATOR_RK4  0
+#define ASTROZ_INTEGRATOR_DP87 1
+#define ASTROZ_NUMERICAL_OK            0
+#define ASTROZ_NUMERICAL_STOPPED       1   /* the reference would loop forever; remaining samples zero-filled */
+#define ASTROZ_NUMERICAL_SUBSTEP_LIMIT 2   /* some DP87 interval hit 10,000 substeps: that sample is the reference's, not
+                                              at its nominal time */
+#define ASTROZ_NUMERICAL_NON_FINITE    3   /* an RK4 trajectory went to NaN or inf (the values are kept) */
+
+/* The sample times of the batch calls (Propagator.zig:32-45 evaluated on the host, the one home of the sampling rule):
+ * *count = number of samples; times (nullable) receives them.  Same argument errors as the batch calls. */
+int32_t astroz_cuda_numerical_times(double t0, double duration, double dt, double *times, uint64_t *count);
+
+/* HOST buffers: states[n][6]; drag_cd / drag_area / drag_mass [n] each (NULL unless drag is on); out / status / steps as
+ * above.  States are processed in chunks, upload / kernel / download overlapped; pageable buffers go through a pinned
+ * ring and the host copy pool, pinned and registered ones receive their results by direct DMA.  The device slots are
+ * returned before the call returns; per device, two streams and (after the first pageable transfer) the 96 MB pinned
+ * ring stay for the life of the process.  n = 0 is a no-op. */
+int32_t astroz_cuda_propagate_numerical(const double *states, uint32_t n, double t0, double duration, double dt,
+                                        double mu, int32_t forces, const double *j2, const double *r_eq,
+                                        const double *drag_cd, const double *drag_area, const double *drag_mass,
+                                        int32_t integrator, double rtol, double atol, int32_t device, double *out,
+                                        uint8_t *status, uint64_t *steps);
+/* Same with DEVICE pointers on `device` (j2 / r_eq stay host scalars).  Asynchronous on `stream` (a cudaStream_t, NULL =
+ * the legacy default stream): the step sizes travel in the launch's parameters, so the call queues one kernel and
+ * returns. */
+int32_t astroz_cuda_propagate_numerical_device(const double *d_states, uint32_t n, double t0, double duration,
+                                               double dt, double mu, int32_t forces, const double *j2,
+                                               const double *r_eq, const double *d_drag_cd,
+                                               const double *d_drag_area, const double *d_drag_mass,
+                                               int32_t integrator, double rtol, double atol, int32_t device,
+                                               double *d_out, uint8_t *d_status, uint64_t *d_steps, void *stream);
+
 /* ---- measurement helpers --------------------------------------------------------------------- */
 /* DFMA microbenchmark on `device`: achieved fp64 TFLOP/s (FMA = 2) -- the measured roofline denominator */
 int32_t astroz_cuda_fp64_peak(int32_t device, double *tflops);

@@ -36,7 +36,7 @@ def zig_type(ctype: str, name: str) -> str:
         "const uint32_t *": "?[*]const u32",
         "uint32_t *": "?[*]u32",
         "int32_t *": "?[*]i32",
-        "uint64_t *": "*u64",
+        "uint64_t *": "?[*]u64" if name in ("steps", "d_steps") else "*u64",
         "void *": "?*anyopaque",
         "void *const *": "?[*]const ?*anyopaque",
         "astroz_constellation_t": "Handle",

@@ -51,6 +51,9 @@ pub extern fn astroz_cuda_sgp4_propagate(h: Handle, tsince: f64, pos: *[3]f64, v
 pub extern fn astroz_cuda_sgp4_propagate_batch(h: Handle, times: ?[*]const f64, results: ?[*]f64, count: u32) i32;
 pub extern fn astroz_cuda_sgp4_array(h: Handle, jd: ?[*]const f64, fr: ?[*]const f64, epoch_jd: f64, results: ?[*]f64, count: u32) i32;
 pub extern fn astroz_cuda_constellation_propagate_device_f32(h: Handle, jd: ?[*]const f64, fr: ?[*]const f64, n_times: u32, d_pos: ?[*]f64, d_vel: ?[*]f64, phase64: i32, stream: ?*anyopaque) i32;
+pub extern fn astroz_cuda_numerical_times(t0: f64, duration: f64, dt: f64, times: ?[*]f64, count: *u64) i32;
+pub extern fn astroz_cuda_propagate_numerical(states: ?[*]const f64, n: u32, t0: f64, duration: f64, dt: f64, mu: f64, forces: i32, j2: ?[*]const f64, r_eq: ?[*]const f64, drag_cd: ?[*]const f64, drag_area: ?[*]const f64, drag_mass: ?[*]const f64, integrator: i32, rtol: f64, atol: f64, device: i32, out: ?[*]f64, status: ?[*]u8, steps: ?[*]u64) i32;
+pub extern fn astroz_cuda_propagate_numerical_device(d_states: ?[*]const f64, n: u32, t0: f64, duration: f64, dt: f64, mu: f64, forces: i32, j2: ?[*]const f64, r_eq: ?[*]const f64, d_drag_cd: ?[*]const f64, d_drag_area: ?[*]const f64, d_drag_mass: ?[*]const f64, integrator: i32, rtol: f64, atol: f64, device: i32, d_out: ?[*]f64, d_status: ?[*]u8, d_steps: ?[*]u64, stream: ?*anyopaque) i32;
 pub extern fn astroz_cuda_fp64_peak(device: i32, tflops: ?[*]f64) i32;
 pub extern fn astroz_cuda_fp64_pipe_peak(device: i32, tflops: ?[*]f64) i32;
 
