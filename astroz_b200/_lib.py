@@ -110,6 +110,10 @@ def lib() -> C.CDLL:
         "astroz_cuda_propagate_numerical_device": (i32, [vp, u32, C.c_double, C.c_double, C.c_double, C.c_double, i32,
                                                          dp, dp, vp, vp, vp, i32, C.c_double, C.c_double, i32, vp, vp,
                                                          vp, vp]),
+        "astroz_cuda_propagate_numerical_models": (i32, [vp, u32, C.c_double, C.c_double, C.c_double, vp, u32, i32,
+                                                         C.c_double, C.c_double, i32, vp, vp, vp]),
+        "astroz_cuda_propagate_numerical_models_device": (i32, [vp, u32, C.c_double, C.c_double, C.c_double, vp, u32,
+                                                                i32, C.c_double, C.c_double, i32, vp, vp, vp, vp]),
         "astroz_cuda_fp64_peak": (i32, [i32, dp]),
         "astroz_cuda_fp64_pipe_peak": (i32, [i32, dp]),
     }
@@ -142,6 +146,7 @@ EXPORTS = [
     "astroz_cuda_constellation_set_timing", "astroz_cuda_constellation_host_block",
     "astroz_cuda_constellation_propagate_pairs", "astroz_cuda_constellation_propagate_pairs_device",
     "astroz_cuda_numerical_times", "astroz_cuda_propagate_numerical", "astroz_cuda_propagate_numerical_device",
+    "astroz_cuda_propagate_numerical_models", "astroz_cuda_propagate_numerical_models_device",
 ]
 
 

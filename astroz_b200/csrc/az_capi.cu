@@ -14,6 +14,8 @@
 #include <unistd.h>
 
 #include <condition_variable>
+#include <cstddef>
+#include <initializer_list>
 #include <functional>
 #include <map>
 #include <memory>
@@ -2250,36 +2252,36 @@ int32_t astroz_cuda_propagate_numerical_device(const double *d_states, uint32_t 
 }
 
 // Host buffers: chunks of states on two device slots, each chunk's trajectory block at most kNumChunkBytes (eight ring
-// pieces).  Chunk k's states go up and its kernel runs on the compute stream while chunk k-1's results come back on the
-// copy stream (pinned / registered destinations) or through the pinned ring and the copy pool (pageable ones);
-// pageable inputs are staged through the same ring.
+// pieces).  Chunk k's states and per-state columns go up and its kernel runs on the compute stream while chunk k-1's
+// results come back on the copy stream (pinned / registered destinations) or through the pinned ring and the copy pool
+// (pageable ones); pageable inputs are staged through the same ring.  `cols` are the per-state input columns the kernel
+// reads ([n] doubles each; the fixed drag set has three, a model list one per per-state array it names); `tabs` are
+// whole arrays uploaded once per call before the first chunk (a model list's position tables).
+// launch(m, dStates, dCols, dTabs, dTraj, dStatus, dCounts, stream) queues the kernel for one chunk of m states.
 static constexpr size_t kNumChunkBytes = 256u << 20;
-int32_t astroz_cuda_propagate_numerical(const double *states, uint32_t n, double t0, double duration, double dt,
-                                        double mu, int32_t forces, const double *j2, const double *r_eq,
-                                        const double *drag_cd, const double *drag_area, const double *drag_mass,
-                                        int32_t integrator, double rtol, double atol, int32_t device, double *out,
-                                        uint8_t *status, uint64_t *steps) {
-    az::StepTable table{};
-    int32_t rc = numerical_check(n, t0, duration, dt, mu, forces, j2, r_eq, drag_cd, drag_area, drag_mass, integrator,
-                                 rtol, atol, device, &table);
-    if (rc != ASTROZ_OK) return rc;
-    if (n == 0) return ASTROZ_OK;
-    if (!states || !out || !status) return ASTROZ_NULL_POINTER;
-    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
+static constexpr int kNumMaxCols = 3 * (int)az::kMaxModels, kNumMaxTabs = (int)az::kMaxModels;
+extern "C++" {
+template <class Launch>
+static int32_t numerical_host_pipeline(const double *states, uint32_t n, const az::StepTable &table, int nCols,
+                                       const double *const *cols, int nTabs, const double *const *tabs,
+                                       const size_t *tabBytes, int32_t device, double *out, uint8_t *status,
+                                       uint64_t *steps, Launch launch) {
     NumericalContext *c = nullptr;
-    if ((rc = numerical_context(device, &c)) != ASTROZ_OK) return rc;
+    int32_t rc = numerical_context(device, &c);
+    if (rc != ASTROZ_OK) return rc;
     std::lock_guard<std::mutex> lk(c->m);
     AZ_CUDA(cudaSetDevice(device));
     cudaStream_t st = c->stream;
-    const bool drag = (forces & az::kForceDrag) != 0;
     const size_t rowD = ((size_t)table.nFull + table.nTail + 1) * 6;  // doubles of one state's trajectory
     const uint32_t chunk = (uint32_t)std::max<size_t>(1, std::min<size_t>(n, kNumChunkBytes / (rowD * 8)));
     const uint32_t nChunks = (uint32_t)(((uint64_t)n + chunk - 1) / chunk);
     const uint32_t slots = nChunks > 1 ? 2 : 1;
-    // slot layout, in doubles: inputs [states | cd | area | mass], results [trajectories | counts | status]
-    const size_t inD = (size_t)chunk * (drag ? 9 : 6);
+    // slot layout, in doubles: inputs [states | column 0 | column 1 | ...], results [trajectories | counts | status]
+    const size_t inD = (size_t)chunk * (6 + nCols);
     const size_t outD = (size_t)chunk * rowD + (steps ? (size_t)chunk * 2 : 0) + (chunk + 7) / 8;
-    StreamBuf dIn(st), dOut(st);
+    size_t tabD = 0;
+    for (int t = 0; t < nTabs; ++t) tabD += tabBytes[t] / 8;
+    StreamBuf dIn(st), dOut(st), dTab(st);
     // declared after the slots, so it runs before they are freed on any return: the ring's plan is forgotten and both
     // streams have finished with the slots
     struct Settle {
@@ -2292,36 +2294,44 @@ int32_t astroz_cuda_propagate_numerical(const double *states, uint32_t n, double
     } settle{c};
     AZ_CUDA(dIn.alloc(inD * slots * 8));
     AZ_CUDA(dOut.alloc(outD * slots * 8));
-    az::NumArgs a = numerical_args(n, table, mu, forces, j2, r_eq, rtol, atol);
-    const bool inPageable = az::is_pageable(states) ||
-                            (drag && (az::is_pageable(drag_cd) || az::is_pageable(drag_area) || az::is_pageable(drag_mass)));
+    const double *dTabs[kNumMaxTabs] = {};
+    if (nTabs) {
+        AZ_CUDA(dTab.alloc(tabD * 8));
+        double *at = static_cast<double *>(dTab.p);
+        for (int t = 0; t < nTabs; ++t) {
+            AZ_CUDA(cudaMemcpyAsync(at, tabs[t], tabBytes[t], cudaMemcpyHostToDevice, st));
+            dTabs[t] = at;
+            at += tabBytes[t] / 8;
+        }
+    }
+    bool inPageable = az::is_pageable(states);
+    for (int k = 0; k < nCols; ++k) inPageable = inPageable || az::is_pageable(cols[k]);
     const bool outPg = az::is_pageable(out), stPg = az::is_pageable(status), cntPg = steps && az::is_pageable(steps);
     const bool outPageable = outPg || stPg || cntPg;
-    const size_t inBytes[4] = {48, 8, 8, 8};
+    size_t inBytes[1 + kNumMaxCols];
+    inBytes[0] = 48;
+    for (int k = 0; k < nCols; ++k) inBytes[1 + k] = 8;
     c->ring.discard();
     for (uint32_t k = 0; k < nChunks; ++k) {
         const uint32_t slot = k % slots;
         const uint32_t s0 = k * chunk, m = std::min(chunk, n - s0);
         double *dStates = static_cast<double *>(dIn.p) + slot * inD;
-        double *dCd = dStates + (size_t)chunk * 6, *dArea = dCd + chunk, *dMass = dArea + chunk;
+        double *dCols[kNumMaxCols] = {};
+        for (int q = 0; q < nCols; ++q) dCols[q] = dStates + (size_t)chunk * (6 + q);
         double *dTraj = static_cast<double *>(dOut.p) + slot * outD;
         uint64_t *dCounts = steps ? reinterpret_cast<uint64_t *>(dTraj + (size_t)chunk * rowD) : nullptr;
         uint8_t *dSt = reinterpret_cast<uint8_t *>(dTraj + (size_t)chunk * rowD + (steps ? (size_t)chunk * 2 : 0));
         if (k >= slots) AZ_CUDA(cudaEventSynchronize(c->copyDone[slot]));  // chunk k-2's results have left this slot
-        const void *src[4] = {states + (size_t)s0 * 6, drag ? drag_cd + s0 : nullptr, drag ? drag_area + s0 : nullptr,
-                              drag ? drag_mass + s0 : nullptr};
-        void *const dst[4] = {dStates, dCd, dArea, dMass};
-        AZ_CUDA(c->ring.upload(inPageable, drag ? 4 : 1, src, dst, inBytes, m, st));
+        const void *src[1 + kNumMaxCols] = {states + (size_t)s0 * 6};
+        void *dst[1 + kNumMaxCols] = {dStates};
+        for (int q = 0; q < nCols; ++q) {
+            src[1 + q] = cols[q] + s0;
+            dst[1 + q] = dCols[q];
+        }
+        AZ_CUDA(c->ring.upload(inPageable, 1 + nCols, src, dst, inBytes, m, st));
         AZ_CUDA(cudaEventRecord(c->inputsDone, st));
-        a.n = m;
-        a.states = dStates;
-        a.cd = drag ? dCd : nullptr;
-        a.area = drag ? dArea : nullptr;
-        a.mass = drag ? dMass : nullptr;
-        a.out = dTraj;
-        a.status = dSt;
-        a.counts = dCounts;
-        AZ_CUDA(az::launch_numerical(a, integrator, forces, st));
+        AZ_CUDA(launch(m, dStates, static_cast<const double *const *>(dCols), static_cast<const double *const *>(dTabs),
+                       dTraj, dSt, dCounts, st));
         const cudaEvent_t ready = c->kernelDone[slot];
         AZ_CUDA(cudaEventRecord(ready, st));
         if (outPageable) {
@@ -2345,8 +2355,184 @@ int32_t astroz_cuda_propagate_numerical(const double *states, uint32_t n, double
     // give the slots back before returning (the default pool keeps nothing across a synchronisation)
     AZ_CUDA(dIn.release());
     AZ_CUDA(dOut.release());
+    AZ_CUDA(dTab.release());
     AZ_CUDA(cudaStreamSynchronize(st));
     return ASTROZ_OK;
+}
+}  // extern "C++"
+
+int32_t astroz_cuda_propagate_numerical(const double *states, uint32_t n, double t0, double duration, double dt,
+                                        double mu, int32_t forces, const double *j2, const double *r_eq,
+                                        const double *drag_cd, const double *drag_area, const double *drag_mass,
+                                        int32_t integrator, double rtol, double atol, int32_t device, double *out,
+                                        uint8_t *status, uint64_t *steps) {
+    az::StepTable table{};
+    int32_t rc = numerical_check(n, t0, duration, dt, mu, forces, j2, r_eq, drag_cd, drag_area, drag_mass, integrator,
+                                 rtol, atol, device, &table);
+    if (rc != ASTROZ_OK) return rc;
+    if (n == 0) return ASTROZ_OK;
+    if (!states || !out || !status) return ASTROZ_NULL_POINTER;
+    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
+    const bool drag = (forces & az::kForceDrag) != 0;
+    const double *cols[3] = {drag_cd, drag_area, drag_mass};
+    az::NumArgs a = numerical_args(n, table, mu, forces, j2, r_eq, rtol, atol);
+    return numerical_host_pipeline(
+        states, n, table, drag ? 3 : 0, cols, 0, nullptr, nullptr, device, out, status, steps,
+        [&](uint32_t m, const double *dStates, const double *const *dCols, const double *const *, double *dTraj,
+            uint8_t *dSt, uint64_t *dCounts, cudaStream_t s) {
+            a.n = m;
+            a.states = dStates;
+            a.cd = drag ? dCols[0] : nullptr;
+            a.area = drag ? dCols[1] : nullptr;
+            a.mass = drag ? dCols[2] : nullptr;
+            a.out = dTraj;
+            a.status = dSt;
+            a.counts = dCounts;
+            return az::launch_numerical(a, integrator, forces, s);
+        });
+}
+
+// ---- model lists (astroz_force_model_t) ----
+static_assert(sizeof(astroz_force_model_t) == sizeof(az::ForceModel), "astroz_force_model_t is az::ForceModel");
+static_assert(offsetof(astroz_force_model_t, pos) == offsetof(az::ForceModel, pos), "pos");
+static_assert(offsetof(astroz_force_model_t, c_per_state) == offsetof(az::ForceModel, c_arr), "c_per_state");
+static_assert(offsetof(astroz_force_model_t, pos_table) == offsetof(az::ForceModel, pos_table), "pos_table");
+static_assert(ASTROZ_MAX_MODELS == az::kMaxModels && ASTROZ_MODEL_THIRD_BODY + 1 == az::kModelKinds, "model kinds");
+static_assert(ASTROZ_MODEL_PER_STATE_C == az::kModelPerStateC && ASTROZ_MODEL_PER_STATE_AREA == az::kModelPerStateArea &&
+                  ASTROZ_MODEL_PER_STATE_MASS == az::kModelPerStateMass && ASTROZ_MODEL_POS_TABLE == az::kModelPosTable,
+              "model flags");
+
+// Checks of a model list, before anything is read, written or allocated, and the list as the kernel reads it: each
+// model's pointers kept only where its flags name them.
+static int32_t models_check(const astroz_force_model_t *models, uint32_t nModels, az::ModelList *list) {
+    auto bad = [](const char *why) {
+        g_lastError = why;
+        return ASTROZ_VALUE_ERROR;
+    };
+    if (nModels == 0 || nModels > az::kMaxModels) return bad("a model list has 1 to 16 models");
+    if (!models) return bad("models is NULL");
+    *list = az::ModelList{};
+    list->count = nModels;
+    constexpr uint32_t kPerState = az::kModelPerStateC | az::kModelPerStateArea | az::kModelPerStateMass;
+    for (uint32_t j = 0; j < nModels; ++j) {
+        const astroz_force_model_t &d = models[j];
+        az::ForceModel &m = list->m[j];
+        std::memcpy(&m, &d, sizeof m);
+        m.c_arr = m.area_arr = m.mass_arr = m.pos_table = nullptr;
+        // the scalar fields the kind reads, and the flags it accepts
+        double used[10];
+        int nUsed = 0;
+        auto use = [&](std::initializer_list<double> v) {
+            for (double x : v) used[nUsed++] = x;
+        };
+        uint32_t allowed = 0;
+        switch (d.kind) {
+            case az::kModelTwoBody: use({d.mu}); break;
+            case az::kModelJ2:
+            case az::kModelJ3:
+            case az::kModelJ4: use({d.mu, d.coef, d.r_eq}); break;
+            case az::kModelDrag: use({d.r_eq, d.rho0, d.scale_height, d.max_altitude}), allowed = kPerState; break;
+            case az::kModelImprovedDrag: use({d.r_eq, d.max_altitude, d.f107}), allowed = kPerState; break;
+            case az::kModelSrp: use({d.r_eq}), allowed = kPerState | az::kModelPosTable; break;
+            case az::kModelThirdBody: use({d.mu}), allowed = az::kModelPosTable; break;
+            default: return bad("unknown model kind");
+        }
+        if (d.flags & ~allowed) return bad("a model flag its kind does not take");
+        if (allowed & kPerState) {
+            const double *arr[3] = {d.c_per_state, d.area_per_state, d.mass_per_state};
+            const double sc[3] = {d.c, d.area, d.mass};
+            const double **dst[3] = {&m.c_arr, &m.area_arr, &m.mass_arr};
+            for (int q = 0; q < 3; ++q) {
+                if (d.flags & (az::kModelPerStateC << q)) {
+                    if (!arr[q]) return bad("a per-state flag is set and its array is NULL");
+                    *dst[q] = arr[q];
+                } else {
+                    use({sc[q]});
+                }
+            }
+        }
+        if (allowed & az::kModelPosTable) {
+            if (d.flags & az::kModelPosTable) {
+                if (!d.pos_table) return bad("ASTROZ_MODEL_POS_TABLE is set and pos_table is NULL");
+                m.pos_table = d.pos_table;
+            } else {
+                use({d.pos[0], d.pos[1], d.pos[2]});
+            }
+        }
+        for (int q = 0; q < nUsed; ++q)
+            if (!std::isfinite(used[q])) return bad("a model's scalar parameter is not finite");
+    }
+    return ASTROZ_OK;
+}
+
+int32_t astroz_cuda_propagate_numerical_models_device(const double *d_states, uint32_t n, double t0, double duration,
+                                                      double dt, const astroz_force_model_t *models, uint32_t n_models,
+                                                      int32_t integrator, double rtol, double atol, int32_t device,
+                                                      double *d_out, uint8_t *d_status, uint64_t *d_steps,
+                                                      void *stream) {
+    az::StepTable table{};
+    az::ModelArgs ma{};
+    int32_t rc = models_check(models, n_models, &ma.models);
+    if (rc != ASTROZ_OK) return rc;
+    rc = numerical_check(n, t0, duration, dt, 0.0, 0, nullptr, nullptr, nullptr, nullptr, nullptr, integrator, rtol,
+                         atol, device, &table);
+    if (rc != ASTROZ_OK) return rc;
+    if (n == 0) return ASTROZ_OK;
+    if (!d_states || !d_out || !d_status) return ASTROZ_NULL_POINTER;
+    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
+    AZ_CUDA(cudaSetDevice(device));
+    ma.a = numerical_args(n, table, 0.0, 0, nullptr, nullptr, rtol, atol);
+    ma.a.states = d_states;
+    ma.a.out = d_out;
+    ma.a.status = d_status;
+    ma.a.counts = d_steps;
+    // the step table and the model list travel in the launch's parameters: the call only queues the kernel
+    AZ_CUDA(az::launch_numerical_models(ma, integrator, static_cast<cudaStream_t>(stream)));
+    return ASTROZ_OK;
+}
+
+int32_t astroz_cuda_propagate_numerical_models(const double *states, uint32_t n, double t0, double duration, double dt,
+                                               const astroz_force_model_t *models, uint32_t n_models,
+                                               int32_t integrator, double rtol, double atol, int32_t device,
+                                               double *out, uint8_t *status, uint64_t *steps) {
+    az::StepTable table{};
+    az::ModelArgs ma{};
+    int32_t rc = models_check(models, n_models, &ma.models);
+    if (rc != ASTROZ_OK) return rc;
+    rc = numerical_check(n, t0, duration, dt, 0.0, 0, nullptr, nullptr, nullptr, nullptr, nullptr, integrator, rtol,
+                         atol, device, &table);
+    if (rc != ASTROZ_OK) return rc;
+    if (n == 0) return ASTROZ_OK;
+    if (!states || !out || !status) return ASTROZ_NULL_POINTER;
+    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
+    // per-state columns in list order, and the position tables ([K][3] each)
+    const double *cols[kNumMaxCols];
+    const double **colOf[kNumMaxCols];
+    const double *tabs[kNumMaxTabs];
+    const double **tabOf[kNumMaxTabs];
+    size_t tabBytes[kNumMaxTabs];
+    int nCols = 0, nTabs = 0;
+    const size_t K = (size_t)table.nFull + table.nTail;
+    for (uint32_t j = 0; j < n_models; ++j) {
+        az::ForceModel &m = ma.models.m[j];
+        for (const double **p : {&m.c_arr, &m.area_arr, &m.mass_arr})
+            if (*p) cols[nCols] = *p, colOf[nCols++] = p;
+        if (m.pos_table) tabs[nTabs] = m.pos_table, tabOf[nTabs] = &m.pos_table, tabBytes[nTabs++] = K * 24;
+    }
+    ma.a = numerical_args(n, table, 0.0, 0, nullptr, nullptr, rtol, atol);
+    return numerical_host_pipeline(
+        states, n, table, nCols, cols, nTabs, tabs, tabBytes, device, out, status, steps,
+        [&](uint32_t m, const double *dStates, const double *const *dCols, const double *const *dTabs, double *dTraj,
+            uint8_t *dSt, uint64_t *dCounts, cudaStream_t s) {
+            for (int q = 0; q < nCols; ++q) *colOf[q] = dCols[q];
+            for (int t = 0; t < nTabs; ++t) *tabOf[t] = dTabs[t];
+            ma.a.n = m;
+            ma.a.states = dStates;
+            ma.a.out = dTraj;
+            ma.a.status = dSt;
+            ma.a.counts = dCounts;
+            return az::launch_numerical_models(ma, integrator, s);
+        });
 }
 
 int32_t astroz_cuda_fp64_peak(int32_t device, double *tflops) {

@@ -43,7 +43,41 @@ cudaError_t launch_forces(const NumArgs &a, int forces, dim3 grid, cudaStream_t 
     return cudaGetLastError();
 }
 
+// The model-list specialisations: the integrator is a template parameter, the list a __grid_constant__ launch parameter
+// the same for every thread, so each branch on a model's kind is warp-uniform and the list is read in place.
+template <int kInt>
+__global__ void __launch_bounds__(kNumThreads) numerical_models_kernel(const __grid_constant__ ModelArgs m) {
+    const NumArgs &a = m.a;
+    const uint32_t i = blockIdx.x * kNumThreads + threadIdx.x;
+    if (i >= a.n) return;
+    double y0[6];
+#pragma unroll
+    for (int c = 0; c < 6; ++c) y0[c] = a.states[(size_t)i * 6 + c];
+    uint64_t counts[2];
+    const size_t samples = (size_t)a.steps.nFull + a.steps.nTail + 1;
+    const uint8_t st = propagate_state_models<kInt>(y0, m.models, i, a.p, a.steps, a.out + (size_t)i * samples * 6,
+                                                    counts);
+    a.status[i] = st;
+    if (a.counts) {
+        a.counts[(size_t)i * 2] = counts[0];
+        a.counts[(size_t)i * 2 + 1] = counts[1];
+    }
+}
+
 }  // namespace
+
+cudaError_t launch_numerical_models(const ModelArgs &m, int integrator, cudaStream_t s) {
+    if (m.a.n == 0) return cudaSuccess;
+    const dim3 grid((m.a.n + kNumThreads - 1) / kNumThreads);
+    if (integrator == kIntRk4) {
+        numerical_models_kernel<kIntRk4><<<grid, kNumThreads, 0, s>>>(m);
+    } else if (integrator == kIntDp87) {
+        numerical_models_kernel<kIntDp87><<<grid, kNumThreads, 0, s>>>(m);
+    } else {
+        return cudaErrorInvalidValue;
+    }
+    return cudaGetLastError();
+}
 
 cudaError_t launch_numerical(const NumArgs &a, int integrator, int forces, cudaStream_t s) {
     if (a.n == 0) return cudaSuccess;

@@ -141,11 +141,22 @@ AZ_HD void accel(const double s[6], const NumParams &p, const DragBody &d, doubl
     }
 }
 
-// derivative of Integrator.zig:47-50 / :261-264: (velocity, acceleration)
+// The integrators below take the force as a policy F: f(s, acc) writes the acceleration at state s, and
+// f.interval(k) is called before output interval k is integrated.  FixedForces is the binding's force list of the
+// eight fixed specialisations; ListForces (further down) is a caller's ordered model list.
 template <int kForces>
-AZ_HD void deriv(const double s[6], const NumParams &p, const DragBody &d, double k[6]) {
+struct FixedForces {
+    const NumParams &p;
+    const DragBody &d;
+    AZ_HD void operator()(const double s[6], double acc[3]) const { accel<kForces>(s, p, d, acc); }
+    AZ_HD void interval(uint32_t) {}
+};
+
+// derivative of Integrator.zig:47-50 / :261-264: (velocity, acceleration)
+template <class F>
+AZ_HD void deriv(const double s[6], const F &f, double k[6]) {
     double a[3];
-    accel<kForces>(s, p, d, a);
+    f(s, a);
     k[0] = s[3];
     k[1] = s[4];
     k[2] = s[5];
@@ -155,20 +166,20 @@ AZ_HD void deriv(const double s[6], const NumParams &p, const DragBody &d, doubl
 }
 
 // Rk4.step (Integrator.zig:28-45); y is replaced by the state after dt
-template <int kForces>
-AZ_HD void rk4_step(double y[6], double dt, const NumParams &p, const DragBody &d) {
+template <class F>
+AZ_HD void rk4_step(double y[6], double dt, const F &f) {
     double k1[6], k2[6], k3[6], k4[6], s[6];
     const double half = 0.5 * dt;
-    deriv<kForces>(y, p, d, k1);
+    deriv(y, f, k1);
 #pragma unroll
     for (int c = 0; c < 6; ++c) s[c] = y[c] + k1[c] * half;
-    deriv<kForces>(s, p, d, k2);
+    deriv(s, f, k2);
 #pragma unroll
     for (int c = 0; c < 6; ++c) s[c] = y[c] + k2[c] * half;
-    deriv<kForces>(s, p, d, k3);
+    deriv(s, f, k3);
 #pragma unroll
     for (int c = 0; c < 6; ++c) s[c] = y[c] + k3[c] * dt;
-    deriv<kForces>(s, p, d, k4);
+    deriv(s, f, k4);
     const double factor = dt / 6.0;
 #pragma unroll
     for (int c = 0; c < 6; ++c) y[c] = y[c] + factor * (k1[c] + 2.0 * k2[c] + 2.0 * k3[c] + k4[c]);
@@ -178,8 +189,8 @@ AZ_HD void rk4_step(double y[6], double dt, const NumParams &p, const DragBody &
 // solution, the return value is errNorm.  The 8th- and 7th-order sums are accumulated as each stage is formed; that is
 // the reference's order of additions (stage by stage, zero weights skipped), so only stages still read by later rows
 // stay live.
-template <int kForces>
-AZ_HD double dp87_attempt(const double y[6], double h, const NumParams &p, const DragBody &d, double y8[6]) {
+template <class F>
+AZ_HD double dp87_attempt(const double y[6], double h, const F &f, const NumParams &p, double y8[6]) {
     double k[13][6];
     double y7[6];
 #pragma unroll
@@ -197,7 +208,7 @@ AZ_HD double dp87_attempt(const double y[6], double h, const NumParams &p, const
                 for (int c = 0; c < 6; ++c) ys[c] = ys[c] + ah * k[j][c];
             }
         }
-        deriv<kForces>(ys, p, d, k[i]);
+        deriv(ys, f, k[i]);
         if (dp87_b8_nz(i)) {
             const double bh = AZ_DP87(b8[i]) * h;
 #pragma unroll
@@ -238,8 +249,8 @@ AZ_HD double dp87_next_h(double h, double errNorm) {
 // interval.  Returns kNumOk, kNumSubstepLimit (10,000 accepted substeps and the interval not finished: y is where the
 // reference leaves it) or kNumStopped: an attempt rejected at h == hMin, which the reference retries with the same y
 // and h forever (this is also where a non-finite errNorm ends).  counts[0] / counts[1] add accepted / rejected attempts.
-template <int kForces>
-AZ_HD uint8_t dp87_interval(double y[6], double &hCur, double dt, const NumParams &p, const DragBody &d,
+template <class F>
+AZ_HD uint8_t dp87_interval(double y[6], double &hCur, double dt, const F &f, const NumParams &p,
                             uint64_t counts[2]) {
     double remaining = dt;
     uint32_t substeps = 0;
@@ -248,7 +259,7 @@ AZ_HD uint8_t dp87_interval(double y[6], double &hCur, double dt, const NumParam
         h = fmin(h, remaining);
         h = fmax(h, kDpHMin);
         double y8[6];
-        const double errNorm = dp87_attempt<kForces>(y, h, p, d, y8);
+        const double errNorm = dp87_attempt(y, h, f, p, y8);
         const double hNew = dp87_next_h(h, errNorm);
         if (errNorm <= 1.0) {
 #pragma unroll
@@ -299,10 +310,10 @@ inline bool step_table_push(StepTable &t, double step) {
 // One state's trajectory (Propagator.propagate, src/propagators/Propagator.zig:22-48): y0 at out[0..6), then the state
 // after each of the K intervals of `steps` (the sampling loop's step sizes, built once on the host) at out[6 (k + 1)).
 // A stopped state's later samples are zero-filled.  Returns the status byte; counts[2] receives accepted / rejected
-// steps (RK4: one accepted step per interval).
-template <int kInt, int kForces>
-AZ_HD uint8_t propagate_state(const double y0[6], const DragBody &d, const NumParams &p, const StepTable &steps,
-                              double *out, uint64_t counts[2]) {
+// steps (RK4: one accepted step per interval).  f is the force policy; f.interval(k) runs before interval k.
+template <int kInt, class F>
+AZ_HD uint8_t propagate_with(const double y0[6], F &f, const NumParams &p, const StepTable &steps, double *out,
+                             uint64_t counts[2]) {
     const uint32_t K = steps.nFull + steps.nTail;
     double y[6];
 #pragma unroll
@@ -312,12 +323,13 @@ AZ_HD uint8_t propagate_state(const double y0[6], const DragBody &d, const NumPa
     double hCur = kDpHStart;
     for (uint32_t k = 0; k < K; ++k) {
         const double dt = steps.step(k);
+        f.interval(k);
         if (kInt == kIntRk4) {
-            rk4_step<kForces>(y, dt, p, d);
+            rk4_step(y, dt, f);
             ++counts[0];
             if (status == kNumOk && !all_finite(y)) status = kNumNonFinite;
         } else {
-            const uint8_t st = dp87_interval<kForces>(y, hCur, dt, p, d, counts);
+            const uint8_t st = dp87_interval(y, hCur, dt, f, p, counts);
             if (st == kNumStopped) {
                 for (size_t w = (size_t)(k + 1) * 6; w < (size_t)(K + 1) * 6; ++w) out[w] = 0.0;
                 return kNumStopped;
@@ -329,6 +341,220 @@ AZ_HD uint8_t propagate_state(const double y0[6], const DragBody &d, const NumPa
         for (int c = 0; c < 6; ++c) o[c] = y[c];
     }
     return status;
+}
+
+// The fixed force sets of the eight K7 kernels
+template <int kInt, int kForces>
+AZ_HD uint8_t propagate_state(const double y0[6], const DragBody &d, const NumParams &p, const StepTable &steps,
+                              double *out, uint64_t counts[2]) {
+    FixedForces<kForces> f{p, d};
+    return propagate_with<kInt>(y0, f, p, steps, out, counts);
+}
+
+// ---- model lists: the force models of the reference's propagators module (src/propagators/ForceModel.zig) ----------
+// kinds (ASTROZ_MODEL_*) and descriptor flags (ASTROZ_MODEL_PER_STATE_*, ASTROZ_MODEL_POS_TABLE)
+constexpr int32_t kModelTwoBody = 0, kModelJ2 = 1, kModelJ3 = 2, kModelJ4 = 3, kModelDrag = 4, kModelImprovedDrag = 5,
+                  kModelSrp = 6, kModelThirdBody = 7, kModelKinds = 8;
+constexpr uint32_t kModelPerStateC = 1, kModelPerStateArea = 2, kModelPerStateMass = 4, kModelPosTable = 8;
+constexpr uint32_t kMaxModels = 16;
+// SolarRadiationPressure: pressure at 1 AU [N/m^2] and the AU [km] (src/constants.zig:27-28); ImprovedDrag: the
+// atmosphere's rotation rate [rad/s] (ForceModel.zig:292)
+constexpr double kSrpPressure = 4.56e-6, kAuKm = 1.495978707e8, kEarthOmega = 7.2921150e-5;
+
+// One model of a list, the layout of astroz_force_model_t.  c is cd (Drag, ImprovedDrag) or cr (SRP); c_arr / area_arr /
+// mass_arr, when set, replace the scalar by one value per state; pos is SRP's sunPos or ThirdBody's pos, and pos_table,
+// when set, replaces it by one row per output interval ([K][3]).
+struct ForceModel {
+    int32_t kind;
+    uint32_t flags;
+    double mu, coef, r_eq;
+    double rho0, scale_height, max_altitude, f107;
+    double c, area, mass;
+    double pos[3];
+    const double *c_arr, *area_arr, *mass_arr;
+    const double *pos_table;
+};
+struct ModelList {
+    uint32_t count;  // 1..kMaxModels
+    ForceModel m[kMaxModels];
+};
+
+AZ_HD double per_state(const double *arr, double scalar, uint32_t i) { return arr ? arr[i] : scalar; }
+
+// ImprovedDrag.getDensity (ForceModel.zig:283-320): the last of the five layers with altitude >= baseAlt (the first
+// below 200 km), exponential decay from its base, scaled by f107 / 150
+AZ_HD double improved_density(double altitude, double f107) {
+    double base = 100.0, rho = 5.297e-7, H = 5.877;
+    if (altitude >= 200.0) base = 200.0, rho = 2.789e-10, H = 37.105;
+    if (altitude >= 400.0) base = 400.0, rho = 3.725e-12, H = 62.822;
+    if (altitude >= 600.0) base = 600.0, rho = 2.418e-13, H = 79.864;
+    if (altitude >= 1000.0) base = 1000.0, rho = 3.561e-15, H = 200.0;
+    const double deltaH = altitude - base;
+    double r = rho * exp(-deltaH / H);
+    const double f107Scale = f107 / 150.0;
+    r *= f107Scale;
+    return r;
+}
+
+// One model's acceleration at state s of batch item i during output interval k, line for line as the reference's
+// acceleration() of that kind; a guard that returns zeros there writes zeros here.
+AZ_HD void model_accel(const ForceModel &m, const double s[6], uint32_t i, uint32_t k, double a[3]) {
+    const double x = s[0], y = s[1], z = s[2];
+    a[0] = a[1] = a[2] = 0.0;
+    switch (m.kind) {
+        case kModelTwoBody: {  // :49-55
+            const double r = sqrt(x * x + y * y + z * z);
+            const double factor = -m.mu / (r * r * r);
+            a[0] = factor * x, a[1] = factor * y, a[2] = factor * z;
+            break;
+        }
+        case kModelJ2: {  // :67-79
+            const double r2 = x * x + y * y + z * z;
+            const double r = sqrt(r2);
+            const double factor = -1.5 * m.coef * m.mu * m.r_eq * m.r_eq / (r2 * r2 * r);
+            const double z2R2 = (z * z) / r2;
+            a[0] = factor * x * (5.0 * z2R2 - 1.0);
+            a[1] = factor * y * (5.0 * z2R2 - 1.0);
+            a[2] = factor * z * (5.0 * z2R2 - 3.0);
+            break;
+        }
+        case kModelJ3: {  // :122-142; the x / y coefficient carries a 1/r its z term does not (kept)
+            const double r2 = x * x + y * y + z * z;
+            const double r = sqrt(r2);
+            const double rEq3 = m.r_eq * m.r_eq * m.r_eq;
+            const double factor = 2.5 * m.coef * m.mu * rEq3 / (r2 * r2 * r2 * r);
+            const double z2R2 = (z * z) / r2;
+            const double xyCoeff = 3.0 * z / r - 7.0 * z * z2R2 / r;
+            const double zCoeff = 6.0 * z * z - 7.0 * z * z * z2R2 - 0.6 * r2;
+            a[0] = factor * x * xyCoeff, a[1] = factor * y * xyCoeff, a[2] = factor * zCoeff;
+            break;
+        }
+        case kModelJ4: {  // :154-175; divides by r^9 (kept)
+            const double r2 = x * x + y * y + z * z;
+            const double r = sqrt(r2);
+            const double r4 = r2 * r2;
+            const double z2 = z * z;
+            const double z4 = z2 * z2;
+            const double z2R2 = z2 / r2;
+            const double z4R4 = z4 / r4;
+            const double rEq4 = m.r_eq * m.r_eq * m.r_eq * m.r_eq;
+            const double factor = 1.875 * m.coef * m.mu * rEq4 / (r4 * r4 * r);
+            const double xyTerm = 3.0 - 42.0 * z2R2 + 63.0 * z4R4;
+            const double zTerm = 15.0 - 70.0 * z2R2 + 63.0 * z4R4;
+            a[0] = factor * x * xyTerm, a[1] = factor * y * xyTerm, a[2] = factor * z * zTerm;
+            break;
+        }
+        case kModelDrag: {  // :95-110
+            const double vx = s[3], vy = s[4], vz = s[5];
+            const double r = sqrt(x * x + y * y + z * z);
+            const double altitude = r - m.r_eq;
+            if (altitude > m.max_altitude) break;
+            const double v = sqrt(vx * vx + vy * vy + vz * vz);
+            if (v < 1e-10) break;
+            const double rho = m.rho0 * exp(-altitude / m.scale_height);
+            const double factor = -0.5 * per_state(m.c_arr, m.c, i) * per_state(m.area_arr, m.area, i) * rho * v * 1e3 /
+                                  per_state(m.mass_arr, m.mass, i);
+            a[0] = factor * vx / v, a[1] = factor * vy / v, a[2] = factor * vz / v;
+            break;
+        }
+        case kModelImprovedDrag: {  // :322-348; zero below 100 km (kept)
+            const double vx = s[3], vy = s[4], vz = s[5];
+            const double r = sqrt(x * x + y * y + z * z);
+            const double altitude = r - m.r_eq;
+            if (altitude > m.max_altitude || altitude < 100.0) break;
+            const double vrelX = vx + kEarthOmega * y;
+            const double vrelY = vy - kEarthOmega * x;
+            const double vrelZ = vz;
+            const double vrel = sqrt(vrelX * vrelX + vrelY * vrelY + vrelZ * vrelZ);
+            if (vrel < 1e-10) break;
+            const double rho = improved_density(altitude, m.f107);
+            const double factor = -0.5 * per_state(m.c_arr, m.c, i) * per_state(m.area_arr, m.area, i) * rho * vrel *
+                                  1e3 / per_state(m.mass_arr, m.mass, i);
+            a[0] = factor * vrelX / vrel, a[1] = factor * vrelY / vrel, a[2] = factor * vrelZ / vrel;
+            break;
+        }
+        case kModelSrp: {  // :197-227
+            double sx, sy, sz;
+            if (m.pos_table) {
+                const double *q = m.pos_table + (size_t)k * 3;
+                sx = q[0], sy = q[1], sz = q[2];
+            } else {
+                sx = m.pos[0], sy = m.pos[1], sz = m.pos[2];
+            }
+            const double dx = sx - x, dy = sy - y, dz = sz - z;
+            const double dist = sqrt(dx * dx + dy * dy + dz * dz);
+            if (dist < 1e-10) break;
+            const double sunDirX = dx / dist, sunDirY = dy / dist, sunDirZ = dz / dist;
+            const double sunDist = sqrt(sx * sx + sy * sy + sz * sz);
+            if (sunDist < 1e-10) break;
+            const double hx = sx / sunDist, hy = sy / sunDist, hz = sz / sunDist;
+            const double proj = x * hx + y * hy + z * hz;
+            if (proj < 0) {
+                const double perpX = x - proj * hx, perpY = y - proj * hy, perpZ = z - proj * hz;
+                const double rho = sqrt(perpX * perpX + perpY * perpY + perpZ * perpZ);
+                if (rho < m.r_eq) break;
+            }
+            const double scale = (kAuKm / dist) * (kAuKm / dist);
+            const double factor = -per_state(m.c_arr, m.c, i) * kSrpPressure * scale * per_state(m.area_arr, m.area, i) /
+                                  per_state(m.mass_arr, m.mass, i) * 1e-3;
+            a[0] = factor * sunDirX, a[1] = factor * sunDirY, a[2] = factor * sunDirZ;
+            break;
+        }
+        case kModelThirdBody: {  // :244-265
+            double qx, qy, qz;
+            if (m.pos_table) {
+                const double *q = m.pos_table + (size_t)k * 3;
+                qx = q[0], qy = q[1], qz = q[2];
+            } else {
+                qx = m.pos[0], qy = m.pos[1], qz = m.pos[2];
+            }
+            const double qMag = sqrt(qx * qx + qy * qy + qz * qz);
+            if (qMag < 1e-10) break;
+            const double qMag3 = qMag * qMag * qMag;
+            const double dx = qx - x, dy = qy - y, dz = qz - z;
+            const double dMag = sqrt(dx * dx + dy * dy + dz * dz);
+            if (dMag < 1e-10) break;
+            const double dMag3 = dMag * dMag * dMag;
+            a[0] = m.mu * (dx / dMag3 - qx / qMag3);
+            a[1] = m.mu * (dy / dMag3 - qy / qMag3);
+            a[2] = m.mu * (dz / dMag3 - qz / qMag3);
+            break;
+        }
+        default: break;
+    }
+}
+
+// A caller's model list for batch item i: one model's acceleration as it is (the binding's rule,
+// bindings/python/src/propagator.zig:138-146), several summed by Composite (ForceModel.zig:365-374) into a total that
+// starts at zero, in list order.  L stays where the launch put it (a __grid_constant__ parameter on the device), and the
+// list is walked by a loop that is not unrolled, so neither it nor a per-model array is copied into local memory.
+struct ListForces {
+    const ModelList &L;
+    uint32_t i;      // batch item: its per-state coefficients
+    uint32_t k = 0;  // output interval: its row of every position table
+    AZ_HD void interval(uint32_t kk) { k = kk; }
+    AZ_HD void operator()(const double s[6], double acc[3]) const {
+        if (L.count == 1) {
+            model_accel(L.m[0], s, i, k, acc);
+            return;
+        }
+        acc[0] = acc[1] = acc[2] = 0.0;
+#pragma unroll 1
+        for (uint32_t j = 0; j < L.count; ++j) {
+            double a[3];
+            model_accel(L.m[j], s, i, k, a);
+            acc[0] += a[0];
+            acc[1] += a[1];
+            acc[2] += a[2];
+        }
+    }
+};
+
+template <int kInt>
+AZ_HD uint8_t propagate_state_models(const double y0[6], const ModelList &L, uint32_t i, const NumParams &p,
+                                     const StepTable &steps, double *out, uint64_t counts[2]) {
+    ListForces f{L, i};
+    return propagate_with<kInt>(y0, f, p, steps, out, counts);
 }
 
 }  // namespace az
@@ -347,5 +573,12 @@ struct NumArgs {
 };
 // Queue K7 for `integrator` / `forces` on s.
 cudaError_t launch_numerical(const NumArgs &a, int integrator, int forces, cudaStream_t s);
+// K7 with a model list: a.cd / a.area / a.mass are unused (per-state coefficients come with the models); the list's
+// pointers are device pointers.  The list travels in the launch's parameters.
+struct ModelArgs {
+    NumArgs a;
+    ModelList models;
+};
+cudaError_t launch_numerical_models(const ModelArgs &a, int integrator, cudaStream_t s);
 }  // namespace az
 #endif

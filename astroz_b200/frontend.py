@@ -197,6 +197,10 @@ def screen(source, times, threshold=10.0, *, target=None, start_time=None, norad
 EARTH_MU = 398600.5
 EARTH_R_EQ = 6378.137
 EARTH_J2 = 0.00108262998905
+# gravitational parameters of the Sun and the Moon [km^3/s^2] (src/constants.zig:97, :170), the values the reference
+# exports as SUN_MU / MOON_MU (bindings/python/src/main.zig:73-74): the mu of a ThirdBody model (astroz_b200.numerical)
+SUN_MU = 1.32712e11
+MOON_MU = 4902.80
 
 
 def propagate_numerical(state, t0, duration, dt, mu, j2=None, r_eq=None, drag_cd=None, drag_area=None, drag_mass=None,
@@ -236,4 +240,4 @@ def propagate_numerical(state, t0, duration, dt, mu, j2=None, r_eq=None, drag_cd
 
 
 __all__ = ["Constellation", "propagate", "screen", "parse_tle_pairs", "omm_to_tle_pairs", "propagate_numerical",
-           "EARTH_MU", "EARTH_R_EQ", "EARTH_J2"]
+           "EARTH_MU", "EARTH_R_EQ", "EARTH_J2", "SUN_MU", "MOON_MU"]

@@ -117,5 +117,223 @@ def propagate_numerical_batch_device(states, t0, duration, dt, mu, out, status, 
         ptr(status), ptr(steps), C.c_void_p(stream) if stream else None))
 
 
+# ---- model lists: the force models of the reference's propagators module (src/propagators/ForceModel.zig) -------------
+# kinds and flags of astroz_force_model_t (ASTROZ_MODEL_*)
+_TWO_BODY, _J2, _J3, _J4, _DRAG, _IMPROVED_DRAG, _SRP, _THIRD_BODY = range(8)
+_PER_STATE = {"c": 1, "area": 2, "mass": 4}
+_POS_TABLE = 8
+MAX_MODELS = 16
+AU_KM = 1.495978707e8   # src/constants.zig:28, SolarRadiationPressure's default Sun distance
+
+
+class _ForceModelC(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("flags", C.c_uint32)] + \
+               [(f, C.c_double) for f in ("mu", "coef", "r_eq", "rho0", "scale_height", "max_altitude", "f107", "c",
+                                          "area", "mass")] + \
+               [("pos", C.c_double * 3), ("c_per_state", C.c_void_p), ("area_per_state", C.c_void_p),
+                ("mass_per_state", C.c_void_p), ("pos_table", C.c_void_p)]
+
+
+class _Model:
+    """A force model of a list: its scalar fields, its coefficients that may vary per state (c, area, mass: a scalar or
+    one value per state) and its position (a fixed 3-vector or one row per output interval)."""
+    kind = -1
+
+    def __init__(self, scalars, coefs=None, pos=None):
+        self._scalars, self._coefs, self._pos = scalars, coefs or {}, pos
+
+    def __repr__(self):
+        fields = {**self._scalars, **self._coefs, **({} if self._pos is None else {"pos": self._pos})}
+        return f"{type(self).__name__}({', '.join(f'{k}={v!r}' for k, v in fields.items())})"
+
+
+class TwoBody(_Model):
+    """TwoBody(mu): ForceModel.zig:42-56"""
+    kind = _TWO_BODY
+
+    def __init__(self, mu):
+        super().__init__({"mu": float(mu)})
+
+
+class _Zonal(_Model):
+    def __init__(self, mu, coef, r_eq):
+        super().__init__({"mu": float(mu), "coef": float(coef), "r_eq": float(r_eq)})
+
+
+class J2(_Zonal):
+    """J2(mu, j2, r_eq): ForceModel.zig:58-80"""
+    kind = _J2
+
+
+class J3(_Zonal):
+    """J3(mu, j3, r_eq): ForceModel.zig:113-143.  Its x / y terms carry an extra 1/r, as the reference's do."""
+    kind = _J3
+
+
+class J4(_Zonal):
+    """J4(mu, j4, r_eq): ForceModel.zig:145-176.  Divides by r^9, as the reference does."""
+    kind = _J4
+
+
+class Drag(_Model):
+    """Drag(r_eq, rho0, H, cd, area, mass, max_altitude): exponential atmosphere, ForceModel.zig:82-111.  cd, area [m^2]
+    and mass [kg] are scalars or one value per state."""
+    kind = _DRAG
+
+    def __init__(self, r_eq, rho0, H, cd, area, mass, max_altitude):
+        super().__init__({"r_eq": float(r_eq), "rho0": float(rho0), "scale_height": float(H),
+                          "max_altitude": float(max_altitude)}, {"c": cd, "area": area, "mass": mass})
+
+
+class ImprovedDrag(_Model):
+    """ImprovedDrag(r_eq, cd, area, mass, max_altitude, f107): five-layer atmosphere rotating with the Earth, scaled by
+    F10.7, ForceModel.zig:268-349.  Zero below 100 km, as the reference.  cd, area [m^2] and mass [kg] are scalars or one
+    value per state."""
+    kind = _IMPROVED_DRAG
+
+    def __init__(self, r_eq, cd, area, mass, max_altitude, f107):
+        super().__init__({"r_eq": float(r_eq), "max_altitude": float(max_altitude), "f107": float(f107)},
+                         {"c": cd, "area": area, "mass": mass})
+
+
+class SolarRadiationPressure(_Model):
+    """SolarRadiationPressure(cr, area, mass, r_eq, sun_pos=None): ForceModel.zig:178-228, with a cylindrical shadow of
+    radius r_eq.  cr, area [m^2] and mass [kg] are scalars or one value per state.  sun_pos [km] is a 3-vector (default
+    (AU, 0, 0), as init sets it) or a (K, 3) table whose row k holds for output interval k (K = samples - 1)."""
+    kind = _SRP
+
+    def __init__(self, cr, area, mass, r_eq, sun_pos=None):
+        super().__init__({"r_eq": float(r_eq)}, {"c": cr, "area": area, "mass": mass},
+                         (AU_KM, 0.0, 0.0) if sun_pos is None else sun_pos)
+
+
+class ThirdBody(_Model):
+    """ThirdBody(mu, pos): Battin's formula, ForceModel.zig:230-266.  pos [km] is a 3-vector or a (K, 3) table whose row
+    k holds for output interval k (K = samples - 1)."""
+    kind = _THIRD_BODY
+
+    def __init__(self, mu, pos):
+        super().__init__({"mu": float(mu)}, pos=pos)
+
+
+def _descriptors(models, n, K, array):
+    """The astroz_force_model_t array of `models`.  array(x, shape, name) returns (pointer, keep-alive) for a per-state
+    array or a position table, or None when x is a scalar / a fixed 3-vector."""
+    models = list(models)
+    if not models or not all(isinstance(m, _Model) for m in models):
+        raise ValueError("models must be a non-empty list of TwoBody / J2 / J3 / J4 / Drag / ImprovedDrag / "
+                         "SolarRadiationPressure / ThirdBody")
+    if len(models) > MAX_MODELS:
+        raise ValueError(f"at most {MAX_MODELS} models")
+    descs = (_ForceModelC * len(models))()
+    keep = []
+    for d, m in zip(descs, models):
+        d.kind = m.kind
+        for k, v in m._scalars.items():
+            setattr(d, k, v)
+        for k, v in m._coefs.items():
+            a = array(v, (n,), k)
+            if a is None:
+                setattr(d, k, float(v))
+            else:
+                d.flags |= _PER_STATE[k]
+                setattr(d, k + "_per_state", a[0])
+                keep.append(a[1])
+        if m._pos is not None:
+            a = array(m._pos, (K, 3), "pos")
+            if a is None:
+                d.pos[:] = [float(x) for x in m._pos]
+            else:
+                d.flags |= _POS_TABLE
+                d.pos_table = a[0]
+                keep.append(a[1])
+    return descs, keep
+
+
+def _host_array(x, shape, name):
+    a = np.asarray(x, dtype=np.float64)
+    if a.ndim == 0 or (name == "pos" and a.ndim == 1):
+        if name == "pos" and a.shape != (3,):
+            raise ValueError("a position is a 3-vector or a (K, 3) table")
+        return None
+    if a.shape != shape:
+        raise ValueError(f"{name} must be a scalar{' or 3-vector' if name == 'pos' else ''} or have shape {shape}")
+    a = np.ascontiguousarray(a)
+    return C.c_void_p(a.ctypes.data), a
+
+
+def propagate_models_batch(states, t0, duration, dt, models, *, integrator="dp87", rtol=1e-9, atol=1e-12, device=0,
+                           out=None):
+    """Integrate n initial states over the shared sample times under an ordered list of force models (at most 16):
+    one model is used as it is, several are summed as the reference's Composite sums them, in list order.
+
+    states: (n, 6).  models: TwoBody / J2 / J3 / J4 / Drag / ImprovedDrag / SolarRadiationPressure / ThirdBody, whose
+    coefficients may be (n,) arrays and whose positions may be (K, 3) tables, K = samples - 1.
+    Returns (times[samples], traj[n, samples, 6], status[n] uint8, steps[n, 2] uint64 accepted / rejected), as
+    propagate_numerical_batch does."""
+    states = np.ascontiguousarray(states, dtype=np.float64)
+    if states.ndim != 2 or states.shape[1] != 6:
+        raise ValueError("states must have shape (n, 6)")
+    n = states.shape[0]
+    times = numerical_times(t0, duration, dt)
+    descs, keep = _descriptors(models, n, len(times) - 1, _host_array)
+    shape = (n, len(times), 6)
+    if out is None:
+        out = np.empty(shape)
+    elif out.shape != shape or out.dtype != np.float64 or not out.flags.c_contiguous:
+        raise ValueError(f"out must be a C-contiguous float64 array of shape {shape}")
+    status = np.zeros(n, dtype=np.uint8)
+    steps = np.zeros((n, 2), dtype=np.uint64)
+    vp = lambda a: C.c_void_p(a.ctypes.data)  # noqa: E731
+    check(lib().astroz_cuda_propagate_numerical_models(
+        vp(states), n, float(t0), float(duration), float(dt), C.cast(descs, C.c_void_p), len(descs),
+        _integrator(integrator), float(rtol), float(atol), int(device), vp(out), vp(status), vp(steps)))
+    del keep
+    return times, out, status, steps
+
+
+def propagate_models_batch_device(states, t0, duration, dt, models, out, status, steps=None, *, integrator="dp87",
+                                  rtol=1e-9, atol=1e-12, stream: int = 0) -> None:
+    """`propagate_models_batch` with torch CUDA tensors on one device: states (n, 6) float64; per-state coefficients as
+    (n,) float64 tensors and position tables as (K, 3) float64 tensors on the same device (scalars and fixed 3-vectors
+    as Python numbers); out (n, samples, 6) float64, status (n,) uint8 and steps (n, 2) int64 (optional) receive the
+    results.  Asynchronous on `stream` (a raw cudaStream_t value, 0 = the default stream)."""
+    import torch
+
+    n = int(states.shape[0]) if states.dim() == 2 else -1
+    if n < 0 or states.shape[1] != 6 or states.dtype != torch.float64 or not states.is_cuda:
+        raise ValueError("states must be a CUDA float64 tensor of shape (n, 6)")
+    samples = len(numerical_times(t0, duration, dt))
+
+    def tensor_or_none(x, shape, name):
+        if not isinstance(x, torch.Tensor):
+            return _host_array(x, shape, name)   # a scalar or a fixed 3-vector; a host array is refused below
+        if x.dtype != torch.float64 or not x.is_contiguous() or tuple(x.shape) != shape or x.device != states.device:
+            raise ValueError(f"{name} must be a contiguous float64 tensor of shape {shape} on {states.device}")
+        return C.c_void_p(x.data_ptr()), x
+
+    def array(x, shape, name):
+        r = tensor_or_none(x, shape, name)
+        if r is not None and not isinstance(r[1], torch.Tensor):
+            raise ValueError(f"{name}: per-state arrays and position tables must be CUDA tensors here")
+        return r
+
+    descs, keep = _descriptors(models, n, samples - 1, array)
+    for name, t, size, dtype in (("out", out, n * samples * 6, torch.float64), ("status", status, n, torch.uint8),
+                                 ("steps", steps, n * 2, torch.int64)):
+        if t is None and name == "steps":
+            continue
+        if not isinstance(t, torch.Tensor) or t.dtype != dtype or not t.is_contiguous() or int(t.numel()) != size \
+                or t.device != states.device:
+            raise ValueError(f"{name} must be a contiguous {dtype} tensor of {size} elements on {states.device}")
+    ptr = lambda t: None if t is None else C.c_void_p(t.data_ptr())  # noqa: E731
+    check(lib().astroz_cuda_propagate_numerical_models_device(
+        ptr(states), n, float(t0), float(duration), float(dt), C.cast(descs, C.c_void_p), len(descs),
+        _integrator(integrator), float(rtol), float(atol), int(states.device.index), ptr(out), ptr(status), ptr(steps),
+        C.c_void_p(stream) if stream else None))
+    del keep
+
+
 __all__ = ["propagate_numerical_batch", "propagate_numerical_batch_device", "numerical_times", "AstrozCudaError",
-           "OK", "STOPPED", "SUBSTEP_LIMIT", "NON_FINITE"]
+           "OK", "STOPPED", "SUBSTEP_LIMIT", "NON_FINITE", "propagate_models_batch", "propagate_models_batch_device",
+           "TwoBody", "J2", "J3", "J4", "Drag", "ImprovedDrag", "SolarRadiationPressure", "ThirdBody", "MAX_MODELS"]

@@ -396,6 +396,80 @@ int32_t astroz_cuda_propagate_numerical_device(const double *d_states, uint32_t 
                                                int32_t integrator, double rtol, double atol, int32_t device,
                                                double *d_out, uint8_t *d_status, uint64_t *d_steps, void *stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Numerical propagation under a caller's ordered list of force models: the force models of the reference's propagators
+ * module (src/propagators/ForceModel.zig) for a batch of states.  State i's trajectory is what Propagator.propagate
+ * (src/propagators/Propagator.zig:22-48) returns for states[i] with the chosen integrator and, as its force, the list:
+ *   one model: that model's acceleration as it is (bindings/python/src/propagator.zig:138-146);
+ *   several:   Composite (ForceModel.zig:365-374): a total starting at zero, the models added in list order, component by
+ *              component (the order changes the low bits and is part of the result).  At most 16 models; kinds repeat.
+ * Sampling, integrators, tolerances, status bytes, zero-filled stopped states and step counts are those of
+ * astroz_cuda_propagate_numerical above.
+ * Each model's fields, by kind (the reference's parameters, with its arithmetic line for line):
+ *   ASTROZ_MODEL_TWO_BODY      mu                                               ForceModel.zig:42-56
+ *   ASTROZ_MODEL_J2 / J3 / J4  mu, coef (j2 / j3 / j4), r_eq                    :58-80, :113-143, :145-176
+ *   ASTROZ_MODEL_DRAG          r_eq, rho0, scale_height, c (cd), area, mass, max_altitude          :82-111
+ *   ASTROZ_MODEL_IMPROVED_DRAG r_eq, c (cd), area, mass, max_altitude, f107     :268-349 (five layers, the atmosphere
+ *                              rotating at 7.2921150e-5 rad/s, zero below 100 km and above max_altitude)
+ *   ASTROZ_MODEL_SRP           c (cr), area, mass, r_eq, pos (sunPos)           :178-228 (P = 4.56e-6 N/m^2, AU =
+ *                              1.495978707e8 km, src/constants.zig:27-28; cylindrical shadow of radius r_eq)
+ *   ASTROZ_MODEL_THIRD_BODY    mu, pos                                          :230-266 (Battin's formula)
+ * Fields a kind does not use are ignored.  Flags: ASTROZ_MODEL_PER_STATE_C / _AREA / _MASS take c / area / mass from
+ * c_per_state / area_per_state / mass_per_state[n] instead (drag kinds and SRP); ASTROZ_MODEL_POS_TABLE takes pos from
+ * pos_table[K][3] instead (SRP and third body), K = samples - 1: row k holds for every force evaluation of output interval
+ * k, DP87 substeps and rejected attempts included -- the batch form of updateSunPos / updatePos between steps.
+ * The reference's quirks are kept: J3's x / y terms carry an extra 1/r, J4 divides by r^9, ImprovedDrag is zero below
+ * 100 km.
+ * ASTROZ_VALUE_ERROR, nothing written or allocated: n_models 0 or > 16; an unknown kind or flag; a non-finite scalar field
+ * the kind uses; a flag set and its pointer NULL; device = -1; and every error of astroz_cuda_propagate_numerical. */
+#define ASTROZ_MODEL_TWO_BODY      0
+#define ASTROZ_MODEL_J2            1
+#define ASTROZ_MODEL_J3            2
+#define ASTROZ_MODEL_J4            3
+#define ASTROZ_MODEL_DRAG          4
+#define ASTROZ_MODEL_IMPROVED_DRAG 5
+#define ASTROZ_MODEL_SRP           6
+#define ASTROZ_MODEL_THIRD_BODY    7
+#define ASTROZ_MODEL_PER_STATE_C    1u
+#define ASTROZ_MODEL_PER_STATE_AREA 2u
+#define ASTROZ_MODEL_PER_STATE_MASS 4u
+#define ASTROZ_MODEL_POS_TABLE      8u
+#define ASTROZ_MAX_MODELS          16
+typedef struct {
+    int32_t kind;
+    uint32_t flags;
+    double mu;
+    double coef;
+    double r_eq;
+    double rho0;
+    double scale_height;
+    double max_altitude;
+    double f107;
+    double c;
+    double area;
+    double mass;
+    double pos[3];
+    const double *c_per_state;
+    const double *area_per_state;
+    const double *mass_per_state;
+    const double *pos_table;
+} astroz_force_model_t;
+
+/* HOST buffers: states[n][6], the per-state arrays [n] and position tables [K][3] the models name, out / status / steps
+ * as astroz_cuda_propagate_numerical.  The same chunked pipeline; the position tables are uploaded once per call. */
+int32_t astroz_cuda_propagate_numerical_models(const double *states, uint32_t n, double t0, double duration, double dt,
+                                               const astroz_force_model_t *models, uint32_t n_models,
+                                               int32_t integrator, double rtol, double atol, int32_t device,
+                                               double *out, uint8_t *status, uint64_t *steps);
+/* Same with DEVICE pointers on `device` for the states, outputs and every per-state array and position table the models
+ * name (the descriptors themselves are host memory).  Asynchronous on `stream`: the model list travels in the launch's
+ * parameters, so the call queues one kernel and returns. */
+int32_t astroz_cuda_propagate_numerical_models_device(const double *d_states, uint32_t n, double t0, double duration,
+                                                      double dt, const astroz_force_model_t *models, uint32_t n_models,
+                                                      int32_t integrator, double rtol, double atol, int32_t device,
+                                                      double *d_out, uint8_t *d_status, uint64_t *d_steps,
+                                                      void *stream);
+
 /* ---- measurement helpers --------------------------------------------------------------------- */
 /* DFMA microbenchmark on `device`: achieved fp64 TFLOP/s (FMA = 2) -- the measured roofline denominator */
 int32_t astroz_cuda_fp64_peak(int32_t device, double *tflops);

@@ -42,6 +42,7 @@ def zig_type(ctype: str, name: str) -> str:
         "astroz_constellation_t": "Handle",
         "astroz_sgp4_t": "Handle",
         "astroz_constellation_t *": "*Handle",
+        "const astroz_force_model_t *": "?[*]const astroz_force_model_t",
         "astroz_sgp4_t *": "*Handle",
         "uint32_t": "u32", "int32_t": "i32", "size_t": "usize", "double": "f64",
     }
@@ -67,6 +68,28 @@ def declarations(header: str):
         yield ret, m.group(2), args
 
 
+def structs(header: str):
+    """`typedef struct { <type> <name>; ... } name;` blocks of the header, as (name, [(ctype, field)])"""
+    text = re.sub(r"/\*.*?\*/", "", open(header).read(), flags=re.S)
+    for m in re.finditer(r"typedef struct \{([^}]*)\}\s*(\w+)\s*;", text):
+        fields = []
+        for decl in m.group(1).split(";"):
+            decl = " ".join(decl.split())
+            if decl:
+                mm = re.match(r"(.*?)(\w+(?:\[\d+\])?)$", decl)
+                fields.append((mm.group(1).strip(), mm.group(2)))
+        yield m.group(2), fields
+
+
+FIELD = {"int32_t": "i32", "uint32_t": "u32", "double": "f64", "const double *": "?[*]const f64"}
+
+
+def zig_field(ctype: str, name: str) -> str:
+    arr = re.search(r"\[(\d+)\]$", name)
+    base = FIELD[" ".join(ctype.split())]
+    return f"[{arr.group(1)}]{base}" if arr else base
+
+
 def render() -> str:
     out = [
         "//! CUDA propagation library bindings -- GENERATED from include/astroz_b200.h by tools/gen_zig_bindings.py.",
@@ -78,6 +101,10 @@ def render() -> str:
         "pub const Handle = ?*anyopaque;",
         "",
     ]
+    for name, fields in structs(HEADER):
+        out.append(f"pub const {name} = extern struct {{")
+        out += [f"    {f.split('[')[0]}: {zig_field(t, f)}," for t, f in fields]
+        out += ["};", ""]
     for ret, name, args in declarations(HEADER):
         zargs = ", ".join(f"{n.split('[')[0]}: {zig_type(t, n)}" for t, n in args)
         out.append(f"pub extern fn {name}({zargs}) {RET[ret]};")

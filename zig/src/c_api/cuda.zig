@@ -6,6 +6,26 @@
 
 pub const Handle = ?*anyopaque;
 
+pub const astroz_force_model_t = extern struct {
+    kind: i32,
+    flags: u32,
+    mu: f64,
+    coef: f64,
+    r_eq: f64,
+    rho0: f64,
+    scale_height: f64,
+    max_altitude: f64,
+    f107: f64,
+    c: f64,
+    area: f64,
+    mass: f64,
+    pos: [3]f64,
+    c_per_state: ?[*]const f64,
+    area_per_state: ?[*]const f64,
+    mass_per_state: ?[*]const f64,
+    pos_table: ?[*]const f64,
+};
+
 pub extern fn astroz_cuda_version() u32;
 pub extern fn astroz_cuda_device_count() i32;
 pub extern fn astroz_cuda_last_error() [*:0]const u8;
@@ -54,6 +74,8 @@ pub extern fn astroz_cuda_constellation_propagate_device_f32(h: Handle, jd: ?[*]
 pub extern fn astroz_cuda_numerical_times(t0: f64, duration: f64, dt: f64, times: ?[*]f64, count: *u64) i32;
 pub extern fn astroz_cuda_propagate_numerical(states: ?[*]const f64, n: u32, t0: f64, duration: f64, dt: f64, mu: f64, forces: i32, j2: ?[*]const f64, r_eq: ?[*]const f64, drag_cd: ?[*]const f64, drag_area: ?[*]const f64, drag_mass: ?[*]const f64, integrator: i32, rtol: f64, atol: f64, device: i32, out: ?[*]f64, status: ?[*]u8, steps: ?[*]u64) i32;
 pub extern fn astroz_cuda_propagate_numerical_device(d_states: ?[*]const f64, n: u32, t0: f64, duration: f64, dt: f64, mu: f64, forces: i32, j2: ?[*]const f64, r_eq: ?[*]const f64, d_drag_cd: ?[*]const f64, d_drag_area: ?[*]const f64, d_drag_mass: ?[*]const f64, integrator: i32, rtol: f64, atol: f64, device: i32, d_out: ?[*]f64, d_status: ?[*]u8, d_steps: ?[*]u64, stream: ?*anyopaque) i32;
+pub extern fn astroz_cuda_propagate_numerical_models(states: ?[*]const f64, n: u32, t0: f64, duration: f64, dt: f64, models: ?[*]const astroz_force_model_t, n_models: u32, integrator: i32, rtol: f64, atol: f64, device: i32, out: ?[*]f64, status: ?[*]u8, steps: ?[*]u64) i32;
+pub extern fn astroz_cuda_propagate_numerical_models_device(d_states: ?[*]const f64, n: u32, t0: f64, duration: f64, dt: f64, models: ?[*]const astroz_force_model_t, n_models: u32, integrator: i32, rtol: f64, atol: f64, device: i32, d_out: ?[*]f64, d_status: ?[*]u8, d_steps: ?[*]u64, stream: ?*anyopaque) i32;
 pub extern fn astroz_cuda_fp64_peak(device: i32, tflops: ?[*]f64) i32;
 pub extern fn astroz_cuda_fp64_pipe_peak(device: i32, tflops: ?[*]f64) i32;
 
