@@ -161,9 +161,8 @@ struct Constellation {
     bool timing = false;  // kernel-time events are recorded only on request (astroz_cuda_constellation_set_timing): the
                           // timed event records cost stream time, which is not work
     cudaEvent_t chunkDone[64] = {};  // grid chunk k of a host-buffer propagate has finished
-    // the two-slot pipelines of the pairs call and sgp4_array: slot k's kernels / result copy have finished, and the
-    // current chunk's inputs are on the device
-    cudaEvent_t kernelDone[2] = {}, copyDone[2] = {}, inputsDone = nullptr;
+    // the two-slot pipeline of the pairs call and sgp4_array, and the pinned ring every pageable transfer goes through
+    az::ChunkPipeline pipe;
     int variant = -1;  // -1 = shipped default; >= 0 selects a tuning variant (ASTROZ_SGP4_VARIANT)
     int chunks = 8;
     // Multi-device handle (device = -1 at creation): the catalog is cut into contiguous satellite ranges, one
@@ -176,7 +175,6 @@ struct Constellation {
     DevBuf<double> dFullPos, dFullVel; // per shard: the WHOLE block, for the replicated (all-gather) propagate
     ShardWorkers *workers = nullptr;   // multi-device handle: parked host threads, one per shard after the first
     bool multi() const { return !shards.empty(); }
-    az::HostRing ring;  // pinned transfers from / to pageable caller memory
 
     // The members are destroyed after this body, on the device it makes current.
     ~Constellation() {
@@ -190,9 +188,6 @@ struct Constellation {
         if (axisReady) cudaEventDestroy(axisReady);
         for (auto &pair : ev) for (auto &e : pair) if (e) cudaEventDestroy(e);
         for (auto &e : chunkDone) if (e) cudaEventDestroy(e);
-        for (auto &e : kernelDone) if (e) cudaEventDestroy(e);
-        for (auto &e : copyDone) if (e) cudaEventDestroy(e);
-        if (inputsDone) cudaEventDestroy(inputsDone);
         if (stream) cudaStreamDestroy(stream);
         if (copyStream) cudaStreamDestroy(copyStream);
         if (auxStream) cudaStreamDestroy(auxStream);
@@ -227,9 +222,7 @@ int32_t open_device(Constellation *c, int device) {
     for (auto &pair : c->ev)
         for (auto &ev : pair) AZ_CUDA(cudaEventCreate(&ev));
     for (auto &ev : c->chunkDone) AZ_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-    for (auto &ev : c->kernelDone) AZ_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-    for (auto &ev : c->copyDone) AZ_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-    AZ_CUDA(cudaEventCreateWithFlags(&c->inputsDone, cudaEventDisableTiming));
+    AZ_CUDA(c->pipe.create());
     if (const char *v = std::getenv("ASTROZ_SGP4_VARIANT")) c->variant = std::atoi(v);
     if (const char *v = std::getenv("ASTROZ_SDP4_VARIANT")) az::set_sdp4_variant(std::atoi(v));
     if (const char *v = std::getenv("ASTROZ_TIMING")) c->timing = std::atoi(v) != 0;
@@ -1068,7 +1061,7 @@ static int32_t propagate_host_queue(Constellation *c, const double *jd, const do
     // cell takes, i.e. every result bit -- the same however the call is chunked (one device or many, any chunk count)
     if (byTime && nChunks > 1) per = (per + 191) / 192 * 192;
     const bool posPageable = az::is_pageable(pos), velPageable = vel && az::is_pageable(vel);
-    c->ring.discard();
+    c->pipe.ring.discard();
     // last_kernel_ms after a host-buffer call: the span from the first kernel of the first chunk to the last kernel of
     // the last chunk (copies overlapping) in all three slots
     time_begin(c);
@@ -1102,13 +1095,13 @@ static int32_t propagate_host_queue(Constellation *c, const double *jd, const do
             const bool pg = which ? velPageable : posPageable;
             const cudaEvent_t ready = c->chunkDone[k];
             if (layout == 0) {  // this handle's rows are one contiguous run of the (possibly wider) host block
-                AZ_CUDA(c->ring.deliver(pg, ready, dsrc, hdst + (size_t)rowOffset * n_times * 3 + off, 1, cnt * 8, cnt * 8,
-                                        c->copyStream));
+                AZ_CUDA(c->pipe.ring.deliver(pg, ready, dsrc, hdst + (size_t)rowOffset * n_times * 3 + off, 1, cnt * 8,
+                                             cnt * 8, c->copyStream));
             } else if (totalRows == n) {
-                AZ_CUDA(c->ring.deliver(pg, ready, dsrc, hdst + off, 1, cnt * 8, cnt * 8, c->copyStream));
+                AZ_CUDA(c->pipe.ring.deliver(pg, ready, dsrc, hdst + off, 1, cnt * 8, cnt * 8, c->copyStream));
             } else {            // time-major into a wider block: n*24 bytes per epoch at a pitch of totalRows*24
-                AZ_CUDA(c->ring.deliver(pg, ready, dsrc, hdst + ((size_t)u0 * totalRows + rowOffset) * 3, u1 - u0,
-                                        (size_t)n * 24, (size_t)totalRows * 24, c->copyStream));
+                AZ_CUDA(c->pipe.ring.deliver(pg, ready, dsrc, hdst + ((size_t)u0 * totalRows + rowOffset) * 3, u1 - u0,
+                                             (size_t)n * 24, (size_t)totalRows * 24, c->copyStream));
             }
         }
     }
@@ -1119,7 +1112,7 @@ static int32_t propagate_host_queue(Constellation *c, const double *jd, const do
 static int32_t propagate_host_wait(Constellation *c) {
     if (!c->stream) return ASTROZ_OK;
     AZ_CUDA(cudaSetDevice(c->device));
-    AZ_CUDA(c->ring.drain(c->copyStream));
+    AZ_CUDA(c->pipe.ring.drain(c->copyStream));
     AZ_CUDA(cudaStreamSynchronize(c->copyStream));
     AZ_CUDA(cudaStreamSynchronize(c->stream));
     return ASTROZ_OK;
@@ -1291,9 +1284,7 @@ int32_t astroz_cuda_constellation_propagate_pairs_device(astroz_constellation_t 
     return pairs_queue(c, d_sat, d_jd, d_fr, n, mode, d_pos, d_vel, d_status, s);
 }
 
-// Host buffers: chunks of pairsChunk queries on two device slots.  Chunk k's queries go up and its kernels run on the
-// compute stream while chunk k-1's results come back on the copy stream (pinned / registered destinations) or through
-// the pinned ring and the copy pool (pageable ones); pageable queries are staged through the same ring.
+// Host buffers: chunks of pairsChunk queries through the handle's two-slot pipeline (az::ChunkPipeline).
 int32_t astroz_cuda_constellation_propagate_pairs(astroz_constellation_t h, const uint32_t *sat, const double *jd,
                                                   const double *fr, uint32_t n, int32_t mode, double *pos, double *vel,
                                                   uint8_t *status) {
@@ -1322,53 +1313,21 @@ int32_t astroz_cuda_constellation_propagate_pairs(astroz_constellation_t h, cons
         if (rc != ASTROZ_OK) return rc;
     }
     const uint32_t chunk = std::min(n, c->pairsChunk);
-    const uint32_t nChunks = (uint32_t)(((uint64_t)n + chunk - 1) / chunk);
-    const uint32_t slots = nChunks > 1 ? 2 : 1;
-    // slot layout, in doubles: queries [jd | fr | sat], results [pos | vel | status]
-    const size_t inD = (size_t)chunk * 2 + (chunk + 1) / 2;
-    const size_t outD = (size_t)chunk * (vel ? 6 : 3) + (status ? (chunk + 7) / 8 : 0);
-    AZ_CUDA(c->dPairsIn.reserve(inD * slots));
-    AZ_CUDA(c->dPairsOut.reserve(outD * slots));
-    const bool inPageable = az::is_pageable(sat) || az::is_pageable(jd) || az::is_pageable(fr);
-    const bool posPg = az::is_pageable(pos), velPg = vel && az::is_pageable(vel);
-    const bool stPg = status && az::is_pageable(status);
-    const bool outPageable = posPg || velPg || stPg;
-    const size_t inBytes[3] = {8, 8, 4};
-    c->ring.discard();
-    for (uint32_t k = 0; k < nChunks; ++k) {
-        const uint32_t slot = k % slots;
-        const uint32_t q0 = k * chunk, m = std::min(chunk, n - q0);
-        double *dJd = c->dPairsIn.p + slot * inD, *dFr = dJd + chunk;
-        uint32_t *dSat = reinterpret_cast<uint32_t *>(dFr + chunk);
-        double *dPos = c->dPairsOut.p + slot * outD, *dVel = vel ? dPos + (size_t)chunk * 3 : nullptr;
-        uint8_t *dSt = status ? reinterpret_cast<uint8_t *>(dPos + (size_t)chunk * (vel ? 6 : 3)) : nullptr;
-        if (k >= slots) AZ_CUDA(cudaEventSynchronize(c->copyDone[slot]));  // chunk k-2's results have left this slot
-        const void *src[3] = {jd + q0, fr + q0, sat + q0};
-        void *const dst[3] = {dJd, dFr, dSat};
-        AZ_CUDA(c->ring.upload(inPageable, 3, src, dst, inBytes, m, st));
-        AZ_CUDA(cudaEventRecord(c->inputsDone, st));
-        rc = pairs_queue(c, dSat, dJd, dFr, m, mode, dPos, dVel, dSt, st);
-        if (rc != ASTROZ_OK) return rc;
-        const cudaEvent_t ready = c->kernelDone[slot];
-        AZ_CUDA(cudaEventRecord(ready, st));
-        if (outPageable) {
-            // chunk k-1's pageable results go through the ring while chunk k computes; the ring is free once this
-            // chunk's queries have left it
-            AZ_CUDA(cudaEventSynchronize(c->inputsDone));
-            AZ_CUDA(c->ring.drain(c->copyStream));
-        }
-        AZ_CUDA(cudaStreamWaitEvent(c->copyStream, ready, 0));
-        AZ_CUDA(c->ring.deliver(posPg, ready, dPos, pos + (size_t)q0 * 3, 1, (size_t)m * 24, (size_t)m * 24,
-                                c->copyStream));
-        if (vel)
-            AZ_CUDA(c->ring.deliver(velPg, ready, dVel, vel + (size_t)q0 * 3, 1, (size_t)m * 24, (size_t)m * 24,
-                                    c->copyStream));
-        if (status) AZ_CUDA(c->ring.deliver(stPg, ready, dSt, status + q0, 1, m, m, c->copyStream));
-        AZ_CUDA(cudaEventRecord(c->copyDone[slot], c->copyStream));
-    }
-    AZ_CUDA(c->ring.drain(c->copyStream));
-    AZ_CUDA(cudaStreamSynchronize(c->copyStream));
-    AZ_CUDA(cudaStreamSynchronize(st));
+    const az::HostIn in[3] = {{jd, 8}, {fr, 8}, {sat, 4}};
+    const az::HostOut out[3] = {{pos, 24}, {vel, 24}, {status, 1}};
+    AZ_CUDA(c->dPairsIn.reserve(az::chunk_slots_bytes(in, 3, n, chunk) / 8));
+    AZ_CUDA(c->dPairsOut.reserve(az::chunk_slots_bytes(out, 3, n, chunk) / 8));
+    int32_t queued = ASTROZ_OK;  // pairs_queue's own code; its message is the last error
+    const cudaError_t e = c->pipe.run(
+        st, c->copyStream, n, chunk, 3, in, 3, out, c->dPairsIn.p, c->dPairsOut.p,
+        [&](uint32_t, uint32_t, uint32_t m, void *const *dIn, void *const *dOut, cudaStream_t s) {
+            queued = pairs_queue(c, static_cast<const uint32_t *>(dIn[2]), static_cast<const double *>(dIn[0]),
+                                 static_cast<const double *>(dIn[1]), m, mode, static_cast<double *>(dOut[0]),
+                                 static_cast<double *>(dOut[1]), static_cast<uint8_t *>(dOut[2]), s);
+            return queued == ASTROZ_OK ? cudaSuccess : cudaErrorUnknown;  // stops the run; `queued` is returned
+        });
+    if (queued != ASTROZ_OK) return queued;
+    AZ_CUDA(e);
     return ASTROZ_OK;
 }
 
@@ -1529,7 +1488,7 @@ static int32_t sgp4_into_host_queue(Constellation *c, const double *times, uint3
     int32_t rc = sgp4_into_common(c, times, n_times, epoch_offsets, c->dPos.p, vel ? c->dVel.p : nullptr, mode,
                                   reference_jd, layout, s, 3, mask, ns);
     if (rc != ASTROZ_OK) return rc;
-    c->ring.discard();
+    c->pipe.ring.discard();
     const cudaEvent_t ready = c->chunkDone[0];
     AZ_CUDA(cudaEventRecord(ready, s));
     AZ_CUDA(cudaStreamWaitEvent(c->copyStream, ready, 0));
@@ -1537,8 +1496,9 @@ static int32_t sgp4_into_host_queue(Constellation *c, const double *times, uint3
         double *dst = host_at(which ? vel : pos);
         const double *src = which ? c->dVel.p : c->dPos.p;
         const bool pg = az::is_pageable(which ? vel : pos);
-        if (!strided) AZ_CUDA(c->ring.deliver(pg, ready, src, dst, 1, dense * 8, dense * 8, c->copyStream));
-        else AZ_CUDA(c->ring.deliver(pg, ready, src, dst, n_times, (size_t)ns * 24, (size_t)rows * 24, c->copyStream));
+        if (!strided) AZ_CUDA(c->pipe.ring.deliver(pg, ready, src, dst, 1, dense * 8, dense * 8, c->copyStream));
+        else AZ_CUDA(c->pipe.ring.deliver(pg, ready, src, dst, n_times, (size_t)ns * 24, (size_t)rows * 24,
+                                          c->copyStream));
     }
     return ASTROZ_OK;
 }
@@ -1857,30 +1817,19 @@ int32_t astroz_cuda_sgp4_array(astroz_sgp4_t h, const double *jd, const double *
     cudaStream_t st = c->stream;
     c->cacheValid = false;  // dTime holds [jd | fr] slots here
     // A long axis ("1 year at one second" = 31.5 M epochs: 0.5 GB of jd/fr in, 1.5 GB of records out) is cut into
-    // chunks on a two-slot pipeline: while chunk k is propagated, chunk k+1's epochs are staged and uploaded and chunk
-    // k-1's records travel back, so the call runs at the PCIe rate of its 48 B/epoch result instead of the sum of three
-    // serial phases.  jd / fr usually are pageable (numpy): the copy pool stages them into pinned slots.
+    // chunks on the handle's two-slot pipeline (az::ChunkPipeline): while chunk k is propagated, chunk k+1's epochs
+    // are staged and uploaded and chunk k-1's records travel back, so the call runs at the PCIe rate of its 48 B/epoch
+    // result instead of the sum of three serial phases.  jd / fr usually are pageable (numpy) and go up through the
+    // pinned ring; pageable results come back through it too, in ring-sized pieces.
     constexpr uint32_t kChunk = 1u << 21;   // epochs per chunk: 32 MB of epochs, 96 MB of records
     const uint32_t nChunks = (count + kChunk - 1) / kChunk;
     const uint32_t chunk = ((count + nChunks - 1) / nChunks + 31) / 32 * 32;   // balanced: no short last chunk
-    const int slots = nChunks > 1 ? 2 : 1;
-    AZ_CUDA(c->dTime.reserve((size_t)chunk * 2 * slots));
-    AZ_CUDA(c->dPos.reserve((size_t)chunk * 6 * slots));
-    // pageable jd / fr are staged through the handle's pinned ring; pageable results are not (a 96 MB chunk does not
-    // fit a ring slot) -- they go through cudaMemcpyAsync's own staging
-    const bool inPageable = az::is_pageable(jd) || az::is_pageable(fr);
-    const size_t inBytes[2] = {8, 8};
-    time_begin(c);
-    AZ_CUDA(time_mark(c, kTimeK1, false, st));
-    for (uint32_t k = 0; k < nChunks; ++k) {
-        const int slot = (int)(k & 1u) % slots;
-        const uint32_t t0 = k * chunk, n = std::min(chunk, count - t0);
-        double *dJd = c->dTime.p + (size_t)slot * chunk * 2, *dFr = dJd + chunk;
-        double *dOut = c->dPos.p + (size_t)slot * chunk * 6;
-        if (k >= (uint32_t)slots) AZ_CUDA(cudaEventSynchronize(c->copyDone[slot]));  // chunk k-2 has left this slot
-        const void *src[2] = {jd + t0, fr + t0};
-        void *const dst[2] = {dJd, dFr};
-        AZ_CUDA(c->ring.upload(inPageable, 2, src, dst, inBytes, n, st));
+    const az::HostIn in[2] = {{jd, 8}, {fr, 8}};
+    const az::HostOut out[1] = {{results, 48}};
+    AZ_CUDA(c->dTime.reserve(az::chunk_slots_bytes(in, 2, count, chunk) / 8));
+    AZ_CUDA(c->dPos.reserve(az::chunk_slots_bytes(out, 1, count, chunk) / 8));
+    auto launch = [&](uint32_t k, uint32_t t0, uint32_t n, void *const *dIn, void *const *dOut, cudaStream_t s) {
+        double *dJd = static_cast<double *>(dIn[0]), *dRec = static_cast<double *>(dOut[0]);
         az::GridArgs a;
         a.g = c->g;
         a.sgp4Tiles = c->dTiles.p;
@@ -1888,23 +1837,23 @@ int32_t astroz_cuda_sgp4_array(astroz_sgp4_t h, const double *jd, const double *
         a.orig = c->dIdentity.p;
         a.nSats = 1;
         a.jdArr = dJd;
-        a.frArr = dFr;
+        a.frArr = static_cast<double *>(dIn[1]);
         a.tbase = dJd;
         a.epochJd = epoch_jd;
         a.nTimes = n;
-        a.pos = dOut;
-        a.vel = dOut + 3;
+        a.pos = dRec;
+        a.vel = dRec + 3;
         a.outNumSats = 1;
         a.recStride = 6;
-        AZ_CUDA(az::launch_sgp4_grid(a, ASTROZ_MODE_TEME, ASTROZ_LAYOUT_SATELLITE_MAJOR, st, c->variant));
-        AZ_CUDA(cudaEventRecord(c->kernelDone[slot], st));
-        AZ_CUDA(cudaStreamWaitEvent(c->copyStream, c->kernelDone[slot], 0));
-        AZ_CUDA(cudaMemcpyAsync(results + (size_t)t0 * 6, dOut, (size_t)n * 48, cudaMemcpyDeviceToHost, c->copyStream));
-        AZ_CUDA(cudaEventRecord(c->copyDone[slot], c->copyStream));
-    }
-    AZ_CUDA(time_mark(c, kTimeK1, true, st));
-    AZ_CUDA(cudaStreamSynchronize(c->copyStream));
-    AZ_CUDA(cudaStreamSynchronize(st));
+        // K1's span: from before the first chunk's kernel to after the last one's
+        cudaError_t e = k == 0 ? time_mark(c, kTimeK1, false, s) : cudaSuccess;
+        if (e == cudaSuccess)
+            e = az::launch_sgp4_grid(a, ASTROZ_MODE_TEME, ASTROZ_LAYOUT_SATELLITE_MAJOR, s, c->variant);
+        if (e == cudaSuccess && t0 + n == count) e = time_mark(c, kTimeK1, true, s);
+        return e;
+    };
+    time_begin(c);
+    AZ_CUDA(c->pipe.run(st, c->copyStream, count, chunk, 2, in, 1, out, c->dTime.p, c->dPos.p, launch));
     return ASTROZ_OK;
 }
 
@@ -2093,6 +2042,11 @@ int32_t astroz_cuda_constellation_propagate_replicated(astroz_constellation_t h,
 }
 
 // ---- numerical propagation (K7, az_numerical.cu) -------------------------------------------------------------------
+// ASTROZ_VALUE_ERROR with `why` as the last error: the argument checks' refusal
+static int32_t value_error(const char *why) {
+    g_lastError = why;
+    return ASTROZ_VALUE_ERROR;
+}
 // The sampling rule of Propagator.propagate (src/propagators/Propagator.zig:32-45), stated here and nowhere else:
 //   t = t0; t_end = t0 + duration; while (t < t_end) { step = min(dt, t_end - t); ...; t += step; }
 // *count = samples (the initial state plus one per step); times (nullable) receives the sample times, table (nullable)
@@ -2102,28 +2056,19 @@ static constexpr uint64_t kMaxNumSteps = 0xfffffffeull;  // K7 counts intervals 
 static int32_t numerical_schedule(double t0, double duration, double dt, double *times, az::StepTable *table,
                                   uint64_t *count) {
     const double tEnd = t0 + duration;
-    if (!std::isfinite(t0) || !std::isfinite(duration) || !std::isfinite(dt) || !std::isfinite(tEnd) || !(dt > 0.0)) {
-        g_lastError = "t0, duration and dt must be finite and dt > 0";
-        return ASTROZ_VALUE_ERROR;
-    }
-    if (duration / dt > (double)kMaxNumSteps) {
-        g_lastError = "duration / dt exceeds the step limit";
-        return ASTROZ_VALUE_ERROR;
-    }
+    if (!std::isfinite(t0) || !std::isfinite(duration) || !std::isfinite(dt) || !std::isfinite(tEnd) || !(dt > 0.0))
+        return value_error("t0, duration and dt must be finite and dt > 0");
+    if (duration / dt > (double)kMaxNumSteps) return value_error("duration / dt exceeds the step limit");
     if (table) *table = az::StepTable{dt, 0, 0, {}};
     double t = t0;
     uint64_t k = 0;
     if (times) times[0] = t;
     while (t < tEnd) {
         const double step = std::min(dt, tEnd - t);
-        if (t + step == t || ++k > kMaxNumSteps) {
-            g_lastError = "the sampling loop would not end: t0 + step rounds to t0";
-            return ASTROZ_VALUE_ERROR;
-        }
-        if (table && !az::step_table_push(*table, step)) {
-            g_lastError = "the sampling loop's steps do not fit the step table";
-            return ASTROZ_VALUE_ERROR;
-        }
+        if (t + step == t || ++k > kMaxNumSteps)
+            return value_error("the sampling loop would not end: t0 + step rounds to t0");
+        if (table && !az::step_table_push(*table, step))
+            return value_error("the sampling loop's steps do not fit the step table");
         t += step;
         if (times) times[k] = t;
     }
@@ -2131,51 +2076,48 @@ static int32_t numerical_schedule(double t0, double duration, double dt, double 
     return ASTROZ_OK;
 }
 
-// Argument checks shared by both batch calls, before anything is read, written or allocated.  *table receives the steps.
-static int32_t numerical_check(uint32_t n, double t0, double duration, double dt, double mu, int32_t forces,
-                               const double *j2, const double *r_eq, const double *cd, const double *area,
-                               const double *mass, int32_t integrator, double rtol, double atol, int32_t device,
-                               az::StepTable *table) {
-    auto bad = [](const char *why) {
-        g_lastError = why;
-        return ASTROZ_VALUE_ERROR;
-    };
-    if (device < 0) return bad("numerical propagation runs on one device: pass its ordinal");
-    if (integrator != az::kIntRk4 && integrator != az::kIntDp87) return bad("integrator must be RK4 (0) or DP87 (1)");
-    if (forces & ~(az::kForceJ2 | az::kForceDrag)) return bad("unknown force bit");
-    if (!std::isfinite(mu) || !std::isfinite(rtol) || !std::isfinite(atol)) return bad("mu, rtol and atol must be finite");
-    if ((forces & az::kForceJ2) && (!j2 || !std::isfinite(*j2))) return bad("J2 needs a finite j2");
-    if (forces && (!r_eq || !std::isfinite(*r_eq))) return bad("J2 and drag need a finite r_eq");
-    if ((forces & az::kForceDrag) && (!cd || !area || !mass)) return bad("drag needs drag_cd, drag_area and drag_mass");
+// Argument checks of every batch call, before anything is read, written or allocated.  On success a receives n, the
+// steps and the tolerances.
+static int32_t numerical_check(uint32_t n, double t0, double duration, double dt, int32_t integrator, double rtol,
+                               double atol, int32_t device, az::NumArgs *a) {
+    if (device < 0) return value_error("numerical propagation runs on one device: pass its ordinal");
+    if (integrator != az::kIntRk4 && integrator != az::kIntDp87)
+        return value_error("integrator must be RK4 (0) or DP87 (1)");
+    if (!std::isfinite(rtol) || !std::isfinite(atol)) return value_error("rtol and atol must be finite");
     uint64_t samples = 0;
-    const int32_t rc = numerical_schedule(t0, duration, dt, nullptr, table, &samples);
+    const int32_t rc = numerical_schedule(t0, duration, dt, nullptr, &a->steps, &samples);
     if (rc != ASTROZ_OK) return rc;
-    if ((uint64_t)n * samples > SIZE_MAX / 48) return bad("the output size overflows");
+    if ((uint64_t)n * samples > SIZE_MAX / 48) return value_error("the output size overflows");
+    a->n = n;
+    a->p.rtol = rtol;
+    a->p.atol = atol;
     return ASTROZ_OK;
 }
 
-static az::NumArgs numerical_args(uint32_t n, const az::StepTable &table, double mu, int32_t forces, const double *j2,
-                                  const double *r_eq, double rtol, double atol) {
-    az::NumArgs a{};
-    a.n = n;
-    a.steps = table;
-    a.p.mu = mu;
-    a.p.j2 = (forces & az::kForceJ2) ? *j2 : 0.0;
-    a.p.rEq = forces ? *r_eq : 0.0;
-    a.p.rtol = rtol;
-    a.p.atol = atol;
-    return a;
+// Checks of the fixed force set (two-body, J2, exponential drag), before anything is read, written or allocated.  On
+// success p receives mu, j2 and r_eq.
+static int32_t forces_check(double mu, int32_t forces, const double *j2, const double *r_eq, const double *cd,
+                            const double *area, const double *mass, az::NumParams *p) {
+    if (forces & ~(az::kForceJ2 | az::kForceDrag)) return value_error("unknown force bit");
+    if (!std::isfinite(mu)) return value_error("mu must be finite");
+    if ((forces & az::kForceJ2) && (!j2 || !std::isfinite(*j2))) return value_error("J2 needs a finite j2");
+    if (forces && (!r_eq || !std::isfinite(*r_eq))) return value_error("J2 and drag need a finite r_eq");
+    if ((forces & az::kForceDrag) && (!cd || !area || !mass))
+        return value_error("drag needs drag_cd, drag_area and drag_mass");
+    p->mu = mu;
+    p->j2 = (forces & az::kForceJ2) ? *j2 : 0.0;
+    p->rEq = forces ? *r_eq : 0.0;
+    return ASTROZ_OK;
 }
 
-// Per-device state of the host-buffer call: its two streams, the two-slot pipeline's events and the pinned ring (three
-// 32 MB pieces, allocated on the first pageable transfer).  Process-wide, created on first use and never destroyed, like
+// Per-device state of the host-buffer call: its two streams and its two-slot pipeline (whose pinned ring of three 32 MB
+// pieces is allocated on the first pageable transfer).  Process-wide, created on first use and never destroyed, like
 // the host copy pool; a mutex serialises the calls that share it.  The device slots are not kept: each call allocates
 // them stream-ordered and returns them before it returns.
 struct NumericalContext {
     std::mutex m;
     cudaStream_t stream = nullptr, copyStream = nullptr;
-    cudaEvent_t kernelDone[2] = {}, copyDone[2] = {}, inputsDone = nullptr;
-    az::HostRing ring;
+    az::ChunkPipeline pipe;
 };
 
 static int32_t numerical_context(int device, NumericalContext **out) {
@@ -2189,9 +2131,7 @@ static int32_t numerical_context(int device, NumericalContext **out) {
         AZ_CUDA(cudaSetDevice(device));
         AZ_CUDA(cudaStreamCreateWithFlags(&fresh->stream, cudaStreamNonBlocking));
         AZ_CUDA(cudaStreamCreateWithFlags(&fresh->copyStream, cudaStreamNonBlocking));
-        for (auto &e : fresh->kernelDone) AZ_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-        for (auto &e : fresh->copyDone) AZ_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-        AZ_CUDA(cudaEventCreateWithFlags(&fresh->inputsDone, cudaEventDisableTiming));
+        AZ_CUDA(fresh->pipe.create());
         c = fresh.release();
     }
     *out = c;
@@ -2230,15 +2170,14 @@ int32_t astroz_cuda_propagate_numerical_device(const double *d_states, uint32_t 
                                                const double *d_drag_area, const double *d_drag_mass,
                                                int32_t integrator, double rtol, double atol, int32_t device,
                                                double *d_out, uint8_t *d_status, uint64_t *d_steps, void *stream) {
-    az::StepTable table{};
-    int32_t rc = numerical_check(n, t0, duration, dt, mu, forces, j2, r_eq, d_drag_cd, d_drag_area, d_drag_mass,
-                                 integrator, rtol, atol, device, &table);
+    az::NumArgs a{};
+    int32_t rc = forces_check(mu, forces, j2, r_eq, d_drag_cd, d_drag_area, d_drag_mass, &a.p);
+    if (rc == ASTROZ_OK) rc = numerical_check(n, t0, duration, dt, integrator, rtol, atol, device, &a);
     if (rc != ASTROZ_OK) return rc;
     if (n == 0) return ASTROZ_OK;
     if (!d_states || !d_out || !d_status) return ASTROZ_NULL_POINTER;
     if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
     AZ_CUDA(cudaSetDevice(device));
-    az::NumArgs a = numerical_args(n, table, mu, forces, j2, r_eq, rtol, atol);
     a.states = d_states;
     a.cd = d_drag_cd;
     a.area = d_drag_area;
@@ -2251,107 +2190,53 @@ int32_t astroz_cuda_propagate_numerical_device(const double *d_states, uint32_t 
     return ASTROZ_OK;
 }
 
-// Host buffers: chunks of states on two device slots, each chunk's trajectory block at most kNumChunkBytes (eight ring
-// pieces).  Chunk k's states and per-state columns go up and its kernel runs on the compute stream while chunk k-1's
-// results come back on the copy stream (pinned / registered destinations) or through the pinned ring and the copy pool
-// (pageable ones); pageable inputs are staged through the same ring.  `cols` are the per-state input columns the kernel
-// reads ([n] doubles each; the fixed drag set has three, a model list one per per-state array it names); `tabs` are
-// whole arrays uploaded once per call before the first chunk (a model list's position tables).
-// launch(m, dStates, dCols, dTabs, dTraj, dStatus, dCounts, stream) queues the kernel for one chunk of m states.
+// Host buffers: chunks of states, each chunk's trajectory block at most kNumChunkBytes (eight ring pieces), through the
+// device's two-slot pipeline (az::ChunkPipeline).  `cols` are the per-state input columns the kernel reads ([n] doubles
+// each; the fixed drag set has three, a model list one per per-state array it names); `tabs` are whole arrays of
+// tabBytes each, uploaded once per call before the first chunk (a model list's position tables).  a holds the checked
+// arguments; for each chunk its n, states, out, status and counts are set to the chunk's and launch(dCols, dTabs, s)
+// queues the kernel.
 static constexpr size_t kNumChunkBytes = 256u << 20;
 static constexpr int kNumMaxCols = 3 * (int)az::kMaxModels, kNumMaxTabs = (int)az::kMaxModels;
-extern "C++" {
-template <class Launch>
-static int32_t numerical_host_pipeline(const double *states, uint32_t n, const az::StepTable &table, int nCols,
-                                       const double *const *cols, int nTabs, const double *const *tabs,
-                                       const size_t *tabBytes, int32_t device, double *out, uint8_t *status,
-                                       uint64_t *steps, Launch launch) {
+using NumLaunch = std::function<cudaError_t(const double *const *dCols, const double *const *dTabs, cudaStream_t s)>;
+static int32_t numerical_host(az::NumArgs &a, const double *states, int nCols, const double *const *cols, int nTabs,
+                              const double *const *tabs, size_t tabBytes, int32_t device, double *out, uint8_t *status,
+                              uint64_t *steps, const NumLaunch &launch) {
     NumericalContext *c = nullptr;
     int32_t rc = numerical_context(device, &c);
     if (rc != ASTROZ_OK) return rc;
     std::lock_guard<std::mutex> lk(c->m);
     AZ_CUDA(cudaSetDevice(device));
     cudaStream_t st = c->stream;
-    const size_t rowD = ((size_t)table.nFull + table.nTail + 1) * 6;  // doubles of one state's trajectory
-    const uint32_t chunk = (uint32_t)std::max<size_t>(1, std::min<size_t>(n, kNumChunkBytes / (rowD * 8)));
-    const uint32_t nChunks = (uint32_t)(((uint64_t)n + chunk - 1) / chunk);
-    const uint32_t slots = nChunks > 1 ? 2 : 1;
-    // slot layout, in doubles: inputs [states | column 0 | column 1 | ...], results [trajectories | counts | status]
-    const size_t inD = (size_t)chunk * (6 + nCols);
-    const size_t outD = (size_t)chunk * rowD + (steps ? (size_t)chunk * 2 : 0) + (chunk + 7) / 8;
-    size_t tabD = 0;
-    for (int t = 0; t < nTabs; ++t) tabD += tabBytes[t] / 8;
+    const uint32_t n = a.n;
+    const size_t rowBytes = ((size_t)a.steps.nFull + a.steps.nTail + 1) * 48;  // one state's trajectory
+    const uint32_t chunk = (uint32_t)std::max<size_t>(1, std::min<size_t>(n, kNumChunkBytes / rowBytes));
+    az::HostIn in[1 + kNumMaxCols] = {{states, 48}};
+    for (int q = 0; q < nCols; ++q) in[1 + q] = {cols[q], 8};
+    const az::HostOut res[3] = {{out, rowBytes}, {status, 1}, {steps, 16}};
     StreamBuf dIn(st), dOut(st), dTab(st);
-    // declared after the slots, so it runs before they are freed on any return: the ring's plan is forgotten and both
-    // streams have finished with the slots
-    struct Settle {
-        NumericalContext *c;
-        ~Settle() {
-            c->ring.discard();
-            cudaStreamSynchronize(c->copyStream);
-            cudaStreamSynchronize(c->stream);
-        }
-    } settle{c};
-    AZ_CUDA(dIn.alloc(inD * slots * 8));
-    AZ_CUDA(dOut.alloc(outD * slots * 8));
+    AZ_CUDA(dIn.alloc(az::chunk_slots_bytes(in, 1 + nCols, n, chunk)));
+    AZ_CUDA(dOut.alloc(az::chunk_slots_bytes(res, 3, n, chunk)));
     const double *dTabs[kNumMaxTabs] = {};
     if (nTabs) {
-        AZ_CUDA(dTab.alloc(tabD * 8));
-        double *at = static_cast<double *>(dTab.p);
+        AZ_CUDA(dTab.alloc(nTabs * tabBytes));
         for (int t = 0; t < nTabs; ++t) {
-            AZ_CUDA(cudaMemcpyAsync(at, tabs[t], tabBytes[t], cudaMemcpyHostToDevice, st));
+            double *at = static_cast<double *>(dTab.p) + t * (tabBytes / 8);
+            AZ_CUDA(cudaMemcpyAsync(at, tabs[t], tabBytes, cudaMemcpyHostToDevice, st));
             dTabs[t] = at;
-            at += tabBytes[t] / 8;
         }
     }
-    bool inPageable = az::is_pageable(states);
-    for (int k = 0; k < nCols; ++k) inPageable = inPageable || az::is_pageable(cols[k]);
-    const bool outPg = az::is_pageable(out), stPg = az::is_pageable(status), cntPg = steps && az::is_pageable(steps);
-    const bool outPageable = outPg || stPg || cntPg;
-    size_t inBytes[1 + kNumMaxCols];
-    inBytes[0] = 48;
-    for (int k = 0; k < nCols; ++k) inBytes[1 + k] = 8;
-    c->ring.discard();
-    for (uint32_t k = 0; k < nChunks; ++k) {
-        const uint32_t slot = k % slots;
-        const uint32_t s0 = k * chunk, m = std::min(chunk, n - s0);
-        double *dStates = static_cast<double *>(dIn.p) + slot * inD;
-        double *dCols[kNumMaxCols] = {};
-        for (int q = 0; q < nCols; ++q) dCols[q] = dStates + (size_t)chunk * (6 + q);
-        double *dTraj = static_cast<double *>(dOut.p) + slot * outD;
-        uint64_t *dCounts = steps ? reinterpret_cast<uint64_t *>(dTraj + (size_t)chunk * rowD) : nullptr;
-        uint8_t *dSt = reinterpret_cast<uint8_t *>(dTraj + (size_t)chunk * rowD + (steps ? (size_t)chunk * 2 : 0));
-        if (k >= slots) AZ_CUDA(cudaEventSynchronize(c->copyDone[slot]));  // chunk k-2's results have left this slot
-        const void *src[1 + kNumMaxCols] = {states + (size_t)s0 * 6};
-        void *dst[1 + kNumMaxCols] = {dStates};
-        for (int q = 0; q < nCols; ++q) {
-            src[1 + q] = cols[q] + s0;
-            dst[1 + q] = dCols[q];
-        }
-        AZ_CUDA(c->ring.upload(inPageable, 1 + nCols, src, dst, inBytes, m, st));
-        AZ_CUDA(cudaEventRecord(c->inputsDone, st));
-        AZ_CUDA(launch(m, dStates, static_cast<const double *const *>(dCols), static_cast<const double *const *>(dTabs),
-                       dTraj, dSt, dCounts, st));
-        const cudaEvent_t ready = c->kernelDone[slot];
-        AZ_CUDA(cudaEventRecord(ready, st));
-        if (outPageable) {
-            // chunk k-1's pageable results go through the ring while chunk k computes; the ring is free once this
-            // chunk's inputs have left it
-            AZ_CUDA(cudaEventSynchronize(c->inputsDone));
-            AZ_CUDA(c->ring.drain(c->copyStream));
-        }
-        AZ_CUDA(cudaStreamWaitEvent(c->copyStream, ready, 0));
-        AZ_CUDA(c->ring.deliver(outPg, ready, dTraj, out + (size_t)s0 * rowD, 1, (size_t)m * rowD * 8,
-                                (size_t)m * rowD * 8, c->copyStream));
-        AZ_CUDA(c->ring.deliver(stPg, ready, dSt, status + s0, 1, m, m, c->copyStream));
-        if (steps)
-            AZ_CUDA(c->ring.deliver(cntPg, ready, dCounts, steps + (size_t)s0 * 2, 1, (size_t)m * 16, (size_t)m * 16,
-                                    c->copyStream));
-        AZ_CUDA(cudaEventRecord(c->copyDone[slot], c->copyStream));
-    }
-    AZ_CUDA(c->ring.drain(c->copyStream));
-    AZ_CUDA(cudaStreamSynchronize(c->copyStream));
-    AZ_CUDA(cudaStreamSynchronize(st));
+    AZ_CUDA(c->pipe.run(st, c->copyStream, n, chunk, 1 + nCols, in, 3, res, dIn.p, dOut.p,
+                        [&](uint32_t, uint32_t, uint32_t m, void *const *dI, void *const *dO, cudaStream_t s) {
+                            const double *dCols[kNumMaxCols] = {};
+                            for (int q = 0; q < nCols; ++q) dCols[q] = static_cast<const double *>(dI[1 + q]);
+                            a.n = m;
+                            a.states = static_cast<const double *>(dI[0]);
+                            a.out = static_cast<double *>(dO[0]);
+                            a.status = static_cast<uint8_t *>(dO[1]);
+                            a.counts = static_cast<uint64_t *>(dO[2]);
+                            return launch(dCols, dTabs, s);
+                        }));
     // give the slots back before returning (the default pool keeps nothing across a synchronisation)
     AZ_CUDA(dIn.release());
     AZ_CUDA(dOut.release());
@@ -2359,37 +2244,28 @@ static int32_t numerical_host_pipeline(const double *states, uint32_t n, const a
     AZ_CUDA(cudaStreamSynchronize(st));
     return ASTROZ_OK;
 }
-}  // extern "C++"
 
 int32_t astroz_cuda_propagate_numerical(const double *states, uint32_t n, double t0, double duration, double dt,
                                         double mu, int32_t forces, const double *j2, const double *r_eq,
                                         const double *drag_cd, const double *drag_area, const double *drag_mass,
                                         int32_t integrator, double rtol, double atol, int32_t device, double *out,
                                         uint8_t *status, uint64_t *steps) {
-    az::StepTable table{};
-    int32_t rc = numerical_check(n, t0, duration, dt, mu, forces, j2, r_eq, drag_cd, drag_area, drag_mass, integrator,
-                                 rtol, atol, device, &table);
+    az::NumArgs a{};
+    int32_t rc = forces_check(mu, forces, j2, r_eq, drag_cd, drag_area, drag_mass, &a.p);
+    if (rc == ASTROZ_OK) rc = numerical_check(n, t0, duration, dt, integrator, rtol, atol, device, &a);
     if (rc != ASTROZ_OK) return rc;
     if (n == 0) return ASTROZ_OK;
     if (!states || !out || !status) return ASTROZ_NULL_POINTER;
     if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
     const bool drag = (forces & az::kForceDrag) != 0;
     const double *cols[3] = {drag_cd, drag_area, drag_mass};
-    az::NumArgs a = numerical_args(n, table, mu, forces, j2, r_eq, rtol, atol);
-    return numerical_host_pipeline(
-        states, n, table, drag ? 3 : 0, cols, 0, nullptr, nullptr, device, out, status, steps,
-        [&](uint32_t m, const double *dStates, const double *const *dCols, const double *const *, double *dTraj,
-            uint8_t *dSt, uint64_t *dCounts, cudaStream_t s) {
-            a.n = m;
-            a.states = dStates;
-            a.cd = drag ? dCols[0] : nullptr;
-            a.area = drag ? dCols[1] : nullptr;
-            a.mass = drag ? dCols[2] : nullptr;
-            a.out = dTraj;
-            a.status = dSt;
-            a.counts = dCounts;
-            return az::launch_numerical(a, integrator, forces, s);
-        });
+    return numerical_host(a, states, drag ? 3 : 0, cols, 0, nullptr, 0, device, out, status, steps,
+                          [&](const double *const *dCols, const double *const *, cudaStream_t s) {
+                              a.cd = drag ? dCols[0] : nullptr;
+                              a.area = drag ? dCols[1] : nullptr;
+                              a.mass = drag ? dCols[2] : nullptr;
+                              return az::launch_numerical(a, integrator, forces, s);
+                          });
 }
 
 // ---- model lists (astroz_force_model_t) ----
@@ -2405,12 +2281,8 @@ static_assert(ASTROZ_MODEL_PER_STATE_C == az::kModelPerStateC && ASTROZ_MODEL_PE
 // Checks of a model list, before anything is read, written or allocated, and the list as the kernel reads it: each
 // model's pointers kept only where its flags name them.
 static int32_t models_check(const astroz_force_model_t *models, uint32_t nModels, az::ModelList *list) {
-    auto bad = [](const char *why) {
-        g_lastError = why;
-        return ASTROZ_VALUE_ERROR;
-    };
-    if (nModels == 0 || nModels > az::kMaxModels) return bad("a model list has 1 to 16 models");
-    if (!models) return bad("models is NULL");
+    if (nModels == 0 || nModels > az::kMaxModels) return value_error("a model list has 1 to 16 models");
+    if (!models) return value_error("models is NULL");
     *list = az::ModelList{};
     list->count = nModels;
     constexpr uint32_t kPerState = az::kModelPerStateC | az::kModelPerStateArea | az::kModelPerStateMass;
@@ -2435,16 +2307,16 @@ static int32_t models_check(const astroz_force_model_t *models, uint32_t nModels
             case az::kModelImprovedDrag: use({d.r_eq, d.max_altitude, d.f107}), allowed = kPerState; break;
             case az::kModelSrp: use({d.r_eq}), allowed = kPerState | az::kModelPosTable; break;
             case az::kModelThirdBody: use({d.mu}), allowed = az::kModelPosTable; break;
-            default: return bad("unknown model kind");
+            default: return value_error("unknown model kind");
         }
-        if (d.flags & ~allowed) return bad("a model flag its kind does not take");
+        if (d.flags & ~allowed) return value_error("a model flag its kind does not take");
         if (allowed & kPerState) {
             const double *arr[3] = {d.c_per_state, d.area_per_state, d.mass_per_state};
             const double sc[3] = {d.c, d.area, d.mass};
             const double **dst[3] = {&m.c_arr, &m.area_arr, &m.mass_arr};
             for (int q = 0; q < 3; ++q) {
                 if (d.flags & (az::kModelPerStateC << q)) {
-                    if (!arr[q]) return bad("a per-state flag is set and its array is NULL");
+                    if (!arr[q]) return value_error("a per-state flag is set and its array is NULL");
                     *dst[q] = arr[q];
                 } else {
                     use({sc[q]});
@@ -2453,14 +2325,14 @@ static int32_t models_check(const astroz_force_model_t *models, uint32_t nModels
         }
         if (allowed & az::kModelPosTable) {
             if (d.flags & az::kModelPosTable) {
-                if (!d.pos_table) return bad("ASTROZ_MODEL_POS_TABLE is set and pos_table is NULL");
+                if (!d.pos_table) return value_error("ASTROZ_MODEL_POS_TABLE is set and pos_table is NULL");
                 m.pos_table = d.pos_table;
             } else {
                 use({d.pos[0], d.pos[1], d.pos[2]});
             }
         }
         for (int q = 0; q < nUsed; ++q)
-            if (!std::isfinite(used[q])) return bad("a model's scalar parameter is not finite");
+            if (!std::isfinite(used[q])) return value_error("a model's scalar parameter is not finite");
     }
     return ASTROZ_OK;
 }
@@ -2470,18 +2342,14 @@ int32_t astroz_cuda_propagate_numerical_models_device(const double *d_states, ui
                                                       int32_t integrator, double rtol, double atol, int32_t device,
                                                       double *d_out, uint8_t *d_status, uint64_t *d_steps,
                                                       void *stream) {
-    az::StepTable table{};
     az::ModelArgs ma{};
     int32_t rc = models_check(models, n_models, &ma.models);
-    if (rc != ASTROZ_OK) return rc;
-    rc = numerical_check(n, t0, duration, dt, 0.0, 0, nullptr, nullptr, nullptr, nullptr, nullptr, integrator, rtol,
-                         atol, device, &table);
+    if (rc == ASTROZ_OK) rc = numerical_check(n, t0, duration, dt, integrator, rtol, atol, device, &ma.a);
     if (rc != ASTROZ_OK) return rc;
     if (n == 0) return ASTROZ_OK;
     if (!d_states || !d_out || !d_status) return ASTROZ_NULL_POINTER;
     if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
     AZ_CUDA(cudaSetDevice(device));
-    ma.a = numerical_args(n, table, 0.0, 0, nullptr, nullptr, rtol, atol);
     ma.a.states = d_states;
     ma.a.out = d_out;
     ma.a.status = d_status;
@@ -2495,12 +2363,9 @@ int32_t astroz_cuda_propagate_numerical_models(const double *states, uint32_t n,
                                                const astroz_force_model_t *models, uint32_t n_models,
                                                int32_t integrator, double rtol, double atol, int32_t device,
                                                double *out, uint8_t *status, uint64_t *steps) {
-    az::StepTable table{};
     az::ModelArgs ma{};
     int32_t rc = models_check(models, n_models, &ma.models);
-    if (rc != ASTROZ_OK) return rc;
-    rc = numerical_check(n, t0, duration, dt, 0.0, 0, nullptr, nullptr, nullptr, nullptr, nullptr, integrator, rtol,
-                         atol, device, &table);
+    if (rc == ASTROZ_OK) rc = numerical_check(n, t0, duration, dt, integrator, rtol, atol, device, &ma.a);
     if (rc != ASTROZ_OK) return rc;
     if (n == 0) return ASTROZ_OK;
     if (!states || !out || !status) return ASTROZ_NULL_POINTER;
@@ -2510,29 +2375,20 @@ int32_t astroz_cuda_propagate_numerical_models(const double *states, uint32_t n,
     const double **colOf[kNumMaxCols];
     const double *tabs[kNumMaxTabs];
     const double **tabOf[kNumMaxTabs];
-    size_t tabBytes[kNumMaxTabs];
     int nCols = 0, nTabs = 0;
-    const size_t K = (size_t)table.nFull + table.nTail;
     for (uint32_t j = 0; j < n_models; ++j) {
         az::ForceModel &m = ma.models.m[j];
         for (const double **p : {&m.c_arr, &m.area_arr, &m.mass_arr})
             if (*p) cols[nCols] = *p, colOf[nCols++] = p;
-        if (m.pos_table) tabs[nTabs] = m.pos_table, tabOf[nTabs] = &m.pos_table, tabBytes[nTabs++] = K * 24;
+        if (m.pos_table) tabs[nTabs] = m.pos_table, tabOf[nTabs++] = &m.pos_table;
     }
-    ma.a = numerical_args(n, table, 0.0, 0, nullptr, nullptr, rtol, atol);
-    return numerical_host_pipeline(
-        states, n, table, nCols, cols, nTabs, tabs, tabBytes, device, out, status, steps,
-        [&](uint32_t m, const double *dStates, const double *const *dCols, const double *const *dTabs, double *dTraj,
-            uint8_t *dSt, uint64_t *dCounts, cudaStream_t s) {
-            for (int q = 0; q < nCols; ++q) *colOf[q] = dCols[q];
-            for (int t = 0; t < nTabs; ++t) *tabOf[t] = dTabs[t];
-            ma.a.n = m;
-            ma.a.states = dStates;
-            ma.a.out = dTraj;
-            ma.a.status = dSt;
-            ma.a.counts = dCounts;
-            return az::launch_numerical_models(ma, integrator, s);
-        });
+    const size_t tabBytes = ((size_t)ma.a.steps.nFull + ma.a.steps.nTail) * 24;
+    return numerical_host(ma.a, states, nCols, cols, nTabs, tabs, tabBytes, device, out, status, steps,
+                          [&](const double *const *dCols, const double *const *dTabs, cudaStream_t s) {
+                              for (int q = 0; q < nCols; ++q) *colOf[q] = dCols[q];
+                              for (int t = 0; t < nTabs; ++t) *tabOf[t] = dTabs[t];
+                              return az::launch_numerical_models(ma, integrator, s);
+                          });
 }
 
 int32_t astroz_cuda_fp64_peak(int32_t device, double *tflops) {

@@ -1,4 +1,4 @@
-// az_hostcopy.cu -- the pinned ring and the host copy pool behind az_hostcopy.cuh.
+// az_hostcopy.cu -- the pinned ring, the host copy pool and the two-slot chunk pipeline behind az_hostcopy.cuh.
 #include "az_hostcopy.cuh"
 
 #include <algorithm>
@@ -9,6 +9,7 @@
 #include <cstring>
 #include <deque>
 #include <functional>
+#include <initializer_list>
 #include <mutex>
 #include <thread>
 
@@ -245,6 +246,93 @@ cudaError_t HostRing::upload(bool pageable, int nArrays, const void *const *src,
         if (e != cudaSuccess) return e;
     }
     return cudaSuccess;
+}
+
+#define AZ_TRY(expr) do { const cudaError_t e_ = (expr); if (e_ != cudaSuccess) return e_; } while (0)
+
+ChunkPipeline::~ChunkPipeline() {
+    for (cudaEvent_t e : {kernelDone[0], kernelDone[1], copyDone[0], copyDone[1], inputsDone})
+        if (e) cudaEventDestroy(e);
+}
+
+cudaError_t ChunkPipeline::create() {
+    for (cudaEvent_t *e : {&kernelDone[0], &kernelDone[1], &copyDone[0], &copyDone[1], &inputsDone})
+        if (!*e) AZ_TRY(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+    return cudaSuccess;
+}
+
+// Slot reuse.  Chunk k takes slot k % 2, which chunk k-2 used, so before chunk k's inputs go up the pipeline waits on
+// copyDone[slot], recorded on `copy` after chunk k-2's deliveries were queued.  For a pinned / registered destination
+// that event completes once the D2H copy has read the slot.  For a pageable one it does not cover the data: the
+// deliveries were only planned when it was recorded.  They were drained during chunk k-1, though (each chunk drains the
+// previous chunk's plan before queueing its own deliveries), and drain returns only when every planned piece is in its
+// final place, so chunk k-2's data has left the slot by then.  Uploads and deliveries share the ring's slots, and drain
+// fills them without waiting for an upload: before each drain the pipeline waits on inputsDone, this chunk's inputs
+// having left the ring.
+cudaError_t ChunkPipeline::run(cudaStream_t stream, cudaStream_t copy, uint32_t n, uint32_t chunk, int nIn,
+                               const HostIn *in, int nOut, const HostOut *out, void *dIn, void *dOut,
+                               const ChunkLaunch &launch) {
+    const uint32_t nChunks = (uint32_t)(((uint64_t)n + chunk - 1) / chunk), slots = nChunks > 1 ? 2 : 1;
+    // the bytes of one slot: what a single chunk needs
+    const size_t inSlot = chunk_slots_bytes(in, nIn, 1, chunk), outSlot = chunk_slots_bytes(out, nOut, 1, chunk);
+    std::vector<const void *> src(nIn);
+    std::vector<void *> dI(nIn), dO(nOut);
+    std::vector<size_t> inBytes(nIn);
+    std::vector<char> outPg(nOut);
+    bool inPageable = false, outPageable = false;
+    for (int a = 0; a < nIn; ++a) {
+        inPageable = inPageable || is_pageable(in[a].p);
+        inBytes[a] = in[a].bytes;
+    }
+    for (int j = 0; j < nOut; ++j) {
+        outPg[j] = out[j].p && is_pageable(out[j].p);
+        outPageable = outPageable || outPg[j];
+    }
+    auto chunks = [&]() -> cudaError_t {
+        for (uint32_t k = 0; k < nChunks; ++k) {
+            const uint32_t slot = k % slots, first = k * chunk, m = std::min(chunk, n - first);
+            char *at = static_cast<char *>(dIn) + slot * inSlot;
+            for (int a = 0; a < nIn; ++a) {
+                src[a] = static_cast<const char *>(in[a].p) + (size_t)first * in[a].bytes;
+                dI[a] = at;
+                at += chunk_col_bytes(chunk, in[a].bytes);
+            }
+            at = static_cast<char *>(dOut) + slot * outSlot;
+            for (int j = 0; j < nOut; ++j) {
+                dO[j] = out[j].p ? at : nullptr;
+                if (out[j].p) at += chunk_col_bytes(chunk, out[j].bytes);
+            }
+            if (k >= slots) AZ_TRY(cudaEventSynchronize(copyDone[slot]));  // chunk k-2's results have left this slot
+            AZ_TRY(ring.upload(inPageable, nIn, src.data(), dI.data(), inBytes.data(), m, stream));
+            AZ_TRY(cudaEventRecord(inputsDone, stream));
+            AZ_TRY(launch(k, first, m, dI.data(), dO.data(), stream));
+            const cudaEvent_t ready = kernelDone[slot];
+            AZ_TRY(cudaEventRecord(ready, stream));
+            if (outPageable) {  // chunk k-1's pageable results go through the ring while chunk k computes
+                AZ_TRY(cudaEventSynchronize(inputsDone));
+                AZ_TRY(ring.drain(copy));
+            }
+            AZ_TRY(cudaStreamWaitEvent(copy, ready, 0));
+            for (int j = 0; j < nOut; ++j) {
+                if (!out[j].p) continue;
+                char *dst = static_cast<char *>(out[j].p) + (size_t)first * out[j].bytes;
+                const size_t b = (size_t)m * out[j].bytes;
+                AZ_TRY(ring.deliver(outPg[j], ready, dO[j], dst, 1, b, b, copy));
+            }
+            AZ_TRY(cudaEventRecord(copyDone[slot], copy));
+        }
+        AZ_TRY(ring.drain(copy));
+        AZ_TRY(cudaStreamSynchronize(copy));
+        return cudaStreamSynchronize(stream);
+    };
+    ring.discard();
+    const cudaError_t e = chunks();
+    if (e != cudaSuccess) {  // nothing may write to the caller's memory, or read the slots, after the return
+        ring.discard();
+        cudaStreamSynchronize(copy);
+        cudaStreamSynchronize(stream);
+    }
+    return e;
 }
 
 }  // namespace az

@@ -2,12 +2,15 @@
 // az_capi.cu.  A DMA to or from PAGEABLE memory is staged by the driver through a small internal buffer, synchronously,
 // at a fraction of the PCIe rate.  Instead such transfers go through a ring of pinned slots owned by the handle
 // (full-rate DMA), and a small pool of host threads copies each piece between its slot and the caller's memory while
-// the next pieces are in flight.
+// the next pieces are in flight.  ChunkPipeline runs the host-buffer calls that cut their items into chunks over two
+// device slots.
 #pragma once
 
 #include <cuda_runtime.h>
 #include <stddef.h>
+#include <stdint.h>
 
+#include <functional>
 #include <vector>
 
 namespace az {
@@ -81,6 +84,50 @@ private:
     cudaEvent_t ev_[kSlots] = {};  // recorded after each slot's last transfer
     std::vector<Piece> plan_;
     size_t uploads_ = 0;  // granules staged so far: the next upload takes slot uploads_ % kSlots
+};
+
+// A host column of a chunked call: item i at p + i * bytes.  An output column with p = nullptr is not wanted: it takes
+// no device memory and its launch pointer is nullptr.
+struct HostIn { const void *p; size_t bytes; };
+struct HostOut { void *p; size_t bytes; };
+
+// Device bytes of one column of a chunk within its slot: the next column starts 16-byte aligned.
+inline size_t chunk_col_bytes(uint32_t chunk, size_t bytes) { return ((size_t)chunk * bytes + 15) & ~size_t(15); }
+// Device bytes ChunkPipeline::run needs for the columns of one side (HostIn or HostOut) over n items in chunks of
+// `chunk`: one slot, or two when n spans several chunks.
+template <class Col>
+size_t chunk_slots_bytes(const Col *cols, int nCols, uint32_t n, uint32_t chunk) {
+    size_t b = 0;
+    for (int k = 0; k < nCols; ++k)
+        if (cols[k].p) b += chunk_col_bytes(chunk, cols[k].bytes);
+    return (n > chunk ? 2 : 1) * b;
+}
+
+// launch(k, first, count, dIn, dOut, s) queues chunk k's work on s: items [first, first + count), with the device copy
+// of input column a at dIn[a] and output column j to be written at dOut[j].
+using ChunkLaunch = std::function<cudaError_t(uint32_t k, uint32_t first, uint32_t count, void *const *dIn,
+                                              void *const *dOut, cudaStream_t s)>;
+
+// The two-slot chunk pipeline of the host-buffer calls: n items are cut into chunks of `chunk` on two device slots.
+// Chunk k's inputs go up and its work runs on `stream` while chunk k-1's results leave on `copy` (pinned / registered
+// destinations) or through the ring and the copy pool (pageable ones); pageable inputs are staged through the ring too.
+// Not copyable (the ring is not).
+class ChunkPipeline {
+public:
+    ~ChunkPipeline();
+    cudaError_t create();  // the events, on the current device
+
+    // Run the chunks.  dIn / dOut are device memory of chunk_slots_bytes() for `in` / `out`.  Returns once every
+    // result is in place and both streams are idle -- also on failure, when the ring's plan is forgotten first, so no
+    // copy into the caller's memory is still queued after the call returns.
+    cudaError_t run(cudaStream_t stream, cudaStream_t copy, uint32_t n, uint32_t chunk, int nIn, const HostIn *in,
+                    int nOut, const HostOut *out, void *dIn, void *dOut, const ChunkLaunch &launch);
+
+    HostRing ring;  // pinned transfers from / to pageable caller memory (also used outside run)
+
+private:
+    // slot k's work / result copy has finished; the current chunk's inputs are on the device
+    cudaEvent_t kernelDone[2] = {}, copyDone[2] = {}, inputsDone = nullptr;
 };
 
 }  // namespace az
