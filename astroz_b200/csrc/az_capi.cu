@@ -25,6 +25,7 @@
 #include <thread>
 #include <vector>
 
+#include "az_fit.cuh"
 #include "az_hostcopy.cuh"
 #include "az_ingest.cuh"
 #include "az_kernels.cuh"
@@ -2389,6 +2390,145 @@ int32_t astroz_cuda_propagate_numerical_models(const double *states, uint32_t n,
                               for (int t = 0; t < nTabs; ++t) *tabOf[t] = dTabs[t];
                               return az::launch_numerical_models(ma, integrator, s);
                           });
+}
+
+// ---- element fits (K8, az_fit.cu) ------------------------------------------------------------------------------------
+static_assert(ASTROZ_FIT_CONVERGED == az::kFitConverged && ASTROZ_FIT_ITERATION_LIMIT == az::kFitIterLimit &&
+                  ASTROZ_FIT_INIT_FAILED == az::kFitInitFailed && ASTROZ_FIT_DEEP_SPACE == az::kFitDeepSpace &&
+                  ASTROZ_FIT_TOO_FEW_OBSERVATIONS == az::kFitTooFew,
+              "fit status bytes");
+
+// Scalar checks of both fit calls, before anything is read, written or allocated; a receives the scalars.
+static int32_t fit_check(uint32_t n, int32_t grav, double pos_sigma, double vel_sigma, int32_t fit_bstar,
+                         uint32_t max_iter, int32_t device, az::FitArgs *a) {
+    if (device < 0) return value_error("an element fit runs on one device: pass its ordinal");
+    if (grav != ASTROZ_WGS72 && grav != ASTROZ_WGS84) return value_error("grav must be ASTROZ_WGS72 or ASTROZ_WGS84");
+    if (!std::isfinite(pos_sigma) || !(pos_sigma > 0.0) || !std::isfinite(vel_sigma) || !(vel_sigma > 0.0))
+        return value_error("pos_sigma and vel_sigma must be finite and > 0");
+    if (max_iter == 0) return value_error("max_iter must be at least 1");
+    a->n = n;
+    a->grav = grav;
+    a->g = az::grav_consts(az::gravity(grav));
+    a->wp = 1.0 / pos_sigma;
+    a->wv = 1.0 / vel_sigma;
+    a->fitBstar = fit_bstar != 0;
+    a->maxIter = max_iter;
+    return ASTROZ_OK;
+}
+
+static bool all_finite(const double *p, size_t count) {
+    for (size_t i = 0; i < count; ++i)
+        if (!std::isfinite(p[i])) return false;
+    return true;
+}
+
+int32_t astroz_cuda_fit_elements_device(const double *d_elements, uint32_t n, int32_t grav, const uint32_t *d_offsets,
+                                        const double *d_jd, const double *d_fr, const double *d_pos,
+                                        const double *d_vel, double pos_sigma, double vel_sigma, int32_t fit_bstar,
+                                        uint32_t max_iter, int32_t device, double *d_fitted, double *d_rms,
+                                        uint32_t *d_iterations, uint8_t *d_status, void *stream) {
+    az::FitArgs a{};
+    int32_t rc = fit_check(n, grav, pos_sigma, vel_sigma, fit_bstar, max_iter, device, &a);
+    if (rc != ASTROZ_OK) return rc;
+    if (n == 0) return ASTROZ_OK;
+    if (!d_elements || !d_offsets || !d_jd || !d_fr || !d_pos || !d_fitted || !d_rms || !d_iterations || !d_status)
+        return ASTROZ_NULL_POINTER;
+    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
+    AZ_CUDA(cudaSetDevice(device));
+    a.elements = d_elements;
+    a.offsets = d_offsets;
+    a.jd = d_jd;
+    a.fr = d_fr;
+    a.pos = d_pos;
+    a.vel = d_vel;
+    a.fitted = d_fitted;
+    a.rms = d_rms;
+    a.iterations = d_iterations;
+    a.status = d_status;
+    AZ_CUDA(az::launch_fit(a, static_cast<cudaStream_t>(stream)));
+    return ASTROZ_OK;
+}
+
+// Host buffers: a fit is compute-bound (each observation is propagated some 8 x iterations times for its ~56 bytes),
+// so the whole batch goes up at once -- pageable arrays through the device's pinned ring, pinned ones by direct DMA --
+// and one launch fits it.  The results (~90 bytes per satellite) come back by plain copies.
+int32_t astroz_cuda_fit_elements(const double *elements, uint32_t n, int32_t grav, const uint32_t *offsets,
+                                 const double *jd, const double *fr, const double *pos, const double *vel, uint32_t m,
+                                 double pos_sigma, double vel_sigma, int32_t fit_bstar, uint32_t max_iter,
+                                 int32_t device, double *fitted, double *rms, uint32_t *iterations, uint8_t *status) {
+    az::FitArgs a{};
+    int32_t rc = fit_check(n, grav, pos_sigma, vel_sigma, fit_bstar, max_iter, device, &a);
+    if (rc != ASTROZ_OK) return rc;
+    if (n == 0) return ASTROZ_OK;
+    if (!elements || !offsets || !fitted || !rms || !iterations || !status) return ASTROZ_NULL_POINTER;
+    if (m && (!jd || !fr || !pos)) return ASTROZ_NULL_POINTER;
+    for (uint32_t s = 0; s < n; ++s)
+        if (offsets[s + 1] < offsets[s]) return value_error("offsets must be non-decreasing");
+    if (offsets[n] != m) return value_error("offsets[n] must equal the observation count m");
+    if (!all_finite(elements, (size_t)8 * n) || !all_finite(jd, m) || !all_finite(fr, m) ||
+        !all_finite(pos, (size_t)3 * m) || (vel && !all_finite(vel, (size_t)3 * m)))
+        return value_error("elements and observations must be finite");
+    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
+    NumericalContext *c = nullptr;
+    if ((rc = numerical_context(device, &c)) != ASTROZ_OK) return rc;
+    std::lock_guard<std::mutex> lk(c->m);
+    AZ_CUDA(cudaSetDevice(device));
+    cudaStream_t st = c->stream;
+    // one device block: elements | fitted | rms | jd | fr | pos | vel | offsets | iterations | status
+    const size_t nObs = std::max<uint32_t>(m, 1);
+    const size_t words[] = {(size_t)8 * n, (size_t)8 * n, (size_t)2 * n, nObs, nObs, 3 * nObs, vel ? 3 * nObs : 0};
+    size_t at[7], total = 0;
+    for (int k = 0; k < 7; ++k) at[k] = total, total += (words[k] * 8 + 15) & ~size_t(15);
+    const size_t offAt = total;
+    total += ((size_t)(n + 1) * 4 + 15) & ~size_t(15);
+    const size_t iterAt = total;
+    total += ((size_t)n * 4 + 15) & ~size_t(15);
+    const size_t statusAt = total;
+    total += n;
+    StreamBuf dBuf(st);
+    AZ_CUDA(dBuf.alloc(total));
+    char *base = static_cast<char *>(dBuf.p);
+    auto dp = [&](int k) { return reinterpret_cast<double *>(base + at[k]); };
+    auto up = [&](const void *src, void *dst, size_t elemBytes, size_t count) {
+        void *const d[1] = {dst};
+        const void *const s[1] = {src};
+        return c->pipe.ring.upload(az::is_pageable(src), 1, s, d, &elemBytes, count, st);
+    };
+    AZ_CUDA(up(elements, dp(0), 8, (size_t)8 * n));
+    AZ_CUDA(up(offsets, base + offAt, 4, (size_t)n + 1));
+    if (m) {
+        AZ_CUDA(up(jd, dp(3), 8, m));
+        AZ_CUDA(up(fr, dp(4), 8, m));
+        AZ_CUDA(up(pos, dp(5), 24, m));
+        if (vel) AZ_CUDA(up(vel, dp(6), 24, m));
+    }
+    a.elements = dp(0);
+    a.offsets = reinterpret_cast<const uint32_t *>(base + offAt);
+    a.jd = dp(3);
+    a.fr = dp(4);
+    a.pos = dp(5);
+    a.vel = vel ? dp(6) : nullptr;
+    a.fitted = dp(1);
+    a.rms = dp(2);
+    a.iterations = reinterpret_cast<uint32_t *>(base + iterAt);
+    a.status = reinterpret_cast<uint8_t *>(base + statusAt);
+    AZ_CUDA(az::launch_fit(a, st));
+    AZ_CUDA(cudaMemcpyAsync(fitted, a.fitted, (size_t)8 * n * 8, cudaMemcpyDeviceToHost, st));
+    AZ_CUDA(cudaMemcpyAsync(rms, a.rms, (size_t)2 * n * 8, cudaMemcpyDeviceToHost, st));
+    AZ_CUDA(cudaMemcpyAsync(iterations, a.iterations, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
+    AZ_CUDA(cudaMemcpyAsync(status, a.status, n, cudaMemcpyDeviceToHost, st));
+    AZ_CUDA(dBuf.release());
+    AZ_CUDA(cudaStreamSynchronize(st));
+    return ASTROZ_OK;
+}
+
+int32_t astroz_cuda_parse_tle(const char *line1, const char *line2, double *elements) {
+    if (!line1 || !line2 || !elements) return ASTROZ_NULL_POINTER;
+    az::TleRecord t;
+    if (az::parse_tle(line1, line2, t) != az::kOk) return ASTROZ_BAD_TLE_LENGTH;
+    const double cols[8] = {t.epochJd, t.revPerDay, t.ecc, t.inclDeg, t.raanDeg, t.argpDeg, t.maDeg, t.bstar};
+    std::memcpy(elements, cols, sizeof cols);
+    return ASTROZ_OK;
 }
 
 int32_t astroz_cuda_fp64_peak(int32_t device, double *tflops) {

@@ -1,0 +1,292 @@
+// az_fit.cuh -- K8: least-squares fit of SGP4 mean elements to TEME ephemerides, one satellite at a time.
+// __host__ __device__, so the kernel (az_fit.cu) and the host emulation (tests/host_emul/emul_fit.cu) run this source.
+//
+// The model is the library's near-earth path: a trial element set goes through build_near_earth and sgp4_columns, the
+// way every near-earth table is built, and is propagated by sgp4_cell<1> at tsince = ((jd + fr) - epoch) * 1440,
+// formed uncontracted like K6 and Satrec.sgp4.  Seven variables, six when B* is held:
+//   x = [n (rev/day), e cos w, e sin w, i (rad), node (rad), lambda = M + w (rad), B* (1/ER)]
+// The pairs (e cos w, e sin w) and lambda stay well conditioned as e -> 0, where (w, M) alone do not.  Levenberg-
+// Marquardt over the weighted residuals (pos / pos_sigma, vel / vel_sigma): forward-difference Jacobian with the steps
+// of fit_step(), Marquardt damping lambda diag(J^T J), the normal equations solved by Cholesky on their unit-diagonal
+// scaling, lambda / 10 after an accepted step and x 10 after a rejected one.
+#pragma once
+
+#include "az_pairs.cuh"
+#include "az_tables.hpp"
+
+namespace az {
+
+// per-satellite status bytes (ASTROZ_FIT_*)
+enum FitStatus : uint8_t { kFitConverged = 0, kFitIterLimit = 1, kFitInitFailed = 2, kFitDeepSpace = 3, kFitTooFew = 4 };
+
+constexpr int kFitVars = 7;              // variables with B* free
+constexpr int kFitSets = 1 + kFitVars;   // nominal set + one perturbed set per variable
+constexpr int kFitN = kFitVars * (kFitVars + 1) / 2;  // J^T J upper triangle, row-major
+constexpr double kFitTol = 1e-10;        // the fit stops when a step changes the cost by at most this fraction of it
+constexpr double kFitNoise = 1e-12;      // ... or when every residual is at the rounding floor: kFitNoise x |state|
+constexpr double kFitLambda0 = 1e-3;     // initial Marquardt damping
+
+// Forward-difference step of variable j: 1e-8 rev/day, 1e-8 on e cos w / e sin w, 1e-8 rad on the angles, 1e-8 / ER
+// on B*.  Each moves a LEO position by 1e-4 .. 1e-3 km over a day: some 1e8 times the propagation's rounding, and small
+// enough that the truncation error of the difference (~ step / value) stays below 1e-8 of the column.  When the
+// forward set is not a near-earth element set (the period would cross 225 min, the perigee 1 earth radius) the
+// backward step is taken instead.
+AZ_HD double fit_step(int) { return 1e-8; }
+
+struct FitSums {             // one pass over a satellite's observations under the nominal set and its perturbations
+    double F;                // weighted cost: sum of r^2, r = (observed - model) / sigma
+    double pos2, vel2;       // unweighted sums of |dr|^2 [km^2] and |dv|^2 [km^2/s^2]
+    double floor;            // kFitNoise^2 sum of (|r_obs| / pos_sigma)^2 + (|v_obs| / vel_sigma)^2: the rounding floor of F
+    double N[kFitN];         // J^T J, J = d(model)/dx weighted
+    double g[kFitVars];      // J^T r
+};
+constexpr int kFitSumWords = 4 + kFitN + kFitVars;
+
+AZ_HD double *fit_words(FitSums &s) { return &s.F; }
+static_assert(sizeof(FitSums) == kFitSumWords * sizeof(double), "FitSums is a flat array of doubles");
+
+AZ_HD int fit_tri(int j, int k) { return j * kFitVars - j * (j - 1) / 2 + (k - j); }  // entry (j, k), j <= k
+
+// Variables -> the eight element columns (epoch, n, e, i, node, w, M in degrees, B*): w = atan2(e sin w, e cos w) and
+// M = lambda - w, node, w and M reduced to [0, 360).  The fit's output is this conversion of its final iterate.
+AZ_HD void fit_elements_of(const double (&x)[kFitVars], double epochJd, TleRecord &t) {
+    using detail::kDeg;
+    const double r2d = 1.0 / kDeg;
+    t = TleRecord{};
+    t.epochJd = epochJd;
+    t.revPerDay = x[0];
+    t.ecc = std::sqrt(x[1] * x[1] + x[2] * x[2]);
+    const double w = std::atan2(x[2], x[1]);
+    t.argpDeg = detail::wrap(w * r2d, 360.0);
+    t.inclDeg = x[3] * r2d;
+    t.raanDeg = detail::wrap(x[4] * r2d, 360.0);
+    t.maDeg = detail::wrap((x[5] - w) * r2d, 360.0);
+    t.bstar = x[6];
+}
+
+// el[c] = column c of the element set (epoch JD, n rev/day, e, i, node, w, M deg, B*) -> variables
+AZ_HD void fit_vars_of(const double *el, double (&x)[kFitVars]) {
+    using detail::kDeg;
+    const double w = el[5] * kDeg;
+    x[0] = el[1];
+    x[1] = el[2] * std::cos(w);
+    x[2] = el[2] * std::sin(w);
+    x[3] = el[3] * kDeg;
+    x[4] = el[4] * kDeg;
+    x[5] = el[6] * kDeg + w;
+    x[6] = el[7];
+}
+
+AZ_HD int fit_columns(const TleRecord &t, const Gravity &grav, double *cols) {
+    NearEarth ne;
+    const int rc = build_near_earth(t, grav, ne);
+    if (rc == kOk) sgp4_columns(ne, cols);
+    return rc;
+}
+
+// Set k of an iteration into cols[kSgp4Cols]: k = 0 the nominal set x, k = 1 + j the set with variable j stepped
+// (forward, or backward when the forward set is not near-earth).  inv[0] = 0, inv[k] = 1 / (the step actually taken,
+// x'[j] - x[j] in fp64).  Returns false when the set cannot be built.
+AZ_HD bool fit_build_set(const double (&x)[kFitVars], int k, double epochJd, const Gravity &grav, double *cols,
+                                double &inv) {
+    TleRecord t;
+    inv = 0.0;
+    if (k == 0) {
+        fit_elements_of(x, epochJd, t);
+        return fit_columns(t, grav, cols) == kOk;
+    }
+    const int j = k - 1;
+    double xs[kFitVars];
+    for (int q = 0; q < kFitVars; ++q) xs[q] = x[q];
+    for (int dir = 0; dir < 2; ++dir) {
+        xs[j] = dir == 0 ? x[j] + fit_step(j) : x[j] - fit_step(j);
+        fit_elements_of(xs, epochJd, t);
+        if (fit_columns(t, grav, cols) == kOk) {
+            inv = 1.0 / (xs[j] - x[j]);
+            return true;
+        }
+    }
+    return false;
+}
+
+// One observation's contribution to s: the model under set 0 and under sets 1..nvar (set(k) = column accessor of set
+// k), the weighted residual and the difference columns of the Jacobian.  J is scratch for the 6 x nvar Jacobian of
+// this observation, entry (j, c) at J[(j * 6 + c) * stride]; word q of the FitSums being accumulated is
+// acc[q * stride].  vel = nullptr: positions only.
+template <typename SetFn>
+AZ_HD void fit_accumulate(SetFn set, int nvar, const double *inv, double jdFull, double epochJd, const double *pos,
+                          const double *vel, double wp, double wv, const GravConsts &g, double *J, double *acc,
+                          int stride) {
+    const double ts[1] = {mul_rn(sub_rn(jdFull, epochJd), 1440.0)};
+    const int nc = vel ? 6 : 3;
+    double obs[6], w[6], f0[6];
+    for (int c = 0; c < 3; ++c) {
+        obs[c] = pos[c];
+        w[c] = wp;
+        obs[3 + c] = vel ? vel[c] : 0.0;
+        w[3 + c] = wv;
+    }
+    {
+        CellOut o[1];
+        sgp4_cell<1>(set(0), ts, g, o);
+        f0[0] = o[0].rx; f0[1] = o[0].ry; f0[2] = o[0].rz;
+        f0[3] = o[0].vx; f0[4] = o[0].vy; f0[5] = o[0].vz;
+    }
+    double r[6];
+    for (int c = 0; c < 6; ++c) r[c] = c < nc ? (obs[c] - f0[c]) * w[c] : 0.0;
+    {
+        double F = acc[0], pos2 = acc[stride], vel2 = acc[2 * stride], fl = acc[3 * stride];
+        for (int c = 0; c < 3; ++c) {
+            const double dp = obs[c] - f0[c], dv = obs[3 + c] - f0[3 + c];
+            pos2 += dp * dp;
+            if (vel) vel2 += dv * dv;
+            F += r[c] * r[c];
+            if (vel) F += r[3 + c] * r[3 + c];
+            const double fp = obs[c] * wp * kFitNoise, fv = obs[3 + c] * wv * kFitNoise;
+            fl += fp * fp;
+            if (vel) fl += fv * fv;
+        }
+        acc[0] = F;
+        acc[stride] = pos2;
+        acc[2 * stride] = vel2;
+        acc[3 * stride] = fl;
+    }
+#ifdef __CUDA_ARCH__
+#pragma unroll 1
+#endif
+    for (int j = 0; j < nvar; ++j) {
+        CellOut o[1];
+        sgp4_cell<1>(set(1 + j), ts, g, o);
+        const double f[6] = {o[0].rx, o[0].ry, o[0].rz, o[0].vx, o[0].vy, o[0].vz};
+        for (int c = 0; c < 6; ++c) J[(j * 6 + c) * stride] = c < nc ? (f[c] - f0[c]) * w[c] * inv[1 + j] : 0.0;
+    }
+    // all kFitVars columns, the held B* column as zeros, so the sums keep static indices (registers on the device)
+#pragma unroll
+    for (int j = 0; j < kFitVars; ++j) {
+        double jc[6];
+#pragma unroll
+        for (int c = 0; c < 6; ++c) jc[c] = j < nvar ? J[(j * 6 + c) * stride] : 0.0;
+        double gj = 0.0;
+#pragma unroll
+        for (int c = 0; c < 6; ++c) gj += jc[c] * r[c];
+        acc[(4 + kFitN + j) * stride] += gj;
+#pragma unroll
+        for (int k = j; k < kFitVars; ++k) {
+            double njk = 0.0;
+#pragma unroll
+            for (int c = 0; c < 6; ++c) njk += jc[c] * (k < nvar ? J[(k * 6 + c) * stride] : 0.0);
+            acc[(4 + fit_tri(j, k)) * stride] += njk;
+        }
+    }
+}
+
+// Solve (N + lambda diag N) d = g for the nvar variables, on the unit-diagonal scaling of N (a variable whose column
+// is zero gets d = 0).  Returns false when the Cholesky factorisation meets a pivot that is not positive and finite.
+AZ_HD bool fit_solve(const FitSums &s, int nvar, double lambda, double (&d)[kFitVars]) {
+    double sc[kFitVars], L[kFitVars][kFitVars], y[kFitVars];
+    for (int j = 0; j < kFitVars; ++j) {
+        const double njj = j < nvar ? s.N[fit_tri(j, j)] : 0.0;
+        sc[j] = njj > 0.0 ? 1.0 / std::sqrt(njj) : 0.0;
+        d[j] = 0.0;
+    }
+    for (int j = 0; j < nvar; ++j) {
+        for (int k = 0; k <= j; ++k) {
+            double a = (k == j) ? (sc[j] > 0.0 ? 1.0 + lambda : 1.0) : s.N[fit_tri(k, j)] * sc[j] * sc[k];
+            for (int q = 0; q < k; ++q) a -= L[j][q] * L[k][q];
+            if (k == j) {
+                if (!(a > 0.0) || !(a < INFINITY)) return false;
+                L[j][j] = std::sqrt(a);
+            } else {
+                L[j][k] = a / L[k][k];
+            }
+        }
+    }
+    for (int j = 0; j < nvar; ++j) {
+        double b = s.g[j] * sc[j];
+        for (int q = 0; q < j; ++q) b -= L[j][q] * y[q];
+        y[j] = b / L[j][j];
+    }
+    for (int j = nvar - 1; j >= 0; --j) {
+        double b = y[j];
+        for (int q = j + 1; q < nvar; ++q) b -= L[q][j] * d[q];
+        d[j] = b / L[j][j];
+    }
+    for (int j = 0; j < nvar; ++j) d[j] *= sc[j];
+    return true;
+}
+
+struct FitResult {
+    double el[8];            // fitted columns (epoch, n, e, i, node, w, M, B*)
+    double rmsPos, rmsVel;   // sqrt(mean |dr|^2) [km], sqrt(mean |dv|^2) [km/s] (0 without velocities)
+    uint32_t iters;          // LM steps tried (accepted or rejected)
+    uint8_t status;
+};
+
+// The whole fit of one satellite.  pass(x, s) evaluates the nominal set x and its nvar perturbed sets over the
+// satellite's nObs observations into s (zeroed by the caller) and returns false when a set cannot be built; it must
+// return the same bits wherever it is called for the same x.  Failing satellites (init, deep space, too few
+// observations) return their initial columns with zero RMS and no iterations.
+template <typename PassFn>
+AZ_HD void fit_satellite(const double *el0, const Gravity &grav, bool fitBstar, uint32_t maxIter, uint32_t nObs,
+                         bool haveVel, PassFn pass, FitResult &out) {
+    const int nvar = fitBstar ? kFitVars : kFitVars - 1;
+    for (int c = 0; c < 8; ++c) out.el[c] = el0[c];
+    out.rmsPos = out.rmsVel = 0.0;
+    out.iters = 0;
+    {
+        TleRecord t;
+        t.epochJd = el0[0]; t.revPerDay = el0[1]; t.ecc = el0[2]; t.inclDeg = el0[3];
+        t.raanDeg = el0[4]; t.argpDeg = el0[5]; t.maDeg = el0[6]; t.bstar = el0[7];
+        NearEarth ne;
+        const int rc = build_near_earth(t, grav, ne);
+        if (rc != kOk) {
+            out.status = rc == kDeepSpace ? kFitDeepSpace : kFitInitFailed;
+            return;
+        }
+    }
+    if ((uint64_t)nObs * (haveVel ? 6 : 3) < (uint64_t)nvar) {
+        out.status = kFitTooFew;
+        return;
+    }
+    double x[kFitVars];
+    fit_vars_of(el0, x);
+    FitSums s = {};
+    if (!pass(x, s)) {
+        out.status = kFitInitFailed;
+        return;
+    }
+    uint8_t status = kFitIterLimit;
+    double lambda = kFitLambda0;
+    uint32_t it = 0;
+    if (s.F <= s.floor) status = kFitConverged;
+    while (status != kFitConverged && it < maxIter) {
+        ++it;
+        double d[kFitVars], xt[kFitVars];
+        FitSums t = {};
+        bool ok = fit_solve(s, nvar, lambda, d);
+        if (ok) {
+            for (int j = 0; j < kFitVars; ++j) xt[j] = x[j] + d[j];
+            ok = pass(xt, t);
+        }
+        if (!ok || !(t.F < s.F)) {   // rejected (also a non-finite cost)
+            if (ok && t.F - s.F <= kFitTol * s.F) status = kFitConverged;
+            lambda *= 10.0;
+            continue;
+        }
+        const bool small = s.F - t.F <= kFitTol * s.F;
+        for (int j = 0; j < kFitVars; ++j) x[j] = xt[j];
+        s = t;
+        lambda *= 0.1;
+        if (small || s.F <= s.floor) status = kFitConverged;
+    }
+    TleRecord t;
+    fit_elements_of(x, el0[0], t);
+    out.el[0] = t.epochJd; out.el[1] = t.revPerDay; out.el[2] = t.ecc; out.el[3] = t.inclDeg;
+    out.el[4] = t.raanDeg; out.el[5] = t.argpDeg; out.el[6] = t.maDeg; out.el[7] = t.bstar;
+    out.rmsPos = std::sqrt(s.pos2 / nObs);
+    out.rmsVel = haveVel ? std::sqrt(s.vel2 / nObs) : 0.0;
+    out.iters = it;
+    out.status = status;
+}
+
+}  // namespace az

@@ -128,6 +128,27 @@ cudaError_t pairs_sort_scratch_bytes(uint32_t n, uint32_t nRows, size_t *bytes);
 cudaError_t launch_pairs_range(const double *jd, const double *fr, uint32_t n, double *scratch, cudaStream_t stream);
 size_t pairs_range_scratch_doubles();
 
+// K8: fit SGP4 mean elements to TEME ephemerides, one warp per satellite (az_fit.cu, az_fit.cuh).  All pointers are
+// device pointers.
+struct FitArgs {
+    const double *elements = nullptr;    // [8][n] initial columns: epoch JD, n rev/day, e, i, node, w, M deg, B*
+    uint32_t n = 0;
+    const uint32_t *offsets = nullptr;   // [n + 1]: satellite s owns observations [offsets[s], offsets[s + 1])
+    const double *jd = nullptr, *fr = nullptr;
+    const double *pos = nullptr;         // [m][3] TEME km
+    const double *vel = nullptr;         // [m][3] TEME km/s, nullable
+    double wp = 1.0, wv = 1.0;           // 1 / pos_sigma, 1 / vel_sigma
+    int fitBstar = 1;
+    uint32_t maxIter = 25;
+    int grav = 1;                        // ASTROZ_WGS72 / ASTROZ_WGS84
+    GravConsts g{};
+    double *fitted = nullptr;            // [8][n]
+    double *rms = nullptr;               // [n][2]: position km, velocity km/s
+    uint32_t *iterations = nullptr;      // [n]
+    uint8_t *status = nullptr;           // [n] ASTROZ_FIT_*
+};
+cudaError_t launch_fit(const FitArgs &a, cudaStream_t stream);
+
 // DFMA throughput microbenchmark: returns achieved fp64 FLOP/s (FMA = 2).
 cudaError_t measure_fp64_peak(double *flops);
 // Arithmetic peak of the fp64 pipe: SMs x 64 lanes x 2 FLOP x the maximum SM clock.

@@ -65,6 +65,23 @@ def _implied_decimal(x: float) -> str:
     return f"{'-' if x < 0 else ' '}{digits:05d}{exp:+d}"
 
 
+def tle_line_pair(norad: int, year: int, doy: float, incl: float, raan: float, ecc: float, argp: float, ma: float,
+                  mean_motion: float, bstar: float, *, classification: str = "U", designator: str = "00000A  ",
+                  ndot: float = 0.0, nddot: float = 0.0, ephemeris_type: int = 0, element_set_no: int = 0,
+                  rev_at_epoch: int = 0) -> tuple[str, str]:
+    """One element set as a checksummed TLE line pair, with TLE column precision (angles in degrees, day of year from
+    1.0 at Jan 1 00:00, B* in 1 / earth radii)."""
+    ndot_txt = ("-" if ndot < 0 else " ") + f"{abs(ndot):.8f}"[1:]
+    head = (f"1 {norad:05d}{classification} {designator} {year % 100:02d}{doy:012.8f} {ndot_txt} "
+            f"{_implied_decimal(nddot)} {_implied_decimal(bstar)} {ephemeris_type} {element_set_no:4d}")
+    head = head[:68].ljust(68)
+    ecc_txt = f"{ecc:.7f}"[2:]
+    tail = (f"2 {norad:05d} {incl:8.4f} {raan:8.4f} {ecc_txt} {argp:8.4f} {ma:8.4f} {mean_motion:11.8f}"
+            f"{rev_at_epoch:5d}")
+    tail = tail[:68].ljust(68)
+    return head + _checksum(head), tail + _checksum(tail)
+
+
 def omm_to_tle_pairs(json_text: str) -> list[tuple[str, str]]:
     """OMM JSON (one record or an array) rendered as TLE line pairs, with TLE column precision -- the reference
     converts OMM input the same way before initialising (__init__.py:203-279), so an OMM catalogue propagates to
@@ -83,18 +100,12 @@ def omm_to_tle_pairs(json_text: str) -> list[tuple[str, str]]:
             designator = f"{obj:<8s}"
         when = datetime.fromisoformat(rec["EPOCH"]).replace(tzinfo=None)
         doy = (when - datetime(when.year, 1, 1)).total_seconds() / 86400.0 + 1.0
-        ndot = rec.get("MEAN_MOTION_DOT") or 0
-        ndot_txt = ("-" if ndot < 0 else " ") + f"{abs(ndot):.8f}"[1:]
-        head = (f"1 {norad:05d}{cls} {designator} {when.year % 100:02d}{doy:012.8f} {ndot_txt} "
-                f"{_implied_decimal(rec.get('MEAN_MOTION_DDOT') or 0)} {_implied_decimal(rec['BSTAR'])} "
-                f"{rec.get('EPHEMERIS_TYPE') or 0} {rec.get('ELEMENT_SET_NO') or 0:4d}")
-        head = head[:68].ljust(68)
-        ecc_txt = f"{rec['ECCENTRICITY']:.7f}"[2:]
-        tail = (f"2 {norad:05d} {rec['INCLINATION']:8.4f} {rec['RA_OF_ASC_NODE']:8.4f} {ecc_txt} "
-                f"{rec['ARG_OF_PERICENTER']:8.4f} {rec['MEAN_ANOMALY']:8.4f} {rec['MEAN_MOTION']:11.8f}"
-                f"{rec.get('REV_AT_EPOCH') or 0:5d}")
-        tail = tail[:68].ljust(68)
-        pairs.append((head + _checksum(head), tail + _checksum(tail)))
+        pairs.append(tle_line_pair(
+            norad, when.year, doy, rec["INCLINATION"], rec["RA_OF_ASC_NODE"], rec["ECCENTRICITY"],
+            rec["ARG_OF_PERICENTER"], rec["MEAN_ANOMALY"], rec["MEAN_MOTION"], rec["BSTAR"], classification=cls,
+            designator=designator, ndot=rec.get("MEAN_MOTION_DOT") or 0, nddot=rec.get("MEAN_MOTION_DDOT") or 0,
+            ephemeris_type=rec.get("EPHEMERIS_TYPE") or 0, element_set_no=rec.get("ELEMENT_SET_NO") or 0,
+            rev_at_epoch=rec.get("REV_AT_EPOCH") or 0))
     return pairs
 
 

@@ -371,6 +371,12 @@ int32_t astroz_cuda_constellation_propagate_device_f32(astroz_constellation_t h,
 #define ASTROZ_NUMERICAL_SUBSTEP_LIMIT 2   /* some DP87 interval hit 10,000 substeps: that sample is the reference's, not
                                               at its nominal time */
 #define ASTROZ_NUMERICAL_NON_FINITE    3   /* an RK4 trajectory went to NaN or inf (the values are kept) */
+/* per-satellite status bytes of the element fits (astroz_cuda_fit_elements below) */
+#define ASTROZ_FIT_CONVERGED            0   /* the cost stopped changing, or reached the rounding floor */
+#define ASTROZ_FIT_ITERATION_LIMIT      1   /* max_iter steps tried: the best accepted iterate is returned */
+#define ASTROZ_FIT_INIT_FAILED          2   /* the initial set fails SGP4 init (e outside [0, 1), perigee below 1 ER) */
+#define ASTROZ_FIT_DEEP_SPACE           3   /* period > 225 min: deep-space sets are not fitted */
+#define ASTROZ_FIT_TOO_FEW_OBSERVATIONS 4   /* fewer scalar residuals than fitted variables */
 
 /* The sample times of the batch calls (Propagator.zig:32-45 evaluated on the host, the one home of the sampling rule):
  * *count = number of samples; times (nullable) receives them.  Same argument errors as the batch calls. */
@@ -469,6 +475,43 @@ int32_t astroz_cuda_propagate_numerical_models_device(const double *d_states, ui
                                                       int32_t integrator, double rtol, double atol, int32_t device,
                                                       double *d_out, uint8_t *d_status, uint64_t *d_steps,
                                                       void *stream);
+
+/* ---- element fits (K8): SGP4 mean elements from TEME ephemerides ------------------------------------------------------
+ * For each satellite s of a batch, Levenberg-Marquardt finds the near-earth mean elements whose SGP4 states best match
+ * its observations in the weighted least-squares sense, residuals (pos - model) / pos_sigma and (vel - model) / vel_sigma.
+ *   elements[8][n]: initial columns as astroz_cuda_constellation_create_from_elements takes them -- epoch JD, mean motion
+ *            [rev/day], eccentricity, inclination, RAAN, argument of perigee, mean anomaly [deg], B*; grav ASTROZ_WGS72 or
+ *            ASTROZ_WGS84.  The epoch is held: the fitted elements are mean elements at that epoch;
+ *   observations: satellite s owns [offsets[s], offsets[s + 1]) of jd[m], fr[m], pos[m][3] (TEME km) and vel[m][3]
+ *            (TEME km/s, nullable: positions only); tsince = ((jd + fr) - epoch) * 1440, as propagate_pairs forms it;
+ *   variables: n, e cos w, e sin w, i, RAAN, M + w and B* (held at its initial value when fit_bstar = 0); forward-
+ *            difference Jacobian, Marquardt damping x10 / /10, at most max_iter steps (25 is a good default);
+ *   model:   every trial set goes through the library's near-earth init and propagation, so the fitted columns passed to
+ *            create_from_elements and propagated with propagate_pairs at the observation times give back the RMS.
+ * Outputs: fitted[8][n] (epoch unchanged; RAAN, w and M in [0, 360)), rms[n][2] (sqrt of the mean squared position
+ * residual [km], and velocity residual [km/s] or 0 without velocities), iterations[n] (steps tried), status[n]
+ * (ASTROZ_FIT_*).  A satellite that does not converge returns its best accepted iterate; one that is not fitted (init
+ * failure, deep space, too few observations) returns its initial columns with zero RMS.  No output is NaN.  A
+ * satellite's bytes depend on its own inputs alone, not on the rest of the batch.
+ * ASTROZ_VALUE_ERROR, nothing written: device = -1 (a fit runs on one device); pos_sigma or vel_sigma not finite or
+ * <= 0; max_iter = 0; an unknown grav; and for the host call offsets that decrease or offsets[n] != m, or a non-finite
+ * element or observation value.  n = 0 is a no-op.  Without a device: ASTROZ_NO_DEVICE.
+ * HOST buffers: the inputs go up once (pageable ones through a pinned ring, pinned ones by direct DMA), one launch fits
+ * the batch, and the call returns with the results in place. */
+int32_t astroz_cuda_fit_elements(const double *elements, uint32_t n, int32_t grav, const uint32_t *offsets,
+                                 const double *jd, const double *fr, const double *pos, const double *vel, uint32_t m,
+                                 double pos_sigma, double vel_sigma, int32_t fit_bstar, uint32_t max_iter,
+                                 int32_t device, double *fitted, double *rms, uint32_t *iterations, uint8_t *status);
+/* Same with DEVICE pointers on `device` (the observation count is d_offsets[n]).  One launch on `stream`: no allocation,
+ * no synchronisation, and only the scalar arguments are checked -- the offsets and values must be valid. */
+int32_t astroz_cuda_fit_elements_device(const double *d_elements, uint32_t n, int32_t grav, const uint32_t *d_offsets,
+                                        const double *d_jd, const double *d_fr, const double *d_pos,
+                                        const double *d_vel, double pos_sigma, double vel_sigma, int32_t fit_bstar,
+                                        uint32_t max_iter, int32_t device, double *d_fitted, double *d_rms,
+                                        uint32_t *d_iterations, uint8_t *d_status, void *stream);
+/* One TLE line pair read by the library's own parser (src/Tle.zig:49-101) into the eight element columns above, the
+ * numbers astroz_cuda_constellation_create would use.  ASTROZ_BAD_TLE_LENGTH when the pair cannot be read. */
+int32_t astroz_cuda_parse_tle(const char *line1, const char *line2, double *elements);
 
 /* ---- measurement helpers --------------------------------------------------------------------- */
 /* DFMA microbenchmark on `device`: achieved fp64 TFLOP/s (FMA = 2) -- the measured roofline denominator */
