@@ -118,6 +118,10 @@ def lib() -> C.CDLL:
                                            i32, vp, vp, vp, vp]),
         "astroz_cuda_fit_elements_device": (i32, [vp, u32, i32, vp, vp, vp, vp, vp, C.c_double, C.c_double, i32, u32,
                                                   i32, vp, vp, vp, vp, vp]),
+        "astroz_cuda_fit_elements_mixed": (i32, [vp, u32, i32, vp, vp, vp, vp, vp, u32, C.c_double, C.c_double, i32,
+                                                 u32, i32, vp, vp, vp, vp]),
+        "astroz_cuda_fit_elements_mixed_device": (i32, [vp, u32, i32, vp, vp, vp, vp, vp, C.c_double, C.c_double, i32,
+                                                        u32, i32, vp, vp, vp, vp, vp]),
         "astroz_cuda_parse_tle": (i32, [C.c_char_p, C.c_char_p, dp]),
         "astroz_cuda_fp64_peak": (i32, [i32, dp]),
         "astroz_cuda_fp64_pipe_peak": (i32, [i32, dp]),
@@ -152,7 +156,8 @@ EXPORTS = [
     "astroz_cuda_constellation_propagate_pairs", "astroz_cuda_constellation_propagate_pairs_device",
     "astroz_cuda_numerical_times", "astroz_cuda_propagate_numerical", "astroz_cuda_propagate_numerical_device",
     "astroz_cuda_propagate_numerical_models", "astroz_cuda_propagate_numerical_models_device",
-    "astroz_cuda_fit_elements", "astroz_cuda_fit_elements_device", "astroz_cuda_parse_tle",
+    "astroz_cuda_fit_elements", "astroz_cuda_fit_elements_device", "astroz_cuda_fit_elements_mixed",
+    "astroz_cuda_fit_elements_mixed_device", "astroz_cuda_parse_tle",
 ]
 
 

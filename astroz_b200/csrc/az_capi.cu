@@ -2422,11 +2422,15 @@ static bool all_finite(const double *p, size_t count) {
     return true;
 }
 
-int32_t astroz_cuda_fit_elements_device(const double *d_elements, uint32_t n, int32_t grav, const uint32_t *d_offsets,
-                                        const double *d_jd, const double *d_fr, const double *d_pos,
-                                        const double *d_vel, double pos_sigma, double vel_sigma, int32_t fit_bstar,
-                                        uint32_t max_iter, int32_t device, double *d_fitted, double *d_rms,
-                                        uint32_t *d_iterations, uint8_t *d_status, void *stream) {
+// The kernels one fit call queues on its stream: launch_fit, or launch_fit_mixed below.
+using FitLaunch = cudaError_t (*)(const az::FitArgs &a, cudaStream_t stream);
+
+// The device-pointer calls: checks, then launch(a, stream) queues the kernels.
+static int32_t fit_device(const double *d_elements, uint32_t n, int32_t grav, const uint32_t *d_offsets,
+                          const double *d_jd, const double *d_fr, const double *d_pos, const double *d_vel,
+                          double pos_sigma, double vel_sigma, int32_t fit_bstar, uint32_t max_iter, int32_t device,
+                          double *d_fitted, double *d_rms, uint32_t *d_iterations, uint8_t *d_status, void *stream,
+                          FitLaunch launch) {
     az::FitArgs a{};
     int32_t rc = fit_check(n, grav, pos_sigma, vel_sigma, fit_bstar, max_iter, device, &a);
     if (rc != ASTROZ_OK) return rc;
@@ -2445,17 +2449,43 @@ int32_t astroz_cuda_fit_elements_device(const double *d_elements, uint32_t n, in
     a.rms = d_rms;
     a.iterations = d_iterations;
     a.status = d_status;
-    AZ_CUDA(az::launch_fit(a, static_cast<cudaStream_t>(stream)));
+    AZ_CUDA(launch(a, static_cast<cudaStream_t>(stream)));
     return ASTROZ_OK;
+}
+
+// A mixed batch: the near-earth fit writes every row (DEEP_SPACE on the deep-space ones), then the deep-space fit
+// overwrites the deep-space rows on the same stream.  The near-earth rows are therefore the near-earth call's bytes.
+static cudaError_t launch_fit_mixed(const az::FitArgs &a, cudaStream_t st) {
+    const cudaError_t e = az::launch_fit(a, st);
+    return e != cudaSuccess ? e : az::launch_fit_deep(a, st);
+}
+
+int32_t astroz_cuda_fit_elements_device(const double *d_elements, uint32_t n, int32_t grav, const uint32_t *d_offsets,
+                                        const double *d_jd, const double *d_fr, const double *d_pos,
+                                        const double *d_vel, double pos_sigma, double vel_sigma, int32_t fit_bstar,
+                                        uint32_t max_iter, int32_t device, double *d_fitted, double *d_rms,
+                                        uint32_t *d_iterations, uint8_t *d_status, void *stream) {
+    return fit_device(d_elements, n, grav, d_offsets, d_jd, d_fr, d_pos, d_vel, pos_sigma, vel_sigma, fit_bstar,
+                      max_iter, device, d_fitted, d_rms, d_iterations, d_status, stream, az::launch_fit);
+}
+
+int32_t astroz_cuda_fit_elements_mixed_device(const double *d_elements, uint32_t n, int32_t grav,
+                                              const uint32_t *d_offsets, const double *d_jd, const double *d_fr,
+                                              const double *d_pos, const double *d_vel, double pos_sigma,
+                                              double vel_sigma, int32_t fit_bstar, uint32_t max_iter, int32_t device,
+                                              double *d_fitted, double *d_rms, uint32_t *d_iterations,
+                                              uint8_t *d_status, void *stream) {
+    return fit_device(d_elements, n, grav, d_offsets, d_jd, d_fr, d_pos, d_vel, pos_sigma, vel_sigma, fit_bstar,
+                      max_iter, device, d_fitted, d_rms, d_iterations, d_status, stream, launch_fit_mixed);
 }
 
 // Host buffers: a fit is compute-bound (each observation is propagated some 8 x iterations times for its ~56 bytes),
 // so the whole batch goes up at once -- pageable arrays through the device's pinned ring, pinned ones by direct DMA --
-// and one launch fits it.  The results (~90 bytes per satellite) come back by plain copies.
-int32_t astroz_cuda_fit_elements(const double *elements, uint32_t n, int32_t grav, const uint32_t *offsets,
-                                 const double *jd, const double *fr, const double *pos, const double *vel, uint32_t m,
-                                 double pos_sigma, double vel_sigma, int32_t fit_bstar, uint32_t max_iter,
-                                 int32_t device, double *fitted, double *rms, uint32_t *iterations, uint8_t *status) {
+// and launch(a, stream) fits it.  The results (~90 bytes per satellite) come back by plain copies.
+static int32_t fit_host(const double *elements, uint32_t n, int32_t grav, const uint32_t *offsets, const double *jd,
+                        const double *fr, const double *pos, const double *vel, uint32_t m, double pos_sigma,
+                        double vel_sigma, int32_t fit_bstar, uint32_t max_iter, int32_t device, double *fitted,
+                        double *rms, uint32_t *iterations, uint8_t *status, FitLaunch launch) {
     az::FitArgs a{};
     int32_t rc = fit_check(n, grav, pos_sigma, vel_sigma, fit_bstar, max_iter, device, &a);
     if (rc != ASTROZ_OK) return rc;
@@ -2512,7 +2542,7 @@ int32_t astroz_cuda_fit_elements(const double *elements, uint32_t n, int32_t gra
     a.rms = dp(2);
     a.iterations = reinterpret_cast<uint32_t *>(base + iterAt);
     a.status = reinterpret_cast<uint8_t *>(base + statusAt);
-    AZ_CUDA(az::launch_fit(a, st));
+    AZ_CUDA(launch(a, st));
     AZ_CUDA(cudaMemcpyAsync(fitted, a.fitted, (size_t)8 * n * 8, cudaMemcpyDeviceToHost, st));
     AZ_CUDA(cudaMemcpyAsync(rms, a.rms, (size_t)2 * n * 8, cudaMemcpyDeviceToHost, st));
     AZ_CUDA(cudaMemcpyAsync(iterations, a.iterations, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
@@ -2520,6 +2550,23 @@ int32_t astroz_cuda_fit_elements(const double *elements, uint32_t n, int32_t gra
     AZ_CUDA(dBuf.release());
     AZ_CUDA(cudaStreamSynchronize(st));
     return ASTROZ_OK;
+}
+
+int32_t astroz_cuda_fit_elements(const double *elements, uint32_t n, int32_t grav, const uint32_t *offsets,
+                                 const double *jd, const double *fr, const double *pos, const double *vel, uint32_t m,
+                                 double pos_sigma, double vel_sigma, int32_t fit_bstar, uint32_t max_iter,
+                                 int32_t device, double *fitted, double *rms, uint32_t *iterations, uint8_t *status) {
+    return fit_host(elements, n, grav, offsets, jd, fr, pos, vel, m, pos_sigma, vel_sigma, fit_bstar, max_iter, device,
+                    fitted, rms, iterations, status, az::launch_fit);
+}
+
+int32_t astroz_cuda_fit_elements_mixed(const double *elements, uint32_t n, int32_t grav, const uint32_t *offsets,
+                                       const double *jd, const double *fr, const double *pos, const double *vel,
+                                       uint32_t m, double pos_sigma, double vel_sigma, int32_t fit_bstar,
+                                       uint32_t max_iter, int32_t device, double *fitted, double *rms,
+                                       uint32_t *iterations, uint8_t *status) {
+    return fit_host(elements, n, grav, offsets, jd, fr, pos, vel, m, pos_sigma, vel_sigma, fit_bstar, max_iter, device,
+                    fitted, rms, iterations, status, launch_fit_mixed);
 }
 
 int32_t astroz_cuda_parse_tle(const char *line1, const char *line2, double *elements) {

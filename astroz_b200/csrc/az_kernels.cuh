@@ -148,6 +148,9 @@ struct FitArgs {
     uint8_t *status = nullptr;           // [n] ASTROZ_FIT_*
 };
 cudaError_t launch_fit(const FitArgs &a, cudaStream_t stream);
+// The deep-space sets of the batch only (initial period > 225 min), under the deep-space model: every other row is left
+// as it is, so queued after launch_fit on the same arguments it completes a mixed batch.
+cudaError_t launch_fit_deep(const FitArgs &a, cudaStream_t stream);
 
 // DFMA throughput microbenchmark: returns achieved fp64 FLOP/s (FMA = 2).
 cudaError_t measure_fp64_peak(double *flops);

@@ -9,6 +9,11 @@ its observations (GPS or precise-ephemeris states, a numerical trajectory, a Mon
 squares sense.  Levenberg-Marquardt over n, e cos w, e sin w, i, RAAN, M + w and B* (optional), every trial element set
 propagated by the library's own near-earth path, one GPU warp per satellite.  The fitted columns, passed to
 `Constellation.from_elements` and propagated at the observation times, give back the reported RMS.
+
+Deep-space sets (period > 225 min: GEO, GPS, Molniya) are fitted with `deep_space=True`, under SDP4 with equinoctial
+variables (n, e cos(w + RAAN), e sin(w + RAAN), tan(i/2) cos RAAN, tan(i/2) sin RAAN, M + w + RAAN, B*), which stay well
+conditioned at i = 0 and e = 0.  Near-earth rows of such a batch are fitted exactly as without it.  By default deep-space
+sets are returned unfitted with status DEEP_SPACE.
 """
 from __future__ import annotations
 
@@ -22,7 +27,7 @@ from ._lib import WGS72, check, lib
 # per-satellite status bytes (ASTROZ_FIT_*)
 CONVERGED, ITERATION_LIMIT, INIT_FAILED, DEEP_SPACE, TOO_FEW_OBSERVATIONS = 0, 1, 2, 3, 4
 STATUS_NAMES = {CONVERGED: "converged", ITERATION_LIMIT: "iteration limit", INIT_FAILED: "initial set fails init",
-                DEEP_SPACE: "deep space, not fitted", TOO_FEW_OBSERVATIONS: "too few observations"}
+                DEEP_SPACE: "deep space, not fitted (deep_space=False)", TOO_FEW_OBSERVATIONS: "too few observations"}
 
 
 def parse_tle(line1: str, line2: str) -> np.ndarray:
@@ -86,12 +91,14 @@ def _csr(n: int, sat):
 
 
 def fit_elements(initial, sat, jd, fr, pos, vel=None, *, pos_sigma: float = 1.0, vel_sigma: float = 1e-3,
-                 fit_bstar: bool = True, max_iter: int = 25, grav: int = WGS72, device: int = 0) -> FitResult:
+                 fit_bstar: bool = True, max_iter: int = 25, grav: int = WGS72, device: int = 0,
+                 deep_space: bool = False) -> FitResult:
     """Fit n satellites at once.
 
     initial: TLE line pairs or an (8, n) array of element columns (epoch JD, n rev/day, e, i, RAAN, w, M deg, B*).
     sat[m], jd[m], fr[m], pos[m, 3] (TEME km), vel[m, 3] (TEME km/s, optional): the observations, in any order; they
-    are sorted stably by satellite.  pos_sigma [km] and vel_sigma [km/s] weight the residuals."""
+    are sorted stably by satellite.  pos_sigma [km] and vel_sigma [km/s] weight the residuals.  deep_space: fit the
+    deep-space sets too (astroz_cuda_fit_elements_mixed) instead of returning them with status DEEP_SPACE."""
     el = _initial_columns(initial)
     n = el.shape[1]
     order, offsets = _csr(n, sat)
@@ -105,19 +112,21 @@ def fit_elements(initial, sat, jd, fr, pos, vel=None, *, pos_sigma: float = 1.0,
     fitted, rms = np.zeros((8, n)), np.zeros((n, 2))
     iters, status = np.zeros(n, dtype=np.uint32), np.zeros(n, dtype=np.uint8)
     vp = lambda a: None if a is None else C.c_void_p(a.ctypes.data)  # noqa: E731
-    check(lib().astroz_cuda_fit_elements(vp(el), n, int(grav), vp(offsets), vp(jd_s), vp(fr_s), vp(pos_s), vp(vel_s),
-                                         m, float(pos_sigma), float(vel_sigma), int(bool(fit_bstar)), int(max_iter),
-                                         int(device), vp(fitted), vp(rms), vp(iters), vp(status)))
+    call = lib().astroz_cuda_fit_elements_mixed if deep_space else lib().astroz_cuda_fit_elements
+    check(call(vp(el), n, int(grav), vp(offsets), vp(jd_s), vp(fr_s), vp(pos_s), vp(vel_s), m, float(pos_sigma),
+               float(vel_sigma), int(bool(fit_bstar)), int(max_iter), int(device), vp(fitted), vp(rms), vp(iters),
+               vp(status)))
     return FitResult(fitted, rms[:, 0].copy(), rms[:, 1].copy(), iters, status)
 
 
 def fit_elements_device(elements, offsets, jd, fr, pos, vel, fitted, rms, iterations, status, *,
                         pos_sigma: float = 1.0, vel_sigma: float = 1e-3, fit_bstar: bool = True, max_iter: int = 25,
-                        grav: int = WGS72, stream: int = 0) -> None:
+                        grav: int = WGS72, stream: int = 0, deep_space: bool = False) -> None:
     """`fit_elements` with torch CUDA tensors on one device, observations already grouped by satellite: elements (8, n)
     float64, offsets (n + 1,) int32 (non-decreasing, offsets[n] = m), jd / fr (m,) float64, pos / vel (m, 3) float64
     (vel may be None); fitted (8, n) float64, rms (n, 2) float64, iterations (n,) int32 and status (n,) uint8 receive
-    the results.  One launch on `stream` (a raw cudaStream_t value, 0 = the default stream)."""
+    the results.  One launch on `stream` (a raw cudaStream_t value, 0 = the default stream); two with deep_space, the
+    deep-space fit after the near-earth one."""
     import torch
 
     n = int(elements.shape[1]) if elements.dim() == 2 and elements.shape[0] == 8 else -1
@@ -136,7 +145,8 @@ def fit_elements_device(elements, offsets, jd, fr, pos, vel, fitted, rms, iterat
                 or t.device != elements.device:
             raise ValueError(f"{name} must be a contiguous {dtype} tensor of {size} elements on {elements.device}")
     ptr = lambda t: None if t is None else C.c_void_p(t.data_ptr())  # noqa: E731
-    check(lib().astroz_cuda_fit_elements_device(
+    call = lib().astroz_cuda_fit_elements_mixed_device if deep_space else lib().astroz_cuda_fit_elements_device
+    check(call(
         ptr(elements), n, int(grav), ptr(offsets), ptr(jd), ptr(fr), ptr(pos), ptr(vel), float(pos_sigma),
         float(vel_sigma), int(bool(fit_bstar)), int(max_iter), int(elements.device.index), ptr(fitted), ptr(rms),
         ptr(iterations), ptr(status), C.c_void_p(stream) if stream else None))

@@ -62,6 +62,8 @@ def _implied_decimal(x: float) -> str:
     mag = abs(x)
     exp = math.floor(math.log10(mag)) + 1
     digits = int(round(mag * 10.0 ** (5 - exp)))
+    if digits == 100000:   # 0.999995.. rounds up to the next power of ten
+        digits, exp = 10000, exp + 1
     return f"{'-' if x < 0 else ' '}{digits:05d}{exp:+d}"
 
 

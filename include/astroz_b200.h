@@ -375,7 +375,8 @@ int32_t astroz_cuda_constellation_propagate_device_f32(astroz_constellation_t h,
 #define ASTROZ_FIT_CONVERGED            0   /* the cost stopped changing, or reached the rounding floor */
 #define ASTROZ_FIT_ITERATION_LIMIT      1   /* max_iter steps tried: the best accepted iterate is returned */
 #define ASTROZ_FIT_INIT_FAILED          2   /* the initial set fails SGP4 init (e outside [0, 1), perigee below 1 ER) */
-#define ASTROZ_FIT_DEEP_SPACE           3   /* period > 225 min: deep-space sets are not fitted */
+#define ASTROZ_FIT_DEEP_SPACE           3   /* period > 225 min: astroz_cuda_fit_elements[_device] do not fit deep-space
+                                               sets (the _mixed calls do, and never return this) */
 #define ASTROZ_FIT_TOO_FEW_OBSERVATIONS 4   /* fewer scalar residuals than fitted variables */
 
 /* The sample times of the batch calls (Propagator.zig:32-45 evaluated on the host, the one home of the sampling rule):
@@ -509,6 +510,30 @@ int32_t astroz_cuda_fit_elements_device(const double *d_elements, uint32_t n, in
                                         const double *d_vel, double pos_sigma, double vel_sigma, int32_t fit_bstar,
                                         uint32_t max_iter, int32_t device, double *d_fitted, double *d_rms,
                                         uint32_t *d_iterations, uint8_t *d_status, void *stream);
+/* Mixed batches: the calls above, plus the deep-space sets (initial period > 225 min) fitted under SDP4.  Same arguments,
+ * checks and return codes.  Each call queues the near-earth fit and then the deep-space fit over the whole batch on one
+ * stream; the second overwrites only the deep-space rows, so every near-earth row is the bytes astroz_cuda_fit_elements
+ * gives it.  A deep-space set:
+ *   variables: equinoctial -- n, e cos(w + RAAN), e sin(w + RAAN), tan(i/2) cos RAAN, tan(i/2) sin RAAN, M + w + RAAN and
+ *            B* -- well conditioned at i = 0 and e = 0 (GEO).  They diverge as i -> 180 deg: retrograde deep-space sets
+ *            near i = 180 deg are out of scope;
+ *   class:   held: a trial set whose period falls to 225 min or below counts as a set that cannot be built (a rejected
+ *            step, or the backward difference);
+ *   model:   every trial set goes through the library's deep-space init and the propagate_pairs deep-space query (its
+ *            resonance integrator included), so create_from_elements + propagate_pairs give back the RMS.  An observation
+ *            the model cannot propagate (decayed, eccentricity out of range) fails the pass: ASTROZ_FIT_INIT_FAILED for
+ *            the initial set, a rejected step for a trial set. */
+int32_t astroz_cuda_fit_elements_mixed(const double *elements, uint32_t n, int32_t grav, const uint32_t *offsets,
+                                       const double *jd, const double *fr, const double *pos, const double *vel,
+                                       uint32_t m, double pos_sigma, double vel_sigma, int32_t fit_bstar,
+                                       uint32_t max_iter, int32_t device, double *fitted, double *rms,
+                                       uint32_t *iterations, uint8_t *status);
+int32_t astroz_cuda_fit_elements_mixed_device(const double *d_elements, uint32_t n, int32_t grav,
+                                              const uint32_t *d_offsets, const double *d_jd, const double *d_fr,
+                                              const double *d_pos, const double *d_vel, double pos_sigma,
+                                              double vel_sigma, int32_t fit_bstar, uint32_t max_iter, int32_t device,
+                                              double *d_fitted, double *d_rms, uint32_t *d_iterations,
+                                              uint8_t *d_status, void *stream);
 /* One TLE line pair read by the library's own parser (src/Tle.zig:49-101) into the eight element columns above, the
  * numbers astroz_cuda_constellation_create would use.  ASTROZ_BAD_TLE_LENGTH when the pair cannot be read. */
 int32_t astroz_cuda_parse_tle(const char *line1, const char *line2, double *elements);

@@ -78,6 +78,8 @@ pub extern fn astroz_cuda_propagate_numerical_models(states: ?[*]const f64, n: u
 pub extern fn astroz_cuda_propagate_numerical_models_device(d_states: ?[*]const f64, n: u32, t0: f64, duration: f64, dt: f64, models: ?[*]const astroz_force_model_t, n_models: u32, integrator: i32, rtol: f64, atol: f64, device: i32, d_out: ?[*]f64, d_status: ?[*]u8, d_steps: ?[*]u64, stream: ?*anyopaque) i32;
 pub extern fn astroz_cuda_fit_elements(elements: ?[*]const f64, n: u32, grav: i32, offsets: ?[*]const u32, jd: ?[*]const f64, fr: ?[*]const f64, pos: ?[*]const f64, vel: ?[*]const f64, m: u32, pos_sigma: f64, vel_sigma: f64, fit_bstar: i32, max_iter: u32, device: i32, fitted: ?[*]f64, rms: ?[*]f64, iterations: ?[*]u32, status: ?[*]u8) i32;
 pub extern fn astroz_cuda_fit_elements_device(d_elements: ?[*]const f64, n: u32, grav: i32, d_offsets: ?[*]const u32, d_jd: ?[*]const f64, d_fr: ?[*]const f64, d_pos: ?[*]const f64, d_vel: ?[*]const f64, pos_sigma: f64, vel_sigma: f64, fit_bstar: i32, max_iter: u32, device: i32, d_fitted: ?[*]f64, d_rms: ?[*]f64, d_iterations: ?[*]u32, d_status: ?[*]u8, stream: ?*anyopaque) i32;
+pub extern fn astroz_cuda_fit_elements_mixed(elements: ?[*]const f64, n: u32, grav: i32, offsets: ?[*]const u32, jd: ?[*]const f64, fr: ?[*]const f64, pos: ?[*]const f64, vel: ?[*]const f64, m: u32, pos_sigma: f64, vel_sigma: f64, fit_bstar: i32, max_iter: u32, device: i32, fitted: ?[*]f64, rms: ?[*]f64, iterations: ?[*]u32, status: ?[*]u8) i32;
+pub extern fn astroz_cuda_fit_elements_mixed_device(d_elements: ?[*]const f64, n: u32, grav: i32, d_offsets: ?[*]const u32, d_jd: ?[*]const f64, d_fr: ?[*]const f64, d_pos: ?[*]const f64, d_vel: ?[*]const f64, pos_sigma: f64, vel_sigma: f64, fit_bstar: i32, max_iter: u32, device: i32, d_fitted: ?[*]f64, d_rms: ?[*]f64, d_iterations: ?[*]u32, d_status: ?[*]u8, stream: ?*anyopaque) i32;
 pub extern fn astroz_cuda_parse_tle(line1: [*:0]const u8, line2: [*:0]const u8, elements: ?[*]f64) i32;
 pub extern fn astroz_cuda_fp64_peak(device: i32, tflops: ?[*]f64) i32;
 pub extern fn astroz_cuda_fp64_pipe_peak(device: i32, tflops: ?[*]f64) i32;
