@@ -15,6 +15,7 @@
 // tensor cores.
 #include "az_kernels.cuh"
 #include "az_device_f32.cuh"
+#include "az_screen.cuh"
 
 #include <algorithm>
 
@@ -782,23 +783,29 @@ cudaError_t launch_sdp4_grid(const GridArgs &a, int mode, int layout, cudaStream
 // replaced by a running (min distance^2, first epoch index) per satellite: a warp owns one satellite
 // over ALL epochs, reduces with shuffles and writes 12 bytes -- the 48 B/cell result block never exists.
 // The reference rotates both vectors to ECEF with the same GMST first (:724,739); a common rotation
-// leaves the distance unchanged, so it is skipped.
+// leaves the distance unchanged, so it is skipped.  Both passes group epochs into lanes the same way
+// (screen_lane_cells), so a satellite with the target's elements meets the track at distance 0.
 // ---------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(128) sgp4_track_kernel(const ScreenArgs a) {
-    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= a.nTimes) return;
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    const uint32_t tw = (i >> 5) * (32u * kScreenLanes), lane = i & 31u;
+    if (tw >= a.nTimes) return;
     const double *tile = a.sgp4Tiles + (size_t)(a.targetIdx / kTileSats) * kSgp4TileDoubles + (a.targetIdx % kTileSats);
-    auto col = [tile](int i) { return __ldg(tile + i * kTileSats); };
-    const double ts[1] = {__ldg(a.tbase + t) + __ldg(a.toff + a.targetIdx)};
-    CellOut o[1];
-    sgp4_cell<1>(col, ts, a.g, o);
-    a.track[(size_t)t * 3 + 0] = o[0].rx;
-    a.track[(size_t)t * 3 + 1] = o[0].ry;
-    a.track[(size_t)t * 3 + 2] = o[0].rz;
+    auto col = [tile](int c) { return __ldg(tile + c * kTileSats); };
+    auto tbase = [&a](uint32_t t) { return __ldg(a.tbase + t); };
+    uint32_t tk[kScreenLanes];
+    CellOut o[kScreenLanes];
+    screen_lane_cells(col, tbase, __ldg(a.toff + a.targetIdx), a.nTimes, tw, lane, a.g, tk, o);
+#pragma unroll
+    for (int k = 0; k < kScreenLanes; ++k) {
+        if (tk[k] >= a.nTimes) continue;
+        a.track[(size_t)tk[k] * 3 + 0] = o[k].rx;
+        a.track[(size_t)tk[k] * 3 + 1] = o[k].ry;
+        a.track[(size_t)tk[k] * 3 + 2] = o[k].rz;
+    }
 }
 
 constexpr int kScreenWarps = 4;
-constexpr int kScreenLanes = 2;
 
 __global__ void __launch_bounds__(kScreenWarps * 32, 3) sgp4_screen_kernel(const ScreenArgs a) {
     __shared__ __align__(128) double tile[kSgp4TileDoubles];
@@ -819,26 +826,21 @@ __global__ void __launch_bounds__(kScreenWarps * 32, 3) sgp4_screen_kernel(const
         const double *colBase = tile + sl;
         auto col = [colBase](int i) { return colBase[i * kTileSats]; };
         const double toff = __ldg(a.toff + sat);
+        auto tbase = [&a](uint32_t t) { return __ldg(a.tbase + t); };
         double best = a.thresholdSq;   // src/Constellation.zig:703-706: start at threshold^2, index 0
         uint32_t bestT = 0;
         if (sat != a.targetIdx) {
 #pragma unroll 1
             for (uint32_t tw = 0; tw < a.nTimes; tw += 32 * kScreenLanes) {
-                double ts[kScreenLanes];
                 uint32_t tk[kScreenLanes];
-#pragma unroll
-                for (int k = 0; k < kScreenLanes; ++k) {
-                    tk[k] = tw + 32u * k + lane;
-                    ts[k] = __ldg(a.tbase + min(tk[k], a.nTimes - 1)) + toff;
-                }
                 CellOut o[kScreenLanes];
-                sgp4_cell<kScreenLanes>(col, ts, a.g, o);
+                screen_lane_cells(col, tbase, toff, a.nTimes, tw, (uint32_t)lane, a.g, tk, o);
 #pragma unroll
                 for (int k = 0; k < kScreenLanes; ++k) {
                     if (tk[k] < a.nTimes) {
                         const double *tg = a.track + (size_t)tk[k] * 3;
                         const double dx = __ldg(tg) - o[k].rx, dy = __ldg(tg + 1) - o[k].ry, dz = __ldg(tg + 2) - o[k].rz;
-                        const double d2 = fma(dx, dx, fma(dy, dy, dz * dz));
+                        const double d2 = screen_d2(dx, dy, dz);
                         if (d2 < best) {  // strict: the earliest epoch of the minimum wins (:745-748)
                             best = d2;
                             bestT = tk[k];
@@ -865,7 +867,8 @@ __global__ void __launch_bounds__(kScreenWarps * 32, 3) sgp4_screen_kernel(const
 
 cudaError_t launch_sgp4_screen(const ScreenArgs &a, cudaStream_t stream) {
     if (a.nSats == 0 || a.nTimes == 0) return cudaSuccess;
-    sgp4_track_kernel<<<(a.nTimes + 127) / 128, 128, 0, stream>>>(a);
+    const uint32_t trackThreads = (a.nTimes + 32 * kScreenLanes - 1) / (32 * kScreenLanes) * 32;
+    sgp4_track_kernel<<<(trackThreads + 127) / 128, 128, 0, stream>>>(a);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
     const uint32_t tiles = (a.nSats + kTileSats - 1) / kTileSats;
@@ -880,20 +883,9 @@ cudaError_t launch_sgp4_screen(const ScreenArgs &a, cudaStream_t stream) {
 // instead of stored, and only the own cell + 13 lexicographically-forward neighbours are visited -- each
 // cross-cell pair is met exactly once from the side whose offset is forward, same-cell pairs by other > s --
 // instead of 27 cells with an other > s filter.  Output order is not the reference's (by epoch, then by
-// satellite): callers get the same SET of (s, other, t) triples.
+// satellite): callers get the same SET of (s, other, t) triples.  The per-(satellite, epoch) search is
+// coarse_search (az_screen.cuh).
 // ---------------------------------------------------------------------------------------------------
-constexpr uint32_t kCoarseEmpty = 0xffffffffu;
-
-__device__ __forceinline__ uint32_t spatial_hash(int cx, int cy, int cz) {  // conjunction.zig:139-148
-    uint32_t h = (uint32_t)cx;
-    h *= 2654435761u;
-    h ^= (uint32_t)cy;
-    h *= 2654435761u;
-    h ^= (uint32_t)cz;
-    h *= 2654435761u;
-    return h;
-}
-
 __device__ __forceinline__ const double *coarse_pos(const CoarseArgs &a, uint32_t s, uint32_t t) {
     return a.pos + ((a.layout == 0) ? ((size_t)s * a.nTimes + t) * 3 : ((size_t)t * a.nSats + s) * 3);
 }
@@ -902,13 +894,9 @@ __global__ void __launch_bounds__(256) coarse_build_kernel(const CoarseArgs a) {
     const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= a.nSats) return;
     const uint32_t tb = blockIdx.y, t = a.t0 + tb;
-    if (a.validMask && a.validMask[s] == 0) return;
     const double *p = coarse_pos(a, s, t);
-    const double x = __ldg(p);
-    if (!isfinite(x)) return;  // conjunction.zig:60-63
-    const double inv = 1.0 / a.threshold;
-    const int cx = (int)floor(x * inv), cy = (int)floor(__ldg(p + 1) * inv), cz = (int)floor(__ldg(p + 2) * inv);
-    const uint32_t h = spatial_hash(cx, cy, cz) & ((1u << a.tableBits) - 1u);
+    if (!coarse_member(a.validMask, s, __ldg(p))) return;
+    const uint32_t h = coarse_bucket(p, 1.0 / a.threshold, (1u << a.tableBits) - 1u);
     a.next[(size_t)tb * a.nSats + s] = atomicExch(a.head + ((size_t)tb << a.tableBits) + h, s);
 }
 
@@ -916,41 +904,19 @@ __global__ void __launch_bounds__(256) coarse_pairs_kernel(const CoarseArgs a) {
     const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= a.nSats) return;
     const uint32_t tb = blockIdx.y, t = a.t0 + tb;
-    if (a.validMask && a.validMask[s] == 0) return;
     const double *p = coarse_pos(a, s, t);
-    const double sx = __ldg(p);
-    if (!isfinite(sx)) return;
-    const double sy = __ldg(p + 1), sz = __ldg(p + 2);
-    const double inv = 1.0 / a.threshold, thr2 = a.threshold * a.threshold;
-    const int scx = (int)floor(sx * inv), scy = (int)floor(sy * inv), scz = (int)floor(sz * inv);
-    const uint32_t mask = (1u << a.tableBits) - 1u;
-    const uint32_t *head = a.head + ((size_t)tb << a.tableBits);
-    const uint32_t *next = a.next + (size_t)tb * a.nSats;
-#pragma unroll 1
-    for (int n = 13; n < 27; ++n) {  // offsets (dx,dy,dz) in lexicographic order: index 13 is (0,0,0), 14..26 are forward
-        const int dx = n / 9 - 1, dy = (n / 3) % 3 - 1, dz = n % 3 - 1;
-        const int ncx = scx + dx, ncy = scy + dy, ncz = scz + dz;
-        uint32_t idx = __ldg(head + (spatial_hash(ncx, ncy, ncz) & mask));
-        while (idx != kCoarseEmpty) {
-            const uint32_t other = idx;
-            idx = __ldg(next + other);
-            if (other == s || (n == 13 && other < s)) continue;
-            if (a.validMask && a.validMask[other] == 0) continue;
-            const double *q = coarse_pos(a, other, t);
-            const double ox = __ldg(q), oy = __ldg(q + 1), oz = __ldg(q + 2);
-            if ((int)floor(ox * inv) != ncx || (int)floor(oy * inv) != ncy || (int)floor(oz * inv) != ncz)
-                continue;  // hash collision: another cell in the same bucket (conjunction.zig:112-113)
-            const double ddx = sx - ox, ddy = sy - oy, ddz = sz - oz;
-            if (ddx * ddx + ddy * ddy + ddz * ddz < thr2) {
-                const unsigned long long k = atomicAdd(a.count, 1ULL);
-                if (k < a.maxResults) {
-                    a.pairs[2 * k] = min(s, other);
-                    a.pairs[2 * k + 1] = max(s, other);
-                    a.tIdx[k] = t;
-                }
-            }
-        }
-    }
+    if (!coarse_member(a.validMask, s, __ldg(p))) return;
+    coarse_search(s, p, 1.0 / a.threshold, a.threshold * a.threshold, a.head + ((size_t)tb << a.tableBits),
+                  a.next + (size_t)tb * a.nSats, (1u << a.tableBits) - 1u, a.validMask,
+                  [&](uint32_t other) { return coarse_pos(a, other, t); },
+                  [&](uint32_t other) {
+                      const unsigned long long k = atomicAdd(a.count, 1ULL);
+                      if (k < a.maxResults) {
+                          a.pairs[2 * k] = min(s, other);
+                          a.pairs[2 * k + 1] = max(s, other);
+                          a.tIdx[k] = t;
+                      }
+                  });
 }
 
 cudaError_t launch_coarse_screen(const CoarseArgs &a, cudaStream_t stream) {

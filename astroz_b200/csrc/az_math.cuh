@@ -52,6 +52,30 @@ AZ_HD double dbl_with_hi(double x, uint32_t hi) {
 #endif
 }
 
+// Rounded fp64 operations nvcc may not contract into an FMA, for expressions that must equal a host evaluation bit for
+// bit (the host compiler does not contract).
+AZ_HD double add_rn(double a, double b) {
+#ifdef __CUDA_ARCH__
+    return __dadd_rn(a, b);
+#else
+    return a + b;
+#endif
+}
+AZ_HD double sub_rn(double a, double b) {
+#ifdef __CUDA_ARCH__
+    return __dsub_rn(a, b);
+#else
+    return a - b;
+#endif
+}
+AZ_HD double mul_rn(double a, double b) {
+#ifdef __CUDA_ARCH__
+    return __dmul_rn(a, b);
+#else
+    return a * b;
+#endif
+}
+
 // Magnitude tests that only steer control flow (which series to use, whether to iterate again) are done on the
 // HIGH WORD of the double with integer instructions: a DSETP occupies the half-rate fp64 pipe like a DFMA does,
 // the integer pipe has idle issue slots.  Ignoring

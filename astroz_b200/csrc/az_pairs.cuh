@@ -14,29 +14,8 @@ namespace az {
 
 constexpr uint8_t kCellBadSatellite = 3;  // ASTROZ_CELL_BAD_SATELLITE: sat[i] is not a catalog row
 
-// Rounded fp64 operations nvcc may not contract into an FMA: the time model and the GMST below must reproduce, bit for
+// The time model and the GMST below are written in add_rn / sub_rn / mul_rn (az_math.cuh): they must reproduce, bit for
 // bit, the expressions the grid path evaluates on the host (upload_time_axis, julian_to_gmst).
-AZ_HD double add_rn(double a, double b) {
-#ifdef __CUDA_ARCH__
-    return __dadd_rn(a, b);
-#else
-    return a + b;
-#endif
-}
-AZ_HD double sub_rn(double a, double b) {
-#ifdef __CUDA_ARCH__
-    return __dsub_rn(a, b);
-#else
-    return a - b;
-#endif
-}
-AZ_HD double mul_rn(double a, double b) {
-#ifdef __CUDA_ARCH__
-    return __dmul_rn(a, b);
-#else
-    return a * b;
-#endif
-}
 
 // Near-earth minutes since epoch: the grid's tbase[t] + toff[s], tbase = ((jd + fr) - referenceEpochJd) * 1440
 // (src/Constellation.zig:425), toff[s] = (referenceEpochJd - epoch[s]) * 1440 from the handle's table.
