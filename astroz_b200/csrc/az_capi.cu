@@ -455,8 +455,24 @@ int32_t upload_time_slot(Constellation *c, size_t nt, unsigned cols, cudaStream_
     return ASTROZ_OK;
 }
 
-// Per-call epoch offsets of the stateless near-earth path, padded to whole tiles, into dToffCall on s.
-int32_t stage_epoch_offsets(Constellation *c, const double *offsets, cudaStream_t s) {
+// Time axis of the stateless near-earth path on s: `times` (minutes from the reference) into column 0, sin / cos of GMST
+// into columns 2 and 3 when mode != TEME, and the per-call epoch offsets, padded to whole tiles, into dToffCall.
+int32_t stage_stateless_axis(Constellation *c, const double *times, uint32_t nt, const double *offsets, int mode,
+                             double reference_jd, cudaStream_t s) {
+    double *tb;
+    int32_t rc = time_slot(c, nt, &tb);
+    if (rc != ASTROZ_OK) return rc;
+    double *gs = tb + 2 * (size_t)nt, *gc = tb + 3 * (size_t)nt;
+    for (uint32_t t = 0; t < nt; ++t) {
+        tb[t] = times[t];
+        if (mode != 0) {  // src/Constellation.zig:573-581
+            const double gm = az::julian_to_gmst(reference_jd + times[t] / 1440.0);
+            gs[t] = std::sin(gm);
+            gc[t] = std::cos(gm);
+        }
+    }
+    rc = upload_time_slot(c, nt, (mode != 0) ? 0xDu : 0x1u, s);
+    if (rc != ASTROZ_OK) return rc;
     const uint32_t ns = c->cat.nSgp4, padded = c->cat.sgp4Padded();
     if (c->toffPending) {  // the previous call's upload of the offsets must have left the staging buffer
         AZ_CUDA(cudaEventSynchronize(c->toffCopied));
@@ -481,6 +497,21 @@ cudaError_t time_mark(Constellation *c, TimedSpan k, bool end, cudaStream_t s) {
     if (!c->timing) return cudaSuccess;
     if (end) c->timedSet |= 1u << k;
     return cudaEventRecord(c->ev[k][end], s);
+}
+
+// Queue launch() on s between the start and end marks of span k (no marks when `timed` is false).
+template <class F> cudaError_t in_span(Constellation *c, TimedSpan k, bool timed, cudaStream_t s, F &&launch) {
+    cudaError_t e = timed ? time_mark(c, k, false, s) : cudaSuccess;
+    if (e == cudaSuccess) e = launch();
+    if (e == cudaSuccess && timed) e = time_mark(c, k, true, s);
+    return e;
+}
+
+// A call of one grid pass: a new timing record holding span k around launch()
+template <class F> int32_t timed_pass(Constellation *c, TimedSpan k, cudaStream_t s, F &&launch) {
+    time_begin(c);
+    AZ_CUDA(in_span(c, k, true, s, launch));
+    return ASTROZ_OK;
 }
 
 int32_t ensure_lattice(Constellation *c, int nodes, cudaStream_t s) {
@@ -508,40 +539,70 @@ struct GatherTargets {  // fused all-gather destinations (see astroz_cuda_conste
     double *peerPos[az::kMaxPeers] = {}, *peerVel[az::kMaxPeers] = {};
 };
 
+// The two builders of a grid pass's arguments: the handle's tables, its gravity constants, the satellite count and the
+// time-axis columns from epoch t0 (dTime as last staged, so they are built after the staging).  The caller adds the
+// outputs and whatever selects a kernel path of its own (tsince, jdArr, mask, gather), which the builders leave null.
+// K1 (near-earth) over tiles [tile0, tile0 + tileCount) of the table, with epoch offsets `toff` and output rows `orig`
+// indexed from the table's first satellite.
+az::GridArgs near_pass(Constellation *c, const double *toff, const uint32_t *orig, uint32_t tile0 = 0,
+                       uint32_t tileCount = UINT32_MAX, uint32_t t0 = 0) {
+    const size_t first = (size_t)tile0 * az::kTileSats;
+    az::GridArgs a;
+    a.g = c->g;
+    a.sgp4Tiles = c->dTiles.p + (size_t)tile0 * az::kSgp4TileDoubles;
+    a.toff = toff + first;
+    a.orig = orig + first;
+    a.nSats = (uint32_t)std::min<uint64_t>(c->cat.nSgp4 - first, (uint64_t)tileCount * az::kTileSats);
+    a.tbase = time_col(c, 0) + t0;
+    a.gsin = time_col(c, 2) + t0;
+    a.gcos = time_col(c, 3) + t0;
+    return a;
+}
+
+// K2 (deep space) over every deep-space record, with output rows `orig`.  The lattice must already reach the call.
+az::GridArgs deep_pass(Constellation *c, const uint32_t *orig, uint32_t t0 = 0) {
+    az::GridArgs a;
+    a.g = c->g;
+    a.sdp4 = c->dSdp4.p;
+    a.orig = orig;
+    a.nSats = c->cat.nSdp4;
+    a.lattice = c->dLattice.p;
+    a.latticeNodes = c->latticeNodes;
+    a.jdFull = time_col(c, 1) + t0;
+    a.gsin = time_col(c, 2) + t0;
+    a.gcos = time_col(c, 3) + t0;
+    return a;
+}
+
 int32_t queue_grid(Constellation *c, const Launch &L, uint32_t ntTotal, double *dPos, double *dVel, uint8_t *dStatus,
                    int mode, int layout, uint32_t outNumSats, uint32_t outSatOffset, cudaStream_t s, bool timeIt,
                    const GatherTargets *gt = nullptr) {
-    const az::CatalogTables &t = c->cat;
-    az::GridArgs a;
-    a.g = c->g;
-    a.nTimes = (layout == 0) ? ntTotal : L.nt;  // satellite-major rows are ntTotal long
-    a.outNumSats = outNumSats;
-    a.tbase = time_col(c, 0) + L.t0;
-    a.jdFull = time_col(c, 1) + L.t0;
-    a.gsin = time_col(c, 2) + L.t0;
-    a.gcos = time_col(c, 3) + L.t0;
-    // outputs: rows are shifted by outSatOffset, epochs by t0
-    size_t shift;
-    if (layout == 0) shift = ((size_t)outSatOffset * ntTotal + L.t0) * 3;
-    else shift = ((size_t)L.t0 * outNumSats + outSatOffset) * 3;
-    a.pos = dPos ? dPos + shift : nullptr;
-    a.vel = dVel ? dVel + shift : nullptr;
-    if (gt && gt->kind) {
-        a.gather = gt->kind;
-        a.nPeers = gt->nPeers;
-        a.mcPos = gt->mcPos ? gt->mcPos + shift : nullptr;
-        a.mcVel = gt->mcVel ? gt->mcVel + shift : nullptr;
-        for (int p = 0; p < gt->nPeers; ++p) {
-            a.peerPos[p] = gt->peerPos[p] ? gt->peerPos[p] + shift : nullptr;
-            a.peerVel[p] = gt->peerVel[p] ? gt->peerVel[p] + shift : nullptr;
-        }
-    }
-    a.status = dStatus ? dStatus + (size_t)outSatOffset * ntTotal + L.t0 : nullptr;
     if (layout == 0 && L.nt != ntTotal) {
         g_lastError = "internal: satellite-major launches cover the whole time axis";
         return ASTROZ_UNKNOWN;
     }
-    const bool doK1 = L.tileCount && t.nSgp4, doK2 = L.deepSpace && t.nSdp4;
+    // outputs: rows are shifted by outSatOffset, epochs by t0
+    const size_t shift = (layout == 0) ? ((size_t)outSatOffset * ntTotal + L.t0) * 3
+                                       : ((size_t)L.t0 * outNumSats + outSatOffset) * 3;
+    auto outputs = [&](az::GridArgs a) {
+        a.nTimes = (layout == 0) ? ntTotal : L.nt;  // satellite-major rows are ntTotal long
+        a.outNumSats = outNumSats;
+        a.pos = dPos ? dPos + shift : nullptr;
+        a.vel = dVel ? dVel + shift : nullptr;
+        if (gt && gt->kind) {
+            a.gather = gt->kind;
+            a.nPeers = gt->nPeers;
+            a.mcPos = gt->mcPos ? gt->mcPos + shift : nullptr;
+            a.mcVel = gt->mcVel ? gt->mcVel + shift : nullptr;
+            for (int p = 0; p < gt->nPeers; ++p) {
+                a.peerPos[p] = gt->peerPos[p] ? gt->peerPos[p] + shift : nullptr;
+                a.peerVel[p] = gt->peerVel[p] ? gt->peerVel[p] + shift : nullptr;
+            }
+        }
+        a.status = dStatus ? dStatus + (size_t)outSatOffset * ntTotal + L.t0 : nullptr;
+        return a;
+    };
+    const bool doK1 = L.tileCount && c->cat.nSgp4, doK2 = L.deepSpace && c->cat.nSdp4;
     // A mixed call runs its two grids side by side: the deep-space grid is small (a few waves of CTAs at lower
     // fp64-pipe utilisation) and goes first, on the auxiliary stream, so the near-earth CTAs fill the SMs as it drains.
     const bool fork = doK1 && doK2;
@@ -555,32 +616,54 @@ int32_t queue_grid(Constellation *c, const Launch &L, uint32_t ntTotal, double *
         AZ_CUDA(cudaStreamWaitEvent(s2, c->forkEv, 0));
     }
     if (doK2) {
-        if (timeIt) AZ_CUDA(time_mark(c, kTimeK2, false, s2));
-        az::GridArgs k2 = a;
-        k2.sdp4 = c->dSdp4.p;
-        k2.orig = c->dSdp4Orig.p;
-        k2.nSats = t.nSdp4;
-        k2.lattice = c->dLattice.p;
-        k2.latticeNodes = c->latticeNodes;
-        AZ_CUDA(az::launch_sdp4_grid(k2, mode, layout, s2));
-        if (timeIt) AZ_CUDA(time_mark(c, kTimeK2, true, s2));
+        const az::GridArgs k2 = outputs(deep_pass(c, c->dSdp4Orig.p, L.t0));
+        AZ_CUDA(in_span(c, kTimeK2, timeIt, s2, [&] { return az::launch_sdp4_grid(k2, mode, layout, s2); }));
     }
     if (doK1) {
-        if (timeIt) AZ_CUDA(time_mark(c, kTimeK1, false, s));
-        az::GridArgs k1 = a;
-        k1.sgp4Tiles = c->dTiles.p + (size_t)L.tile0 * az::kSgp4TileDoubles;
-        k1.toff = c->dToff.p + (size_t)L.tile0 * az::kTileSats;
-        k1.orig = c->dSgp4Orig.p + (size_t)L.tile0 * az::kTileSats;
-        const uint32_t first = L.tile0 * az::kTileSats;
-        k1.nSats = std::min<uint32_t>(t.nSgp4 - first, L.tileCount * az::kTileSats);
-        AZ_CUDA(az::launch_sgp4_grid(k1, mode, layout, s, c->variant));
-        if (timeIt) AZ_CUDA(time_mark(c, kTimeK1, true, s));
+        const az::GridArgs k1 = outputs(near_pass(c, c->dToff.p, c->dSgp4Orig.p, L.tile0, L.tileCount, L.t0));
+        AZ_CUDA(in_span(c, kTimeK1, timeIt, s, [&] { return az::launch_sgp4_grid(k1, mode, layout, s, c->variant); }));
     }
     if (fork) {
         AZ_CUDA(cudaEventRecord(c->joinEv, s2));
         AZ_CUDA(cudaStreamWaitEvent(s, c->joinEv, 0));
     }
     if (timeIt) AZ_CUDA(time_mark(c, kTimeSpan, true, s));
+    return ASTROZ_OK;
+}
+
+// Satellites [row0, row0 + n) x epochs [t0, t0 + m) of a block of totalRows satellites x nt epochs, 3 doubles per cell,
+// in `layout`: `rows` runs of rowBytes, `pitch` bytes apart, from double `at` of the block.  A satellite-major range
+// covers whole rows (t0 = 0, m = nt).  A dense device block of those cells holds the same runs back to back.
+struct HostRows {
+    size_t at, rows, rowBytes, pitch;
+};
+
+HostRows host_rows(int layout, uint32_t row0, uint32_t n, uint32_t totalRows, uint32_t t0, uint32_t m, uint32_t nt) {
+    if (layout == 0) return {((size_t)row0 * nt + t0) * 3, n, (size_t)m * 24, (size_t)nt * 24};  // a run per satellite
+    return {((size_t)t0 * totalRows + row0) * 3, m, (size_t)n * 24, (size_t)totalRows * 24};       // a run per epoch
+}
+
+// Place the dense device blocks dPos / dVel at `h` in the caller's host blocks pos / vel once the work queued so far on
+// c->stream has finished (recorded in `ready`): pinned and registered memory gets a DMA on the copy stream, pageable
+// memory gets ring-sized pieces through the pinned ring, delivered by propagate_host_wait.
+int32_t place_rows(Constellation *c, cudaEvent_t ready, const double *dPos, const double *dVel, double *pos,
+                   double *vel, const HostRows &h) {
+    AZ_CUDA(cudaEventRecord(ready, c->stream));
+    AZ_CUDA(cudaStreamWaitEvent(c->copyStream, ready, 0));
+    for (int which = 0; which < (vel ? 2 : 1); ++which) {
+        double *dst = which ? vel : pos;
+        AZ_CUDA(c->pipe.ring.deliver(az::is_pageable(dst), ready, which ? dVel : dPos, dst + h.at, h.rows, h.rowBytes,
+                                     h.pitch, c->copyStream));
+    }
+    return ASTROZ_OK;
+}
+
+int32_t propagate_host_wait(Constellation *c) {
+    if (!c->stream) return ASTROZ_OK;
+    AZ_CUDA(cudaSetDevice(c->device));
+    AZ_CUDA(c->pipe.ring.drain(c->copyStream));
+    AZ_CUDA(cudaStreamSynchronize(c->copyStream));
+    AZ_CUDA(cudaStreamSynchronize(c->stream));
     return ASTROZ_OK;
 }
 
@@ -875,26 +958,13 @@ static int32_t sdp4_into_common(Constellation *c, const double *jd, const double
     if (rc != ASTROZ_OK) return rc;
     rc = prepare_deep_space(c, jdMin, jdMax, s);
     if (rc != ASTROZ_OK) return rc;
-    az::GridArgs a;
-    a.g = c->g;
+    az::GridArgs a = deep_pass(c, c->dSdp4Identity.p);
     a.nTimes = nt;
     a.outNumSats = outNumSats;
-    a.jdFull = time_col(c, 1);
-    a.gsin = time_col(c, 2);
-    a.gcos = time_col(c, 3);
     const size_t shift = (layout == 0) ? (size_t)satOffset * nt * 3 : (size_t)satOffset * 3;
     a.pos = dPos + shift;
     a.vel = dVel ? dVel + shift : nullptr;
-    a.sdp4 = c->dSdp4.p;
-    a.orig = c->dSdp4Identity.p;
-    a.nSats = nd;
-    a.lattice = c->dLattice.p;
-    a.latticeNodes = c->latticeNodes;
-    time_begin(c);
-    AZ_CUDA(time_mark(c, kTimeK2, false, s));
-    AZ_CUDA(az::launch_sdp4_grid(a, mode, layout, s));
-    AZ_CUDA(time_mark(c, kTimeK2, true, s));
-    return ASTROZ_OK;
+    return timed_pass(c, kTimeK2, s, [&] { return az::launch_sdp4_grid(a, mode, layout, s); });
 }
 
 static int32_t sdp4_into_check(Constellation *c, uint32_t out_num_sats, uint32_t sat_offset, uint32_t *rows) {
@@ -935,26 +1005,19 @@ int32_t astroz_cuda_sdp4_propagate_into(astroz_constellation_t h, const double *
     rc = sdp4_into_check(c, out_num_sats, sat_offset, &rows);
     if (rc != ASTROZ_OK) return rc;
     AZ_CUDA(cudaSetDevice(c->device));
-    cudaStream_t s = c->stream;
-    // the deep-space rows are computed as a dense block on the device and land in the caller's (possibly wider)
-    // block with one strided copy; rows that belong to other satellites are never touched
+    // the deep-space rows are computed as a dense block on the device and placed in the caller's (possibly wider)
+    // block; rows that belong to other satellites are never touched
     const size_t dense = (size_t)nd * n_times * 3;
     AZ_CUDA(c->dPos.reserve(dense));
     if (vel) AZ_CUDA(c->dVel.reserve(dense));
-    rc = sdp4_into_common(c, jd, fr, n_times, c->dPos.p, vel ? c->dVel.p : nullptr, mode, layout, nd, 0, s);
+    double *dVel = vel ? c->dVel.p : nullptr;
+    rc = sdp4_into_common(c, jd, fr, n_times, c->dPos.p, dVel, mode, layout, nd, 0, c->stream);
     if (rc != ASTROZ_OK) return rc;
-    for (int which = 0; which < (vel ? 2 : 1); ++which) {
-        double *dst = which ? vel : pos;
-        const double *src = which ? c->dVel.p : c->dPos.p;
-        if (layout == 0) {
-            AZ_CUDA(cudaMemcpyAsync(dst + (size_t)sat_offset * n_times * 3, src, dense * 8, cudaMemcpyDeviceToHost, s));
-        } else {
-            AZ_CUDA(cudaMemcpy2DAsync(dst + (size_t)sat_offset * 3, (size_t)rows * 24, src, (size_t)nd * 24,
-                                      (size_t)nd * 24, n_times, cudaMemcpyDeviceToHost, s));
-        }
-    }
-    AZ_CUDA(cudaStreamSynchronize(s));
-    return ASTROZ_OK;
+    c->pipe.ring.discard();
+    rc = place_rows(c, c->chunkDone[0], c->dPos.p, dVel, pos, vel, host_rows(layout, sat_offset, nd, rows, 0, n_times,
+                                                                              n_times));
+    if (rc != ASTROZ_OK) return rc;
+    return propagate_host_wait(c);
 }
 
 int32_t astroz_cuda_constellation_propagate_device_f32(astroz_constellation_t h, const double *jd, const double *fr,
@@ -969,22 +1032,12 @@ int32_t astroz_cuda_constellation_propagate_device_f32(astroz_constellation_t h,
     double jdMin, jdMax;
     int32_t rc = upload_time_axis(c, jd, fr, n_times, ASTROZ_MODE_TEME, s, &jdMin, &jdMax);
     if (rc != ASTROZ_OK) return rc;
-    az::GridArgs a;
-    a.g = c->g;
-    a.sgp4Tiles = c->dTiles.p;
-    a.toff = c->dToff.p;
-    a.orig = c->dSgp4Orig.p;
-    a.nSats = c->cat.nSgp4;
-    a.tbase = time_col(c, 0);
+    az::GridArgs a = near_pass(c, c->dToff.p, c->dSgp4Orig.p);
     a.nTimes = n_times;
     a.pos = d_pos;
     a.vel = d_vel;
     a.outNumSats = c->cat.n;
-    time_begin(c);
-    AZ_CUDA(time_mark(c, kTimeK1, false, s));
-    AZ_CUDA(az::launch_sgp4_grid_f32(a, phase64, s));
-    AZ_CUDA(time_mark(c, kTimeK1, true, s));
-    return ASTROZ_OK;
+    return timed_pass(c, kTimeK1, s, [&] { return az::launch_sgp4_grid_f32(a, phase64, s); });
 }
 
 int32_t astroz_cuda_constellation_propagate_gather(astroz_constellation_t h, const double *jd, const double *fr,
@@ -1061,7 +1114,6 @@ static int32_t propagate_host_queue(Constellation *c, const double *jd, const do
     // launch: time chunks that start on multiples of 192 keep every thread's set of epochs -- and with it the series each
     // cell takes, i.e. every result bit -- the same however the call is chunked (one device or many, any chunk count)
     if (byTime && nChunks > 1) per = (per + 191) / 192 * 192;
-    const bool posPageable = az::is_pageable(pos), velPageable = vel && az::is_pageable(vel);
     c->pipe.ring.discard();
     // last_kernel_ms after a host-buffer call: the span from the first kernel of the first chunk to the last kernel of
     // the last chunk (copies overlapping) in all three slots
@@ -1071,51 +1123,25 @@ static int32_t propagate_host_queue(Constellation *c, const double *jd, const do
         const uint32_t u0 = k * per, u1 = std::min(units, u0 + per);
         if (u0 >= u1) break;
         Launch L;
-        size_t off, cnt;
+        uint32_t r0 = 0, r1 = n;  // the chunk's satellites
         if (bySat) {
             L.tile0 = u0; L.tileCount = u1 - u0; L.deepSpace = false; L.t0 = 0; L.nt = n_times;
-            const size_t r0 = (size_t)u0 * az::kTileSats, r1 = std::min<size_t>(n, (size_t)u1 * az::kTileSats);
-            off = r0 * n_times * 3;
-            cnt = (r1 - r0) * n_times * 3;
+            r0 = u0 * az::kTileSats;
+            r1 = (uint32_t)std::min<size_t>(n, (size_t)u1 * az::kTileSats);
         } else if (byTime) {
             L.tile0 = 0; L.tileCount = tiles; L.deepSpace = true; L.t0 = u0; L.nt = u1 - u0;
-            off = (size_t)u0 * n * 3;
-            cnt = (size_t)(u1 - u0) * n * 3;
         } else {
             L.tile0 = 0; L.tileCount = tiles; L.deepSpace = true; L.t0 = 0; L.nt = n_times;
-            off = 0;
-            cnt = total;
         }
         rc = queue_grid(c, L, n_times, dPos, dVel, nullptr, mode, layout, n, 0, s, false);
         if (rc != ASTROZ_OK) return rc;
-        AZ_CUDA(cudaEventRecord(c->chunkDone[k], s));
-        AZ_CUDA(cudaStreamWaitEvent(c->copyStream, c->chunkDone[k], 0));
-        for (int which = 0; which < (vel ? 2 : 1); ++which) {
-            double *hdst = which ? vel : pos;
-            const double *dsrc = (which ? dVel : dPos) + off;
-            const bool pg = which ? velPageable : posPageable;
-            const cudaEvent_t ready = c->chunkDone[k];
-            if (layout == 0) {  // this handle's rows are one contiguous run of the (possibly wider) host block
-                AZ_CUDA(c->pipe.ring.deliver(pg, ready, dsrc, hdst + (size_t)rowOffset * n_times * 3 + off, 1, cnt * 8,
-                                             cnt * 8, c->copyStream));
-            } else if (totalRows == n) {
-                AZ_CUDA(c->pipe.ring.deliver(pg, ready, dsrc, hdst + off, 1, cnt * 8, cnt * 8, c->copyStream));
-            } else {            // time-major into a wider block: n*24 bytes per epoch at a pitch of totalRows*24
-                AZ_CUDA(c->pipe.ring.deliver(pg, ready, dsrc, hdst + ((size_t)u0 * totalRows + rowOffset) * 3, u1 - u0,
-                                             (size_t)n * 24, (size_t)totalRows * 24, c->copyStream));
-            }
-        }
+        // the device block is this handle's alone: the chunk's cells sit there as they would in a host block of n rows
+        const size_t off = host_rows(layout, r0, r1 - r0, n, L.t0, L.nt, n_times).at;
+        rc = place_rows(c, c->chunkDone[k], dPos + off, dVel ? dVel + off : nullptr, pos, vel,
+                        host_rows(layout, rowOffset + r0, r1 - r0, totalRows, L.t0, L.nt, n_times));
+        if (rc != ASTROZ_OK) return rc;
     }
     AZ_CUDA(time_mark(c, kTimeSpan, true, s));
-    return ASTROZ_OK;
-}
-
-static int32_t propagate_host_wait(Constellation *c) {
-    if (!c->stream) return ASTROZ_OK;
-    AZ_CUDA(cudaSetDevice(c->device));
-    AZ_CUDA(c->pipe.ring.drain(c->copyStream));
-    AZ_CUDA(cudaStreamSynchronize(c->copyStream));
-    AZ_CUDA(cudaStreamSynchronize(c->stream));
     return ASTROZ_OK;
 }
 
@@ -1175,24 +1201,33 @@ static int32_t for_each_shard(Constellation *c, const std::function<int32_t(size
     return c->workers->run(work);
 }
 
-int32_t astroz_cuda_constellation_propagate(astroz_constellation_t h, const double *jd, const double *fr,
-                                            uint32_t n_times, double *pos, double *vel, int32_t mode, int32_t layout) {
-    Constellation *c = static_cast<Constellation *>(h);
-    int32_t rc = check_args(c, jd, fr, pos, mode, layout);
-    if (rc != ASTROZ_OK) return rc;
-    if (n_times == 0 || c->cat.n == 0) return ASTROZ_OK;
+// A host-buffer call on every device of the handle: queue(target, row0, near0) then propagate_host_wait(target), on the
+// handle itself (row0 = near0 = 0), or on each shard side by side with its first catalog row and first near-earth index.
+// Each shard computes its own satellite range and copies it over its own PCIe link into its slice of the caller's
+// block: no collective is needed for a host-resident result.
+static int32_t queue_and_wait(Constellation *c,
+                              const std::function<int32_t(Constellation *, uint32_t, uint32_t)> &queue) {
     if (!c->multi()) {
-        rc = propagate_host_queue(c, jd, fr, n_times, pos, vel, mode, layout, 0, c->cat.n);
+        const int32_t rc = queue(c, 0, 0);
         if (rc != ASTROZ_OK) return rc;
         return propagate_host_wait(c);
     }
-    // one call, every device: each shard computes its satellite range and copies it over its own PCIe link into its
-    // slice of the caller's block; no collective is needed for a host-resident result
     return for_each_shard(c, [&](size_t k) -> int32_t {
         Constellation *sh = c->shards[k];
-        const int32_t q = propagate_host_queue(sh, jd, fr, n_times, pos, vel, mode, layout, c->shardRow0[k], c->cat.n);
+        const int32_t q = queue(sh, c->shardRow0[k], c->shardNear0[k]);
         const int32_t w = propagate_host_wait(sh);   // also drains what was queued before a failure
         return q != ASTROZ_OK ? q : w;
+    });
+}
+
+int32_t astroz_cuda_constellation_propagate(astroz_constellation_t h, const double *jd, const double *fr,
+                                            uint32_t n_times, double *pos, double *vel, int32_t mode, int32_t layout) {
+    Constellation *c = static_cast<Constellation *>(h);
+    const int32_t rc = check_args(c, jd, fr, pos, mode, layout);
+    if (rc != ASTROZ_OK) return rc;
+    if (n_times == 0 || c->cat.n == 0) return ASTROZ_OK;
+    return queue_and_wait(c, [&](Constellation *sh, uint32_t row0, uint32_t) {
+        return propagate_host_queue(sh, jd, fr, n_times, pos, vel, mode, layout, row0, c->cat.n);
     });
 }
 
@@ -1397,31 +1432,9 @@ static int32_t sgp4_into_common(Constellation *c, const double *times, uint32_t 
                                 double *dPos, double *dVel, int mode, double reference_jd, int layout, cudaStream_t s,
                                 uint32_t recStride = 3, const uint8_t *mask = nullptr, uint32_t outNumSats = 0) {
     const uint32_t ns = c->cat.nSgp4;
-    double *tb;
-    int32_t rc = time_slot(c, nt, &tb);
+    const int32_t rc = stage_stateless_axis(c, times, nt, epoch_offsets, mode, reference_jd, s);
     if (rc != ASTROZ_OK) return rc;
-    double *gs = tb + 2 * (size_t)nt, *gc = tb + 3 * (size_t)nt;
-    for (uint32_t t = 0; t < nt; ++t) {
-        tb[t] = times[t];
-        if (mode != 0) {  // src/Constellation.zig:573-581
-            const double gm = az::julian_to_gmst(reference_jd + times[t] / 1440.0);
-            gs[t] = std::sin(gm);
-            gc[t] = std::cos(gm);
-        }
-    }
-    rc = upload_time_slot(c, nt, (mode != 0) ? 0xDu : 0x1u, s);
-    if (rc == ASTROZ_OK) rc = stage_epoch_offsets(c, epoch_offsets, s);
-    if (rc != ASTROZ_OK) return rc;
-
-    az::GridArgs a;
-    a.g = c->g;
-    a.sgp4Tiles = c->dTiles.p;
-    a.toff = c->dToffCall.p;
-    a.orig = c->dIdentity.p;  // satellite i -> output row i (src/Constellation.zig:561-565)
-    a.nSats = ns;
-    a.tbase = time_col(c, 0);
-    a.gsin = time_col(c, 2);
-    a.gcos = time_col(c, 3);
+    az::GridArgs a = near_pass(c, c->dToffCall.p, c->dIdentity.p);  // satellite i -> row i, src/Constellation.zig:561-565
     a.nTimes = nt;
     a.pos = dPos;
     a.vel = dVel;
@@ -1432,11 +1445,7 @@ static int32_t sgp4_into_common(Constellation *c, const double *times, uint32_t 
         AZ_CUDA(cudaMemcpyAsync(c->dMask.p, mask, ns, cudaMemcpyHostToDevice, s));
         a.mask = c->dMask.p;
     }
-    time_begin(c);
-    AZ_CUDA(time_mark(c, kTimeK1, false, s));
-    AZ_CUDA(az::launch_sgp4_grid(a, mode, layout, s, c->variant));
-    AZ_CUDA(time_mark(c, kTimeK1, true, s));
-    return ASTROZ_OK;
+    return timed_pass(c, kTimeK1, s, [&] { return az::launch_sgp4_grid(a, mode, layout, s, c->variant); });
 }
 
 int32_t astroz_cuda_sgp4_propagate_into_device(astroz_constellation_t h, const double *times, uint32_t n_times,
@@ -1469,39 +1478,26 @@ static int32_t sgp4_into_host_queue(Constellation *c, const double *times, uint3
     AZ_CUDA(cudaSetDevice(c->device));
     cudaStream_t s = c->stream;
     // the near-earth rows are computed as a dense (ns, n_times) block on the device and placed in the caller's
-    // (possibly wider) block with one strided copy per array; rows that belong to other satellites are never touched
+    // (possibly wider) block; rows that belong to other satellites are never touched
     const size_t dense = (size_t)ns * n_times * 3;
     AZ_CUDA(c->dPos.reserve(dense));
     if (vel) AZ_CUDA(c->dVel.reserve(dense));
-    const bool strided = (layout == 1 && rows != ns);
-    auto host_at = [&](double *base) {
-        return base + (layout == 0 ? (size_t)rowOffset * n_times * 3 : (size_t)rowOffset * 3);
-    };
+    double *dVel = vel ? c->dVel.p : nullptr;
+    const HostRows at = host_rows(layout, rowOffset, ns, rows, 0, n_times, n_times);
     if (mask) {  // masked rows must keep the caller's contents: stage the caller's rows, overwrite the active ones
         for (int which = 0; which < (vel ? 2 : 1); ++which) {
-            double *dst = which ? c->dVel.p : c->dPos.p;
-            const double *src = host_at(which ? vel : pos);
-            if (!strided) AZ_CUDA(cudaMemcpyAsync(dst, src, dense * 8, cudaMemcpyHostToDevice, s));
-            else AZ_CUDA(cudaMemcpy2DAsync(dst, (size_t)ns * 24, src, (size_t)rows * 24, (size_t)ns * 24, n_times,
-                                           cudaMemcpyHostToDevice, s));
+            double *dst = which ? dVel : c->dPos.p;
+            const double *src = (which ? vel : pos) + at.at;
+            if (at.pitch == at.rowBytes) AZ_CUDA(cudaMemcpyAsync(dst, src, dense * 8, cudaMemcpyHostToDevice, s));
+            else AZ_CUDA(cudaMemcpy2DAsync(dst, at.rowBytes, src, at.pitch, at.rowBytes, at.rows, cudaMemcpyHostToDevice,
+                                           s));
         }
     }
-    int32_t rc = sgp4_into_common(c, times, n_times, epoch_offsets, c->dPos.p, vel ? c->dVel.p : nullptr, mode,
-                                  reference_jd, layout, s, 3, mask, ns);
+    const int32_t rc = sgp4_into_common(c, times, n_times, epoch_offsets, c->dPos.p, dVel, mode, reference_jd, layout, s,
+                                        3, mask, ns);
     if (rc != ASTROZ_OK) return rc;
     c->pipe.ring.discard();
-    const cudaEvent_t ready = c->chunkDone[0];
-    AZ_CUDA(cudaEventRecord(ready, s));
-    AZ_CUDA(cudaStreamWaitEvent(c->copyStream, ready, 0));
-    for (int which = 0; which < (vel ? 2 : 1); ++which) {
-        double *dst = host_at(which ? vel : pos);
-        const double *src = which ? c->dVel.p : c->dPos.p;
-        const bool pg = az::is_pageable(which ? vel : pos);
-        if (!strided) AZ_CUDA(c->pipe.ring.deliver(pg, ready, src, dst, 1, dense * 8, dense * 8, c->copyStream));
-        else AZ_CUDA(c->pipe.ring.deliver(pg, ready, src, dst, n_times, (size_t)ns * 24, (size_t)rows * 24,
-                                          c->copyStream));
-    }
-    return ASTROZ_OK;
+    return place_rows(c, c->chunkDone[0], c->dPos.p, dVel, pos, vel, at);
 }
 
 int32_t astroz_cuda_sgp4_propagate_into(astroz_constellation_t h, const double *times, uint32_t n_times,
@@ -1518,26 +1514,15 @@ int32_t astroz_cuda_sgp4_propagate_into(astroz_constellation_t h, const double *
         g_lastError = "out_num_sats smaller than the number of near-earth satellites";
         return ASTROZ_VALUE_ERROR;
     }
-    if (!c->multi()) {
-        rc = sgp4_into_host_queue(c, times, n_times, epoch_offsets, pos, vel, mode, reference_jd, layout, satellite_mask,
-                                  rows, 0);
-        if (rc != ASTROZ_OK) return rc;
-        return propagate_host_wait(c);
-    }
-    return for_each_shard(c, [&](size_t k) -> int32_t {
-        Constellation *sh = c->shards[k];
-        const uint32_t near0 = c->shardNear0[k];
-        const int32_t q = sgp4_into_host_queue(sh, times, n_times, epoch_offsets + near0, pos, vel, mode, reference_jd, layout,
-                                               satellite_mask ? satellite_mask + near0 : nullptr, rows, near0);
-        const int32_t w = propagate_host_wait(sh);
-        return q != ASTROZ_OK ? q : w;
+    return queue_and_wait(c, [&](Constellation *sh, uint32_t, uint32_t near0) {
+        return sgp4_into_host_queue(sh, times, n_times, epoch_offsets + near0, pos, vel, mode, reference_jd, layout,
+                                    satellite_mask ? satellite_mask + near0 : nullptr, rows, near0);
     });
 }
 
 int32_t astroz_cuda_sgp4_screen(astroz_constellation_t h, const double *times, uint32_t n_times,
                                 const double *epoch_offsets, uint32_t target_idx, double threshold,
                                 double reference_jd, double *out_min_dists, uint32_t *out_min_t) {
-    (void)reference_jd;
     Constellation *c = static_cast<Constellation *>(h);
     if (const int32_t rc = refuse_multi(c); rc != ASTROZ_OK) return rc;
     if (!c || !times || !epoch_offsets || !out_min_dists || !out_min_t) return ASTROZ_NULL_POINTER;
@@ -1549,12 +1534,7 @@ int32_t astroz_cuda_sgp4_screen(astroz_constellation_t h, const double *times, u
     }
     AZ_CUDA(cudaSetDevice(c->device));
     cudaStream_t s = c->stream;
-    double *tb;
-    int32_t rc = time_slot(c, n_times, &tb);
-    if (rc != ASTROZ_OK) return rc;
-    std::memcpy(tb, times, (size_t)n_times * 8);
-    rc = upload_time_slot(c, n_times, 0x1u, s);
-    if (rc == ASTROZ_OK) rc = stage_epoch_offsets(c, epoch_offsets, s);
+    int32_t rc = stage_stateless_axis(c, times, n_times, epoch_offsets, ASTROZ_MODE_TEME, reference_jd, s);
     if (rc != ASTROZ_OK) return rc;
     // scratch: target track [nt][3] | minDist [ns] | minT [ns] (as doubles' worth of space)
     AZ_CUDA(c->dPos.reserve((size_t)n_times * 3 + 2 * (size_t)ns + 2));
@@ -1570,10 +1550,8 @@ int32_t astroz_cuda_sgp4_screen(astroz_constellation_t h, const double *times, u
     a.minDist = c->dPos.p + (size_t)n_times * 3;
     a.minT = reinterpret_cast<uint32_t *>(a.minDist + ns);
     a.g = c->g;
-    time_begin(c);
-    AZ_CUDA(time_mark(c, kTimeK1, false, s));
-    AZ_CUDA(az::launch_sgp4_screen(a, s));
-    AZ_CUDA(time_mark(c, kTimeK1, true, s));
+    rc = timed_pass(c, kTimeK1, s, [&] { return az::launch_sgp4_screen(a, s); });
+    if (rc != ASTROZ_OK) return rc;
     AZ_CUDA(cudaMemcpyAsync(out_min_dists, a.minDist, (size_t)ns * 8, cudaMemcpyDeviceToHost, s));
     AZ_CUDA(cudaMemcpyAsync(out_min_t, a.minT, (size_t)ns * 4, cudaMemcpyDeviceToHost, s));
     AZ_CUDA(cudaStreamSynchronize(s));
@@ -1730,71 +1708,66 @@ int32_t astroz_cuda_sgp4_propagate_batch(astroz_sgp4_t h, const double *times, d
     }
     Constellation *c = s->c.get();
     AZ_CUDA(cudaSetDevice(c->device));
-    const bool fast = !s->deep && count >= 64;
-    std::vector<double> pos(fast ? 0 : (size_t)count * 3), vel(fast ? 0 : (size_t)count * 3);
-    int32_t rc;
+    cudaStream_t st = c->stream;
+    const size_t n3 = (size_t)count * 3;
+    AZ_CUDA(c->dPos.reserve(2 * n3));
+    double *dPos = c->dPos.p, *dVel = c->dPos.p + n3;
+    const double zero = 0.0;
+    if (!s->deep && count >= 64) {
+        // the time-parallel kernel (K1t) writes x y z vx vy vz records straight into one block that is copied to
+        // `results` in a single transfer (src/c_api/sgp4.zig:60-100 layout)
+        const int32_t rc = sgp4_into_common(c, times, count, &zero, dPos, dPos + 3, ASTROZ_MODE_TEME, 0.0,
+                                            ASTROZ_LAYOUT_SATELLITE_MAJOR, st, 6);
+        if (rc != ASTROZ_OK) return rc;
+        AZ_CUDA(cudaMemcpyAsync(results, dPos, n3 * 16, cudaMemcpyDeviceToHost, st));
+        AZ_CUDA(cudaStreamSynchronize(st));
+        return ASTROZ_OK;
+    }
+    // a position block and a velocity block, interleaved into records here: below 64 epochs K1 runs one epoch per
+    // thread instead of K1t's two (the series a cell takes, and so its bits, may differ between the two)
+    DevBuf<uint8_t> dSt;
+    std::vector<uint8_t> cell;
     if (!s->deep) {
-        // near earth: the time-parallel kernel writes x y z vx vy vz records straight into one block that
-        // is copied to `results` in a single transfer (src/c_api/sgp4.zig:60-100 layout)
-        const double zero = 0.0;
-        if (count >= 64) {
-            AZ_CUDA(c->dPos.reserve((size_t)count * 6));
-            rc = sgp4_into_common(c, times, count, &zero, c->dPos.p, c->dPos.p + 3, ASTROZ_MODE_TEME, 0.0,
-                                  ASTROZ_LAYOUT_SATELLITE_MAJOR, c->stream, 6);
-            if (rc != ASTROZ_OK) return rc;
-            AZ_CUDA(cudaMemcpyAsync(results, c->dPos.p, (size_t)count * 48, cudaMemcpyDeviceToHost, c->stream));
-            AZ_CUDA(cudaStreamSynchronize(c->stream));
-            return ASTROZ_OK;
-        }
-        rc = astroz_cuda_sgp4_propagate_into(c, times, count, &zero, pos.data(), vel.data(), ASTROZ_MODE_TEME, 0.0,
-                                             ASTROZ_LAYOUT_SATELLITE_MAJOR, nullptr, 0);
+        const int32_t rc = sgp4_into_common(c, times, count, &zero, dPos, dVel, ASTROZ_MODE_TEME, 0.0,
+                                            ASTROZ_LAYOUT_SATELLITE_MAJOR, st);
         if (rc != ASTROZ_OK) return rc;
     } else {
         // deep space: minutes since epoch go to the kernel directly (no Julian-date round trip)
         double *tb;
-        rc = time_slot(c, count, &tb);
+        int32_t rc = time_slot(c, count, &tb);
         if (rc != ASTROZ_OK) return rc;
         double reach = 0.0;
         for (uint32_t i = 0; i < count; ++i) {
             tb[i] = times[i];
             reach = std::max(reach, std::fabs(times[i]));
         }
-        cudaStream_t st = c->stream;
         rc = upload_time_slot(c, count, 0x1u, st);
         if (rc != ASTROZ_OK) return rc;
         rc = ensure_lattice(c, (int)std::floor(reach / az::kStepp) + 2, st);
         if (rc != ASTROZ_OK) return rc;
-        const size_t total = (size_t)count * 3;
-        DevBuf<uint8_t> dSt;
-        AZ_CUDA(c->dPos.reserve(total));
-        AZ_CUDA(c->dVel.reserve(total));
         AZ_CUDA(dSt.reserve(count));
-        az::GridArgs a;
-        a.g = c->g;
-        a.sdp4 = c->dSdp4.p;
-        a.orig = c->dSdp4Orig.p;
-        a.nSats = 1;
-        a.lattice = c->dLattice.p;
-        a.latticeNodes = c->latticeNodes;
+        az::GridArgs a = deep_pass(c, c->dSdp4Orig.p);
         a.tsince = time_col(c, 0);
         a.nTimes = count;
-        a.pos = c->dPos.p;
-        a.vel = c->dVel.p;
+        a.pos = dPos;
+        a.vel = dVel;
         a.status = dSt.p;
         a.outNumSats = 1;
-        std::vector<uint8_t> cell(count);
+        cell.resize(count);
         AZ_CUDA(az::launch_sdp4_grid(a, ASTROZ_MODE_TEME, ASTROZ_LAYOUT_SATELLITE_MAJOR, st));
-        AZ_CUDA(cudaMemcpyAsync(pos.data(), c->dPos.p, total * 8, cudaMemcpyDeviceToHost, st));
-        AZ_CUDA(cudaMemcpyAsync(vel.data(), c->dVel.p, total * 8, cudaMemcpyDeviceToHost, st));
         AZ_CUDA(cudaMemcpyAsync(cell.data(), dSt.p, count, cudaMemcpyDeviceToHost, st));
-        AZ_CUDA(cudaStreamSynchronize(st));
-        for (uint32_t i = 0; i < count; ++i)
-            if (cell[i] != 0) rc = status_to_code(cell[i]);  // failing cells stay zero-filled; last failure reported
     }
+    std::vector<double> pv(2 * n3);
+    AZ_CUDA(cudaMemcpyAsync(pv.data(), dPos, 2 * n3 * 8, cudaMemcpyDeviceToHost, st));
+    AZ_CUDA(cudaStreamSynchronize(st));
+    int32_t rc = ASTROZ_OK;
+    for (uint8_t code : cell)
+        if (code != 0) rc = status_to_code(code);  // failing cells stay zero-filled; last failure reported
     for (uint32_t i = 0; i < count; ++i) {
         double *r = results + (size_t)i * 6;
-        r[0] = pos[i * 3]; r[1] = pos[i * 3 + 1]; r[2] = pos[i * 3 + 2];
-        r[3] = vel[i * 3]; r[4] = vel[i * 3 + 1]; r[5] = vel[i * 3 + 2];
+        const double *p = pv.data() + (size_t)i * 3, *v = p + n3;
+        r[0] = p[0]; r[1] = p[1]; r[2] = p[2];
+        r[3] = v[0]; r[4] = v[1]; r[5] = v[2];
     }
     return rc;
 }
@@ -1831,15 +1804,9 @@ int32_t astroz_cuda_sgp4_array(astroz_sgp4_t h, const double *jd, const double *
     AZ_CUDA(c->dPos.reserve(az::chunk_slots_bytes(out, 1, count, chunk) / 8));
     auto launch = [&](uint32_t k, uint32_t t0, uint32_t n, void *const *dIn, void *const *dOut, cudaStream_t s) {
         double *dJd = static_cast<double *>(dIn[0]), *dRec = static_cast<double *>(dOut[0]);
-        az::GridArgs a;
-        a.g = c->g;
-        a.sgp4Tiles = c->dTiles.p;
-        a.toff = c->dToff.p;
-        a.orig = c->dIdentity.p;
-        a.nSats = 1;
+        az::GridArgs a = near_pass(c, c->dToff.p, c->dIdentity.p);
         a.jdArr = dJd;
         a.frArr = static_cast<double *>(dIn[1]);
-        a.tbase = dJd;
         a.epochJd = epoch_jd;
         a.nTimes = n;
         a.pos = dRec;

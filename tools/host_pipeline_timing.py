@@ -1,14 +1,28 @@
 #!/usr/bin/env python
-"""Host-buffer calls that run the two-slot chunk pipeline (astroz_b200/csrc/az_hostcopy.cu, ChunkPipeline), each with
-pinned and with pageable buffers: host clock around calls that end in a synchronise, best of --reps after a warm-up
-call, and a SHA-256 of the result bytes.  Prints one JSON line with the card's name, power limit and
-maximum SM clock.
+"""Host orchestration of the C ABI (astroz_b200/csrc/az_capi.cu, az_hostcopy.cu): the calls that run the two-slot chunk
+pipeline (ChunkPipeline), the calls that place grid results in the caller's host block, and the single-pass calls
+around them.  Host-buffer calls run with pinned and with pageable buffers.  Host clock around calls that end in a
+synchronise, best of --reps after a warm-up call, and a SHA-256 of the result bytes.  Prints one JSON line with the
+card's name, power limit and maximum SM clock.
 
   pairs W1 / W4  tools/pairs_timing.py's W1 (19,408,320 queries over the config-2 catalogue) and W4 (100,000 queries),
                  TEME with velocities and status
   sgp4_array     the ISS over 31,536,000 epochs at one second ("1 year (second)"), through astroz_cuda_sgp4_array
   numerical N1   tools/numerical_timing.py's N1 (100,000 LEO states, J2 + drag, one day at 60 s, DP87) through
                  astroz_cuda_propagate_numerical
+  propagate      the config-2 mixed catalogue (13,478 satellites, 1,024 GEO, 256 Molniya, 256 GPS) over 1,440 epochs,
+                 TEME with velocities, satellite- and time-major; also on a three-shard handle of one GPU
+                 (ASTROZ_DEVICE_LIST=0,0,0)
+  sgp4_into      astroz_cuda_sgp4_propagate_into, the 13,478 near-earth satellites over 1,440 epochs with a seeded
+                 9-in-10 mask and per-satellite epoch offsets into a block 512 rows wider than the catalogue
+  sdp4_into      astroz_cuda_sdp4_propagate_into, the mixed catalogue's deep-space members over 1,440 epochs at row 32 of
+                 a block 64 rows wider, both layouts
+  batch          astroz_cuda_sgp4_propagate_batch, the ISS (near) and a GEO satellite (deep) at 1, 63, 64 and 10,000
+                 seeded epochs within a week of the element epoch
+  screen         astroz_cuda_sgp4_screen (target 0, 10 km) and astroz_cuda_sgp4_screen_all (10 km) over the near-earth
+                 catalogue and 1,440 epochs
+  device         astroz_cuda_constellation_propagate_device_f32 (near-earth catalogue) and
+                 astroz_cuda_sdp4_propagate_into_device (the mixed catalogue's deep-space members), 1,440 epochs
 
     python tools/host_pipeline_timing.py [--reps 3]
     python tools/host_pipeline_timing.py --compare OTHER.so [--rounds 5]
@@ -120,6 +134,97 @@ def numerical_case(y0, area0, samples, pinned, reps):
     return ms, checksum([out, status, steps])
 
 
+def propagate_case(c, jd, fr, layout, pinned, reps):
+    shape = c._shape(len(jd), layout)
+    pos, vel = empty(shape, np.float64, pinned), empty(shape, np.float64, pinned)
+    ms = best_ms(lambda: c.propagate(jd, fr, pos, vel, 0, layout), reps)
+    return ms, checksum([pos, vel])
+
+
+def sgp4_into_case(c, times, off, mask, rows, time_major, pinned, reps):
+    # masked and surplus rows keep what the block held before the call: a fill that is part of the checksum
+    shape = (len(times), rows, 3) if time_major else (rows, len(times), 3)
+    pos, vel = like(np.full(shape, 0.5), pinned), like(np.full(shape, -0.5), pinned)
+    ms = best_ms(lambda: c.propagate_into(times, pos, vel, epoch_offsets=off, satellite_mask=mask,
+                                          time_major=time_major, output_stride=rows), reps)
+    return ms, checksum([pos, vel])
+
+
+def sdp4_into_case(c, jd, fr, rows, offset, time_major, pinned, reps):
+    shape = (len(jd), rows, 3) if time_major else (rows, len(jd), 3)
+    pos, vel = like(np.full(shape, 0.5), pinned), like(np.full(shape, -0.5), pinned)
+    ms = best_ms(lambda: c.propagate_sdp4_into(jd, fr, pos, vel, time_major=time_major, output_stride=rows,
+                                               sat_offset=offset), reps)
+    return ms, checksum([pos, vel])
+
+
+def batch_case(s, times, reps):
+    from astroz_b200 import _lib
+
+    out = np.zeros((len(times), 6))
+    L = _lib.lib()
+    ms = best_ms(lambda: _lib.check(L.astroz_cuda_sgp4_propagate_batch(s._h, _lib.dptr(times), _lib.dptr(out),
+                                                                       len(times))), reps)
+    return ms, checksum([out])
+
+
+def screen_case(c, times, off, reps):
+    out = [None]
+
+    def call():
+        out[0] = c.screen_conjunction(times, 0, 10.0, epoch_offsets=off)
+
+    return best_ms(call, reps), checksum(out[0])
+
+
+def screen_all_case(c, times, off, reps):
+    from astroz_b200 import _lib
+
+    ns, cap = c.numSgp4, 2_000_000
+    pairs, tidx, cnt = np.empty((cap, 2), np.uint32), np.empty(cap, np.uint32), C.c_uint64()
+    L = _lib.lib()
+    u32p = C.POINTER(C.c_uint32)
+    ms = best_ms(lambda: _lib.check(L.astroz_cuda_sgp4_screen_all(
+        c._h, _lib.dptr(times), len(times), _lib.dptr(off[:ns]), 10.0, pairs.ctypes.data_as(u32p),
+        tidx.ctypes.data_as(u32p), cap, C.byref(cnt))), reps)
+    # hits are appended in whatever order the threads find them: the hit set is compared in the API's sorted order
+    from astroz_b200.constellation import _sorted_hits
+
+    k = min(cnt.value, cap)
+    return ms, checksum([np.array([cnt.value], np.uint64), *_sorted_hits(pairs[:k], tidx[:k])])
+
+
+def device_f32_case(c, jd, fr, reps):
+    import torch
+
+    pos = torch.zeros((c.numSatellites, len(jd), 3), dtype=torch.float64, device="cuda:0")
+    vel = torch.zeros_like(pos)
+
+    def call():
+        c.propagate_device_f32(jd, fr, pos, vel)
+        torch.cuda.synchronize()
+
+    return best_ms(call, reps), checksum([pos.cpu().numpy(), vel.cpu().numpy()])
+
+
+def sdp4_device_case(c, jd, fr, reps):
+    import torch
+
+    from astroz_b200 import _lib
+
+    nd = c.numSdp4
+    block = torch.zeros((2, nd, len(jd), 3), dtype=torch.float64, device="cuda:0")
+    L = _lib.lib()
+
+    def call():
+        _lib.check(L.astroz_cuda_sdp4_propagate_into_device(
+            c._h, _lib.dptr(jd), _lib.dptr(fr), len(jd), C.c_void_p(block[0].data_ptr()),
+            C.c_void_p(block[1].data_ptr()), 0, 0, nd, 0, None))
+        c.synchronize()
+
+    return best_ms(call, reps), checksum([block.cpu().numpy()])
+
+
 def measure(reps: int) -> dict:
     import astroz_b200
     from astroz_b200 import _lib, numerical, synth
@@ -131,10 +236,16 @@ def measure(reps: int) -> dict:
     _lib.require_device()
     res = {"card_power_limit_max_sm_clock": card(), "lib": os.path.relpath(_lib.LIB_PATH, ROOT), "reps": reps}
 
+    def record(name, ms, digest):
+        res[name] = {"ms": round(ms, 3), "checksum": digest}
+        print(f"{name}: {ms:.3f} ms", file=sys.stderr, flush=True)   # progress of a long run
+
     def both(name, case, *args):
         for pinned in (True, False):
-            ms, digest = case(*args, pinned, reps)
-            res[f"{name}_{'pinned' if pinned else 'pageable'}"] = {"ms": round(ms, 3), "checksum": digest}
+            record(f"{name}_{'pinned' if pinned else 'pageable'}", *case(*args, pinned, reps))
+
+    def one(name, case, *args):
+        record(name, *case(*args, reps))
 
     near = synth.near_earth_catalog()
     c = astroz_b200.Constellation(near)
@@ -149,6 +260,41 @@ def measure(reps: int) -> dict:
     y1 = teme_states(synth.monte_carlo_catalog(100_000), synth.BENCH_JD0, 0.0)
     area = rng.uniform(1.0, 20.0, len(y1))
     both("numerical_N1", numerical_case, y1, area, len(numerical.numerical_times(0.0, 86400.0, 60.0)))
+
+    jd, fr = synth.time_grid(1440)
+    mixed = synth.mixed_catalog()
+    c = astroz_b200.Constellation(mixed)
+    for layout, tag in ((0, "sat"), (1, "time")):
+        both(f"propagate_mixed_{tag}", propagate_case, c, jd, fr, layout)
+    for time_major, tag in ((False, "sat"), (True, "time")):
+        both(f"sdp4_into_wide_{tag}", sdp4_into_case, c, jd, fr, c.numSdp4 + 64, 32, time_major)
+    one("sdp4_into_device", sdp4_device_case, c, jd, fr)
+    del c
+    os.environ["ASTROZ_DEVICE_LIST"] = "0,0,0"   # read when a device = -1 handle is made
+    c = astroz_b200.Constellation(mixed, device=-1)
+    del os.environ["ASTROZ_DEVICE_LIST"]
+    for layout, tag in ((0, "sat"), (1, "time")):
+        both(f"propagate_mixed_3shards_{tag}", propagate_case, c, jd, fr, layout)
+    del c
+
+    c = astroz_b200.Constellation(near)
+    ns = c.numSgp4
+    rng = np.random.default_rng(3)
+    times = np.arange(1440, dtype=np.float64)
+    off = rng.uniform(-1440.0, 0.0, ns)
+    mask = (rng.uniform(size=ns) < 0.9).astype(np.uint8)
+    for time_major, tag in ((False, "sat"), (True, "time")):
+        both(f"sgp4_into_masked_wide_{tag}", sgp4_into_case, c, times, off, mask, ns + 512, time_major)
+    one("sgp4_screen", screen_case, c, times, off)
+    one("screen_all", screen_all_case, c, times, off)
+    one("propagate_device_f32", device_f32_case, c, jd, fr)
+    del c
+
+    for tag, tle in (("near", G.ISS), ("deep", G.GEO28626)):
+        s = Satrec.twoline2rv(*tle, WGS72)
+        for n in (1, 63, 64, 10_000):
+            one(f"batch_{tag}_{n}", batch_case, s, np.sort(np.random.default_rng(n).uniform(-1440.0, 10080.0, n)))
+        del s
     return res
 
 
@@ -160,8 +306,9 @@ def compare(other: str, rounds: int, reps: int) -> dict:
             env.pop("ASTROZ_B200_LIB", None)
             if label == "other":
                 env["ASTROZ_B200_LIB"] = os.path.abspath(other)
+            print(f"round {r}: {label}", file=sys.stderr, flush=True)
             p = subprocess.run([sys.executable, os.path.abspath(__file__), "--reps", str(reps)], env=env,
-                               capture_output=True, text=True, check=True)
+                               stdout=subprocess.PIPE, text=True, check=True)
             runs[label].append(json.loads(p.stdout.strip().splitlines()[-1]))
     first = runs["this"][0]
     res = {"card_power_limit_max_sm_clock": first["card_power_limit_max_sm_clock"], "other": other, "rounds": rounds,
