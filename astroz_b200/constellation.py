@@ -235,7 +235,9 @@ class Constellation:
                          out_sat_offset: int = 0, stream: int = 0) -> None:
         """Same computation, results left in HBM.  pos / vel / status are torch CUDA tensors (or anything
         with .data_ptr()) on this constellation's device; asynchronous on `stream` (a raw cudaStream_t
-        value, 0 = the handle's own stream)."""
+        value, 0 = the handle's own stream).  out_num_sats / out_sat_offset place this handle's rows inside a larger
+        pos / vel block; status is this handle's own (numSatellites, n_times) uint8 block, satellite-major, satellite
+        i at row i whatever the offset."""
         jd, fr = as_f64(jd), as_f64(fr)
         nt = jd.shape[0]
         rows = self.numSatellites if out_num_sats is None else int(out_num_sats)

@@ -581,6 +581,13 @@ int32_t queue_grid(Constellation *c, const Launch &L, uint32_t ntTotal, double *
         g_lastError = "internal: satellite-major launches cover the whole time axis";
         return ASTROZ_UNKNOWN;
     }
+    // The status block is the handle's own n x ntTotal bytes, satellite-major, whatever block the positions land in:
+    // the kernels index it by output row and a.nTimes, which is the chunk length for a time-major chunk, so it only
+    // comes with launches over the whole time axis.
+    if (dStatus && (L.t0 != 0 || L.nt != ntTotal)) {
+        g_lastError = "internal: a status block needs a launch over the whole time axis";
+        return ASTROZ_UNKNOWN;
+    }
     // outputs: rows are shifted by outSatOffset, epochs by t0
     const size_t shift = (layout == 0) ? ((size_t)outSatOffset * ntTotal + L.t0) * 3
                                        : ((size_t)L.t0 * outNumSats + outSatOffset) * 3;
@@ -599,7 +606,7 @@ int32_t queue_grid(Constellation *c, const Launch &L, uint32_t ntTotal, double *
                 a.peerVel[p] = gt->peerVel[p] ? gt->peerVel[p] + shift : nullptr;
             }
         }
-        a.status = dStatus ? dStatus + (size_t)outSatOffset * ntTotal + L.t0 : nullptr;
+        a.status = dStatus;  // row i of the handle at i * ntTotal, not shifted by outSatOffset
         return a;
     };
     const bool doK1 = L.tileCount && c->cat.nSgp4, doK2 = L.deepSpace && c->cat.nSdp4;

@@ -148,7 +148,8 @@ int32_t astroz_cuda_constellation_propagate(astroz_constellation_t h, const doub
  * out_num_sats / out_sat_offset place this handle's satellites inside a larger output block
  * (the reference's numSatellites-as-stride convention, src/Constellation.zig:46-51 and
  * bindings/python/src/sgp4.zig:216); pass n and 0 for a stand-alone constellation.
- * d_status (nullable): n*n_times bytes, satellite-major, per-cell ASTROZ_CELL_* code.
+ * d_status (nullable): n*n_times bytes, satellite-major, per-cell ASTROZ_CELL_* code: this handle's satellite i at
+ * i*n_times whatever out_num_sats / out_sat_offset are (the status block is not part of the larger block).
  * stream: a cudaStream_t (NULL = the handle's own stream); the call is asynchronous on it. */
 int32_t astroz_cuda_constellation_propagate_device(astroz_constellation_t h, const double *jd, const double *fr,
                                                    uint32_t n_times, double *d_pos, double *d_vel, uint8_t *d_status,
