@@ -114,6 +114,12 @@ def lib() -> C.CDLL:
                                                          C.c_double, C.c_double, i32, vp, vp, vp]),
         "astroz_cuda_propagate_numerical_models_device": (i32, [vp, u32, C.c_double, C.c_double, C.c_double, vp, u32,
                                                                 i32, C.c_double, C.c_double, i32, vp, vp, vp, vp]),
+        "astroz_cuda_propagate_maneuvers": (i32, [vp, u32, C.c_double, C.c_double, C.c_double, C.c_double, vp, vp,
+                                                  u32, vp, u32, i32, C.c_double, C.c_double, u32, i32, vp, vp, vp, vp,
+                                                  vp]),
+        "astroz_cuda_propagate_maneuvers_device": (i32, [vp, u32, C.c_double, C.c_double, C.c_double, C.c_double, vp,
+                                                         vp, u32, vp, u32, i32, C.c_double, C.c_double, u32, i32, vp, vp,
+                                                         vp, vp, vp, vp]),
         "astroz_cuda_fit_elements": (i32, [vp, u32, i32, vp, vp, vp, vp, vp, u32, C.c_double, C.c_double, i32, u32,
                                            i32, vp, vp, vp, vp]),
         "astroz_cuda_fit_elements_device": (i32, [vp, u32, i32, vp, vp, vp, vp, vp, C.c_double, C.c_double, i32, u32,
@@ -156,6 +162,7 @@ EXPORTS = [
     "astroz_cuda_constellation_propagate_pairs", "astroz_cuda_constellation_propagate_pairs_device",
     "astroz_cuda_numerical_times", "astroz_cuda_propagate_numerical", "astroz_cuda_propagate_numerical_device",
     "astroz_cuda_propagate_numerical_models", "astroz_cuda_propagate_numerical_models_device",
+    "astroz_cuda_propagate_maneuvers", "astroz_cuda_propagate_maneuvers_device",
     "astroz_cuda_fit_elements", "astroz_cuda_fit_elements_device", "astroz_cuda_fit_elements_mixed",
     "astroz_cuda_fit_elements_mixed_device", "astroz_cuda_parse_tle",
 ]

@@ -2168,30 +2168,31 @@ int32_t astroz_cuda_propagate_numerical_device(const double *d_states, uint32_t 
 // Host buffers: chunks of states, each chunk's trajectory block at most kNumChunkBytes (eight ring pieces), through the
 // device's two-slot pipeline (az::ChunkPipeline).  `cols` are the per-state input columns the kernel reads ([n] doubles
 // each; the fixed drag set has three, a model list one per per-state array it names); `tabs` are whole arrays of
-// tabBytes each, uploaded once per call before the first chunk (a model list's position tables).  a holds the checked
-// arguments; for each chunk its n, states, out, status and counts are set to the chunk's and launch(dCols, dTabs, s)
-// queues the kernel.
+// tabBytes each, uploaded once per call before the first chunk (a model list's position tables, a maneuver call's
+// schedules).  The per-state results are the columns res[nRes]; rowBytes, the bytes of one state's trajectory, sizes the
+// chunks.  For each chunk, launch(first, m, dStates, dRes, dCols, dTabs, s) queues the kernel.
 static constexpr size_t kNumChunkBytes = 256u << 20;
 static constexpr int kNumMaxCols = 3 * (int)az::kMaxModels, kNumMaxTabs = (int)az::kMaxModels;
 using NumLaunch = std::function<cudaError_t(const double *const *dCols, const double *const *dTabs, cudaStream_t s)>;
-static int32_t numerical_host(az::NumArgs &a, const double *states, int nCols, const double *const *cols, int nTabs,
-                              const double *const *tabs, size_t tabBytes, int32_t device, double *out, uint8_t *status,
-                              uint64_t *steps, const NumLaunch &launch) {
+// one chunk: its first state, its state count, its device states and result columns, the per-state columns and tables
+using NumRowsLaunch =
+    std::function<cudaError_t(uint32_t first, uint32_t m, const double *dStates, void *const *dRes,
+                              const double *const *dCols, const double *const *dTabs, cudaStream_t s)>;
+static int32_t numerical_host_rows(uint32_t n, const double *states, int nCols, const double *const *cols, int nTabs,
+                                   const double *const *tabs, size_t tabBytes, int32_t device, int nRes,
+                                   const az::HostOut *res, size_t rowBytes, const NumRowsLaunch &launch) {
     NumericalContext *c = nullptr;
     int32_t rc = numerical_context(device, &c);
     if (rc != ASTROZ_OK) return rc;
     std::lock_guard<std::mutex> lk(c->m);
     AZ_CUDA(cudaSetDevice(device));
     cudaStream_t st = c->stream;
-    const uint32_t n = a.n;
-    const size_t rowBytes = ((size_t)a.steps.nFull + a.steps.nTail + 1) * 48;  // one state's trajectory
     const uint32_t chunk = (uint32_t)std::max<size_t>(1, std::min<size_t>(n, kNumChunkBytes / rowBytes));
     az::HostIn in[1 + kNumMaxCols] = {{states, 48}};
     for (int q = 0; q < nCols; ++q) in[1 + q] = {cols[q], 8};
-    const az::HostOut res[3] = {{out, rowBytes}, {status, 1}, {steps, 16}};
     StreamBuf dIn(st), dOut(st), dTab(st);
     AZ_CUDA(dIn.alloc(az::chunk_slots_bytes(in, 1 + nCols, n, chunk)));
-    AZ_CUDA(dOut.alloc(az::chunk_slots_bytes(res, 3, n, chunk)));
+    AZ_CUDA(dOut.alloc(az::chunk_slots_bytes(res, nRes, n, chunk)));
     const double *dTabs[kNumMaxTabs] = {};
     if (nTabs) {
         AZ_CUDA(dTab.alloc(nTabs * tabBytes));
@@ -2201,16 +2202,11 @@ static int32_t numerical_host(az::NumArgs &a, const double *states, int nCols, c
             dTabs[t] = at;
         }
     }
-    AZ_CUDA(c->pipe.run(st, c->copyStream, n, chunk, 1 + nCols, in, 3, res, dIn.p, dOut.p,
-                        [&](uint32_t, uint32_t, uint32_t m, void *const *dI, void *const *dO, cudaStream_t s) {
+    AZ_CUDA(c->pipe.run(st, c->copyStream, n, chunk, 1 + nCols, in, nRes, res, dIn.p, dOut.p,
+                        [&](uint32_t, uint32_t first, uint32_t m, void *const *dI, void *const *dO, cudaStream_t s) {
                             const double *dCols[kNumMaxCols] = {};
                             for (int q = 0; q < nCols; ++q) dCols[q] = static_cast<const double *>(dI[1 + q]);
-                            a.n = m;
-                            a.states = static_cast<const double *>(dI[0]);
-                            a.out = static_cast<double *>(dO[0]);
-                            a.status = static_cast<uint8_t *>(dO[1]);
-                            a.counts = static_cast<uint64_t *>(dO[2]);
-                            return launch(dCols, dTabs, s);
+                            return launch(first, m, static_cast<const double *>(dI[0]), dO, dCols, dTabs, s);
                         }));
     // give the slots back before returning (the default pool keeps nothing across a synchronisation)
     AZ_CUDA(dIn.release());
@@ -2218,6 +2214,25 @@ static int32_t numerical_host(az::NumArgs &a, const double *states, int nCols, c
     AZ_CUDA(dTab.release());
     AZ_CUDA(cudaStreamSynchronize(st));
     return ASTROZ_OK;
+}
+
+// K7's results: trajectory rows, status bytes and step counts.  a holds the checked arguments; for each chunk its n,
+// states, out, status and counts are set to the chunk's and launch(dCols, dTabs, s) queues the kernel.
+static int32_t numerical_host(az::NumArgs &a, const double *states, int nCols, const double *const *cols, int nTabs,
+                              const double *const *tabs, size_t tabBytes, int32_t device, double *out, uint8_t *status,
+                              uint64_t *steps, const NumLaunch &launch) {
+    const size_t rowBytes = ((size_t)a.steps.nFull + a.steps.nTail + 1) * 48;  // one state's trajectory
+    const az::HostOut res[3] = {{out, rowBytes}, {status, 1}, {steps, 16}};
+    return numerical_host_rows(a.n, states, nCols, cols, nTabs, tabs, tabBytes, device, 3, res, rowBytes,
+                               [&](uint32_t, uint32_t m, const double *dStates, void *const *dO,
+                                   const double *const *dCols, const double *const *dTabs, cudaStream_t s) {
+                                   a.n = m;
+                                   a.states = dStates;
+                                   a.out = static_cast<double *>(dO[0]);
+                                   a.status = static_cast<uint8_t *>(dO[1]);
+                                   a.counts = static_cast<uint64_t *>(dO[2]);
+                                   return launch(dCols, dTabs, s);
+                               });
 }
 
 int32_t astroz_cuda_propagate_numerical(const double *states, uint32_t n, double t0, double duration, double dt,
@@ -2364,6 +2379,132 @@ int32_t astroz_cuda_propagate_numerical_models(const double *states, uint32_t n,
                               for (int t = 0; t < nTabs; ++t) *tabOf[t] = dTabs[t];
                               return az::launch_numerical_models(ma, integrator, s);
                           });
+}
+
+// ---- impulsive maneuvers (K7 maneuvers, az_numerical.cu) ----
+static_assert(sizeof(astroz_impulse_t) == sizeof(az::Impulse) &&
+                  offsetof(astroz_impulse_t, p) == offsetof(az::Impulse, p),
+              "astroz_impulse_t is az::Impulse");
+static_assert(ASTROZ_IMPULSE_ABSOLUTE == az::kImpAbsolute && ASTROZ_IMPULSE_PROGRADE == az::kImpPrograde &&
+                  ASTROZ_IMPULSE_PHASE == az::kImpPhase && ASTROZ_IMPULSE_PLANE_CHANGE == az::kImpPlaneChange &&
+                  ASTROZ_MANEUVER_ABNORMAL == az::kManAbnormal && ASTROZ_MANEUVER_TRUNCATED == az::kManTruncated,
+              "impulse kinds and maneuver status bytes");
+
+// Checks of every maneuver call, before anything is read, written or allocated (the impulses and offsets only where
+// they are host memory).  On success a receives the scalars and the model list.
+static int32_t maneuvers_check(uint32_t n, double t0, double duration, double h, double mu,
+                               const uint32_t *offsets, const astroz_impulse_t *impulses, uint32_t m, bool host,
+                               const astroz_force_model_t *models, uint32_t nModels, int32_t integrator, double rtol,
+                               double atol, uint32_t maxSamples, int32_t device, az::ManeuverArgs *a) {
+    int32_t rc = models_check(models, nModels, &a->models);
+    if (rc != ASTROZ_OK) return rc;
+    for (uint32_t j = 0; j < nModels; ++j)
+        if (models[j].flags & ASTROZ_MODEL_POS_TABLE)
+            return value_error("position tables follow K7's shared output intervals: a maneuver call refuses them");
+    az::NumArgs na{};
+    if ((rc = numerical_check(n, t0, duration, h, integrator, rtol, atol, device, &na)) != ASTROZ_OK) return rc;
+    if (!std::isfinite(mu)) return value_error("mu must be finite");
+    if (maxSamples == 0) return value_error("max_samples must be at least 1");
+    if ((uint64_t)n * maxSamples > SIZE_MAX / 56) return value_error("the output size overflows");
+    if (host) {
+        if (!offsets || (m && !impulses)) return ASTROZ_NULL_POINTER;
+        for (uint32_t i = 0; i < n; ++i)
+            if (offsets[i + 1] < offsets[i]) return value_error("impulse_offsets decrease");
+        if (offsets[n] != m) return value_error("impulse_offsets[n] must equal m");
+        for (uint32_t k = 0; k < m; ++k) {
+            const astroz_impulse_t &b = impulses[k];
+            if (b.kind < ASTROZ_IMPULSE_ABSOLUTE || b.kind > ASTROZ_IMPULSE_PLANE_CHANGE)
+                return value_error("unknown impulse kind");
+            if (!std::isfinite(b.time) || !std::isfinite(b.p[0]) || !std::isfinite(b.p[1]) || !std::isfinite(b.p[2]))
+                return value_error("an impulse's time or parameter is not finite");
+            if (b.kind == ASTROZ_IMPULSE_PHASE && !(b.p[1] > 0.0)) return value_error("a phasing burn needs orbits > 0");
+        }
+    }
+    a->n = n;
+    a->t0 = t0;
+    a->tf = t0 + duration;
+    a->h = h;
+    a->p = az::NumParams{mu, 0.0, 0.0, rtol, atol};
+    a->maxSamples = maxSamples;
+    return ASTROZ_OK;
+}
+
+int32_t astroz_cuda_propagate_maneuvers_device(const double *d_states, uint32_t n, double t0, double duration, double h,
+                                               double mu, const uint32_t *d_impulse_offsets,
+                                               const astroz_impulse_t *d_impulses, uint32_t m,
+                                               const astroz_force_model_t *models, uint32_t n_models, int32_t integrator,
+                                               double rtol, double atol, uint32_t max_samples, int32_t device,
+                                               double *d_times, double *d_out, uint64_t *d_n_samples, uint8_t *d_status,
+                                               uint64_t *d_steps, void *stream) {
+    az::ManeuverArgs a{};
+    int32_t rc = maneuvers_check(n, t0, duration, h, mu, nullptr, nullptr, m, false, models, n_models, integrator, rtol,
+                                 atol, max_samples, device, &a);
+    if (rc != ASTROZ_OK) return rc;
+    if (n == 0) return ASTROZ_OK;
+    if (!d_states || !d_impulse_offsets || (m && !d_impulses) || !d_times || !d_out || !d_n_samples || !d_status)
+        return ASTROZ_NULL_POINTER;
+    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
+    AZ_CUDA(cudaSetDevice(device));
+    a.states = d_states;
+    a.offsets = d_impulse_offsets;
+    a.impulses = reinterpret_cast<const az::Impulse *>(d_impulses);
+    a.times = d_times;
+    a.out = d_out;
+    a.count = d_n_samples;
+    a.status = d_status;
+    a.counts = d_steps;
+    // the scalars and the model list travel in the launch's parameters: the call only queues the kernel
+    AZ_CUDA(az::launch_maneuvers(a, integrator, static_cast<cudaStream_t>(stream)));
+    return ASTROZ_OK;
+}
+
+int32_t astroz_cuda_propagate_maneuvers(const double *states, uint32_t n, double t0, double duration, double h, double mu,
+                                        const uint32_t *impulse_offsets, const astroz_impulse_t *impulses, uint32_t m,
+                                        const astroz_force_model_t *models, uint32_t n_models, int32_t integrator,
+                                        double rtol, double atol, uint32_t max_samples, int32_t device, double *times,
+                                        double *out, uint64_t *n_samples, uint8_t *status, uint64_t *steps) {
+    az::ManeuverArgs a{};
+    int32_t rc = maneuvers_check(n, t0, duration, h, mu, impulse_offsets, impulses, m, true, models, n_models,
+                                 integrator, rtol, atol, max_samples, device, &a);
+    if (rc != ASTROZ_OK) return rc;
+    if (n == 0) return ASTROZ_OK;
+    if (!states || !times || !out || !n_samples || !status) return ASTROZ_NULL_POINTER;
+    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
+    // per-state columns in list order (as for model lists), and the schedules as one whole array: the impulses, then
+    // the offsets, uploaded once per call
+    const double *cols[kNumMaxCols];
+    const double **colOf[kNumMaxCols];
+    int nCols = 0;
+    for (uint32_t j = 0; j < n_models; ++j) {
+        az::ForceModel &fm = a.models.m[j];
+        for (const double **p : {&fm.c_arr, &fm.area_arr, &fm.mass_arr})
+            if (*p) cols[nCols] = *p, colOf[nCols++] = p;
+    }
+    const size_t impBytes = (size_t)m * sizeof(astroz_impulse_t), offBytes = ((size_t)n + 1) * 4;
+    std::vector<double> sched((impBytes + offBytes + 7) / 8);
+    if (m) std::memcpy(sched.data(), impulses, impBytes);
+    std::memcpy(reinterpret_cast<char *>(sched.data()) + impBytes, impulse_offsets, offBytes);
+    const double *tabs[1] = {sched.data()};
+    const size_t rowSamples = max_samples;
+    const az::HostOut res[5] = {
+        {times, rowSamples * 8}, {out, rowSamples * 48}, {n_samples, 8}, {status, 1}, {steps, 16}};
+    return numerical_host_rows(n, states, nCols, cols, 1, tabs, sched.size() * 8, device, 5, res, rowSamples * 56,
+                               [&](uint32_t first, uint32_t cm, const double *dStates, void *const *dO,
+                                   const double *const *dCols, const double *const *dTabs, cudaStream_t s) {
+                                   for (int q = 0; q < nCols; ++q) *colOf[q] = dCols[q];
+                                   a.n = cm;
+                                   a.first = first;
+                                   a.states = dStates;
+                                   a.impulses = reinterpret_cast<const az::Impulse *>(dTabs[0]);
+                                   a.offsets = reinterpret_cast<const uint32_t *>(
+                                       reinterpret_cast<const char *>(dTabs[0]) + impBytes);
+                                   a.times = static_cast<double *>(dO[0]);
+                                   a.out = static_cast<double *>(dO[1]);
+                                   a.count = static_cast<uint64_t *>(dO[2]);
+                                   a.status = static_cast<uint8_t *>(dO[3]);
+                                   a.counts = static_cast<uint64_t *>(dO[4]);
+                                   return az::launch_maneuvers(a, integrator, s);
+                               });
 }
 
 // ---- element fits (K8, az_fit.cu) ------------------------------------------------------------------------------------

@@ -64,7 +64,42 @@ __global__ void __launch_bounds__(kNumThreads) numerical_models_kernel(const __g
     }
 }
 
+// Maneuver schedules: one state per thread, the list a __grid_constant__ parameter as above; each thread walks its own
+// impulses, so a warp's lanes diverge where their schedules differ.
+template <int kInt>
+__global__ void __launch_bounds__(kNumThreads) maneuvers_kernel(const __grid_constant__ ManeuverArgs a) {
+    const uint32_t i = blockIdx.x * kNumThreads + threadIdx.x;
+    if (i >= a.n) return;
+    double y0[6];
+#pragma unroll
+    for (int c = 0; c < 6; ++c) y0[c] = a.states[(size_t)i * 6 + c];
+    const uint32_t b = a.offsets[a.first + i], e = a.offsets[a.first + i + 1];
+    ManeuverRow row{a.times + (size_t)i * a.maxSamples, a.out + (size_t)i * a.maxSamples * 6, a.maxSamples, 0};
+    uint64_t counts[2];
+    const uint8_t st = maneuver_state_models<kInt>(y0, a.models, i, a.p, a.t0, a.tf, a.h, a.impulses + b, e - b, row,
+                                                   counts);
+    a.status[i] = st;
+    a.count[i] = row.count;
+    if (a.counts) {
+        a.counts[(size_t)i * 2] = counts[0];
+        a.counts[(size_t)i * 2 + 1] = counts[1];
+    }
+}
+
 }  // namespace
+
+cudaError_t launch_maneuvers(const ManeuverArgs &a, int integrator, cudaStream_t s) {
+    if (a.n == 0) return cudaSuccess;
+    const dim3 grid((a.n + kNumThreads - 1) / kNumThreads);
+    if (integrator == kIntRk4) {
+        maneuvers_kernel<kIntRk4><<<grid, kNumThreads, 0, s>>>(a);
+    } else if (integrator == kIntDp87) {
+        maneuvers_kernel<kIntDp87><<<grid, kNumThreads, 0, s>>>(a);
+    } else {
+        return cudaErrorInvalidValue;
+    }
+    return cudaGetLastError();
+}
 
 cudaError_t launch_numerical_models(const ModelArgs &m, int integrator, cudaStream_t s) {
     if (m.a.n == 0) return cudaSuccess;

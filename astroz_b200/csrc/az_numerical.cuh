@@ -557,6 +557,182 @@ AZ_HD uint8_t propagate_state_models(const double y0[6], const ModelList &L, uin
     return propagate_with<kInt>(y0, f, p, steps, out, counts);
 }
 
+// ---- impulsive maneuvers: Spacecraft.propagate's loop (src/Spacecraft.zig:172-323) over a model list -----------------
+// impulse kinds (ASTROZ_IMPULSE_*) and the status bytes of the maneuver calls beyond K7's (ASTROZ_MANEUVER_*)
+constexpr int32_t kImpAbsolute = 0, kImpPrograde = 1, kImpPhase = 2, kImpPlaneChange = 3;
+constexpr uint8_t kManAbnormal = 4, kManTruncated = 5;
+// a trajectory has at most this many samples; one more stops the state (bounds a phasing coast of huge `orbits`)
+constexpr uint64_t kManMaxSamples = 0xfffffffeull;
+
+// One impulse of a schedule, the layout of astroz_impulse_t.  p: ABSOLUTE dv[3] km/s; PROGRADE p[0] = dv km/s; PHASE
+// p[0] = angle rad, p[1] = orbits; PLANE_CHANGE p[0] = delta inclination rad, p[1] = delta RAAN rad.
+struct Impulse {
+    double time;
+    int32_t kind;
+    uint32_t reserved;
+    double p[3];
+};
+
+// std.math.pow(f64, x, 3) as Zig evaluates an integral exponent (repeated squaring of the significand): x * (x * x)
+AZ_HD double zig_pow3(double x) { return x * (x * x); }
+// std.math.pow(f64, x, 2.0 / 3.0) as Zig evaluates it: the fractional part above 0.5 becomes 2/3 - 1 through exp(log),
+// the integral part 1 multiplies the significand back in
+AZ_HD double zig_pow_two_thirds(double x) { return exp((2.0 / 3.0 - 1.0) * log(x)) * x; }
+
+// calculatePhaseChange (Spacecraft.zig:310-323): the prograde dv of a phasing orbit from radius r
+AZ_HD double phase_dv(double radius, double phaseAngle, double transferOrbits, double mu) {
+    const double vCircular = sqrt(mu / radius);
+    const double period = 2.0 * kPi * sqrt(zig_pow3(radius) / mu);
+    const double deltaT = phaseAngle * period / (2.0 * kPi * transferOrbits);
+    const double transferPeriod = period + deltaT;
+    const double aTransfer = zig_pow_two_thirds(transferPeriod * sqrt(mu) / (2.0 * kPi));
+    const double vTransfer = sqrt(mu * (2.0 / radius - 1.0 / aTransfer));
+    return vTransfer - vCircular;
+}
+
+// progradeVec (Spacecraft.zig:260-263)
+AZ_HD void prograde_vec(const double y[6], double dvMag, double dv[3]) {
+    const double vMag = sqrt(y[3] * y[3] + y[4] * y[4] + y[5] * y[5]);
+    dv[0] = y[3] / vMag * dvMag, dv[1] = y[4] / vMag * dvMag, dv[2] = y[5] / vMag * dvMag;
+}
+
+// calculations.impulse (calculations.zig:480-485)
+AZ_HD void apply_dv(double y[6], double dx, double dy, double dz) {
+    y[3] = y[3] + dx, y[4] = y[4] + dy, y[5] = y[5] + dz;
+}
+
+// applyPlaneChange (Spacecraft.zig:272-307), its "simplified" direction kept: dv = (hx sin di, hy sin di, hz cos di) *
+// dvMag / |h|, which is the reference's result and not the textbook plane change
+AZ_HD void plane_change(double y[6], double deltaInclination, double deltaRaan) {
+    const double vMag = sqrt(y[3] * y[3] + y[4] * y[4] + y[5] * y[5]);
+    const double totalAngle = sqrt(deltaInclination * deltaInclination + deltaRaan * deltaRaan);
+    if (totalAngle < 1e-10) return;
+    const double dvMag = 2.0 * vMag * sin(totalAngle / 2.0);
+    const double hx = y[1] * y[5] - y[2] * y[4];
+    const double hy = y[2] * y[3] - y[0] * y[5];
+    const double hz = y[0] * y[4] - y[1] * y[3];
+    const double hMag = sqrt(hx * hx + hy * hy + hz * hz);
+    const double si = sin(deltaInclination), ci = cos(deltaInclination);
+    apply_dv(y, hx / hMag * dvMag * si, hy / hMag * dvMag * si, hz / hMag * dvMag * ci);
+}
+
+// One state's row of a maneuver call: sample j's time at times[j] and state at out[6 j] while j < cap; count counts
+// every sample, written or not.
+struct ManeuverRow {
+    double *times, *out;
+    uint64_t cap, count;
+    // false when the sample would pass kManMaxSamples
+    AZ_HD bool append(double t, const double y[6]) {
+        if (count == kManMaxSamples) return false;
+        if (count < cap) {
+            times[count] = t;
+#pragma unroll
+            for (int c = 0; c < 6; ++c) out[count * 6 + c] = y[c];
+        }
+        ++count;
+        return true;
+    }
+};
+
+// Spacecraft.propagate (Spacecraft.zig:172-270) for one state, line for line, with the force f, the integrator kInt and
+// the impulses imp[m] in list order:
+//   append (t0, y0); while t < tf { fire every impulse with time <= t + h (a partial step to it when it lies ahead, the
+//   burn, a sample); a regular step of min(h, tf - t); a sample; stop when the orbit is abnormal }.
+// A DP87 step carries hCur through every call (partial steps, phasing coasts, regular steps).  Writes row.count
+// samples (the first row.cap of them) and zero-fills the rest of the row.  Status: kManTruncated when count > cap, else
+// kNumStopped (a DP87 rejection at hMin, or a sample past kManMaxSamples), kNumSubstepLimit, kNumNonFinite,
+// kManAbnormal (the reference's abnormal-orbit stop), kNumOk.
+template <int kInt, class F>
+AZ_HD uint8_t maneuver_with(const double y0[6], F &f, const NumParams &p, double t0, double tf, double h,
+                            const Impulse *imp, uint32_t m, ManeuverRow &row, uint64_t counts[2]) {
+    double y[6];
+#pragma unroll
+    for (int c = 0; c < 6; ++c) y[c] = y0[c];
+    counts[0] = counts[1] = 0;
+    row.count = 0;
+    uint8_t status = kNumOk;
+    bool stopped = false, abnormal = false;
+    double hCur = kDpHStart;
+    double t = t0;
+    // Integrator.step of length dt from y; false when the state stops
+    auto step = [&](double dt) -> bool {
+        if (kInt == kIntRk4) {
+            rk4_step(y, dt, f);
+            ++counts[0];
+            if (status == kNumOk && !all_finite(y)) status = kNumNonFinite;
+            return true;
+        }
+        const uint8_t st = dp87_interval(y, hCur, dt, f, p, counts);
+        if (st == kNumSubstepLimit) status = kNumSubstepLimit;
+        return st != kNumStopped;
+    };
+    row.append(t, y);
+    uint32_t idx = 0;
+    while (t < tf && !stopped) {
+        while (idx < m && imp[idx].time <= t + h) {
+            const Impulse &b = imp[idx];
+            const double dt = b.time - t;
+            if (dt > 0) {
+                if (!step(dt)) { stopped = true; break; }
+                t += dt;
+                if (!row.append(t, y)) { stopped = true; break; }
+            }
+            if (b.kind == kImpAbsolute) {
+                apply_dv(y, b.p[0], b.p[1], b.p[2]);
+            } else if (b.kind == kImpPrograde) {
+                double dv[3];
+                prograde_vec(y, b.p[0], dv);
+                apply_dv(y, dv[0], dv[1], dv[2]);
+            } else if (b.kind == kImpPhase) {  // applyImpulse's .phase (Spacecraft.zig:237-252)
+                const double r = sqrt(y[0] * y[0] + y[1] * y[1] + y[2] * y[2]);
+                double dv[3];
+                prograde_vec(y, phase_dv(r, b.p[0], b.p[1], p.mu), dv);
+                apply_dv(y, dv[0], dv[1], dv[2]);
+                const double period = 2.0 * kPi * sqrt(zig_pow3(r) / p.mu);
+                const double tEnd = t + period * b.p[1];
+                for (; t < tEnd && !stopped; t += h)
+                    stopped = !step(h) || !row.append(t + h, y);
+                if (stopped) break;
+                apply_dv(y, -dv[0], -dv[1], -dv[2]);
+            } else {
+                plane_change(y, b.p[0], b.p[1]);
+            }
+            if (!row.append(t, y)) { stopped = true; break; }
+            ++idx;
+        }
+        if (stopped) break;
+        const double s = fmin(h, tf - t);
+        if (!step(s)) { stopped = true; break; }
+        t += s;
+        if (!row.append(t, y)) { stopped = true; break; }
+        // the abnormal-orbit test (Spacecraft.zig:263-269, calculateEnergy :265-269)
+        const double r = sqrt(y[0] * y[0] + y[1] * y[1] + y[2] * y[2]);
+        const double v = sqrt(y[3] * y[3] + y[4] * y[4] + y[5] * y[5]);
+        const double energy = 0.5 * v * v - p.mu / r;
+        if (energy > 0 || isnan(energy) || r > 100000) {
+            abnormal = true;
+            break;
+        }
+    }
+    for (uint64_t j = row.count; j < row.cap; ++j) {
+        row.times[j] = 0.0;
+#pragma unroll
+        for (int c = 0; c < 6; ++c) row.out[j * 6 + c] = 0.0;
+    }
+    if (row.count > row.cap) return kManTruncated;
+    if (stopped) return kNumStopped;
+    if (status != kNumOk) return status;
+    return abnormal ? kManAbnormal : kNumOk;
+}
+
+template <int kInt>
+AZ_HD uint8_t maneuver_state_models(const double y0[6], const ModelList &L, uint32_t i, const NumParams &p, double t0,
+                                    double tf, double h, const Impulse *imp, uint32_t m, ManeuverRow &row,
+                                    uint64_t counts[2]) {
+    ListForces f{L, i};
+    return maneuver_with<kInt>(y0, f, p, t0, tf, h, imp, m, row, counts);
+}
+
 }  // namespace az
 
 #ifndef AZ_NUMERICAL_CORES_ONLY
@@ -580,5 +756,23 @@ struct ModelArgs {
     ModelList models;
 };
 cudaError_t launch_numerical_models(const ModelArgs &a, int integrator, cudaStream_t s);
+// K7 maneuvers: a model list (no position tables) and per-state impulse schedules.  State i (of this launch; `first` +
+// i of the call) fires impulses[offsets[first + i] .. offsets[first + i + 1]).
+struct ManeuverArgs {
+    const double *states;      // [n][6]
+    uint32_t n, first;
+    double t0, tf, h;
+    NumParams p;               // mu: the central body's; rtol / atol: DP87's
+    const uint32_t *offsets;   // [call's n + 1]
+    const Impulse *impulses;   // [m]
+    uint32_t maxSamples;
+    double *times;             // [n][maxSamples]
+    double *out;               // [n][maxSamples][6]
+    uint64_t *count;           // [n]
+    uint8_t *status;           // [n]
+    uint64_t *counts;          // [n][2] or nullptr
+    ModelList models;
+};
+cudaError_t launch_maneuvers(const ManeuverArgs &a, int integrator, cudaStream_t s);
 }  // namespace az
 #endif

@@ -334,6 +334,230 @@ def propagate_models_batch_device(states, t0, duration, dt, models, out, status,
     del keep
 
 
+# ---- impulsive maneuvers: the loop of the reference's Spacecraft.propagate (src/Spacecraft.zig:172-323) -------------
+# status bytes beyond the batch calls' (ASTROZ_MANEUVER_*)
+ABNORMAL, TRUNCATED = 4, 5
+EARTH_MU = 398600.5   # WGS-84 (src/constants.zig:55-58), the reference's default orbitingObject.mu
+# astroz_impulse_t
+IMPULSE_DTYPE = np.dtype([("time", "<f8"), ("kind", "<i4"), ("reserved", "<u4"), ("p", "<f8", (3,))])
+
+
+class _Impulse:
+    """An impulse of a schedule: its time [s, the states' clock] and the kind's parameters."""
+    kind = -1
+
+    def __init__(self, t, *p):
+        self.time, self.p = float(t), tuple(float(x) for x in p) + (0.0,) * (3 - len(p))
+
+    def __repr__(self):
+        return f"{type(self).__name__}({self.time!r}, {', '.join(repr(x) for x in self.p)})"
+
+
+class Absolute(_Impulse):
+    """Absolute(t, dv): velocity += dv (a 3-vector, km/s), calculations.impulse (calculations.zig:480-485)"""
+    kind = 0
+
+    def __init__(self, t, dv):
+        dv = [float(x) for x in dv]
+        if len(dv) != 3:
+            raise ValueError("dv is a 3-vector")
+        super().__init__(t, *dv)
+
+
+class Prograde(_Impulse):
+    """Prograde(t, dv): dv km/s along the velocity (Spacecraft.zig:260-263)"""
+    kind = 1
+
+    def __init__(self, t, dv):
+        super().__init__(t, dv)
+
+
+class Phase(_Impulse):
+    """Phase(t, angle, orbits=1.0): the reference's phasing maneuver (Spacecraft.zig:237-252, :310-323): a prograde
+    burn, a coast of `orbits` periods of the circular orbit at the burn's radius sampled every h, then the opposite
+    burn.  angle in rad, orbits > 0."""
+    kind = 2
+
+    def __init__(self, t, angle, orbits=1.0):
+        super().__init__(t, angle, orbits)
+
+
+class PlaneChange(_Impulse):
+    """PlaneChange(t, d_incl, d_raan): the reference's applyPlaneChange (Spacecraft.zig:272-307), nothing below 1e-10
+    rad.  Its Δv points along (hx sin di, hy sin di, hz cos di) / |h|, the reference's "simplified" direction -- not
+    the textbook plane change."""
+    kind = 3
+
+    def __init__(self, t, d_incl, d_raan):
+        super().__init__(t, d_incl, d_raan)
+
+
+def pack_schedules(schedules, n):
+    """(offsets[n + 1] uint32, impulses[m] IMPULSE_DTYPE) of `schedules`: one list of impulses shared by every state,
+    or n lists.  Impulse kinds and parameters are checked as the C ABI checks them."""
+    schedules = list(schedules)
+    if all(isinstance(b, _Impulse) for b in schedules):
+        schedules = [schedules] * n
+    elif len(schedules) != n:
+        raise ValueError(f"schedules must be one list of impulses or {n} lists")
+    lengths = [len(s) for s in schedules]
+    offsets = np.zeros(n + 1, dtype=np.uint32)
+    np.cumsum(lengths, out=offsets[1:])
+    imp = np.zeros(int(offsets[-1]), dtype=IMPULSE_DTYPE)
+    k = 0
+    for s in schedules:
+        for b in s:
+            if not isinstance(b, _Impulse):
+                raise ValueError("a schedule holds Absolute / Prograde / Phase / PlaneChange impulses")
+            if not (np.isfinite(b.time) and all(np.isfinite(b.p))):
+                raise ValueError(f"{b!r}: time and parameters must be finite")
+            if b.kind == Phase.kind and not b.p[1] > 0:
+                raise ValueError(f"{b!r}: orbits must be > 0")
+            imp[k] = (b.time, b.kind, 0, b.p)
+            k += 1
+    return offsets, imp
+
+
+def _estimate_samples(states, t0, duration, h, offsets, imp, mu):
+    """Rows for a first call: the regular samples, 3 per burn (the partial step, the burn sample, one more regular step
+    on the shifted grid) and every phasing coast at the state's initial radius with 10 % slack."""
+    base = len(numerical_times(t0, duration, h)) + 3 * int(np.max(np.diff(offsets), initial=0))
+    phase = np.flatnonzero(imp["kind"] == Phase.kind)
+    if len(phase) == 0:
+        return base
+    owner = np.searchsorted(offsets, phase, side="right") - 1
+    r = np.linalg.norm(states[owner, :3], axis=1)
+    coast = np.ceil(1.1 * 2.0 * np.pi * np.sqrt(r ** 3 / mu) * imp["p"][phase, 1] / h) + 2
+    extra = np.zeros(len(states))
+    np.add.at(extra, owner, coast)
+    return int(min(base + extra.max(), 0xfffffffe))
+
+
+def _subset(models, idx):
+    """The models with their per-state coefficients cut to the states idx"""
+    import copy
+
+    out = []
+    for m in models:
+        c = copy.copy(m)
+        c._coefs = {k: (np.asarray(v)[idx] if np.ndim(v) == 1 else v) for k, v in m._coefs.items()}
+        out.append(c)
+    return out
+
+
+def _maneuvers_call(states, t0, duration, h, models, offsets, imp, mu, integrator, rtol, atol, max_samples, device):
+    n = states.shape[0]
+    descs, keep = _descriptors(models, n, 0, _host_array)
+    times = np.empty((n, max_samples))
+    traj = np.empty((n, max_samples, 6))
+    count = np.zeros(n, dtype=np.uint64)
+    status = np.zeros(n, dtype=np.uint8)
+    steps = np.zeros((n, 2), dtype=np.uint64)
+    vp = lambda a: C.c_void_p(a.ctypes.data)  # noqa: E731
+    check(lib().astroz_cuda_propagate_maneuvers(
+        vp(states), n, float(t0), float(duration), float(h), float(mu), vp(offsets), vp(imp) if len(imp) else None,
+        len(imp), C.cast(descs, C.c_void_p), len(descs), _integrator(integrator), float(rtol), float(atol),
+        int(max_samples), int(device), vp(times), vp(traj), vp(count), vp(status), vp(steps)))
+    del keep
+    return times, traj, count, status, steps
+
+
+def propagate_maneuvers_batch(states, t0, duration, h, models, schedules, *, mu=EARTH_MU, integrator="rk4", rtol=1e-9,
+                              atol=1e-12, max_samples=None, device=0):
+    """Propagate n states through impulse schedules, as the reference's Spacecraft.propagate does for one: step h
+    from t0 to t0 + duration under the model list, the impulses of each schedule fired in list order when their time
+    comes within the next step (an impulse before t0 fires at once), each burn sampled, stopping on an abnormal orbit.
+
+    states: (n, 6) km, km/s.  models: as propagate_models_batch (fixed positions only).  schedules: one list of
+    Absolute / Prograde / Phase / PlaneChange shared by every state, or n lists.  mu: the central body's parameter
+    (phasing burns and the abnormal-orbit test).  integrator: "rk4" (the reference's) or "dp87".
+    max_samples: the row length; None sizes the rows from an estimate and reruns the states that did not fit, once, at
+    their own sample count (a state's result depends on its own inputs only, so the bytes are those of an ample call).
+    Returns (times[n, S], traj[n, S, 6], n_samples[n] uint64, status[n] uint8, steps[n, 2] uint64).  Row i holds
+    n_samples[i] samples and zeros after them (all S when the state was TRUNCATED); sample times repeat at burns and the
+    last step can be negative after a phasing coast that passes t0 + duration."""
+    states = np.ascontiguousarray(states, dtype=np.float64)
+    if states.ndim != 2 or states.shape[1] != 6:
+        raise ValueError("states must have shape (n, 6)")
+    n = states.shape[0]
+    offsets, imp = pack_schedules(schedules, n)
+    models = list(models)
+    if max_samples is not None:
+        return _maneuvers_call(states, t0, duration, h, models, offsets, imp, mu, integrator, rtol, atol,
+                               int(max_samples), device)
+    first = _estimate_samples(states, t0, duration, h, offsets, imp, mu)
+    times, traj, count, status, steps = _maneuvers_call(states, t0, duration, h, models, offsets, imp, mu, integrator,
+                                                        rtol, atol, first, device)
+    again = np.flatnonzero(status == TRUNCATED)
+    if len(again) == 0:
+        return times, traj, count, status, steps
+    width = int(count[again].max())
+    sub_off = np.zeros(len(again) + 1, dtype=np.uint32)
+    np.cumsum(np.diff(offsets)[again], out=sub_off[1:])
+    sub_imp = np.concatenate([imp[offsets[i]:offsets[i + 1]] for i in again]) if len(imp) else imp
+    t2, y2, c2, s2, st2 = _maneuvers_call(np.ascontiguousarray(states[again]), t0, duration, h, _subset(models, again),
+                                          sub_off, sub_imp, mu, integrator, rtol, atol, width, device)
+    T = np.zeros((n, width))
+    Y = np.zeros((n, width, 6))
+    T[:, :first], Y[:, :first] = times, traj
+    T[again], Y[again], count[again], status[again], steps[again] = t2, y2, c2, s2, st2
+    return T, Y, count, status, steps
+
+
+def propagate_maneuvers_batch_device(states, t0, duration, h, models, schedules, times, out, n_samples, status,
+                                     steps=None, *, mu=EARTH_MU, integrator="rk4", rtol=1e-9, atol=1e-12,
+                                     stream: int = 0) -> None:
+    """`propagate_maneuvers_batch` with torch CUDA tensors on one device: states (n, 6) float64, per-state coefficients
+    as (n,) float64 tensors; schedules as there (checked here, then uploaded); times (n, S) float64, out (n, S, 6)
+    float64, n_samples (n,) int64, status (n,) uint8 and steps (n, 2) int64 (optional) receive the results, S being the
+    row length.  One kernel, asynchronous on `stream` (a raw cudaStream_t value, 0 = the default stream)."""
+    import torch
+
+    n = int(states.shape[0]) if states.dim() == 2 else -1
+    if n < 0 or states.shape[1] != 6 or states.dtype != torch.float64 or not states.is_cuda:
+        raise ValueError("states must be a CUDA float64 tensor of shape (n, 6)")
+    if not isinstance(times, torch.Tensor) or times.dim() != 2 or times.shape[0] != n:
+        raise ValueError("times must be a tensor of shape (n, max_samples)")
+    S = int(times.shape[1])
+    for name, t, size, dtype in (("times", times, n * S, torch.float64), ("out", out, n * S * 6, torch.float64),
+                                 ("n_samples", n_samples, n, torch.int64), ("status", status, n, torch.uint8),
+                                 ("steps", steps, n * 2, torch.int64)):
+        if t is None and name == "steps":
+            continue
+        if not isinstance(t, torch.Tensor) or t.dtype != dtype or not t.is_contiguous() or int(t.numel()) != size \
+                or t.device != states.device:
+            raise ValueError(f"{name} must be a contiguous {dtype} tensor of {size} elements on {states.device}")
+
+    def array(x, shape, name):
+        if not isinstance(x, torch.Tensor):
+            r = _host_array(x, shape, name)
+            if r is not None:
+                raise ValueError(f"{name}: per-state arrays must be CUDA tensors here")
+            return None
+        if x.dtype != torch.float64 or not x.is_contiguous() or tuple(x.shape) != shape or x.device != states.device:
+            raise ValueError(f"{name} must be a contiguous float64 tensor of shape {shape} on {states.device}")
+        return C.c_void_p(x.data_ptr()), x
+
+    descs, keep = _descriptors(models, n, 0, array)
+    offsets, imp = pack_schedules(schedules, n)
+    d_off = torch.from_numpy(offsets.view(np.int32)).to(states.device)
+    d_imp = torch.from_numpy(imp.view(np.uint8)).to(states.device)
+    torch.cuda.current_stream(states.device).synchronize()   # the uploads have landed before `stream` reads them
+    ptr = lambda t: None if t is None else C.c_void_p(t.data_ptr())  # noqa: E731
+    check(lib().astroz_cuda_propagate_maneuvers_device(
+        ptr(states), n, float(t0), float(duration), float(h), float(mu), ptr(d_off), ptr(d_imp) if len(imp) else None,
+        len(imp), C.cast(descs, C.c_void_p), len(descs), _integrator(integrator), float(rtol), float(atol), S,
+        int(states.device.index), ptr(times), ptr(out), ptr(n_samples), ptr(status), ptr(steps),
+        C.c_void_p(stream) if stream else None))
+    if stream:   # the schedules stay allocated until the kernel on `stream` has read them
+        ext = torch.cuda.ExternalStream(stream, device=states.device)
+        d_off.record_stream(ext)
+        d_imp.record_stream(ext)
+    del keep
+
+
 __all__ = ["propagate_numerical_batch", "propagate_numerical_batch_device", "numerical_times", "AstrozCudaError",
            "OK", "STOPPED", "SUBSTEP_LIMIT", "NON_FINITE", "propagate_models_batch", "propagate_models_batch_device",
-           "TwoBody", "J2", "J3", "J4", "Drag", "ImprovedDrag", "SolarRadiationPressure", "ThirdBody", "MAX_MODELS"]
+           "TwoBody", "J2", "J3", "J4", "Drag", "ImprovedDrag", "SolarRadiationPressure", "ThirdBody", "MAX_MODELS",
+           "ABNORMAL", "TRUNCATED", "EARTH_MU", "Absolute", "Prograde", "Phase", "PlaneChange", "pack_schedules",
+           "propagate_maneuvers_batch", "propagate_maneuvers_batch_device"]

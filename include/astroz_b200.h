@@ -478,6 +478,73 @@ int32_t astroz_cuda_propagate_numerical_models_device(const double *d_states, ui
                                                       double *d_out, uint8_t *d_status, uint64_t *d_steps,
                                                       void *stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Impulsive maneuvers: the loop of Spacecraft.propagate (src/Spacecraft.zig:172-323) for a batch of states, each with
+ * its own impulse schedule.  State i fires impulses[impulse_offsets[i] .. impulse_offsets[i + 1]) in list order (the
+ * list is not sorted), under the model list `models` with RK4 or DP87:
+ *   y = y0; t = t0; tf = t0 + duration; sample (t, y); idx = 0
+ *   while t < tf:
+ *       while idx < count and imp[idx].time <= t + h:     (an impulse before t0 fires at once)
+ *           dt = imp[idx].time - t; if dt > 0: step dt, t += dt, sample
+ *           burn imp[idx] (a phasing burn samples its coast and advances t); sample; idx += 1
+ *       s = min(h, tf - t); step s; t += s; sample    (s <= 0 after a phasing coast that passes tf)
+ *       stop when 0.5 v^2 - mu / r > 0, is NaN, or r > 100,000 km (status ASTROZ_MANEUVER_ABNORMAL)
+ * Burns, operation for operation as the reference's:
+ *   ASTROZ_IMPULSE_ABSOLUTE      velocity += p[0..2]                                   (calculations.zig:480-485)
+ *   ASTROZ_IMPULSE_PROGRADE      velocity += v / |v| * p[0]                            (Spacecraft.zig:260-263)
+ *   ASTROZ_IMPULSE_PHASE         the prograde dv of calculatePhaseChange(|r|, p[0], p[1]) (:310-323), a coast of
+ *                                `while t < tEnd { step h; sample (t + h); t += h }`, tEnd = t + 2 pi sqrt(r^3 / mu)
+ *                                * p[1], then the negated dv (:237-252)
+ *   ASTROZ_IMPULSE_PLANE_CHANGE  applyPlaneChange (:272-307): nothing below 1e-10 rad; otherwise dv = (hx sin di,
+ *                                hy sin di, hz cos di) * 2 |v| sin(angle / 2) / |h|, h = r x v -- the reference's
+ *                                "simplified" direction, not the textbook plane change.
+ * mu is the central body's parameter (the reference's orbitingObject.mu): the phasing burn and the abnormal-orbit test
+ * use it.  A DP87 state carries its step size through every step: partial steps to a burn, coasts and regular steps (a
+ * step of 1e-14 s or less makes no attempt and leaves the step size at min(step size, that step)).
+ * Departures from the reference: the inputs are states, not TLEs, and tf = t0 + duration; where the reference never
+ * returns, the state stops (ASTROZ_NUMERICAL_STOPPED: a DP87 rejection at hMin, or a sample count that would pass
+ * 2^32 - 2); position tables are refused (their rows follow K7's shared output intervals, which do not exist here).
+ * Outputs: rows of max_samples samples per state: times[n][max_samples], out[n][max_samples][6]; n_samples[n] = the
+ * number of samples state i's trajectory has, also when that is more than max_samples (only the first max_samples are
+ * written); samples past n_samples are zero.  Sample times repeat (the sample before and after a burn) and can decrease
+ * (the negative last step).  status[n]: ASTROZ_MANEUVER_TRUNCATED first, then the ASTROZ_NUMERICAL_* codes, then
+ * ASTROZ_MANEUVER_ABNORMAL; steps[n][2] (nullable) as for the batch calls.
+ * ASTROZ_VALUE_ERROR, nothing read, written or allocated: h <= 0; t0, duration, h, mu, rtol or atol not finite; a
+ * regular sampling loop that would not end; an unknown impulse kind; a non-finite impulse time or parameter; orbits <= 0;
+ * offsets that decrease or offsets[n] != m (host call); max_samples = 0; every model-list error, and a position table;
+ * an unknown integrator; device = -1. */
+#define ASTROZ_IMPULSE_ABSOLUTE     0   /* p = dv[3] km/s */
+#define ASTROZ_IMPULSE_PROGRADE     1   /* p[0] = dv km/s */
+#define ASTROZ_IMPULSE_PHASE        2   /* p[0] = angle rad, p[1] = orbits (> 0) */
+#define ASTROZ_IMPULSE_PLANE_CHANGE 3   /* p[0] = delta inclination rad, p[1] = delta RAAN rad */
+typedef struct {
+    double time;
+    int32_t kind;
+    uint32_t reserved;
+    double p[3];
+} astroz_impulse_t;
+#define ASTROZ_MANEUVER_ABNORMAL  4     /* the reference's abnormal-orbit stop; the trajectory ends at that sample */
+#define ASTROZ_MANEUVER_TRUNCATED 5     /* more than max_samples samples: the first max_samples are written */
+
+/* HOST buffers: states[n][6], impulse_offsets[n + 1], impulses[m], the per-state arrays the models name, outputs as
+ * above.  The chunked pipeline of astroz_cuda_propagate_numerical; the schedules are uploaded once per call. */
+int32_t astroz_cuda_propagate_maneuvers(const double *states, uint32_t n, double t0, double duration, double h, double mu,
+                                        const uint32_t *impulse_offsets, const astroz_impulse_t *impulses, uint32_t m,
+                                        const astroz_force_model_t *models, uint32_t n_models, int32_t integrator,
+                                        double rtol, double atol, uint32_t max_samples, int32_t device, double *times,
+                                        double *out, uint64_t *n_samples, uint8_t *status, uint64_t *steps);
+/* Same with DEVICE pointers on `device` for the states, offsets, impulses, per-state arrays and outputs (the descriptors
+ * are host memory).  Asynchronous on `stream`: the call queues one kernel and returns, so it reads neither offsets nor
+ * impulses -- they must pass the host call's checks (astroz_b200.numerical.propagate_maneuvers_batch_device checks
+ * them before they go up). */
+int32_t astroz_cuda_propagate_maneuvers_device(const double *d_states, uint32_t n, double t0, double duration, double h,
+                                               double mu, const uint32_t *d_impulse_offsets,
+                                               const astroz_impulse_t *d_impulses, uint32_t m,
+                                               const astroz_force_model_t *models, uint32_t n_models, int32_t integrator,
+                                               double rtol, double atol, uint32_t max_samples, int32_t device,
+                                               double *d_times, double *d_out, uint64_t *d_n_samples, uint8_t *d_status,
+                                               uint64_t *d_steps, void *stream);
+
 /* ---- element fits (K8): SGP4 mean elements from TEME ephemerides ------------------------------------------------------
  * For each satellite s of a batch, Levenberg-Marquardt finds the near-earth mean elements whose SGP4 states best match
  * its observations in the weighted least-squares sense, residuals (pos - model) / pos_sigma and (vel - model) / vel_sigma.

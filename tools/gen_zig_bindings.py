@@ -36,13 +36,14 @@ def zig_type(ctype: str, name: str) -> str:
         "const uint32_t *": "?[*]const u32",
         "uint32_t *": "?[*]u32",
         "int32_t *": "?[*]i32",
-        "uint64_t *": "?[*]u64" if name in ("steps", "d_steps") else "*u64",
+        "uint64_t *": "?[*]u64" if name in ("steps", "d_steps", "n_samples", "d_n_samples") else "*u64",
         "void *": "?*anyopaque",
         "void *const *": "?[*]const ?*anyopaque",
         "astroz_constellation_t": "Handle",
         "astroz_sgp4_t": "Handle",
         "astroz_constellation_t *": "*Handle",
         "const astroz_force_model_t *": "?[*]const astroz_force_model_t",
+        "const astroz_impulse_t *": "?[*]const astroz_impulse_t",
         "astroz_sgp4_t *": "*Handle",
         "uint32_t": "u32", "int32_t": "i32", "size_t": "usize", "double": "f64",
     }

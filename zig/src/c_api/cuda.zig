@@ -26,6 +26,13 @@ pub const astroz_force_model_t = extern struct {
     pos_table: ?[*]const f64,
 };
 
+pub const astroz_impulse_t = extern struct {
+    time: f64,
+    kind: i32,
+    reserved: u32,
+    p: [3]f64,
+};
+
 pub extern fn astroz_cuda_version() u32;
 pub extern fn astroz_cuda_device_count() i32;
 pub extern fn astroz_cuda_last_error() [*:0]const u8;
@@ -76,6 +83,8 @@ pub extern fn astroz_cuda_propagate_numerical(states: ?[*]const f64, n: u32, t0:
 pub extern fn astroz_cuda_propagate_numerical_device(d_states: ?[*]const f64, n: u32, t0: f64, duration: f64, dt: f64, mu: f64, forces: i32, j2: ?[*]const f64, r_eq: ?[*]const f64, d_drag_cd: ?[*]const f64, d_drag_area: ?[*]const f64, d_drag_mass: ?[*]const f64, integrator: i32, rtol: f64, atol: f64, device: i32, d_out: ?[*]f64, d_status: ?[*]u8, d_steps: ?[*]u64, stream: ?*anyopaque) i32;
 pub extern fn astroz_cuda_propagate_numerical_models(states: ?[*]const f64, n: u32, t0: f64, duration: f64, dt: f64, models: ?[*]const astroz_force_model_t, n_models: u32, integrator: i32, rtol: f64, atol: f64, device: i32, out: ?[*]f64, status: ?[*]u8, steps: ?[*]u64) i32;
 pub extern fn astroz_cuda_propagate_numerical_models_device(d_states: ?[*]const f64, n: u32, t0: f64, duration: f64, dt: f64, models: ?[*]const astroz_force_model_t, n_models: u32, integrator: i32, rtol: f64, atol: f64, device: i32, d_out: ?[*]f64, d_status: ?[*]u8, d_steps: ?[*]u64, stream: ?*anyopaque) i32;
+pub extern fn astroz_cuda_propagate_maneuvers(states: ?[*]const f64, n: u32, t0: f64, duration: f64, h: f64, mu: f64, impulse_offsets: ?[*]const u32, impulses: ?[*]const astroz_impulse_t, m: u32, models: ?[*]const astroz_force_model_t, n_models: u32, integrator: i32, rtol: f64, atol: f64, max_samples: u32, device: i32, times: ?[*]f64, out: ?[*]f64, n_samples: ?[*]u64, status: ?[*]u8, steps: ?[*]u64) i32;
+pub extern fn astroz_cuda_propagate_maneuvers_device(d_states: ?[*]const f64, n: u32, t0: f64, duration: f64, h: f64, mu: f64, d_impulse_offsets: ?[*]const u32, d_impulses: ?[*]const astroz_impulse_t, m: u32, models: ?[*]const astroz_force_model_t, n_models: u32, integrator: i32, rtol: f64, atol: f64, max_samples: u32, device: i32, d_times: ?[*]f64, d_out: ?[*]f64, d_n_samples: ?[*]u64, d_status: ?[*]u8, d_steps: ?[*]u64, stream: ?*anyopaque) i32;
 pub extern fn astroz_cuda_fit_elements(elements: ?[*]const f64, n: u32, grav: i32, offsets: ?[*]const u32, jd: ?[*]const f64, fr: ?[*]const f64, pos: ?[*]const f64, vel: ?[*]const f64, m: u32, pos_sigma: f64, vel_sigma: f64, fit_bstar: i32, max_iter: u32, device: i32, fitted: ?[*]f64, rms: ?[*]f64, iterations: ?[*]u32, status: ?[*]u8) i32;
 pub extern fn astroz_cuda_fit_elements_device(d_elements: ?[*]const f64, n: u32, grav: i32, d_offsets: ?[*]const u32, d_jd: ?[*]const f64, d_fr: ?[*]const f64, d_pos: ?[*]const f64, d_vel: ?[*]const f64, pos_sigma: f64, vel_sigma: f64, fit_bstar: i32, max_iter: u32, device: i32, d_fitted: ?[*]f64, d_rms: ?[*]f64, d_iterations: ?[*]u32, d_status: ?[*]u8, stream: ?*anyopaque) i32;
 pub extern fn astroz_cuda_fit_elements_mixed(elements: ?[*]const f64, n: u32, grav: i32, offsets: ?[*]const u32, jd: ?[*]const f64, fr: ?[*]const f64, pos: ?[*]const f64, vel: ?[*]const f64, m: u32, pos_sigma: f64, vel_sigma: f64, fit_bstar: i32, max_iter: u32, device: i32, fitted: ?[*]f64, rms: ?[*]f64, iterations: ?[*]u32, status: ?[*]u8) i32;
