@@ -18,7 +18,7 @@ from . import _lib
 from ._lib import as_f64, check, dptr, lib
 from .constellation import Constellation, Layout, OutputMode
 
-WGS72OLD = 0  # python-sgp4 numbering (sgp4.api.WGS72OLD / WGS72 / WGS84)
+WGS72OLD = 0  # python-sgp4 numbering (sgp4.api.WGS72OLD / WGS72 / WGS84), not the header's: _grav maps it
 WGS72 = 1
 WGS84 = 2
 accelerated = True

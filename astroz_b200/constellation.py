@@ -11,18 +11,19 @@ from enum import IntEnum
 import numpy as np
 
 from . import _lib
+from ._abi import DEFINES as D
 from ._lib import AstrozCudaError, as_f64, check, dptr, lib
 
 
 class OutputMode(IntEnum):  # src/Constellation.zig:30-34
-    teme = 0
-    ecef = 1
-    geodetic = 2
+    teme = D["ASTROZ_MODE_TEME"]
+    ecef = D["ASTROZ_MODE_ECEF"]
+    geodetic = D["ASTROZ_MODE_GEODETIC"]
 
 
 class Layout(IntEnum):  # src/Constellation.zig:37-42
-    satelliteMajor = 0
-    timeMajor = 1
+    satelliteMajor = D["ASTROZ_LAYOUT_SATELLITE_MAJOR"]
+    timeMajor = D["ASTROZ_LAYOUT_TIME_MAJOR"]
 
 
 def _c_lines(tles):

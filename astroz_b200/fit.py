@@ -22,10 +22,13 @@ from dataclasses import dataclass
 
 import numpy as np
 
+from ._abi import DEFINES as D
 from ._lib import WGS72, check, lib
 
-# per-satellite status bytes (ASTROZ_FIT_*)
-CONVERGED, ITERATION_LIMIT, INIT_FAILED, DEEP_SPACE, TOO_FEW_OBSERVATIONS = 0, 1, 2, 3, 4
+# per-satellite status bytes
+CONVERGED, ITERATION_LIMIT, INIT_FAILED, DEEP_SPACE, TOO_FEW_OBSERVATIONS = (
+    D["ASTROZ_FIT_CONVERGED"], D["ASTROZ_FIT_ITERATION_LIMIT"], D["ASTROZ_FIT_INIT_FAILED"], D["ASTROZ_FIT_DEEP_SPACE"],
+    D["ASTROZ_FIT_TOO_FEW_OBSERVATIONS"])
 STATUS_NAMES = {CONVERGED: "converged", ITERATION_LIMIT: "iteration limit", INIT_FAILED: "initial set fails init",
                 DEEP_SPACE: "deep space, not fitted (deep_space=False)", TOO_FEW_OBSERVATIONS: "too few observations"}
 

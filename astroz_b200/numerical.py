@@ -15,12 +15,15 @@ import ctypes as C
 
 import numpy as np
 
+from . import _abi
+from ._abi import DEFINES as D
 from ._lib import AstrozCudaError, check, lib
 
-FORCE_J2, FORCE_DRAG = 1, 2
-INTEGRATORS = {"rk4": 0, "dp87": 1}
-# per-state status bytes (ASTROZ_NUMERICAL_*)
-OK, STOPPED, SUBSTEP_LIMIT, NON_FINITE = 0, 1, 2, 3
+FORCE_J2, FORCE_DRAG = D["ASTROZ_FORCE_J2"], D["ASTROZ_FORCE_DRAG"]
+INTEGRATORS = {"rk4": D["ASTROZ_INTEGRATOR_RK4"], "dp87": D["ASTROZ_INTEGRATOR_DP87"]}
+# per-state status bytes
+OK, STOPPED, SUBSTEP_LIMIT, NON_FINITE = (D["ASTROZ_NUMERICAL_OK"], D["ASTROZ_NUMERICAL_STOPPED"],
+                                         D["ASTROZ_NUMERICAL_SUBSTEP_LIMIT"], D["ASTROZ_NUMERICAL_NON_FINITE"])
 
 
 def numerical_times(t0: float, duration: float, dt: float) -> np.ndarray:
@@ -118,20 +121,14 @@ def propagate_numerical_batch_device(states, t0, duration, dt, mu, out, status, 
 
 
 # ---- model lists: the force models of the reference's propagators module (src/propagators/ForceModel.zig) -------------
-# kinds and flags of astroz_force_model_t (ASTROZ_MODEL_*)
-_TWO_BODY, _J2, _J3, _J4, _DRAG, _IMPROVED_DRAG, _SRP, _THIRD_BODY = range(8)
-_PER_STATE = {"c": 1, "area": 2, "mass": 4}
-_POS_TABLE = 8
-MAX_MODELS = 16
+# flags of astroz_force_model_t
+_PER_STATE = {"c": D["ASTROZ_MODEL_PER_STATE_C"], "area": D["ASTROZ_MODEL_PER_STATE_AREA"],
+              "mass": D["ASTROZ_MODEL_PER_STATE_MASS"]}
+_POS_TABLE = D["ASTROZ_MODEL_POS_TABLE"]
+MAX_MODELS = D["ASTROZ_MAX_MODELS"]
 AU_KM = 1.495978707e8   # src/constants.zig:28, SolarRadiationPressure's default Sun distance
 
-
-class _ForceModelC(C.Structure):
-    _fields_ = [("kind", C.c_int32), ("flags", C.c_uint32)] + \
-               [(f, C.c_double) for f in ("mu", "coef", "r_eq", "rho0", "scale_height", "max_altitude", "f107", "c",
-                                          "area", "mass")] + \
-               [("pos", C.c_double * 3), ("c_per_state", C.c_void_p), ("area_per_state", C.c_void_p),
-                ("mass_per_state", C.c_void_p), ("pos_table", C.c_void_p)]
+_ForceModelC = _abi.structure("astroz_force_model_t")
 
 
 class _Model:
@@ -149,7 +146,7 @@ class _Model:
 
 class TwoBody(_Model):
     """TwoBody(mu): ForceModel.zig:42-56"""
-    kind = _TWO_BODY
+    kind = D["ASTROZ_MODEL_TWO_BODY"]
 
     def __init__(self, mu):
         super().__init__({"mu": float(mu)})
@@ -162,23 +159,23 @@ class _Zonal(_Model):
 
 class J2(_Zonal):
     """J2(mu, j2, r_eq): ForceModel.zig:58-80"""
-    kind = _J2
+    kind = D["ASTROZ_MODEL_J2"]
 
 
 class J3(_Zonal):
     """J3(mu, j3, r_eq): ForceModel.zig:113-143.  Its x / y terms carry an extra 1/r, as the reference's do."""
-    kind = _J3
+    kind = D["ASTROZ_MODEL_J3"]
 
 
 class J4(_Zonal):
     """J4(mu, j4, r_eq): ForceModel.zig:145-176.  Divides by r^9, as the reference does."""
-    kind = _J4
+    kind = D["ASTROZ_MODEL_J4"]
 
 
 class Drag(_Model):
     """Drag(r_eq, rho0, H, cd, area, mass, max_altitude): exponential atmosphere, ForceModel.zig:82-111.  cd, area [m^2]
     and mass [kg] are scalars or one value per state."""
-    kind = _DRAG
+    kind = D["ASTROZ_MODEL_DRAG"]
 
     def __init__(self, r_eq, rho0, H, cd, area, mass, max_altitude):
         super().__init__({"r_eq": float(r_eq), "rho0": float(rho0), "scale_height": float(H),
@@ -189,7 +186,7 @@ class ImprovedDrag(_Model):
     """ImprovedDrag(r_eq, cd, area, mass, max_altitude, f107): five-layer atmosphere rotating with the Earth, scaled by
     F10.7, ForceModel.zig:268-349.  Zero below 100 km, as the reference.  cd, area [m^2] and mass [kg] are scalars or one
     value per state."""
-    kind = _IMPROVED_DRAG
+    kind = D["ASTROZ_MODEL_IMPROVED_DRAG"]
 
     def __init__(self, r_eq, cd, area, mass, max_altitude, f107):
         super().__init__({"r_eq": float(r_eq), "max_altitude": float(max_altitude), "f107": float(f107)},
@@ -200,7 +197,7 @@ class SolarRadiationPressure(_Model):
     """SolarRadiationPressure(cr, area, mass, r_eq, sun_pos=None): ForceModel.zig:178-228, with a cylindrical shadow of
     radius r_eq.  cr, area [m^2] and mass [kg] are scalars or one value per state.  sun_pos [km] is a 3-vector (default
     (AU, 0, 0), as init sets it) or a (K, 3) table whose row k holds for output interval k (K = samples - 1)."""
-    kind = _SRP
+    kind = D["ASTROZ_MODEL_SRP"]
 
     def __init__(self, cr, area, mass, r_eq, sun_pos=None):
         super().__init__({"r_eq": float(r_eq)}, {"c": cr, "area": area, "mass": mass},
@@ -210,7 +207,7 @@ class SolarRadiationPressure(_Model):
 class ThirdBody(_Model):
     """ThirdBody(mu, pos): Battin's formula, ForceModel.zig:230-266.  pos [km] is a 3-vector or a (K, 3) table whose row
     k holds for output interval k (K = samples - 1)."""
-    kind = _THIRD_BODY
+    kind = D["ASTROZ_MODEL_THIRD_BODY"]
 
     def __init__(self, mu, pos):
         super().__init__({"mu": float(mu)}, pos=pos)
@@ -335,11 +332,10 @@ def propagate_models_batch_device(states, t0, duration, dt, models, out, status,
 
 
 # ---- impulsive maneuvers: the loop of the reference's Spacecraft.propagate (src/Spacecraft.zig:172-323) -------------
-# status bytes beyond the batch calls' (ASTROZ_MANEUVER_*)
-ABNORMAL, TRUNCATED = 4, 5
+# status bytes beyond the batch calls'
+ABNORMAL, TRUNCATED = D["ASTROZ_MANEUVER_ABNORMAL"], D["ASTROZ_MANEUVER_TRUNCATED"]
 EARTH_MU = 398600.5   # WGS-84 (src/constants.zig:55-58), the reference's default orbitingObject.mu
-# astroz_impulse_t
-IMPULSE_DTYPE = np.dtype([("time", "<f8"), ("kind", "<i4"), ("reserved", "<u4"), ("p", "<f8", (3,))])
+IMPULSE_DTYPE = np.dtype(_abi.structure("astroz_impulse_t"))
 
 
 class _Impulse:
@@ -355,7 +351,7 @@ class _Impulse:
 
 class Absolute(_Impulse):
     """Absolute(t, dv): velocity += dv (a 3-vector, km/s), calculations.impulse (calculations.zig:480-485)"""
-    kind = 0
+    kind = D["ASTROZ_IMPULSE_ABSOLUTE"]
 
     def __init__(self, t, dv):
         dv = [float(x) for x in dv]
@@ -366,7 +362,7 @@ class Absolute(_Impulse):
 
 class Prograde(_Impulse):
     """Prograde(t, dv): dv km/s along the velocity (Spacecraft.zig:260-263)"""
-    kind = 1
+    kind = D["ASTROZ_IMPULSE_PROGRADE"]
 
     def __init__(self, t, dv):
         super().__init__(t, dv)
@@ -376,7 +372,7 @@ class Phase(_Impulse):
     """Phase(t, angle, orbits=1.0): the reference's phasing maneuver (Spacecraft.zig:237-252, :310-323): a prograde
     burn, a coast of `orbits` periods of the circular orbit at the burn's radius sampled every h, then the opposite
     burn.  angle in rad, orbits > 0."""
-    kind = 2
+    kind = D["ASTROZ_IMPULSE_PHASE"]
 
     def __init__(self, t, angle, orbits=1.0):
         super().__init__(t, angle, orbits)
@@ -386,7 +382,7 @@ class PlaneChange(_Impulse):
     """PlaneChange(t, d_incl, d_raan): the reference's applyPlaneChange (Spacecraft.zig:272-307), nothing below 1e-10
     rad.  Its Δv points along (hx sin di, hy sin di, hz cos di) / |h|, the reference's "simplified" direction -- not
     the textbook plane change."""
-    kind = 3
+    kind = D["ASTROZ_IMPULSE_PLANE_CHANGE"]
 
     def __init__(self, t, d_incl, d_raan):
         super().__init__(t, d_incl, d_raan)

@@ -13,7 +13,9 @@ import re
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HEADER = os.path.join(ROOT, "include", "astroz_b200.h")
+sys.path.insert(0, ROOT)
+from astroz_b200._abi import declarations, structs  # noqa: E402
+
 OUT = os.path.join(ROOT, "zig", "src", "c_api", "cuda.zig")
 
 RET = {"int32_t": "i32", "uint32_t": "u32", "void": "void", "const char *": "[*:0]const u8", "void *": "?*anyopaque"}
@@ -52,36 +54,6 @@ def zig_type(ctype: str, name: str) -> str:
     return table[t]
 
 
-def declarations(header: str):
-    text = re.sub(r"/\*.*?\*/", "", open(header).read(), flags=re.S)
-    text = re.sub(r"#[^\n]*", "", text)
-    for m in re.finditer(r"([\w \*]+?)\b(astroz_cuda_[a-z0-9_]+)\s*\(([^;{]*?)\)\s*;", text, flags=re.S):
-        ret = " ".join(m.group(1).split())
-        ret = ret if not ret.endswith("*") else ret[:-1].strip() + " *"
-        args = []
-        raw = " ".join(m.group(3).split())
-        if raw and raw != "void":
-            for a in raw.split(","):
-                a = a.strip()
-                mm = re.match(r"(.*?)(\w+(?:\[\d+\])?)$", a)
-                ctype, name = mm.group(1).strip(), mm.group(2)
-                args.append((ctype, name))
-        yield ret, m.group(2), args
-
-
-def structs(header: str):
-    """`typedef struct { <type> <name>; ... } name;` blocks of the header, as (name, [(ctype, field)])"""
-    text = re.sub(r"/\*.*?\*/", "", open(header).read(), flags=re.S)
-    for m in re.finditer(r"typedef struct \{([^}]*)\}\s*(\w+)\s*;", text):
-        fields = []
-        for decl in m.group(1).split(";"):
-            decl = " ".join(decl.split())
-            if decl:
-                mm = re.match(r"(.*?)(\w+(?:\[\d+\])?)$", decl)
-                fields.append((mm.group(1).strip(), mm.group(2)))
-        yield m.group(2), fields
-
-
 FIELD = {"int32_t": "i32", "uint32_t": "u32", "double": "f64", "const double *": "?[*]const f64"}
 
 
@@ -102,11 +74,11 @@ def render() -> str:
         "pub const Handle = ?*anyopaque;",
         "",
     ]
-    for name, fields in structs(HEADER):
+    for name, fields in structs():
         out.append(f"pub const {name} = extern struct {{")
         out += [f"    {f.split('[')[0]}: {zig_field(t, f)}," for t, f in fields]
         out += ["};", ""]
-    for ret, name, args in declarations(HEADER):
+    for ret, name, args in declarations():
         zargs = ", ".join(f"{n.split('[')[0]}: {zig_type(t, n)}" for t, n in args)
         out.append(f"pub extern fn {name}({zargs}) {RET[ret]};")
     out += [
