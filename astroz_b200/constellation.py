@@ -300,6 +300,37 @@ class Constellation:
             int(outputMode), C.c_void_p(pos.data_ptr()), C.c_void_p(vel.data_ptr()) if vel is not None else None,
             C.c_void_p(status.data_ptr()) if status is not None else None, C.c_void_p(stream) if stream else None))
 
+    def porkchop(self, chaser, target, dep_jd, dep_fr, arr_jd, arr_fr, *, mu: float | None = None, max_revs: int = 0):
+        """Porkchop grids between catalog rows: pair p departs from row chaser[p] at each epoch dep_jd + dep_fr and
+        arrives at row target[p] at each epoch arr_jd + arr_fr, both propagated by `propagate_pairs` (TEME).  Cell
+        (p, d, a) is the transfer of least |dv1| + |dv2| over max_revs revolutions, prograde relative to the chaser
+        (astroz_b200.lambert).  mu defaults to the handle's gravity model's.  Returns dv (P, D, A, 2) km/s, slot and
+        status (P, D, A) uint8 (ASTROZ_LAMBERT_*; STATE_FAILED where an endpoint's propagation status is not 0).
+        Single-device handles only."""
+        rows = [np.ascontiguousarray(np.atleast_1d(np.asarray(x))) for x in (chaser, target)]
+        for r in rows:
+            if r.ndim != 1 or (r.size and (not np.issubdtype(r.dtype, np.integer) or r.min() < 0 or
+                                           r.max() > 0xFFFFFFFF)):
+                raise ValueError("chaser and target must be 1-D arrays of catalog rows")
+        if rows[0].shape != rows[1].shape:
+            raise ValueError("chaser and target must have the same length")
+        chaser, target = (r.astype(np.uint32, copy=False) for r in rows)
+        dep_jd, dep_fr, arr_jd, arr_fr = as_f64(dep_jd), as_f64(dep_fr), as_f64(arr_jd), as_f64(arr_fr)
+        if dep_jd.shape != dep_fr.shape or arr_jd.shape != arr_fr.shape or dep_jd.ndim != 1 or arr_jd.ndim != 1:
+            raise ValueError("dep_jd / dep_fr and arr_jd / arr_fr must be 1-D arrays of the same length")
+        if max_revs < 0:
+            raise ValueError("max_revs must be >= 0")
+        if mu is None:
+            mu = 398600.8 if self.grav == _lib.WGS72 else 398600.5   # src/constants.zig:41-58
+        P, Dn, An = len(chaser), len(dep_jd), len(arr_jd)
+        dv = np.zeros((P, Dn, An, 2))
+        slot, status = np.zeros((P, Dn, An), dtype=np.uint8), np.zeros((P, Dn, An), dtype=np.uint8)
+        check(lib().astroz_cuda_constellation_porkchop(
+            self._h, C.c_void_p(chaser.ctypes.data), C.c_void_p(target.ctypes.data), P, dptr(dep_jd), dptr(dep_fr), Dn,
+            dptr(arr_jd), dptr(arr_fr), An, float(mu), int(max_revs), dptr(dv), C.c_void_p(slot.ctypes.data),
+            C.c_void_p(status.ctypes.data)))
+        return dv, slot, status
+
     def propagate_gather(self, jd, fr, peer_pos=None, peer_vel=None, mc_pos: int = 0, mc_vel: int = 0,
                          out_num_sats: int | None = None, out_sat_offset: int = 0, stream: int = 0) -> None:
         """Fused propagate + all-gather (TEME, satellite-major): this constellation's rows are written into

@@ -29,6 +29,7 @@
 #include "az_hostcopy.cuh"
 #include "az_ingest.cuh"
 #include "az_kernels.cuh"
+#include "az_lambert.cuh"
 #include "az_numerical.cuh"
 #include "az_tables.hpp"
 
@@ -2690,6 +2691,200 @@ int32_t astroz_cuda_parse_tle(const char *line1, const char *line2, double *elem
     if (az::parse_tle(line1, line2, t) != az::kOk) return ASTROZ_BAD_TLE_LENGTH;
     const double cols[8] = {t.epochJd, t.revPerDay, t.ecc, t.inclDeg, t.raanDeg, t.argpDeg, t.maDeg, t.bstar};
     std::memcpy(elements, cols, sizeof cols);
+    return ASTROZ_OK;
+}
+
+// ---- Lambert transfers (K9, az_lambert.cu) ---------------------------------------------------------------------------
+static_assert(ASTROZ_LAMBERT_OK == az::kLamOk && ASTROZ_LAMBERT_NO_SOLUTION == az::kLamNoSolution &&
+                  ASTROZ_LAMBERT_DEGENERATE == az::kLamDegenerate &&
+                  ASTROZ_LAMBERT_NOT_CONVERGED == az::kLamNotConverged &&
+                  ASTROZ_LAMBERT_STATE_FAILED == az::kLamStateFailed && ASTROZ_LAMBERT_MAX_REVS == az::kLamMaxRevs,
+              "lambert status bytes");
+
+// Scalar checks of every Lambert call, before anything is read, written or allocated.
+static int32_t lambert_check(double mu, uint32_t max_revs, int32_t device) {
+    if (device < 0) return value_error("a Lambert call runs on one device: pass its ordinal");
+    if (!std::isfinite(mu) || !(mu > 0.0)) return value_error("mu must be finite and > 0");
+    if (max_revs > az::kLamMaxRevs) return value_error("max_revs must be at most 127");
+    return ASTROZ_OK;
+}
+
+// lambert_check, and the grid's size: its byte count and its CTA count (one cell per thread) must be representable.
+static int32_t porkchop_check(uint32_t n_pairs, uint32_t n_dep, uint32_t n_arr, double mu, uint32_t max_revs,
+                              int32_t device) {
+    const int32_t rc = lambert_check(mu, max_revs, device);
+    if (rc != ASTROZ_OK) return rc;
+    const uint64_t perPair = (uint64_t)n_dep * n_arr;
+    if (n_pairs && perPair > (uint64_t)0x7fffffff * 128 / n_pairs) return value_error("the porkchop grid is too large");
+    return ASTROZ_OK;
+}
+
+int32_t astroz_cuda_lambert_device(const double *d_r1, const double *d_r2, const double *d_tof, const double *d_normal,
+                                   uint32_t n, double mu, uint32_t max_revs, int32_t device, double *d_v1,
+                                   double *d_v2, uint8_t *d_status, uint8_t *d_iterations, void *stream) {
+    int32_t rc = lambert_check(mu, max_revs, device);
+    if (rc != ASTROZ_OK) return rc;
+    if (n == 0) return ASTROZ_OK;
+    if (!d_r1 || !d_r2 || !d_tof || !d_v1 || !d_v2 || !d_status) return ASTROZ_NULL_POINTER;
+    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
+    AZ_CUDA(cudaSetDevice(device));
+    const az::LambertArgs a{d_r1, d_r2, d_tof, d_normal, n, max_revs, mu, d_v1, d_v2, d_status, d_iterations};
+    AZ_CUDA(az::launch_lambert(a, static_cast<cudaStream_t>(stream)));
+    return ASTROZ_OK;
+}
+
+// Host buffers: a solve is compute-bound (some 5 iterations of fp64 transcendentals per slot for 56 bytes in), so the
+// batch goes up at once -- pageable arrays through the device's pinned ring, pinned ones by direct DMA -- one launch
+// solves it and the results come back by plain copies.
+int32_t astroz_cuda_lambert(const double *r1, const double *r2, const double *tof, const double *normal, uint32_t n,
+                            double mu, uint32_t max_revs, int32_t device, double *v1, double *v2, uint8_t *status,
+                            uint8_t *iterations) {
+    int32_t rc = lambert_check(mu, max_revs, device);
+    if (rc != ASTROZ_OK) return rc;
+    if (n == 0) return ASTROZ_OK;
+    if (!r1 || !r2 || !tof || !v1 || !v2 || !status) return ASTROZ_NULL_POINTER;
+    if (!all_finite(r1, (size_t)3 * n) || !all_finite(r2, (size_t)3 * n) || !all_finite(tof, n) ||
+        (normal && !all_finite(normal, (size_t)3 * n)))
+        return value_error("r1, r2, tof and normal must be finite");
+    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
+    NumericalContext *c = nullptr;
+    if ((rc = numerical_context(device, &c)) != ASTROZ_OK) return rc;
+    std::lock_guard<std::mutex> lk(c->m);
+    AZ_CUDA(cudaSetDevice(device));
+    cudaStream_t st = c->stream;
+    const size_t slots = (size_t)n * (2 * (size_t)max_revs + 1);
+    // one device block: r1 | r2 | normal | tof | v1 | v2 | status | iterations
+    const size_t bytes[] = {(size_t)24 * n, (size_t)24 * n, normal ? (size_t)24 * n : 0, (size_t)8 * n, 24 * slots,
+                            24 * slots, slots, iterations ? slots : 0};
+    size_t at[8], total = 0;
+    for (int k = 0; k < 8; ++k) at[k] = total, total += (bytes[k] + 15) & ~size_t(15);
+    StreamBuf dBuf(st);
+    AZ_CUDA(dBuf.alloc(total));
+    char *base = static_cast<char *>(dBuf.p);
+    auto up = [&](const void *src, int k, size_t elemBytes, size_t count) {
+        void *const d[1] = {base + at[k]};
+        const void *const s[1] = {src};
+        return c->pipe.ring.upload(az::is_pageable(src), 1, s, d, &elemBytes, count, st);
+    };
+    AZ_CUDA(up(r1, 0, 24, n));
+    AZ_CUDA(up(r2, 1, 24, n));
+    if (normal) AZ_CUDA(up(normal, 2, 24, n));
+    AZ_CUDA(up(tof, 3, 8, n));
+    auto dd = [&](int k) { return reinterpret_cast<double *>(base + at[k]); };
+    auto db = [&](int k) { return reinterpret_cast<uint8_t *>(base + at[k]); };
+    const az::LambertArgs a{dd(0), dd(1), dd(3), normal ? dd(2) : nullptr, n, max_revs, mu, dd(4), dd(5), db(6),
+                            iterations ? db(7) : nullptr};
+    AZ_CUDA(az::launch_lambert(a, st));
+    AZ_CUDA(cudaMemcpyAsync(v1, a.v1, 24 * slots, cudaMemcpyDeviceToHost, st));
+    AZ_CUDA(cudaMemcpyAsync(v2, a.v2, 24 * slots, cudaMemcpyDeviceToHost, st));
+    AZ_CUDA(cudaMemcpyAsync(status, a.status, slots, cudaMemcpyDeviceToHost, st));
+    if (iterations) AZ_CUDA(cudaMemcpyAsync(iterations, a.iterations, slots, cudaMemcpyDeviceToHost, st));
+    AZ_CUDA(dBuf.release());
+    AZ_CUDA(cudaStreamSynchronize(st));
+    return ASTROZ_OK;
+}
+
+int32_t astroz_cuda_lambert_porkchop_device(const double *d_dep, const uint8_t *d_dep_status, const double *d_arr,
+                                            const uint8_t *d_arr_status, uint32_t n_pairs, const double *d_dep_jd,
+                                            const double *d_dep_fr, uint32_t n_dep, const double *d_arr_jd,
+                                            const double *d_arr_fr, uint32_t n_arr, double mu, uint32_t max_revs,
+                                            int32_t device, double *d_dv, uint8_t *d_slot, uint8_t *d_status,
+                                            void *stream) {
+    int32_t rc = porkchop_check(n_pairs, n_dep, n_arr, mu, max_revs, device);
+    if (rc != ASTROZ_OK) return rc;
+    if (!n_pairs || !n_dep || !n_arr) return ASTROZ_OK;
+    if (!d_dep || !d_arr || !d_dep_jd || !d_dep_fr || !d_arr_jd || !d_arr_fr || !d_dv || !d_slot || !d_status)
+        return ASTROZ_NULL_POINTER;
+    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
+    AZ_CUDA(cudaSetDevice(device));
+    const az::PorkchopArgs a{d_dep,    d_dep + 3, d_arr,    d_arr + 3, 6,     d_dep_status, d_arr_status,
+                             d_dep_jd, d_dep_fr,  d_arr_jd, d_arr_fr,  n_pairs, n_dep,      n_arr,
+                             max_revs, mu,        d_dv,     d_slot,    d_status};
+    AZ_CUDA(az::launch_porkchop(a, static_cast<cudaStream_t>(stream)));
+    return ASTROZ_OK;
+}
+
+// Host buffers: chunks of pairs through the handle's two-slot pipeline (az::ChunkPipeline), each chunk's grid block at
+// most kPorkchopChunkBytes with its endpoint states.  A chunk's queries are its pairs' catalog rows (the pipeline's input
+// columns, one row per departure or arrival) against the time axes tiled over the chunk's pairs (uploaded once); the
+// handle's pairs path fills the endpoint states, then the porkchop kernel runs on them, all on the handle's stream.
+static constexpr size_t kPorkchopChunkBytes = 32u << 20;
+int32_t astroz_cuda_constellation_porkchop(astroz_constellation_t h, const uint32_t *chaser, const uint32_t *target,
+                                           uint32_t n_pairs, const double *dep_jd, const double *dep_fr, uint32_t n_dep,
+                                           const double *arr_jd, const double *arr_fr, uint32_t n_arr, double mu,
+                                           uint32_t max_revs, double *dv, uint8_t *slot, uint8_t *status) {
+    Constellation *c = static_cast<Constellation *>(h);
+    if (!c) return ASTROZ_NULL_POINTER;
+    int32_t rc = refuse_multi(c);
+    if (rc == ASTROZ_OK) rc = porkchop_check(n_pairs, n_dep, n_arr, mu, max_revs, c->device);
+    if (rc != ASTROZ_OK) return rc;
+    if (!n_pairs || !n_dep || !n_arr) return ASTROZ_OK;
+    if (!chaser || !target || !dep_jd || !dep_fr || !arr_jd || !arr_fr || !dv || !slot || !status)
+        return ASTROZ_NULL_POINTER;
+    const az::CatalogTables &t = c->cat;
+    for (uint32_t p = 0; p < n_pairs; ++p)
+        if (chaser[p] >= t.n || target[p] >= t.n) {
+            g_lastError = "pair " + std::to_string(p) + ": a catalog row is not in the " + std::to_string(t.n) +
+                          "-row catalog";
+            return ASTROZ_VALUE_ERROR;
+        }
+    if (!all_finite(dep_jd, n_dep) || !all_finite(dep_fr, n_dep) || !all_finite(arr_jd, n_arr) ||
+        !all_finite(arr_fr, n_arr))
+        return value_error("the departure and arrival epochs must be finite");
+    const size_t D = n_dep, A = n_arr;
+    AZ_CUDA(cudaSetDevice(c->device));
+    cudaStream_t st = c->stream;
+    if (t.nSdp4) {
+        double lo = INFINITY, hi = -INFINITY;
+        for (size_t i = 0; i < D; ++i) lo = std::min(lo, dep_jd[i] + dep_fr[i]), hi = std::max(hi, dep_jd[i] + dep_fr[i]);
+        for (size_t i = 0; i < A; ++i) lo = std::min(lo, arr_jd[i] + arr_fr[i]), hi = std::max(hi, arr_jd[i] + arr_fr[i]);
+        if ((rc = prepare_deep_space(c, lo, hi, st)) != ASTROZ_OK) return rc;
+    }
+    const size_t pairBytes = D * A * 18 + (D + A) * 49;   // grid block, and endpoint states and status bytes
+    const uint32_t chunk = (uint32_t)std::max<size_t>(1, std::min<size_t>(n_pairs, kPorkchopChunkBytes / pairBytes));
+    std::vector<uint32_t> satC((size_t)n_pairs * D), satT((size_t)n_pairs * A);
+    for (size_t p = 0; p < n_pairs; ++p) {
+        std::fill_n(satC.begin() + p * D, D, chaser[p]);
+        std::fill_n(satT.begin() + p * A, A, target[p]);
+    }
+    // device scratch: tiled dep jd | dep fr | arr jd | arr fr, then dep pos | dep vel | arr pos | arr vel, status bytes
+    const size_t qd = (size_t)chunk * D, qa = (size_t)chunk * A;
+    std::vector<double> tiles(2 * qd + 2 * qa);
+    for (size_t q = 0; q < qd; ++q) tiles[q] = dep_jd[q % D], tiles[qd + q] = dep_fr[q % D];
+    for (size_t q = 0; q < qa; ++q) tiles[2 * qd + q] = arr_jd[q % A], tiles[2 * qd + qa + q] = arr_fr[q % A];
+    StreamBuf dScratch(st), dIn(st), dOut(st);
+    AZ_CUDA(dScratch.alloc((tiles.size() + 6 * qd + 6 * qa) * 8 + qd + qa));
+    double *dTiles = static_cast<double *>(dScratch.p);
+    AZ_CUDA(cudaMemcpyAsync(dTiles, tiles.data(), tiles.size() * 8, cudaMemcpyHostToDevice, st));
+    const double *depJd = dTiles, *depFr = dTiles + qd, *arrJd = dTiles + 2 * qd, *arrFr = dTiles + 2 * qd + qa;
+    double *depPos = dTiles + tiles.size(), *depVel = depPos + 3 * qd, *arrPos = depVel + 3 * qd,
+           *arrVel = arrPos + 3 * qa;
+    uint8_t *depSt = reinterpret_cast<uint8_t *>(arrVel + 3 * qa), *arrSt = depSt + qd;
+    const az::HostIn in[2] = {{satC.data(), 4 * D}, {satT.data(), 4 * A}};
+    const az::HostOut out[3] = {{dv, 16 * D * A}, {slot, D * A}, {status, D * A}};
+    AZ_CUDA(dIn.alloc(az::chunk_slots_bytes(in, 2, n_pairs, chunk)));
+    AZ_CUDA(dOut.alloc(az::chunk_slots_bytes(out, 3, n_pairs, chunk)));
+    int32_t queued = ASTROZ_OK;  // pairs_queue's own code; its message is the last error
+    const cudaError_t e = c->pipe.run(
+        st, c->copyStream, n_pairs, chunk, 2, in, 3, out, dIn.p, dOut.p,
+        [&](uint32_t, uint32_t, uint32_t m, void *const *dI, void *const *dO, cudaStream_t s) {
+            queued = pairs_queue(c, static_cast<const uint32_t *>(dI[0]), depJd, depFr, (uint32_t)(m * D),
+                                 ASTROZ_MODE_TEME, depPos, depVel, depSt, s);
+            if (queued == ASTROZ_OK)
+                queued = pairs_queue(c, static_cast<const uint32_t *>(dI[1]), arrJd, arrFr, (uint32_t)(m * A),
+                                     ASTROZ_MODE_TEME, arrPos, arrVel, arrSt, s);
+            if (queued != ASTROZ_OK) return cudaErrorUnknown;  // stops the run; `queued` is returned
+            const az::PorkchopArgs a{depPos, depVel, arrPos, arrVel, 3, depSt, arrSt, depJd, depFr, arrJd, arrFr,
+                                     m, n_dep, n_arr, max_revs, mu, static_cast<double *>(dO[0]),
+                                     static_cast<uint8_t *>(dO[1]), static_cast<uint8_t *>(dO[2])};
+            return az::launch_porkchop(a, s);
+        });
+    if (queued != ASTROZ_OK) return queued;
+    AZ_CUDA(e);
+    AZ_CUDA(dIn.release());
+    AZ_CUDA(dOut.release());
+    AZ_CUDA(dScratch.release());
+    AZ_CUDA(cudaStreamSynchronize(st));
     return ASTROZ_OK;
 }
 

@@ -11,6 +11,7 @@ same time convention (`times` in minutes from `start_time`, near-earth tsince = 
 * sources that need the network (CelesTrak group names, URLs, `norad_id=`) raise: this build has no egress and the
   catalogue download is outside the propagation path;
 * the deep-space rows of `propagate()` are filled (the reference leaves them uninitialised, SURVEY.md appendix C);
+* `lambert()` returns the true solution of Lambert's problem; the reference's velocities miss r2 (SURVEY.md appendix C);
 * geodetic output is what the core produces -- latitude / longitude in radians, altitude in km
   (src/Constellation.zig:497) -- like the reference's actual return value, not its docstring.
 """
@@ -252,5 +253,39 @@ def propagate_numerical(state, t0, duration, dt, mu, j2=None, r_eq=None, drag_cd
     return [float(t) for t in times], [tuple(float(x) for x in row) for row in traj[0]]
 
 
-__all__ = ["Constellation", "propagate", "screen", "parse_tle_pairs", "omm_to_tle_pairs", "propagate_numerical",
+_LAMBERT_ERROR = "Lambert solver failed (check inputs: tof>0, non-zero position vectors)"
+
+
+def lambert(mu, r1, r2, tof):
+    """`astroz.lambert(mu, r1, r2, tof)` (bindings/python/src/orbital_mechanics.zig:37-97): a dict with
+    `departure_velocity` and `arrival_velocity` (3-tuples, km/s), `transfer_angle` (rad), `sma` (km) and `tof` (s).
+    The reference's geometry: the short way, transfer angle acos(r1 . r2 / |r1| |r2|) in (0, pi), no revolutions, solved
+    on the device with the normal r1 x r2.  The velocities are the true solution of Lambert's problem, not the
+    reference's (whose departure velocity misses r2, SURVEY.md appendix C); `sma` is that transfer conic's semi-major
+    axis, negative for a hyperbola.  ValueError with the reference's message for tof <= 0, a zero vector or
+    |sin(transfer angle)| < 1e-12 (src/OrbitalMechanics.zig:122-158)."""
+    from . import lambert as K9
+
+    mu, tof = float(mu), float(tof)
+    r1, r2 = [float(x) for x in r1], [float(x) for x in r2]
+    if len(r1) != 3 or len(r2) != 3:
+        raise ValueError("position vectors must have exactly 3 elements")
+    n1, n2 = math.sqrt(sum(x * x for x in r1)), math.sqrt(sum(x * x for x in r2))
+    if tof <= 0 or n1 <= 0 or n2 <= 0:
+        raise ValueError(_LAMBERT_ERROR)
+    cos_angle = max(-1.0, min(1.0, sum(a * b for a, b in zip(r1, r2)) / (n1 * n2)))
+    angle = math.acos(cos_angle)
+    if abs(math.sin(angle)) < 1e-12:
+        raise ValueError(_LAMBERT_ERROR)
+    normal = np.cross(r1, r2)
+    v1, v2, status, _ = K9.lambert_batch([r1], [r2], [tof], mu, normal=normal)
+    if status[0, 0] != K9.OK:
+        raise ValueError(_LAMBERT_ERROR)
+    dep = v1[0, 0]
+    sma = 1.0 / (2.0 / n1 - float(dep @ dep) / mu)   # vis-viva
+    return {"departure_velocity": tuple(float(x) for x in dep), "arrival_velocity": tuple(float(x) for x in v2[0, 0]),
+            "transfer_angle": angle, "sma": sma, "tof": tof}
+
+
+__all__ = ["Constellation", "propagate", "screen", "parse_tle_pairs", "omm_to_tle_pairs", "propagate_numerical", "lambert",
            "EARTH_MU", "EARTH_R_EQ", "EARTH_J2", "SUN_MU", "MOON_MU"]

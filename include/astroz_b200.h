@@ -606,6 +606,76 @@ int32_t astroz_cuda_fit_elements_mixed_device(const double *d_elements, uint32_t
  * numbers astroz_cuda_constellation_create would use.  ASTROZ_BAD_TLE_LENGTH when the pair cannot be read. */
 int32_t astroz_cuda_parse_tle(const char *line1, const char *line2, double *elements);
 
+/* ---- Lambert transfers (K9): replaces astroz.lambert(mu, r1, r2, tof) (bindings/python/src/orbital_mechanics.zig:37-97,
+ * src/OrbitalMechanics.zig:122-183) with a batched multi-revolution solver.  The reference's lambertSolverSimple does not
+ * solve Lambert's problem (its departure velocity, propagated for tof, misses r2: SURVEY.md appendix C); these calls
+ * return the true solutions, by Izzo's algorithm (Celest. Mech. Dyn. Astron. 121, 2015).
+ * Problem i: positions r1[i], r2[i] [km], time of flight tof[i] [s], gravitational parameter mu [km^3/s^2] and a unit
+ * normal normal[i] (nullable: +z for every problem) that sets the sense of motion:
+ *   direction: ih = r1 x r2 / |r1 x r2|; ih . n > 0 is the short way (transfer angle < pi), ih . n < 0 the long way.  A
+ *              retrograde transfer is a negated normal;
+ *   slots:     S = 2 max_revs + 1 per problem: slot 0 is the zero-revolution solution, slot 2M - 1 the left and slot 2M
+ *              the right branch of M revolutions.  A slot of M revolutions exists when tof >= its minimum time of flight;
+ *   numerics:  Householder iterations on Izzo's x until |dx| < 1e-13, at most 15; the minimum time of flight by Halley
+ *              iterations, for the largest candidate M only;
+ *   outputs:   v1[n][S][3], v2[n][S][3] [km/s], status[n][S] (ASTROZ_LAMBERT_*), iterations[n][S] (nullable: Householder
+ *              steps taken, 15 for NOT_CONVERGED, 0 when no iteration ran).  A slot that is not OK is zero-filled.
+ * A problem's bytes depend on its own inputs alone, never on its position in a batch.
+ * ASTROZ_VALUE_ERROR, nothing written: mu not finite or <= 0; max_revs > 127 (slot indices stay inside a byte); device
+ * = -1 or not a visible ordinal; an output size that overflows; and for the host call a non-finite r1, r2, tof or normal.
+ * n = 0 is a no-op.  Without a device: ASTROZ_NO_DEVICE. */
+#define ASTROZ_LAMBERT_OK            0
+#define ASTROZ_LAMBERT_NO_SOLUTION   1   /* tof <= 0, or no M-revolution solution at this tof */
+#define ASTROZ_LAMBERT_DEGENERATE    2   /* |r1| = 0, |r2| = 0, |r1 x r2| < 1e-12 |r1| |r2| (the reference's |sin dnu|
+                                            < 1e-12 rule, OrbitalMechanics.zig:158) or ih . n = 0 */
+#define ASTROZ_LAMBERT_NOT_CONVERGED 3   /* 15 Householder steps without |dx| < 1e-13 */
+#define ASTROZ_LAMBERT_STATE_FAILED  4   /* porkchop only: an endpoint's propagation status was not 0 */
+#define ASTROZ_LAMBERT_MAX_REVS      127
+
+/* HOST buffers: r1[n][3], r2[n][3], tof[n], normal[n][3] (nullable), outputs as above.  Compute-bound: the inputs go up
+ * at once (pageable ones through a pinned ring), one launch solves the batch, the results come back by plain copies. */
+int32_t astroz_cuda_lambert(const double *r1, const double *r2, const double *tof, const double *normal, uint32_t n,
+                            double mu, uint32_t max_revs, int32_t device, double *v1, double *v2, uint8_t *status,
+                            uint8_t *iterations);
+/* Same with DEVICE pointers on `device`.  One launch on `stream` (a cudaStream_t, NULL = the legacy default stream): no
+ * allocation, no synchronisation, and only the scalar arguments are checked -- the values must be finite. */
+int32_t astroz_cuda_lambert_device(const double *d_r1, const double *d_r2, const double *d_tof, const double *d_normal,
+                                   uint32_t n, double mu, uint32_t max_revs, int32_t device, double *d_v1,
+                                   double *d_v2, uint8_t *d_status, uint8_t *d_iterations, void *stream);
+
+/* Porkchop grids: the cost of transfers between n_pairs (chaser, target) pairs over a grid of departure and arrival
+ * epochs.  Cell (p, d, a), arrival index fastest:
+ *   endpoints: the chaser's state at departure d, d_dep[p][d][6] (x y z vx vy vz, km and km/s), and the target's at
+ *              arrival a, d_arr[p][a][6], each with a status byte (d_dep_status[p][d], d_arr_status[p][a], nullable: all
+ *              valid).  States may come from anywhere: propagate_pairs_device, K7 trajectories, ephemerides.  TEME (or
+ *              any frame) is treated as inertial over the transfer;
+ *   time:      tof = ((arr_jd[a] - dep_jd[d]) + (arr_fr[a] - dep_fr[d])) * 86400, evaluated in that order;
+ *   direction: prograde relative to the chaser: the normal is the chaser's r x v at departure;
+ *   selection: every feasible slot of max_revs revolutions is solved and the one with the least
+ *              |v1 - v_chaser| + |v_target - v2| kept, the lowest slot on a tie;
+ *   outputs:   d_dv[p][d][a][2] (|dv1|, |dv2| km/s), d_slot[p][d][a] (the slot kept), d_status[p][d][a]: OK, or
+ *              ASTROZ_LAMBERT_STATE_FAILED when an endpoint's status byte is not 0, or slot 0's status when no slot is
+ *              OK (dv 0 and slot 0 then).
+ * Asynchronous on `stream`; ASTROZ_VALUE_ERROR as for astroz_cuda_lambert_device, and when n_pairs * n_dep * n_arr
+ * overflows. */
+int32_t astroz_cuda_lambert_porkchop_device(const double *d_dep, const uint8_t *d_dep_status, const double *d_arr,
+                                            const uint8_t *d_arr_status, uint32_t n_pairs, const double *d_dep_jd,
+                                            const double *d_dep_fr, uint32_t n_dep, const double *d_arr_jd,
+                                            const double *d_arr_fr, uint32_t n_arr, double mu, uint32_t max_revs,
+                                            int32_t device, double *d_dv, uint8_t *d_slot, uint8_t *d_status,
+                                            void *stream);
+/* The whole porkchop from a handle's catalogue, HOST buffers: pair p departs from catalog row chaser[p] and arrives at
+ * catalog row target[p].  The pairs are cut into chunks on the handle's two-slot pipeline; for each chunk the handle's
+ * pairs path (astroz_cuda_constellation_propagate_pairs, TEME, its status bytes) gives the chaser rows x departures
+ * and the target rows x arrivals, then the porkchop kernel above runs on them.  dv[n_pairs][n_dep][n_arr][2],
+ * slot / status[n_pairs][n_dep][n_arr].
+ * ASTROZ_VALUE_ERROR, nothing written: a row outside the catalog; a multi-device handle (device = -1); mu not finite or
+ * <= 0; max_revs > 127; a non-finite epoch; an output size that overflows.  n_pairs, n_dep or n_arr = 0 is a no-op. */
+int32_t astroz_cuda_constellation_porkchop(astroz_constellation_t h, const uint32_t *chaser, const uint32_t *target,
+                                           uint32_t n_pairs, const double *dep_jd, const double *dep_fr, uint32_t n_dep,
+                                           const double *arr_jd, const double *arr_fr, uint32_t n_arr, double mu,
+                                           uint32_t max_revs, double *dv, uint8_t *slot, uint8_t *status);
+
 /* ---- measurement helpers --------------------------------------------------------------------- */
 /* DFMA microbenchmark on `device`: achieved fp64 TFLOP/s (FMA = 2) -- the measured roofline denominator */
 int32_t astroz_cuda_fp64_peak(int32_t device, double *tflops);

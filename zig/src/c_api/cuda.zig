@@ -90,6 +90,10 @@ pub extern fn astroz_cuda_fit_elements_device(d_elements: ?[*]const f64, n: u32,
 pub extern fn astroz_cuda_fit_elements_mixed(elements: ?[*]const f64, n: u32, grav: i32, offsets: ?[*]const u32, jd: ?[*]const f64, fr: ?[*]const f64, pos: ?[*]const f64, vel: ?[*]const f64, m: u32, pos_sigma: f64, vel_sigma: f64, fit_bstar: i32, max_iter: u32, device: i32, fitted: ?[*]f64, rms: ?[*]f64, iterations: ?[*]u32, status: ?[*]u8) i32;
 pub extern fn astroz_cuda_fit_elements_mixed_device(d_elements: ?[*]const f64, n: u32, grav: i32, d_offsets: ?[*]const u32, d_jd: ?[*]const f64, d_fr: ?[*]const f64, d_pos: ?[*]const f64, d_vel: ?[*]const f64, pos_sigma: f64, vel_sigma: f64, fit_bstar: i32, max_iter: u32, device: i32, d_fitted: ?[*]f64, d_rms: ?[*]f64, d_iterations: ?[*]u32, d_status: ?[*]u8, stream: ?*anyopaque) i32;
 pub extern fn astroz_cuda_parse_tle(line1: [*:0]const u8, line2: [*:0]const u8, elements: ?[*]f64) i32;
+pub extern fn astroz_cuda_lambert(r1: ?[*]const f64, r2: ?[*]const f64, tof: ?[*]const f64, normal: ?[*]const f64, n: u32, mu: f64, max_revs: u32, device: i32, v1: ?[*]f64, v2: ?[*]f64, status: ?[*]u8, iterations: ?[*]u8) i32;
+pub extern fn astroz_cuda_lambert_device(d_r1: ?[*]const f64, d_r2: ?[*]const f64, d_tof: ?[*]const f64, d_normal: ?[*]const f64, n: u32, mu: f64, max_revs: u32, device: i32, d_v1: ?[*]f64, d_v2: ?[*]f64, d_status: ?[*]u8, d_iterations: ?[*]u8, stream: ?*anyopaque) i32;
+pub extern fn astroz_cuda_lambert_porkchop_device(d_dep: ?[*]const f64, d_dep_status: ?[*]const u8, d_arr: ?[*]const f64, d_arr_status: ?[*]const u8, n_pairs: u32, d_dep_jd: ?[*]const f64, d_dep_fr: ?[*]const f64, n_dep: u32, d_arr_jd: ?[*]const f64, d_arr_fr: ?[*]const f64, n_arr: u32, mu: f64, max_revs: u32, device: i32, d_dv: ?[*]f64, d_slot: ?[*]u8, d_status: ?[*]u8, stream: ?*anyopaque) i32;
+pub extern fn astroz_cuda_constellation_porkchop(h: Handle, chaser: ?[*]const u32, target: ?[*]const u32, n_pairs: u32, dep_jd: ?[*]const f64, dep_fr: ?[*]const f64, n_dep: u32, arr_jd: ?[*]const f64, arr_fr: ?[*]const f64, n_arr: u32, mu: f64, max_revs: u32, dv: ?[*]f64, slot: ?[*]u8, status: ?[*]u8) i32;
 pub extern fn astroz_cuda_fp64_peak(device: i32, tflops: ?[*]f64) i32;
 pub extern fn astroz_cuda_fp64_pipe_peak(device: i32, tflops: ?[*]f64) i32;
 
