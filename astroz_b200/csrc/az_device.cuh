@@ -672,7 +672,11 @@ AZ_HD void sdp4_cell_n(const Sdp4Sat &e, const double (&t)[kN], const double (&x
         if (!(am[k] >= 0.95)) am[k] = 1.0;
         // inclination-dependent terms re-derived per cell (src/Sdp4Batch.zig:326-339)
         const double cosip2 = cosip[k] * cosip[k];
-        const double den = 1.0 + cosip[k];
+        // 1 + cos ip.  Near 180 degrees it cancels: cos ip is known to 1e-16 absolute, so 1 + cos ip ~ 1.5e-12 (the guard
+        // below) would keep four digits, and xlcof ~ 1/(1 + cos ip) moves the argument of latitude by kilometres.  A
+        // retrograde cell takes the identity 1 + cos = sin^2 / (1 - cos) instead, exact to the digits of sin ip (the
+        // small rotation of the element set's sin/cos forms it to 1e-20 absolute); other cells keep 1 + cos ip.
+        const double den = cosip[k] < 0.0 ? sinip[k] * sinip[k] * rcp(1.0 - cosip[k]) : 1.0 + cosip[k];
         sa[k].sinio = sinip[k];
         sa[k].cosio = cosip[k];
         sa[k].aycof = -0.5 * g.j3oj2 * sinip[k];
