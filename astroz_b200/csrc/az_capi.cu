@@ -31,6 +31,7 @@
 #include "az_kernels.cuh"
 #include "az_lambert.cuh"
 #include "az_numerical.cuh"
+#include "az_obs.cuh"
 #include "az_tables.hpp"
 
 namespace {
@@ -2683,6 +2684,293 @@ int32_t astroz_cuda_fit_elements_mixed(const double *elements, uint32_t n, int32
                                        uint32_t *iterations, uint8_t *status) {
     return fit_host(elements, n, grav, offsets, jd, fr, pos, vel, m, pos_sigma, vel_sigma, fit_bstar, max_iter, device,
                     fitted, rms, iterations, status, launch_fit_mixed);
+}
+
+// ---- element fits from sensor observations (K8, az_fit_obs.cu, az_obs.cuh) ----------------------------------------
+static_assert(ASTROZ_OBS_TEME_STATE == az::kObsTemeState && ASTROZ_OBS_ECEF_STATE == az::kObsEcefState &&
+                  ASTROZ_OBS_RADAR == az::kObsRadar && ASTROZ_OBS_OPTICAL == az::kObsOptical &&
+                  ASTROZ_OBS_VALUES == az::kObsValues && ASTROZ_FIT_COVARIANCE_WORDS == az::kFitN,
+              "observation kinds and layouts");
+
+// Scalar checks of the observation fits, before anything is read, written or allocated; a receives the scalars.
+static int32_t fit_obs_check(uint32_t n, int32_t grav, int32_t fit_bstar, uint32_t max_iter, int32_t device,
+                             az::FitObsArgs *a) {
+    if (device < 0) return value_error("an element fit runs on one device: pass its ordinal");
+    if (grav != ASTROZ_WGS72 && grav != ASTROZ_WGS84) return value_error("grav must be ASTROZ_WGS72 or ASTROZ_WGS84");
+    if (max_iter == 0) return value_error("max_iter must be at least 1");
+    a->n = n;
+    a->grav = grav;
+    a->g = az::grav_consts(az::gravity(grav));
+    a->fitBstar = fit_bstar != 0;
+    a->maxIter = max_iter;
+    return ASTROZ_OK;
+}
+
+// Host-side value checks of m observations and k stations.  sigma = nullptr: astroz_cuda_observe, which has no sigmas
+// and reads no values.
+static int32_t obs_values_check(const double *jd, const double *fr, const double *value, const double *sigma,
+                                const uint32_t *station, const uint8_t *kind, uint32_t m, const double *stations,
+                                uint32_t k) {
+    if (k && !stations) return ASTROZ_NULL_POINTER;
+    for (uint32_t s = 0; s < k; ++s) {
+        const double *st = stations + (size_t)s * 3;
+        if (!std::isfinite(st[0]) || !std::isfinite(st[1]) || !std::isfinite(st[2]))
+            return value_error("stations must be finite");
+        if (!(std::fabs(st[0]) <= 90.0)) return value_error("a station latitude is outside [-90, 90] deg");
+    }
+    if (!all_finite(jd, m) || !all_finite(fr, m)) return value_error("observation times must be finite");
+    for (uint32_t i = 0; i < m; ++i) {
+        if (kind[i] >= az::kObsKinds) return value_error("unknown observation kind");
+        if (az::obs_uses_station(kind[i])) {
+            if (!station) return ASTROZ_NULL_POINTER;
+            if (station[i] >= k) return value_error("a station index is not below the station count k");
+        }
+        if (!sigma) continue;
+        const double *v = value + (size_t)i * 6, *sg = sigma + (size_t)i * 6;
+        const int count = az::obs_count(kind[i]), wr = az::obs_wrapped(kind[i]);
+        for (int c = 0; c < count; ++c) {
+            if (!(sg[c] > 0.0)) return value_error("sigma must be > 0 (+inf: component not used)");
+            if (sg[c] < INFINITY && !std::isfinite(v[c])) return value_error("a used observation value is not finite");
+        }
+        if (wr >= 0 && sg[wr] < INFINITY && !std::isfinite(v[az::obs_partner(kind[i])]))
+            return value_error("a used azimuth or right ascension needs a finite elevation or declination");
+    }
+    return ASTROZ_OK;
+}
+
+static cudaError_t launch_fit_obs_mixed(const az::FitObsArgs &a, cudaStream_t st) {
+    const cudaError_t e = az::launch_fit_obs(a, st);
+    return e != cudaSuccess ? e : az::launch_fit_obs_deep(a, st);
+}
+using FitObsLaunch = cudaError_t (*)(const az::FitObsArgs &a, cudaStream_t stream);
+
+static int32_t fit_obs_device(const double *d_elements, uint32_t n, int32_t grav, const uint32_t *d_offsets,
+                              const double *d_jd, const double *d_fr, const double *d_value, const double *d_sigma,
+                              const uint32_t *d_station, const uint8_t *d_kind, const double *d_stations,
+                              int32_t fit_bstar, uint32_t max_iter, int32_t device, double *d_fitted, double *d_wrms,
+                              uint32_t *d_n_residuals, double *d_covariance, uint32_t *d_iterations,
+                              uint8_t *d_status, uint8_t *d_model, void *stream, FitObsLaunch launch) {
+    az::FitObsArgs a{};
+    int32_t rc = fit_obs_check(n, grav, fit_bstar, max_iter, device, &a);
+    if (rc != ASTROZ_OK) return rc;
+    if (n == 0) return ASTROZ_OK;
+    if (!d_elements || !d_offsets || !d_jd || !d_fr || !d_value || !d_sigma || !d_kind || !d_fitted || !d_wrms ||
+        !d_n_residuals || !d_covariance || !d_iterations || !d_status || !d_model)
+        return ASTROZ_NULL_POINTER;
+    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
+    AZ_CUDA(cudaSetDevice(device));
+    a.elements = d_elements;
+    a.offsets = d_offsets;
+    a.jd = d_jd;
+    a.fr = d_fr;
+    a.value = d_value;
+    a.sigma = d_sigma;
+    a.station = d_station;
+    a.kind = d_kind;
+    a.stations = d_stations;
+    a.fitted = d_fitted;
+    a.wrms = d_wrms;
+    a.nResiduals = d_n_residuals;
+    a.covariance = d_covariance;
+    a.iterations = d_iterations;
+    a.status = d_status;
+    a.model = d_model;
+    AZ_CUDA(launch(a, static_cast<cudaStream_t>(stream)));
+    return ASTROZ_OK;
+}
+
+// A stream-ordered device block cut into 16-byte aligned pieces of the given byte sizes.
+struct DeviceBlock {
+    StreamBuf buf;
+    std::vector<size_t> at;
+    explicit DeviceBlock(cudaStream_t s) : buf(s) {}
+    cudaError_t alloc(std::initializer_list<size_t> bytes) {
+        size_t total = 0;
+        for (size_t b : bytes) at.push_back(total), total += (b + 15) & ~size_t(15);
+        return buf.alloc(std::max<size_t>(total, 16));
+    }
+    char *piece(int k) { return static_cast<char *>(buf.p) + at[k]; }
+    double *f64(int k) { return reinterpret_cast<double *>(piece(k)); }
+    uint32_t *u32(int k) { return reinterpret_cast<uint32_t *>(piece(k)); }
+    uint8_t *u8(int k) { return reinterpret_cast<uint8_t *>(piece(k)); }
+};
+
+// Host buffers: as fit_host -- the inputs go up once (pageable through the pinned ring, pinned by direct DMA), the
+// launch fits the batch, and the results come back by plain copies.
+static int32_t fit_obs_host(const double *elements, uint32_t n, int32_t grav, const uint32_t *offsets,
+                            const double *jd, const double *fr, const double *value, const double *sigma,
+                            const uint32_t *station, const uint8_t *kind, uint32_t m, const double *stations,
+                            uint32_t k, int32_t fit_bstar, uint32_t max_iter, int32_t device, double *fitted,
+                            double *wrms, uint32_t *n_residuals, double *covariance, uint32_t *iterations,
+                            uint8_t *status, uint8_t *model, FitObsLaunch launch) {
+    az::FitObsArgs a{};
+    int32_t rc = fit_obs_check(n, grav, fit_bstar, max_iter, device, &a);
+    if (rc != ASTROZ_OK) return rc;
+    if (n == 0) return ASTROZ_OK;
+    if (!elements || !offsets || !fitted || !wrms || !n_residuals || !covariance || !iterations || !status || !model)
+        return ASTROZ_NULL_POINTER;
+    if (m && (!jd || !fr || !value || !sigma || !kind)) return ASTROZ_NULL_POINTER;
+    for (uint32_t s = 0; s < n; ++s)
+        if (offsets[s + 1] < offsets[s]) return value_error("offsets must be non-decreasing");
+    if (offsets[n] != m) return value_error("offsets[n] must equal the observation count m");
+    if (!all_finite(elements, (size_t)8 * n)) return value_error("elements must be finite");
+    if ((rc = obs_values_check(jd, fr, value, sigma, station, kind, m, stations, k)) != ASTROZ_OK) return rc;
+    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
+    NumericalContext *c = nullptr;
+    if ((rc = numerical_context(device, &c)) != ASTROZ_OK) return rc;
+    std::lock_guard<std::mutex> lk(c->m);
+    AZ_CUDA(cudaSetDevice(device));
+    cudaStream_t st = c->stream;
+    // elements | offsets | jd | fr | value | sigma | station | kind | stations | fitted | wrms | n_res | cov | iter |
+    // status | model
+    DeviceBlock d(st);
+    AZ_CUDA(d.alloc({(size_t)64 * n, (size_t)4 * (n + 1), (size_t)8 * m, (size_t)8 * m, (size_t)48 * m,
+                     (size_t)48 * m, station ? (size_t)4 * m : 0, (size_t)m, (size_t)24 * k, (size_t)64 * n,
+                     (size_t)8 * n, (size_t)4 * n, (size_t)8 * az::kFitN * n, (size_t)4 * n, (size_t)n, (size_t)n}));
+    auto up = [&](const void *src, void *dst, size_t elemBytes, size_t count) {
+        void *const dd[1] = {dst};
+        const void *const ss[1] = {src};
+        return c->pipe.ring.upload(az::is_pageable(src), 1, ss, dd, &elemBytes, count, st);
+    };
+    AZ_CUDA(up(elements, d.f64(0), 8, (size_t)8 * n));
+    AZ_CUDA(up(offsets, d.u32(1), 4, (size_t)n + 1));
+    if (m) {
+        AZ_CUDA(up(jd, d.f64(2), 8, m));
+        AZ_CUDA(up(fr, d.f64(3), 8, m));
+        AZ_CUDA(up(value, d.f64(4), 48, m));
+        AZ_CUDA(up(sigma, d.f64(5), 48, m));
+        if (station) AZ_CUDA(up(station, d.u32(6), 4, m));
+        AZ_CUDA(up(kind, d.u8(7), 1, m));
+    }
+    if (k) AZ_CUDA(up(stations, d.f64(8), 24, k));
+    a.elements = d.f64(0);
+    a.offsets = d.u32(1);
+    a.jd = d.f64(2);
+    a.fr = d.f64(3);
+    a.value = d.f64(4);
+    a.sigma = d.f64(5);
+    a.station = station ? d.u32(6) : nullptr;
+    a.kind = d.u8(7);
+    a.stations = k ? d.f64(8) : nullptr;
+    a.fitted = d.f64(9);
+    a.wrms = d.f64(10);
+    a.nResiduals = d.u32(11);
+    a.covariance = d.f64(12);
+    a.iterations = d.u32(13);
+    a.status = d.u8(14);
+    a.model = d.u8(15);
+    AZ_CUDA(launch(a, st));
+    AZ_CUDA(cudaMemcpyAsync(fitted, a.fitted, (size_t)64 * n, cudaMemcpyDeviceToHost, st));
+    AZ_CUDA(cudaMemcpyAsync(wrms, a.wrms, (size_t)8 * n, cudaMemcpyDeviceToHost, st));
+    AZ_CUDA(cudaMemcpyAsync(n_residuals, a.nResiduals, (size_t)4 * n, cudaMemcpyDeviceToHost, st));
+    AZ_CUDA(cudaMemcpyAsync(covariance, a.covariance, (size_t)8 * az::kFitN * n, cudaMemcpyDeviceToHost, st));
+    AZ_CUDA(cudaMemcpyAsync(iterations, a.iterations, (size_t)4 * n, cudaMemcpyDeviceToHost, st));
+    AZ_CUDA(cudaMemcpyAsync(status, a.status, n, cudaMemcpyDeviceToHost, st));
+    AZ_CUDA(cudaMemcpyAsync(model, a.model, n, cudaMemcpyDeviceToHost, st));
+    AZ_CUDA(d.buf.release());
+    AZ_CUDA(cudaStreamSynchronize(st));
+    return ASTROZ_OK;
+}
+
+int32_t astroz_cuda_fit_observations(const double *elements, uint32_t n, int32_t grav, const uint32_t *offsets,
+                                     const double *jd, const double *fr, const double *value, const double *sigma,
+                                     const uint32_t *station, const uint8_t *kind, uint32_t m, const double *stations,
+                                     uint32_t k, int32_t fit_bstar, uint32_t max_iter, int32_t device, double *fitted,
+                                     double *wrms, uint32_t *n_residuals, double *covariance, uint32_t *iterations,
+                                     uint8_t *status, uint8_t *model) {
+    return fit_obs_host(elements, n, grav, offsets, jd, fr, value, sigma, station, kind, m, stations, k, fit_bstar,
+                        max_iter, device, fitted, wrms, n_residuals, covariance, iterations, status, model,
+                        az::launch_fit_obs);
+}
+
+int32_t astroz_cuda_fit_observations_mixed(const double *elements, uint32_t n, int32_t grav, const uint32_t *offsets,
+                                           const double *jd, const double *fr, const double *value,
+                                           const double *sigma, const uint32_t *station, const uint8_t *kind,
+                                           uint32_t m, const double *stations, uint32_t k, int32_t fit_bstar,
+                                           uint32_t max_iter, int32_t device, double *fitted, double *wrms,
+                                           uint32_t *n_residuals, double *covariance, uint32_t *iterations,
+                                           uint8_t *status, uint8_t *model) {
+    return fit_obs_host(elements, n, grav, offsets, jd, fr, value, sigma, station, kind, m, stations, k, fit_bstar,
+                        max_iter, device, fitted, wrms, n_residuals, covariance, iterations, status, model,
+                        launch_fit_obs_mixed);
+}
+
+int32_t astroz_cuda_fit_observations_device(const double *d_elements, uint32_t n, int32_t grav,
+                                            const uint32_t *d_offsets, const double *d_jd, const double *d_fr,
+                                            const double *d_value, const double *d_sigma, const uint32_t *d_station,
+                                            const uint8_t *d_kind, const double *d_stations, int32_t fit_bstar,
+                                            uint32_t max_iter, int32_t device, double *d_fitted, double *d_wrms,
+                                            uint32_t *d_n_residuals, double *d_covariance, uint32_t *d_iterations,
+                                            uint8_t *d_status, uint8_t *d_model, void *stream) {
+    return fit_obs_device(d_elements, n, grav, d_offsets, d_jd, d_fr, d_value, d_sigma, d_station, d_kind, d_stations,
+                          fit_bstar, max_iter, device, d_fitted, d_wrms, d_n_residuals, d_covariance, d_iterations,
+                          d_status, d_model, stream, az::launch_fit_obs);
+}
+
+int32_t astroz_cuda_fit_observations_mixed_device(const double *d_elements, uint32_t n, int32_t grav,
+                                                  const uint32_t *d_offsets, const double *d_jd, const double *d_fr,
+                                                  const double *d_value, const double *d_sigma,
+                                                  const uint32_t *d_station, const uint8_t *d_kind,
+                                                  const double *d_stations, int32_t fit_bstar, uint32_t max_iter,
+                                                  int32_t device, double *d_fitted, double *d_wrms,
+                                                  uint32_t *d_n_residuals, double *d_covariance,
+                                                  uint32_t *d_iterations, uint8_t *d_status, uint8_t *d_model,
+                                                  void *stream) {
+    return fit_obs_device(d_elements, n, grav, d_offsets, d_jd, d_fr, d_value, d_sigma, d_station, d_kind, d_stations,
+                          fit_bstar, max_iter, device, d_fitted, d_wrms, d_n_residuals, d_covariance, d_iterations,
+                          d_status, d_model, stream, launch_fit_obs_mixed);
+}
+
+int32_t astroz_cuda_observe(const double *states, const double *jd, const double *fr, const uint8_t *kind,
+                            const uint32_t *station, uint32_t m, const double *stations, uint32_t k, int32_t device,
+                            double *values) {
+    if (device < 0) return value_error("observe runs on one device: pass its ordinal");
+    if (m == 0) return ASTROZ_OK;
+    if (!states || !jd || !fr || !kind || !values) return ASTROZ_NULL_POINTER;
+    int32_t rc = obs_values_check(jd, fr, nullptr, nullptr, station, kind, m, stations, k);
+    if (rc != ASTROZ_OK) return rc;
+    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
+    NumericalContext *c = nullptr;
+    if ((rc = numerical_context(device, &c)) != ASTROZ_OK) return rc;
+    std::lock_guard<std::mutex> lk(c->m);
+    AZ_CUDA(cudaSetDevice(device));
+    cudaStream_t st = c->stream;
+    // states | jd | fr | kind | station | stations | values
+    DeviceBlock d(st);
+    AZ_CUDA(d.alloc({(size_t)48 * m, (size_t)8 * m, (size_t)8 * m, (size_t)m, station ? (size_t)4 * m : 0,
+                     (size_t)24 * k, (size_t)48 * m}));
+    auto up = [&](const void *src, void *dst, size_t elemBytes, size_t count) {
+        void *const dd[1] = {dst};
+        const void *const ss[1] = {src};
+        return c->pipe.ring.upload(az::is_pageable(src), 1, ss, dd, &elemBytes, count, st);
+    };
+    AZ_CUDA(up(states, d.f64(0), 48, m));
+    AZ_CUDA(up(jd, d.f64(1), 8, m));
+    AZ_CUDA(up(fr, d.f64(2), 8, m));
+    AZ_CUDA(up(kind, d.u8(3), 1, m));
+    if (station) AZ_CUDA(up(station, d.u32(4), 4, m));
+    if (k) AZ_CUDA(up(stations, d.f64(5), 24, k));
+    AZ_CUDA(az::launch_observe(d.f64(0), d.f64(1), d.f64(2), d.u8(3),
+                               station ? d.u32(4) : nullptr, k ? d.f64(5) : nullptr, m,
+                               d.f64(6), st));
+    AZ_CUDA(cudaMemcpyAsync(values, d.f64(6), (size_t)48 * m, cudaMemcpyDeviceToHost, st));
+    AZ_CUDA(d.buf.release());
+    AZ_CUDA(cudaStreamSynchronize(st));
+    return ASTROZ_OK;
+}
+
+int32_t astroz_cuda_observe_device(const double *d_states, const double *d_jd, const double *d_fr,
+                                   const uint8_t *d_kind, const uint32_t *d_station, uint32_t m,
+                                   const double *d_stations, int32_t device, double *d_values, void *stream) {
+    if (device < 0) return value_error("observe runs on one device: pass its ordinal");
+    if (m == 0) return ASTROZ_OK;
+    if (!d_states || !d_jd || !d_fr || !d_kind || !d_values) return ASTROZ_NULL_POINTER;
+    int32_t rc = check_device_ordinal(device);
+    if (rc != ASTROZ_OK) return rc;
+    AZ_CUDA(cudaSetDevice(device));
+    AZ_CUDA(az::launch_observe(d_states, d_jd, d_fr, d_kind, d_station, d_stations, m, d_values,
+                               static_cast<cudaStream_t>(stream)));
+    return ASTROZ_OK;
 }
 
 int32_t astroz_cuda_parse_tle(const char *line1, const char *line2, double *elements) {

@@ -183,6 +183,29 @@ AZ_HD bool fit_build_set(const double (&x)[kFitVars], int k, double epochJd, con
     return fit_build_set_of<FitNearEarth>(x, k, epochJd, grav, cols, inv);
 }
 
+// One observation's share of J^T r and J^T J: r[6] its weighted residuals, J its 6 x nvar Jacobian, entry (j, c) at
+// J[(j * 6 + c) * stride]; word q of the FitSums being accumulated is acc[q * stride].
+AZ_HD void fit_accumulate_normal(int nvar, const double (&r)[6], const double *J, double *acc, int stride) {
+    // all kFitVars columns, the held B* column as zeros, so the sums keep static indices (registers on the device)
+#pragma unroll
+    for (int j = 0; j < kFitVars; ++j) {
+        double jc[6];
+#pragma unroll
+        for (int c = 0; c < 6; ++c) jc[c] = j < nvar ? J[(j * 6 + c) * stride] : 0.0;
+        double gj = 0.0;
+#pragma unroll
+        for (int c = 0; c < 6; ++c) gj += jc[c] * r[c];
+        acc[(4 + kFitN + j) * stride] += gj;
+#pragma unroll
+        for (int k = j; k < kFitVars; ++k) {
+            double njk = 0.0;
+#pragma unroll
+            for (int c = 0; c < 6; ++c) njk += jc[c] * (k < nvar ? J[(k * 6 + c) * stride] : 0.0);
+            acc[(4 + fit_tri(j, k)) * stride] += njk;
+        }
+    }
+}
+
 // One observation's contribution to s: the model under set 0 and under sets 1..nvar (eval(k, jdFull, ts, f) = the TEME
 // state f[6] of set k at the observation, false when that set's cell fails), the weighted residual and the difference
 // columns of the Jacobian.  J is scratch for the 6 x nvar Jacobian of this observation, entry (j, c) at
@@ -230,24 +253,7 @@ AZ_HD bool fit_accumulate_model(EvalFn eval, int nvar, const double *inv, double
         ok = eval(1 + j, jdFull, ts, f) && ok;
         for (int c = 0; c < 6; ++c) J[(j * 6 + c) * stride] = c < nc ? (f[c] - f0[c]) * w[c] * inv[1 + j] : 0.0;
     }
-    // all kFitVars columns, the held B* column as zeros, so the sums keep static indices (registers on the device)
-#pragma unroll
-    for (int j = 0; j < kFitVars; ++j) {
-        double jc[6];
-#pragma unroll
-        for (int c = 0; c < 6; ++c) jc[c] = j < nvar ? J[(j * 6 + c) * stride] : 0.0;
-        double gj = 0.0;
-#pragma unroll
-        for (int c = 0; c < 6; ++c) gj += jc[c] * r[c];
-        acc[(4 + kFitN + j) * stride] += gj;
-#pragma unroll
-        for (int k = j; k < kFitVars; ++k) {
-            double njk = 0.0;
-#pragma unroll
-            for (int c = 0; c < 6; ++c) njk += jc[c] * (k < nvar ? J[(k * 6 + c) * stride] : 0.0);
-            acc[(4 + fit_tri(j, k)) * stride] += njk;
-        }
-    }
+    fit_accumulate_normal(nvar, r, J, acc, stride);
     return ok;
 }
 
@@ -347,13 +353,14 @@ struct FitResult {
 };
 
 // The whole fit of one satellite.  pass(x, s) evaluates the nominal set x and its nvar perturbed sets over the
-// satellite's nObs observations into s (zeroed by the caller) and returns false when a set cannot be built; it must
-// return the same bits wherever it is called for the same x.  Failing satellites (init, deep space, too few
-// observations) return their initial columns with zero RMS and no iterations.
+// satellite's observations into s (zeroed by the caller) and returns false when a set cannot be built; it must
+// return the same bits wherever it is called for the same x.  nResiduals is the number of scalar residuals the
+// observations carry.  Failing satellites (init, deep space, too few residuals) return their initial columns with
+// zero RMS and no iterations; for a fitted satellite final(s) receives the sums at its final iterate.
 // Model (FitNearEarth, FitDeepSpace) gives the variables and the class rule of the initial set.
-template <typename PassFn, typename Model = FitNearEarth>
-AZ_HD void fit_satellite(const double *el0, const Gravity &grav, bool fitBstar, uint32_t maxIter, uint32_t nObs,
-                         bool haveVel, PassFn pass, FitResult &out, Model = Model{}) {
+template <typename PassFn, typename FinalFn, typename Model>
+AZ_HD void fit_satellite_run(const double *el0, const Gravity &grav, bool fitBstar, uint32_t maxIter,
+                             uint64_t nResiduals, PassFn pass, FinalFn final, FitResult &out, Model) {
     const int nvar = fitBstar ? kFitVars : kFitVars - 1;
     for (int c = 0; c < 8; ++c) out.el[c] = el0[c];
     out.rmsPos = out.rmsVel = 0.0;
@@ -369,7 +376,7 @@ AZ_HD void fit_satellite(const double *el0, const Gravity &grav, bool fitBstar, 
             return;
         }
     }
-    if ((uint64_t)nObs * (haveVel ? 6 : 3) < (uint64_t)nvar) {
+    if (nResiduals < (uint64_t)nvar) {
         out.status = kFitTooFew;
         return;
     }
@@ -408,10 +415,20 @@ AZ_HD void fit_satellite(const double *el0, const Gravity &grav, bool fitBstar, 
     Model::elements_of(x, el0[0], t);
     out.el[0] = t.epochJd; out.el[1] = t.revPerDay; out.el[2] = t.ecc; out.el[3] = t.inclDeg;
     out.el[4] = t.raanDeg; out.el[5] = t.argpDeg; out.el[6] = t.maDeg; out.el[7] = t.bstar;
-    out.rmsPos = std::sqrt(s.pos2 / nObs);
-    out.rmsVel = haveVel ? std::sqrt(s.vel2 / nObs) : 0.0;
+    final(s);
     out.iters = it;
     out.status = status;
+}
+
+// The fit of TEME ephemerides: nObs positions (and velocities with haveVel), RMS from the final iterate's sums.
+template <typename PassFn, typename Model = FitNearEarth>
+AZ_HD void fit_satellite(const double *el0, const Gravity &grav, bool fitBstar, uint32_t maxIter, uint32_t nObs,
+                         bool haveVel, PassFn pass, FitResult &out, Model model = Model{}) {
+    auto final = [&](const FitSums &s) {
+        out.rmsPos = std::sqrt(s.pos2 / nObs);
+        out.rmsVel = haveVel ? std::sqrt(s.vel2 / nObs) : 0.0;
+    };
+    fit_satellite_run(el0, grav, fitBstar, maxIter, (uint64_t)nObs * (haveVel ? 6 : 3), pass, final, out, model);
 }
 
 }  // namespace az

@@ -152,6 +152,37 @@ cudaError_t launch_fit(const FitArgs &a, cudaStream_t stream);
 // as it is, so queued after launch_fit on the same arguments it completes a mixed batch.
 cudaError_t launch_fit_deep(const FitArgs &a, cudaStream_t stream);
 
+// K8 from sensor observations (az_fit_obs.cu, az_obs.cuh): TEME or ECEF states, radar, optical angles.  Device pointers.
+struct FitObsArgs {
+    const double *elements = nullptr;    // [8][n]
+    uint32_t n = 0;
+    const uint32_t *offsets = nullptr;   // [n + 1]
+    const double *jd = nullptr, *fr = nullptr;
+    const double *value = nullptr;       // [m][6]
+    const double *sigma = nullptr;       // [m][6]: +inf = component not used
+    const uint32_t *station = nullptr;   // [m]: row of stations (radar and optical kinds)
+    const uint8_t *kind = nullptr;       // [m] ASTROZ_OBS_*
+    const double *stations = nullptr;    // [k][3]: geodetic lat deg, lon deg, height km (WGS84)
+    int fitBstar = 1;
+    uint32_t maxIter = 25;
+    int grav = 1;
+    GravConsts g{};
+    double *fitted = nullptr;            // [8][n]
+    double *wrms = nullptr;              // [n]: sqrt(cost / used residuals)
+    uint32_t *nResiduals = nullptr;      // [n]
+    double *covariance = nullptr;        // [n][28]: upper triangle of the fitted variables' covariance
+    uint32_t *iterations = nullptr;      // [n]
+    uint8_t *status = nullptr;           // [n]
+    uint8_t *model = nullptr;            // [n]: 0 near-earth variables, 1 deep-space (equinoctial) variables
+};
+cudaError_t launch_fit_obs(const FitObsArgs &a, cudaStream_t stream);
+// the deep-space rows only, under the deep-space model (as launch_fit_deep)
+cudaError_t launch_fit_obs_deep(const FitObsArgs &a, cudaStream_t stream);
+// h(kind, state) of m observations, one thread each: states[m][6] TEME -> values[m][6] (zero past the kind's count)
+cudaError_t launch_observe(const double *states, const double *jd, const double *fr, const uint8_t *kind,
+                           const uint32_t *station, const double *stations, uint32_t m, double *values,
+                           cudaStream_t stream);
+
 // DFMA throughput microbenchmark: returns achieved fp64 FLOP/s (FMA = 2).
 cudaError_t measure_fp64_peak(double *flops);
 // Arithmetic peak of the fp64 pipe: SMs x 64 lanes x 2 FLOP x the maximum SM clock.

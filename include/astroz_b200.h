@@ -602,6 +602,89 @@ int32_t astroz_cuda_fit_elements_mixed_device(const double *d_elements, uint32_t
                                               double vel_sigma, int32_t fit_bstar, uint32_t max_iter, int32_t device,
                                               double *d_fitted, double *d_rms, uint32_t *d_iterations,
                                               uint8_t *d_status, void *stream);
+
+/* ---- element fits (K8) from sensor observations: Earth-fixed states, radar and optical angles, with covariance ---------
+ * astroz_cuda_fit_elements[_mixed] with a measurement layer between the model's TEME state and the residual.  The
+ * variables, steps, damping, stopping rule, deep-space handling and the mixed calls' row rule are K8's.  Observation i
+ * of satellite s ([offsets[s], offsets[s + 1]) as in K8) is jd[i] + fr[i], kind[i] (ASTROZ_OBS_*), value[i][6] and
+ * sigma[i][6] (components past the kind's count are ignored), and station[i], a row of stations[k][3] = (geodetic
+ * latitude deg, longitude deg, height km) on WGS84, read by the radar and optical kinds only (station may be NULL when
+ * no observation uses one):
+ *   TEME_STATE  x y z [km], vx vy vz [km/s]: K8's observation;
+ *   ECEF_STATE  r_ecef = Rz(GMST) r, the rotation of propagate_pairs' ECEF output (GMST of the observation's jd + fr),
+ *               and the Earth-fixed velocity v_ecef = Rz(GMST) v - omega x r_ecef (omega = 360.98564736629 deg/day).
+ *               Unlike this kind, the library's ECEF output mode leaves omega x r out, as the reference does;
+ *   RADAR       range [km], azimuth [rad, from north through east], elevation [rad], range-rate [km/s] in the station's
+ *               geodetic horizon frame: rho = r_ecef - r_station, range-rate = rho . v_ecef / |rho|;
+ *   OPTICAL     topocentric right ascension and declination [rad] in TEME: rho = r_teme - Rz(GMST)^T r_station.
+ * Observations are geometric and instantaneous: no light time, aberration or refraction.  Polar motion and the TEME ->
+ * GCRF rotation are the caller's: optical angles must be in TEME.
+ *   residuals: (observed - model) / sigma.  Azimuth and right-ascension differences are wrapped to (-pi, pi] and
+ *              multiplied by the cosine of the observed elevation / declination (sigma is an arc on the sky).  sigma =
+ *              +inf: the component is not used (a radar without range-rate, a position-only fix);
+ *   outputs:   fitted[8][n] and iterations[n], status[n] as K8; wrms[n] = sqrt(cost / used residuals), dimensionless,
+ *              about 1 when the sigmas are right; n_residuals[n] the used scalar residuals (ASTROZ_FIT_TOO_FEW_
+ *              OBSERVATIONS when fewer than the fitted variables); covariance[n][28] the upper triangle, row by row, of
+ *              the 7 x 7 covariance (J^T W J)^-1 of the fitted variables at the final iterate, in the fit's own
+ *              variables and order (near-earth: n, e cos w, e sin w, i, RAAN, M + w, B*; deep space: K8's equinoctial
+ *              set), units rev/day, rad and 1/ER.  The B* row and column are zero when B* is held.  All 28 words zero:
+ *              the normal matrix was not positive definite (or the satellite was not fitted); model[n] 0 when row s
+ *              was fitted in the near-earth variables, 1 in the deep-space ones (the _mixed calls' deep-space rows):
+ *              the variables its covariance is stated in.
+ * ASTROZ_VALUE_ERROR, nothing written: device = -1, max_iter = 0, an unknown grav; and for the host calls offsets that
+ * decrease or offsets[n] != m, a non-finite element or time, an unknown kind, a station index >= k (kinds that read
+ * one), a sigma that is <= 0 or NaN, a non-finite value in a used component (or the elevation / declination of a used
+ * azimuth / right ascension), a station that is not finite or whose latitude is outside [-90, 90]. */
+#define ASTROZ_OBS_TEME_STATE 0
+#define ASTROZ_OBS_ECEF_STATE 1
+#define ASTROZ_OBS_RADAR      2
+#define ASTROZ_OBS_OPTICAL    3
+#define ASTROZ_OBS_VALUES     6    /* columns of value and sigma */
+#define ASTROZ_FIT_COVARIANCE_WORDS 28
+/* HOST buffers: one upload (pageable through a pinned ring, pinned by direct DMA), one launch, plain copies back. */
+int32_t astroz_cuda_fit_observations(const double *elements, uint32_t n, int32_t grav, const uint32_t *offsets,
+                                     const double *jd, const double *fr, const double *value, const double *sigma,
+                                     const uint32_t *station, const uint8_t *kind, uint32_t m, const double *stations,
+                                     uint32_t k, int32_t fit_bstar, uint32_t max_iter, int32_t device, double *fitted,
+                                     double *wrms, uint32_t *n_residuals, double *covariance, uint32_t *iterations,
+                                     uint8_t *status, uint8_t *model);
+/* Mixed batches: deep-space rows fitted under SDP4 too, as astroz_cuda_fit_elements_mixed. */
+int32_t astroz_cuda_fit_observations_mixed(const double *elements, uint32_t n, int32_t grav, const uint32_t *offsets,
+                                           const double *jd, const double *fr, const double *value,
+                                           const double *sigma, const uint32_t *station, const uint8_t *kind,
+                                           uint32_t m, const double *stations, uint32_t k, int32_t fit_bstar,
+                                           uint32_t max_iter, int32_t device, double *fitted, double *wrms,
+                                           uint32_t *n_residuals, double *covariance, uint32_t *iterations,
+                                           uint8_t *status, uint8_t *model);
+/* DEVICE pointers on `device` (the observation count is d_offsets[n]): one launch (two for _mixed) on `stream`, no
+ * allocation, no synchronisation; only the scalar arguments are checked -- kinds, stations and sigmas must be valid. */
+int32_t astroz_cuda_fit_observations_device(const double *d_elements, uint32_t n, int32_t grav,
+                                            const uint32_t *d_offsets, const double *d_jd, const double *d_fr,
+                                            const double *d_value, const double *d_sigma, const uint32_t *d_station,
+                                            const uint8_t *d_kind, const double *d_stations, int32_t fit_bstar,
+                                            uint32_t max_iter, int32_t device, double *d_fitted, double *d_wrms,
+                                            uint32_t *d_n_residuals, double *d_covariance, uint32_t *d_iterations,
+                                            uint8_t *d_status, uint8_t *d_model, void *stream);
+int32_t astroz_cuda_fit_observations_mixed_device(const double *d_elements, uint32_t n, int32_t grav,
+                                                  const uint32_t *d_offsets, const double *d_jd, const double *d_fr,
+                                                  const double *d_value, const double *d_sigma,
+                                                  const uint32_t *d_station, const uint8_t *d_kind,
+                                                  const double *d_stations, int32_t fit_bstar, uint32_t max_iter,
+                                                  int32_t device, double *d_fitted, double *d_wrms,
+                                                  uint32_t *d_n_residuals, double *d_covariance,
+                                                  uint32_t *d_iterations, uint8_t *d_status, uint8_t *d_model,
+                                                  void *stream);
+/* The measurement model alone, one thread per observation: states[m][6] (TEME km, km/s) at jd[i] + fr[i] ->
+ * values[m][6], the kind's values (azimuth and right ascension in [0, 2 pi)), zero past its count.  For per-observation
+ * residuals and outlier editing; no visibility search: h is evaluated at the times given.  ASTROZ_VALUE_ERROR, nothing
+ * written: device = -1; for the host call an unknown kind, a station index >= k, a bad station, a non-finite time.
+ * The _device form checks only its scalars and runs on `stream`. */
+int32_t astroz_cuda_observe(const double *states, const double *jd, const double *fr, const uint8_t *kind,
+                            const uint32_t *station, uint32_t m, const double *stations, uint32_t k, int32_t device,
+                            double *values);
+int32_t astroz_cuda_observe_device(const double *d_states, const double *d_jd, const double *d_fr,
+                                   const uint8_t *d_kind, const uint32_t *d_station, uint32_t m,
+                                   const double *d_stations, int32_t device, double *d_values, void *stream);
 /* One TLE line pair read by the library's own parser (src/Tle.zig:49-101) into the eight element columns above, the
  * numbers astroz_cuda_constellation_create would use.  ASTROZ_BAD_TLE_LENGTH when the pair cannot be read. */
 int32_t astroz_cuda_parse_tle(const char *line1, const char *line2, double *elements);
