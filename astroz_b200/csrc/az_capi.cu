@@ -25,6 +25,7 @@
 #include <thread>
 #include <vector>
 
+#include "az_covariance.cuh"
 #include "az_fit.cuh"
 #include "az_hostcopy.cuh"
 #include "az_ingest.cuh"
@@ -2970,6 +2971,120 @@ int32_t astroz_cuda_observe_device(const double *d_states, const double *d_jd, c
     AZ_CUDA(cudaSetDevice(device));
     AZ_CUDA(az::launch_observe(d_states, d_jd, d_fr, d_kind, d_station, d_stations, m, d_values,
                                static_cast<cudaStream_t>(stream)));
+    return ASTROZ_OK;
+}
+
+// ---- state covariance (K10, az_covariance.cu, az_covariance.cuh) ----------------------------------------------------
+static_assert(ASTROZ_COV_OK == az::kCovOk && ASTROZ_COV_INIT_FAILED == az::kCovInitFailed &&
+                  ASTROZ_COV_CELL_FAILED == az::kCovCellFailed && ASTROZ_COV_FRAME_TEME == az::kCovFrameTeme &&
+                  ASTROZ_COV_FRAME_RTN == az::kCovFrameRtn && ASTROZ_STATE_COVARIANCE_WORDS == az::kCovWords,
+              "covariance status bytes, frames and layout");
+
+// Scalar checks of the covariance calls, before anything is read, written or allocated; a receives the scalars.
+static int32_t cov_check(uint32_t n, int32_t grav, uint32_t m, int32_t frame, int32_t device, az::CovArgs *a) {
+    if (device < 0) return value_error("covariance propagation runs on one device: pass its ordinal");
+    if (grav != ASTROZ_WGS72 && grav != ASTROZ_WGS84) return value_error("grav must be ASTROZ_WGS72 or ASTROZ_WGS84");
+    if (frame != ASTROZ_COV_FRAME_TEME && frame != ASTROZ_COV_FRAME_RTN)
+        return value_error("frame must be ASTROZ_COV_FRAME_TEME or ASTROZ_COV_FRAME_RTN");
+    a->n = n;
+    a->m = m;
+    a->grav = grav;
+    a->g = az::grav_consts(az::gravity(grav));
+    a->frame = frame;
+    return ASTROZ_OK;
+}
+
+int32_t astroz_cuda_propagate_covariance_device(const double *d_elements, uint32_t n, int32_t grav,
+                                                const double *d_covariance, const uint8_t *d_model,
+                                                const uint32_t *d_offsets, const double *d_jd, const double *d_fr,
+                                                uint32_t m, int32_t frame, int32_t device, double *d_state,
+                                                double *d_state_covariance, double *d_jacobian, uint8_t *d_status,
+                                                void *stream) {
+    az::CovArgs a{};
+    int32_t rc = cov_check(n, grav, m, frame, device, &a);
+    if (rc != ASTROZ_OK) return rc;
+    if (n == 0 || m == 0) return ASTROZ_OK;
+    if (!d_elements || !d_covariance || !d_offsets || !d_jd || !d_fr || !d_state_covariance || !d_status)
+        return ASTROZ_NULL_POINTER;
+    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
+    AZ_CUDA(cudaSetDevice(device));
+    a.elements = d_elements;
+    a.covariance = d_covariance;
+    a.model = d_model;
+    a.offsets = d_offsets;
+    a.jd = d_jd;
+    a.fr = d_fr;
+    a.state = d_state;
+    a.sigma = d_state_covariance;
+    a.jacobian = d_jacobian;
+    a.status = d_status;
+    AZ_CUDA(az::launch_covariance(a, static_cast<cudaStream_t>(stream)));
+    return ASTROZ_OK;
+}
+
+// Host buffers: as fit_obs_host -- the inputs go up once (pageable through the pinned ring, pinned by direct DMA), the
+// two launches run on the device's stream, and the results come back by plain copies.
+int32_t astroz_cuda_propagate_covariance(const double *elements, uint32_t n, int32_t grav, const double *covariance,
+                                         const uint8_t *model, const uint32_t *offsets, const double *jd,
+                                         const double *fr, uint32_t m, int32_t frame, int32_t device, double *state,
+                                         double *state_covariance, double *jacobian, uint8_t *status) {
+    az::CovArgs a{};
+    int32_t rc = cov_check(n, grav, m, frame, device, &a);
+    if (rc != ASTROZ_OK) return rc;
+    if (!offsets) return ASTROZ_NULL_POINTER;
+    if (n && (!elements || !covariance)) return ASTROZ_NULL_POINTER;
+    if (m && (!jd || !fr || !state_covariance || !status)) return ASTROZ_NULL_POINTER;
+    if (offsets[0] != 0) return value_error("offsets[0] must be 0");
+    for (uint32_t s = 0; s < n; ++s)
+        if (offsets[s + 1] < offsets[s]) return value_error("offsets must be non-decreasing");
+    if (offsets[n] != m) return value_error("offsets[n] must equal the query count m");
+    if (!all_finite(elements, (size_t)8 * n)) return value_error("elements must be finite");
+    if (!all_finite(covariance, (size_t)az::kFitN * n)) return value_error("covariance words must be finite");
+    if (!all_finite(jd, m) || !all_finite(fr, m)) return value_error("query times must be finite");
+    if (model)
+        for (uint32_t s = 0; s < n; ++s)
+            if (model[s] > 1) return value_error("a model byte is not 0 (near-earth) or 1 (deep space)");
+    if (n == 0 || m == 0) return ASTROZ_OK;
+    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
+    NumericalContext *c = nullptr;
+    if ((rc = numerical_context(device, &c)) != ASTROZ_OK) return rc;
+    std::lock_guard<std::mutex> lk(c->m);
+    AZ_CUDA(cudaSetDevice(device));
+    cudaStream_t st = c->stream;
+    // elements | covariance | model | offsets | jd | fr | state | state_covariance | jacobian | status
+    DeviceBlock d(st);
+    AZ_CUDA(d.alloc({(size_t)64 * n, (size_t)8 * az::kFitN * n, model ? (size_t)n : 0, (size_t)4 * (n + 1),
+                     (size_t)8 * m, (size_t)8 * m, state ? (size_t)48 * m : 0, (size_t)8 * az::kCovWords * m,
+                     jacobian ? (size_t)8 * az::kCovJacWords * m : 0, (size_t)m}));
+    auto up = [&](const void *src, void *dst, size_t elemBytes, size_t count) {
+        void *const dd[1] = {dst};
+        const void *const ss[1] = {src};
+        return c->pipe.ring.upload(az::is_pageable(src), 1, ss, dd, &elemBytes, count, st);
+    };
+    AZ_CUDA(up(elements, d.f64(0), 8, (size_t)8 * n));
+    AZ_CUDA(up(covariance, d.f64(1), 8 * az::kFitN, n));
+    if (model) AZ_CUDA(up(model, d.u8(2), 1, n));
+    AZ_CUDA(up(offsets, d.u32(3), 4, (size_t)n + 1));
+    AZ_CUDA(up(jd, d.f64(4), 8, m));
+    AZ_CUDA(up(fr, d.f64(5), 8, m));
+    a.elements = d.f64(0);
+    a.covariance = d.f64(1);
+    a.model = model ? d.u8(2) : nullptr;
+    a.offsets = d.u32(3);
+    a.jd = d.f64(4);
+    a.fr = d.f64(5);
+    a.state = state ? d.f64(6) : nullptr;
+    a.sigma = d.f64(7);
+    a.jacobian = jacobian ? d.f64(8) : nullptr;
+    a.status = d.u8(9);
+    AZ_CUDA(az::launch_covariance(a, st));
+    if (state) AZ_CUDA(cudaMemcpyAsync(state, a.state, (size_t)48 * m, cudaMemcpyDeviceToHost, st));
+    AZ_CUDA(cudaMemcpyAsync(state_covariance, a.sigma, (size_t)8 * az::kCovWords * m, cudaMemcpyDeviceToHost, st));
+    if (jacobian)
+        AZ_CUDA(cudaMemcpyAsync(jacobian, a.jacobian, (size_t)8 * az::kCovJacWords * m, cudaMemcpyDeviceToHost, st));
+    AZ_CUDA(cudaMemcpyAsync(status, a.status, m, cudaMemcpyDeviceToHost, st));
+    AZ_CUDA(d.buf.release());
+    AZ_CUDA(cudaStreamSynchronize(st));
     return ASTROZ_OK;
 }
 

@@ -183,6 +183,28 @@ cudaError_t launch_observe(const double *states, const double *jd, const double 
                            const uint32_t *station, const double *stations, uint32_t m, double *values,
                            cudaStream_t stream);
 
+// K10: fitted covariances carried to state covariances at query times (az_covariance.cu, az_covariance.cuh).  Device
+// pointers.
+struct CovArgs {
+    const double *elements = nullptr;    // [8][n]
+    const double *covariance = nullptr;  // [n][28]: upper triangle of P in the fit's variables
+    const uint8_t *model = nullptr;      // [n], nullable (all 0): 0 near-earth variables, 1 deep-space variables
+    uint32_t n = 0;
+    const uint32_t *offsets = nullptr;   // [n + 1]: satellite s owns queries [offsets[s], offsets[s + 1])
+    const double *jd = nullptr, *fr = nullptr;
+    uint32_t m = 0;
+    uint32_t chunk = 0;                  // queries per work item: launch_covariance sets cov_chunk(m)
+    int frame = 0;                       // ASTROZ_COV_FRAME_*
+    int grav = 1;
+    GravConsts g{};
+    double *state = nullptr;             // [m][6] TEME, nullable
+    double *sigma = nullptr;             // [m][21]
+    double *jacobian = nullptr;          // [m][6][7], nullable
+    uint8_t *status = nullptr;           // [m] ASTROZ_COV_*
+};
+// the near-earth rows' queries (model 0), then on the same stream the deep-space rows' (model 1)
+cudaError_t launch_covariance(const CovArgs &a, cudaStream_t stream);
+
 // DFMA throughput microbenchmark: returns achieved fp64 FLOP/s (FMA = 2).
 cudaError_t measure_fp64_peak(double *flops);
 // Arithmetic peak of the fp64 pipe: SMs x 64 lanes x 2 FLOP x the maximum SM clock.

@@ -685,6 +685,52 @@ int32_t astroz_cuda_observe(const double *states, const double *jd, const double
 int32_t astroz_cuda_observe_device(const double *d_states, const double *d_jd, const double *d_fr,
                                    const uint8_t *d_kind, const uint32_t *d_station, uint32_t m,
                                    const double *d_stations, int32_t device, double *d_values, void *stream);
+/* ---- state covariance (K10): a fitted element set's covariance carried to any time, in TEME or RTN ----------------------
+ * Satellite s has element columns elements[8][n], a covariance covariance[n][28] (the upper triangle, row by row, of a
+ * 7 x 7 matrix P in the element fit's variables: the layout astroz_cuda_fit_observations returns; any positive
+ * semi-definite P, not only a fit's) and model[s] (NULL: all 0), the variables P is stated in: 0 the near-earth set
+ * (n, e cos w, e sin w, i, RAAN, M + w, B*), 1 the deep-space equinoctial set -- the fit's model output.  Query i of
+ * satellite s ([offsets[s], offsets[s + 1]), offsets[0] = 0, offsets[n] = m) is at jd[i] + fr[i]:
+ *   nominal:   the TEME state f(x) of the fit's model (SGP4 for model 0, SDP4 with the K2a lattice for model 1) at
+ *              tsince = ((jd + fr) - epoch) * 1440, x the variables of the element columns;
+ *   Jacobian:  J = df/dx (6 x 7) by the fit's forward differences: a step of 1e-8 in each variable (the backward step
+ *              when the forward set cannot be built), divided by the step actually taken;
+ *   B* held:   when P's B* row is all zero the B* set is not built or propagated and J's B* column is zero;
+ *   frame:     ASTROZ_COV_FRAME_TEME, or ASTROZ_COV_FRAME_RTN of the nominal state: R = r / |r|, N = r x v / |r x v|,
+ *              T = N x R.  The one rotation is applied to the position and the velocity blocks: there is no omega x r
+ *              term, so the RTN velocity block is the TEME velocity covariance rotated, not that of a rotating frame;
+ *   outputs:   state_covariance[m][21] the upper triangle, row by row, of Sigma = J P J^T [km^2, km^2/s, km^2/s^2];
+ *              state[m][6] (nullable) the nominal TEME state [km, km/s]; jacobian[m][6][7] (nullable) J in the output
+ *              frame; status[m] (ASTROZ_COV_*): INIT_FAILED when a set cannot be built under the row's model (model 0
+ *              on a deep-space set, model 1 on a near-earth set, a stepped set that fails in both directions),
+ *              CELL_FAILED when a deep-space cell of the nominal or a stepped set fails (decay, eccentricity).  A
+ *              failed query is zero in every output; a zero P is not an error (zero Sigma, the state filled).
+ *   deep space, B* free: SDP4's drag barely moves a deep-space orbit, so its B* column is rounding noise and a fit's
+ *              B* variance is huge; Sigma is then dominated by their product.  Zero the B* row of P for such rows, or
+ *              supply a B* variance of your own;
+ * A query's bytes depend on its satellite's inputs and its own time alone: no sum runs across queries.
+ * ASTROZ_VALUE_ERROR, nothing written: device = -1, an unknown grav or frame; and for the host call offsets that
+ * decrease, offsets[0] != 0 or offsets[n] != m, a non-finite element, time or covariance word, a model byte > 1. */
+#define ASTROZ_COV_OK          0
+#define ASTROZ_COV_INIT_FAILED 1
+#define ASTROZ_COV_CELL_FAILED 2
+#define ASTROZ_COV_FRAME_TEME  0
+#define ASTROZ_COV_FRAME_RTN   1
+#define ASTROZ_STATE_COVARIANCE_WORDS 21
+/* HOST buffers: one upload (pageable through a pinned ring, pinned by direct DMA), one launch per model, plain copies
+ * back. */
+int32_t astroz_cuda_propagate_covariance(const double *elements, uint32_t n, int32_t grav, const double *covariance,
+                                         const uint8_t *model, const uint32_t *offsets, const double *jd,
+                                         const double *fr, uint32_t m, int32_t frame, int32_t device, double *state,
+                                         double *state_covariance, double *jacobian, uint8_t *status);
+/* DEVICE pointers on `device`: two launches on `stream` (near-earth rows, then deep-space rows; one when d_model is
+ * NULL), no allocation, no synchronisation; only the scalar arguments are checked. */
+int32_t astroz_cuda_propagate_covariance_device(const double *d_elements, uint32_t n, int32_t grav,
+                                                const double *d_covariance, const uint8_t *d_model,
+                                                const uint32_t *d_offsets, const double *d_jd, const double *d_fr,
+                                                uint32_t m, int32_t frame, int32_t device, double *d_state,
+                                                double *d_state_covariance, double *d_jacobian, uint8_t *d_status,
+                                                void *stream);
 /* One TLE line pair read by the library's own parser (src/Tle.zig:49-101) into the eight element columns above, the
  * numbers astroz_cuda_constellation_create would use.  ASTROZ_BAD_TLE_LENGTH when the pair cannot be read. */
 int32_t astroz_cuda_parse_tle(const char *line1, const char *line2, double *elements);
