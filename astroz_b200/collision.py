@@ -1,0 +1,140 @@
+"""Assess candidate conjunctions on the device: time of closest approach, miss, relative state and the 2-D probability of
+collision from both objects' fitted covariances (K11, astroz_b200/csrc/az_conjunction.cu).
+
+    from astroz_b200.collision import conjunctions
+    fit = fit_observations(...)                                   # FitResult with covariance and deep_space
+    res = conjunctions(fit, primary, secondary, jd, fr, window_min=2.0, hbr_km=0.02)
+    res.tca_jd, res.tca_fr, res.miss_km, res.pc, res.c2, res.status
+
+Candidates are inputs: pairs of catalogue rows with a guess time and a half window, from any screen, a conjunction
+message or the caller's own logic; this module does not search for encounters.  For each candidate the TCA is the local
+minimum of the range inside the window, each object's state covariance comes from K10 (astroz_b200.covariance) at the
+TCA, and Pc is the short-encounter 2-D integral over the combined hard-body disk in the encounter plane, with the two
+objects' errors taken as uncorrelated.  For slow encounters (GEO pairs) the short-encounter assumption fails and Pc is
+not the collision probability.
+"""
+from __future__ import annotations
+
+import ctypes as C
+from dataclasses import dataclass
+
+import numpy as np
+
+from ._abi import DEFINES as D
+from ._lib import WGS72, check, lib
+from .covariance import RTN, TEME, _covariance_words  # noqa: F401  (frames re-exported for callers)
+
+OK, INIT_FAILED, CELL_FAILED = D["ASTROZ_CONJ_OK"], D["ASTROZ_CONJ_INIT_FAILED"], D["ASTROZ_CONJ_CELL_FAILED"]
+WINDOW_EDGE, NO_PLANE, BAD_PAIR = D["ASTROZ_CONJ_WINDOW_EDGE"], D["ASTROZ_CONJ_NO_PLANE"], D["ASTROZ_CONJ_BAD_PAIR"]
+STATUS_NAMES = {OK: "ok", INIT_FAILED: "a set cannot be built under the row's model",
+                CELL_FAILED: "a deep-space cell failed (decay, eccentricity)",
+                WINDOW_EDGE: "no minimum inside the window: the nearer window end",
+                NO_PLANE: "zero relative velocity: no encounter plane", BAD_PAIR: "bad row pair"}
+_WORDS = D["ASTROZ_CONJ_RECORD_WORDS"]
+_SIG = D["ASTROZ_STATE_COVARIANCE_WORDS"]
+
+
+@dataclass
+class ConjunctionResult:
+    record: np.ndarray                   # (m, 13) the raw record words (astroz_b200.h, K11)
+    tca_jd: np.ndarray                   # (m,) the TCA as jd + fr: jd as given ...
+    tca_fr: np.ndarray                   # (m,) ... and fr + dt_tca / 1440
+    states: np.ndarray | None            # (m, 2, 6) TEME states of primary and secondary at the TCA, or None
+    state_covariance: np.ndarray | None  # (m, 2, 21) each object's Sigma words at the TCA, or None
+    status: np.ndarray                   # (m,) uint8 ASTROZ_CONJ_*
+
+    dt_tca_min = property(lambda self: self.record[:, 0])
+    miss_km = property(lambda self: self.record[:, 1])
+    rel_speed_km_s = property(lambda self: self.record[:, 2])
+    rel_position_rtn = property(lambda self: self.record[:, 3:6])   # secondary - primary, primary's RTN [km]
+    rel_velocity_rtn = property(lambda self: self.record[:, 6:9])   # [km/s]
+    pc = property(lambda self: self.record[:, 12])
+
+    @property
+    def c2(self) -> np.ndarray:
+        """(m, 2, 2) combined position covariance in the encounter plane [km^2]"""
+        xx, xy, yy = self.record[:, 9], self.record[:, 10], self.record[:, 11]
+        return np.stack([np.stack([xx, xy], -1), np.stack([xy, yy], -1)], -2)
+
+
+def conjunctions(source, primary, secondary, jd, fr, *, window_min, hbr_km, covariance=None, model=None,
+                 frame: int = TEME, states: bool = False, grav: int = WGS72, device: int = 0) -> ConjunctionResult:
+    """Assess m candidate conjunctions (astroz_cuda_conjunction).
+
+    source: a FitResult (elements, covariance and deep_space are taken from it; covariance= or model= override them)
+    or an (8, n) array of element columns with covariance= (n, 28) words or (n, 7, 7) matrices in the fit's variables
+    and model= (n,) 0 / 1 or bool.  Candidate i: rows primary[i] != secondary[i] around jd[i] + fr[i], half window
+    window_min [min] and combined hard-body radius hbr_km [km] (jd, fr, window_min and hbr_km broadcast to primary).
+    frame chooses TEME or each object's own RTN for state_covariance; states=True also returns both TEME states."""
+    if hasattr(source, "elements") and hasattr(source, "deep_space"):
+        el = np.ascontiguousarray(source.elements, dtype=np.float64)
+        covariance = source.covariance if covariance is None else covariance
+        model = source.deep_space if model is None else model
+        if covariance is None:
+            raise ValueError("this FitResult has no covariance (fit_observations returns one)")
+    else:
+        el = np.ascontiguousarray(source, dtype=np.float64)
+        if el.ndim != 2 or el.shape[0] != 8:
+            raise ValueError("source must be a FitResult or an (8, n) array of element columns")
+        if covariance is None:
+            raise ValueError("covariance= is required with an element array")
+    n = el.shape[1]
+    cov = _covariance_words(covariance, n)
+    md = None
+    if model is not None:
+        mm = np.asarray(model).reshape(-1)
+        if len(mm) != n or (mm.size and (mm.min() < 0 or mm.max() > 1)):
+            raise ValueError("model must hold n values, 0 (near-earth) or 1 (deep space)")
+        md = np.ascontiguousarray(mm.astype(np.uint8))
+    rows = []
+    for name, a in (("primary", primary), ("secondary", secondary)):
+        a = np.asarray(a).reshape(-1)
+        if a.size and (not np.issubdtype(a.dtype, np.integer) or a.min() < 0 or a.max() >= n):
+            raise ValueError(f"{name} must hold row indices in [0, n)")
+        rows.append(np.ascontiguousarray(a.astype(np.uint32)))
+    pr, se = rows
+    if len(pr) != len(se):
+        raise ValueError("primary and secondary must have the same length")
+    m = len(pr)
+    f64 = lambda a: np.ascontiguousarray(np.broadcast_to(np.asarray(a, dtype=np.float64), (m,)))  # noqa: E731
+    jd_, fr_, w_, r_ = f64(jd), f64(fr), f64(window_min), f64(hbr_km)
+    rec, stat = np.zeros((m, _WORDS)), np.zeros(m, dtype=np.uint8)
+    st = np.zeros((m, 2, 6)) if states else None
+    sig = np.zeros((m, 2, _SIG))
+    vp = lambda a: None if a is None or a.size == 0 else C.c_void_p(a.ctypes.data)  # noqa: E731
+    check(lib().astroz_cuda_conjunction(vp(el), n, int(grav), vp(cov), vp(md), vp(pr), vp(se), vp(jd_), vp(fr_),
+                                        vp(w_), vp(r_), m, int(frame), int(device), vp(rec), vp(st), vp(sig),
+                                        vp(stat)))
+    return ConjunctionResult(rec, jd_.copy(), fr_ + rec[:, 0] / 1440.0, st, sig, stat)
+
+
+def conjunctions_device(elements, covariance, model, primary, secondary, jd, fr, window_min, hbr_km, record, states,
+                        state_covariance, status, *, frame: int = TEME, grav: int = WGS72, stream: int = 0) -> None:
+    """`conjunctions` with torch CUDA tensors on one device: elements (8, n) float64, covariance (n, 28) float64, model
+    (n,) uint8 or None, primary / secondary (m,) int32, jd / fr / window_min / hbr_km (m,) float64; record (m, 13)
+    float64, states (m, 2, 6) float64 or None, state_covariance (m, 2, 21) float64 or None and status (m,) uint8
+    receive the results.  Two launches on `stream` (a raw cudaStream_t value, 0 = the default stream).  Rows are not
+    checked here: a bad pair gets status BAD_PAIR."""
+    import torch
+
+    n = int(elements.shape[1]) if elements.dim() == 2 and elements.shape[0] == 8 else -1
+    if n < 0 or elements.dtype != torch.float64 or not elements.is_cuda:
+        raise ValueError("elements must be a CUDA float64 tensor of shape (8, n)")
+    m = int(primary.numel())
+    tensors = [("elements", elements, 8 * n, torch.float64), ("covariance", covariance, 28 * n, torch.float64),
+               ("model", model, n, torch.uint8), ("primary", primary, m, torch.int32),
+               ("secondary", secondary, m, torch.int32), ("jd", jd, m, torch.float64), ("fr", fr, m, torch.float64),
+               ("window_min", window_min, m, torch.float64), ("hbr_km", hbr_km, m, torch.float64),
+               ("record", record, _WORDS * m, torch.float64), ("states", states, 12 * m, torch.float64),
+               ("state_covariance", state_covariance, 2 * _SIG * m, torch.float64), ("status", status, m, torch.uint8)]
+    for name, t, size, dtype in tensors:
+        if t is None and name in ("model", "states", "state_covariance"):
+            continue
+        if not isinstance(t, torch.Tensor) or t.dtype != dtype or not t.is_contiguous() or int(t.numel()) != size \
+                or t.device != elements.device:
+            raise ValueError(f"{name} must be a contiguous {dtype} tensor of {size} elements on {elements.device}")
+    ptr = lambda t: None if t is None else C.c_void_p(t.data_ptr())  # noqa: E731
+    check(lib().astroz_cuda_conjunction_device(
+        ptr(elements), n, int(grav), ptr(covariance), ptr(model), ptr(primary), ptr(secondary), ptr(jd), ptr(fr),
+        ptr(window_min), ptr(hbr_km), m, int(frame), int(elements.device.index), ptr(record), ptr(states),
+        ptr(state_covariance), ptr(status), C.c_void_p(stream) if stream else None))

@@ -26,6 +26,7 @@
 #include <vector>
 
 #include "az_covariance.cuh"
+#include "az_conjunction.cuh"
 #include "az_fit.cuh"
 #include "az_hostcopy.cuh"
 #include "az_ingest.cuh"
@@ -3082,6 +3083,136 @@ int32_t astroz_cuda_propagate_covariance(const double *elements, uint32_t n, int
     AZ_CUDA(cudaMemcpyAsync(state_covariance, a.sigma, (size_t)8 * az::kCovWords * m, cudaMemcpyDeviceToHost, st));
     if (jacobian)
         AZ_CUDA(cudaMemcpyAsync(jacobian, a.jacobian, (size_t)8 * az::kCovJacWords * m, cudaMemcpyDeviceToHost, st));
+    AZ_CUDA(cudaMemcpyAsync(status, a.status, m, cudaMemcpyDeviceToHost, st));
+    AZ_CUDA(d.buf.release());
+    AZ_CUDA(cudaStreamSynchronize(st));
+    return ASTROZ_OK;
+}
+
+// ---- conjunction assessment (K11, az_conjunction.cu, az_conjunction.cuh) -------------------------------------------
+static_assert(ASTROZ_CONJ_OK == az::kConjOk && ASTROZ_CONJ_INIT_FAILED == az::kConjInitFailed &&
+                  ASTROZ_CONJ_CELL_FAILED == az::kConjCellFailed && ASTROZ_CONJ_WINDOW_EDGE == az::kConjWindowEdge &&
+                  ASTROZ_CONJ_NO_PLANE == az::kConjNoPlane && ASTROZ_CONJ_BAD_PAIR == az::kConjBadPair &&
+                  ASTROZ_CONJ_RECORD_WORDS == az::kConjRecordWords,
+              "conjunction status bytes and record layout");
+
+// Scalar checks of the conjunction calls, before anything is read, written or allocated; a receives the scalars.
+static int32_t conj_check(uint32_t n, int32_t grav, uint32_t m, int32_t frame, int32_t device, az::ConjArgs *a) {
+    if (device < 0) return value_error("conjunction assessment runs on one device: pass its ordinal");
+    if (grav != ASTROZ_WGS72 && grav != ASTROZ_WGS84) return value_error("grav must be ASTROZ_WGS72 or ASTROZ_WGS84");
+    if (frame != ASTROZ_COV_FRAME_TEME && frame != ASTROZ_COV_FRAME_RTN)
+        return value_error("frame must be ASTROZ_COV_FRAME_TEME or ASTROZ_COV_FRAME_RTN");
+    a->n = n;
+    a->m = m;
+    a->grav = grav;
+    a->g = az::grav_consts(az::gravity(grav));
+    a->frame = frame;
+    return ASTROZ_OK;
+}
+
+int32_t astroz_cuda_conjunction_device(const double *d_elements, uint32_t n, int32_t grav, const double *d_covariance,
+                                       const uint8_t *d_model, const uint32_t *d_primary, const uint32_t *d_secondary,
+                                       const double *d_jd, const double *d_fr, const double *d_window_min,
+                                       const double *d_hbr_km, uint32_t m, int32_t frame, int32_t device,
+                                       double *d_record, double *d_states, double *d_state_covariance,
+                                       uint8_t *d_status, void *stream) {
+    az::ConjArgs a{};
+    int32_t rc = conj_check(n, grav, m, frame, device, &a);
+    if (rc != ASTROZ_OK) return rc;
+    if (m == 0) return ASTROZ_OK;
+    if ((n && (!d_elements || !d_covariance)) || !d_primary || !d_secondary || !d_jd || !d_fr || !d_window_min ||
+        !d_hbr_km || !d_record || !d_status)
+        return ASTROZ_NULL_POINTER;
+    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
+    AZ_CUDA(cudaSetDevice(device));
+    a.elements = d_elements;
+    a.covariance = d_covariance;
+    a.model = d_model;
+    a.primary = d_primary;
+    a.secondary = d_secondary;
+    a.jd = d_jd;
+    a.fr = d_fr;
+    a.window = d_window_min;
+    a.hbr = d_hbr_km;
+    a.record = d_record;
+    a.states = d_states;
+    a.sigma = d_state_covariance;
+    a.status = d_status;
+    AZ_CUDA(az::launch_conjunction(a, static_cast<cudaStream_t>(stream)));
+    return ASTROZ_OK;
+}
+
+// Host buffers: as astroz_cuda_propagate_covariance -- the inputs go up once (pageable through the pinned ring, pinned
+// by direct DMA), the two launches run on the device's stream, and the results come back by plain copies.
+int32_t astroz_cuda_conjunction(const double *elements, uint32_t n, int32_t grav, const double *covariance,
+                                const uint8_t *model, const uint32_t *primary, const uint32_t *secondary,
+                                const double *jd, const double *fr, const double *window_min, const double *hbr_km,
+                                uint32_t m, int32_t frame, int32_t device, double *record, double *states,
+                                double *state_covariance, uint8_t *status) {
+    az::ConjArgs a{};
+    int32_t rc = conj_check(n, grav, m, frame, device, &a);
+    if (rc != ASTROZ_OK) return rc;
+    if (n && (!elements || !covariance)) return ASTROZ_NULL_POINTER;
+    if (m && (!primary || !secondary || !jd || !fr || !window_min || !hbr_km || !record || !status))
+        return ASTROZ_NULL_POINTER;
+    for (uint32_t i = 0; i < m; ++i) {
+        if (primary[i] >= n || secondary[i] >= n) return value_error("a candidate's row is outside the catalogue");
+        if (primary[i] == secondary[i]) return value_error("a candidate pairs a row with itself");
+        if (!(window_min[i] > 0.0) || !std::isfinite(window_min[i]))
+            return value_error("half windows must be finite and > 0 minutes");
+        if (!(hbr_km[i] >= 0.0) || !std::isfinite(hbr_km[i]))
+            return value_error("hard-body radii must be finite and >= 0 km");
+    }
+    if (!all_finite(elements, (size_t)8 * n)) return value_error("elements must be finite");
+    if (!all_finite(covariance, (size_t)az::kFitN * n)) return value_error("covariance words must be finite");
+    if (!all_finite(jd, m) || !all_finite(fr, m)) return value_error("guess times must be finite");
+    if (model)
+        for (uint32_t s = 0; s < n; ++s)
+            if (model[s] > 1) return value_error("a model byte is not 0 (near-earth) or 1 (deep space)");
+    if (m == 0) return ASTROZ_OK;
+    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
+    NumericalContext *c = nullptr;
+    if ((rc = numerical_context(device, &c)) != ASTROZ_OK) return rc;
+    std::lock_guard<std::mutex> lk(c->m);
+    AZ_CUDA(cudaSetDevice(device));
+    cudaStream_t st = c->stream;
+    // elements | covariance | model | primary | secondary | jd | fr | window | hbr | record | states | sigma | status
+    DeviceBlock d(st);
+    AZ_CUDA(d.alloc({(size_t)64 * n, (size_t)8 * az::kFitN * n, model ? (size_t)n : 0, (size_t)4 * m, (size_t)4 * m,
+                     (size_t)8 * m, (size_t)8 * m, (size_t)8 * m, (size_t)8 * m, (size_t)8 * az::kConjRecordWords * m,
+                     states ? (size_t)96 * m : 0, state_covariance ? (size_t)16 * az::kCovWords * m : 0, (size_t)m}));
+    auto up = [&](const void *src, void *dst, size_t elemBytes, size_t count) {
+        void *const dd[1] = {dst};
+        const void *const ss[1] = {src};
+        return c->pipe.ring.upload(az::is_pageable(src), 1, ss, dd, &elemBytes, count, st);
+    };
+    AZ_CUDA(up(elements, d.f64(0), 8, (size_t)8 * n));
+    AZ_CUDA(up(covariance, d.f64(1), 8 * az::kFitN, n));
+    if (model) AZ_CUDA(up(model, d.u8(2), 1, n));
+    AZ_CUDA(up(primary, d.u32(3), 4, m));
+    AZ_CUDA(up(secondary, d.u32(4), 4, m));
+    AZ_CUDA(up(jd, d.f64(5), 8, m));
+    AZ_CUDA(up(fr, d.f64(6), 8, m));
+    AZ_CUDA(up(window_min, d.f64(7), 8, m));
+    AZ_CUDA(up(hbr_km, d.f64(8), 8, m));
+    a.elements = d.f64(0);
+    a.covariance = d.f64(1);
+    a.model = model ? d.u8(2) : nullptr;
+    a.primary = d.u32(3);
+    a.secondary = d.u32(4);
+    a.jd = d.f64(5);
+    a.fr = d.f64(6);
+    a.window = d.f64(7);
+    a.hbr = d.f64(8);
+    a.record = d.f64(9);
+    a.states = states ? d.f64(10) : nullptr;
+    a.sigma = state_covariance ? d.f64(11) : nullptr;
+    a.status = d.u8(12);
+    AZ_CUDA(az::launch_conjunction(a, st));
+    AZ_CUDA(cudaMemcpyAsync(record, a.record, (size_t)8 * az::kConjRecordWords * m, cudaMemcpyDeviceToHost, st));
+    if (states) AZ_CUDA(cudaMemcpyAsync(states, a.states, (size_t)96 * m, cudaMemcpyDeviceToHost, st));
+    if (state_covariance)
+        AZ_CUDA(cudaMemcpyAsync(state_covariance, a.sigma, (size_t)16 * az::kCovWords * m, cudaMemcpyDeviceToHost, st));
     AZ_CUDA(cudaMemcpyAsync(status, a.status, m, cudaMemcpyDeviceToHost, st));
     AZ_CUDA(d.buf.release());
     AZ_CUDA(cudaStreamSynchronize(st));

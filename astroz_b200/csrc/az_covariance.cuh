@@ -73,6 +73,20 @@ AZ_HD void cov_zero(double *J, int stride, double (&f0)[6], double (&sig)[kCovWo
     for (int q = 0; q < kCovJacWords; ++q) J[q * stride] = 0.0;
 }
 
+// Rows R, T, N of the RTN frame of TEME state f: R = r / |r|, N = r x v / |r x v|, T = N x R
+AZ_HD void cov_rtn(const double (&f)[6], double (&R)[3][3]) {
+    const double rn = std::sqrt(f[0] * f[0] + f[1] * f[1] + f[2] * f[2]);
+    const double h[3] = {f[1] * f[5] - f[2] * f[4], f[2] * f[3] - f[0] * f[5], f[0] * f[4] - f[1] * f[3]};
+    const double hn = std::sqrt(h[0] * h[0] + h[1] * h[1] + h[2] * h[2]);
+    for (int c = 0; c < 3; ++c) {
+        R[0][c] = f[c] / rn;
+        R[2][c] = h[c] / hn;
+    }
+    R[1][0] = R[2][1] * R[0][2] - R[2][2] * R[0][1];
+    R[1][1] = R[2][2] * R[0][0] - R[2][0] * R[0][2];
+    R[1][2] = R[2][0] * R[0][1] - R[2][1] * R[0][0];
+}
+
 // One query whose sets are built: eval(k, jdFull, ts, f) = the TEME state f[6] of set k (false when its cell fails),
 // inv[1 + j] = 1 / step of variable j, P the 28 covariance words.  J receives the 6 x 7 Jacobian in the output frame,
 // entry (c, j) at J[(c * kFitVars + j) * stride]; f0 the nominal TEME state; sig the 21 words of Sigma.
@@ -95,17 +109,7 @@ AZ_HD uint8_t cov_query(EvalFn eval, int nvar, const double *inv, const double *
     }
     if (frame == kCovFrameRtn) {
         double R[3][3];
-        const double rn = std::sqrt(f0[0] * f0[0] + f0[1] * f0[1] + f0[2] * f0[2]);
-        const double h[3] = {f0[1] * f0[5] - f0[2] * f0[4], f0[2] * f0[3] - f0[0] * f0[5],
-                             f0[0] * f0[4] - f0[1] * f0[3]};
-        const double hn = std::sqrt(h[0] * h[0] + h[1] * h[1] + h[2] * h[2]);
-        for (int c = 0; c < 3; ++c) {
-            R[0][c] = f0[c] / rn;
-            R[2][c] = h[c] / hn;
-        }
-        R[1][0] = R[2][1] * R[0][2] - R[2][2] * R[0][1];
-        R[1][1] = R[2][2] * R[0][0] - R[2][0] * R[0][2];
-        R[1][2] = R[2][0] * R[0][1] - R[2][1] * R[0][0];
+        cov_rtn(f0, R);
 #ifdef __CUDA_ARCH__
 #pragma unroll 1
 #endif

@@ -205,6 +205,28 @@ struct CovArgs {
 // the near-earth rows' queries (model 0), then on the same stream the deep-space rows' (model 1)
 cudaError_t launch_covariance(const CovArgs &a, cudaStream_t stream);
 
+// K11: candidate conjunctions assessed at their TCA (az_conjunction.cu, az_conjunction.cuh).  Device pointers.
+struct ConjArgs {
+    const double *elements = nullptr;    // [8][n]
+    const double *covariance = nullptr;  // [n][28]: upper triangle of P in the fit's variables
+    const uint8_t *model = nullptr;      // [n], nullable (all 0)
+    uint32_t n = 0;
+    const uint32_t *primary = nullptr, *secondary = nullptr;  // [m] rows
+    const double *jd = nullptr, *fr = nullptr;                 // [m] guess times
+    const double *window = nullptr;      // [m] half window [min]
+    const double *hbr = nullptr;         // [m] combined hard-body radius [km]
+    uint32_t m = 0;
+    int frame = 0;                       // ASTROZ_COV_FRAME_* of the per-object Sigma
+    int grav = 1;
+    GravConsts g{};
+    double *record = nullptr;            // [m][13]
+    double *states = nullptr;            // [m][2][6] TEME at the TCA, nullable
+    double *sigma = nullptr;             // [m][2][21], nullable
+    uint8_t *status = nullptr;           // [m] ASTROZ_CONJ_*
+};
+// the pairs of two near-earth rows, then on the same stream every other pair
+cudaError_t launch_conjunction(const ConjArgs &a, cudaStream_t stream);
+
 // DFMA throughput microbenchmark: returns achieved fp64 FLOP/s (FMA = 2).
 cudaError_t measure_fp64_peak(double *flops);
 // Arithmetic peak of the fp64 pipe: SMs x 64 lanes x 2 FLOP x the maximum SM clock.

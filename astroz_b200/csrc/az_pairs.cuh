@@ -64,13 +64,11 @@ AZ_HD uint8_t pairs_sgp4_query(ColFn col, double jdFull, double refJd, double to
     return st;
 }
 
-// One deep-space query.  lattice = this satellite's [2][nodes] resonance checkpoints (K2a); the state is taken at the
-// node below |tsince| and stepped on from there, exactly as K2 does (so the result does not depend on the lattice's
-// extent).  A failing cell is zero-filled; returns its ASTROZ_CELL_* code.
-template <int kMode, bool kVel>
-AZ_HD uint8_t pairs_sdp4_query(const Sdp4Sat &e, const double2 *lattice, int nodes, double jdFull, const GravConsts &g,
-                               CellOut &o) {
-    const double ts = pairs_tsince_deep(jdFull, e.epochJd);
+// One deep-space cell at tsince ts [min] into o (TEME), its ASTROZ_CELL_* code returned.  lattice = this satellite's
+// [2][nodes] resonance checkpoints (K2a); the state is taken at the node below |tsince| and stepped on from there,
+// exactly as K2 does (so the result does not depend on the lattice's extent).
+AZ_HD int pairs_sdp4_at(const Sdp4Sat &e, const double2 *lattice, int nodes, double ts, const GravConsts &g,
+                        CellOut &o) {
     double xli = e.xlamo, xni = e.no, atime = 0.0;
     if (e.irez != 0) {
         const int node = resonance_node(ts);
@@ -82,7 +80,15 @@ AZ_HD uint8_t pairs_sdp4_query(const Sdp4Sat &e, const double2 *lattice, int nod
         atime = delt * (double)have;
         for (int j = have; j < node; ++j) resonance_step(e, xli, xni, atime, delt);  // beyond the lattice
     }
-    const int st = sdp4_cell(e, ts, xli, xni, atime, g, o);
+    return sdp4_cell(e, ts, xli, xni, atime, g, o);
+}
+
+// One deep-space query at its own epoch jd + fr, in the output frame of kMode.  A failing cell is zero-filled; returns
+// its ASTROZ_CELL_* code.
+template <int kMode, bool kVel>
+AZ_HD uint8_t pairs_sdp4_query(const Sdp4Sat &e, const double2 *lattice, int nodes, double jdFull, const GravConsts &g,
+                               CellOut &o) {
+    const int st = pairs_sdp4_at(e, lattice, nodes, pairs_tsince_deep(jdFull, e.epochJd), g, o);
     if (st != 0) {
         o.rx = o.ry = o.rz = o.vx = o.vy = o.vz = 0.0;
     } else {

@@ -731,6 +731,58 @@ int32_t astroz_cuda_propagate_covariance_device(const double *d_elements, uint32
                                                 uint32_t m, int32_t frame, int32_t device, double *d_state,
                                                 double *d_state_covariance, double *d_jacobian, uint8_t *d_status,
                                                 void *stream);
+/* ---- conjunction assessment (K11): TCA, miss and 2-D Pc of candidate conjunctions from fitted covariances ------------
+ * Candidates come from any screen, a conjunction message or the caller's own logic; nothing here finds them.  The
+ * catalogue is K10's: elements[8][n], covariance[n][28] in the fit's variables and model[n] (NULL: all 0).  Candidate i
+ * pairs rows primary[i] != secondary[i] around the guess time jd[i] + fr[i], with a half window window_min[i] > 0
+ * [min] and a combined hard-body radius hbr_km[i] >= 0 [km]:
+ *   states:    each row's nominal TEME state under its own model at dt minutes from the guess, tsince = ((jd + fr) -
+ *              epoch) * 1440 + dt (K10's nominal at dt = 0); dr = r_s - r_p, dv = v_s - v_p;
+ *   TCA:       a root of g = dr . dv where g goes from - to + in [-w, w], found by 32-point sampling rounds that cut the
+ *              bracket 31x each until it is 1e-9 min wide, then one secant step.  Several roots in the first round's
+ *              32 samples: the one of least |dr|.  No root: the window end with the smaller |dr|, status WINDOW_EDGE;
+ *   Sigma:     each row's 6 x 6 state covariance at the TCA by K10's definition (forward-difference J, B* held when P's
+ *              B* row is zero, a zero P gives a zero Sigma), in TEME or in that row's own RTN frame (frame);
+ *   plane:     z = dv / |dv|, x = dr's part perpendicular to z, normalised (an exact hit takes x from the TEME axis
+ *              least aligned with z), y = z x x.  C2 = the (x, y) block of Sigma_p + Sigma_s: the two objects'
+ *              errors are assumed UNCORRELATED;
+ *   Pc:        the short-encounter 2-D probability: the integral of N((u, v); (d, 0), C2) over the disk u^2 + v^2 <=
+ *              R^2, d = |dr perpendicular to z|.  It assumes a straight-line relative motion over the encounter with
+ *              constant covariance; for slow encounters (GEO pairs, co-orbiting objects) that assumption fails and
+ *              Pc is not the collision probability.  Computed in C2's principal axes as a 1-D Gauss-Legendre
+ *              integral of normal-CDF differences, with exact limits for a singular C2;
+ *   outputs:   record[m][13]: dt_tca [min from jd + fr], miss [km], relative speed [km/s], dr and dv in the primary's
+ *              RTN frame (6 words, no omega x r term), C2 (xx, xy, yy) [km^2], Pc; states[m][2][6] (nullable) the two
+ *              TEME states at the TCA; state_covariance[m][2][21] (nullable) each row's Sigma words, as K10's;
+ *              status[m] (ASTROZ_CONJ_*).  INIT_FAILED and CELL_FAILED mean what K10's do (and INIT_FAILED a model
+ *              byte > 1 on the device call); every output is zero then and for BAD_PAIR (device call only: a row
+ *              outside the catalogue, or primary == secondary).  WINDOW_EDGE and NO_PLANE (|dv| = 0: C2 and Pc zero)
+ *              fill the other outputs.
+ * A candidate's bytes depend on its own inputs and its two rows alone: no sum runs across candidates.
+ * ASTROZ_VALUE_ERROR, nothing written: device = -1, an unknown grav or frame; and for the host call a row outside the
+ * catalogue, primary == secondary, a half window <= 0, a radius < 0, a model byte > 1 or any non-finite input. */
+#define ASTROZ_CONJ_OK           0
+#define ASTROZ_CONJ_INIT_FAILED  1
+#define ASTROZ_CONJ_CELL_FAILED  2
+#define ASTROZ_CONJ_WINDOW_EDGE  3
+#define ASTROZ_CONJ_NO_PLANE     4
+#define ASTROZ_CONJ_BAD_PAIR     5
+#define ASTROZ_CONJ_RECORD_WORDS 13
+/* HOST buffers: one upload (pageable through a pinned ring, pinned by direct DMA), one launch per pair class, plain
+ * copies back. */
+int32_t astroz_cuda_conjunction(const double *elements, uint32_t n, int32_t grav, const double *covariance,
+                                const uint8_t *model, const uint32_t *primary, const uint32_t *secondary,
+                                const double *jd, const double *fr, const double *window_min, const double *hbr_km,
+                                uint32_t m, int32_t frame, int32_t device, double *record, double *states,
+                                double *state_covariance, uint8_t *status);
+/* DEVICE pointers on `device`: two launches on `stream` (pairs of near-earth rows, then every other pair), no
+ * allocation, no synchronisation; only the scalar arguments are checked. */
+int32_t astroz_cuda_conjunction_device(const double *d_elements, uint32_t n, int32_t grav, const double *d_covariance,
+                                       const uint8_t *d_model, const uint32_t *d_primary, const uint32_t *d_secondary,
+                                       const double *d_jd, const double *d_fr, const double *d_window_min,
+                                       const double *d_hbr_km, uint32_t m, int32_t frame, int32_t device,
+                                       double *d_record, double *d_states, double *d_state_covariance,
+                                       uint8_t *d_status, void *stream);
 /* One TLE line pair read by the library's own parser (src/Tle.zig:49-101) into the eight element columns above, the
  * numbers astroz_cuda_constellation_create would use.  ASTROZ_BAD_TLE_LENGTH when the pair cannot be read. */
 int32_t astroz_cuda_parse_tle(const char *line1, const char *line2, double *elements);

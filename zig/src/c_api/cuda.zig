@@ -97,6 +97,8 @@ pub extern fn astroz_cuda_observe(states: ?[*]const f64, jd: ?[*]const f64, fr: 
 pub extern fn astroz_cuda_observe_device(d_states: ?[*]const f64, d_jd: ?[*]const f64, d_fr: ?[*]const f64, d_kind: ?[*]const u8, d_station: ?[*]const u32, m: u32, d_stations: ?[*]const f64, device: i32, d_values: ?[*]f64, stream: ?*anyopaque) i32;
 pub extern fn astroz_cuda_propagate_covariance(elements: ?[*]const f64, n: u32, grav: i32, covariance: ?[*]const f64, model: ?[*]const u8, offsets: ?[*]const u32, jd: ?[*]const f64, fr: ?[*]const f64, m: u32, frame: i32, device: i32, state: ?[*]f64, state_covariance: ?[*]f64, jacobian: ?[*]f64, status: ?[*]u8) i32;
 pub extern fn astroz_cuda_propagate_covariance_device(d_elements: ?[*]const f64, n: u32, grav: i32, d_covariance: ?[*]const f64, d_model: ?[*]const u8, d_offsets: ?[*]const u32, d_jd: ?[*]const f64, d_fr: ?[*]const f64, m: u32, frame: i32, device: i32, d_state: ?[*]f64, d_state_covariance: ?[*]f64, d_jacobian: ?[*]f64, d_status: ?[*]u8, stream: ?*anyopaque) i32;
+pub extern fn astroz_cuda_conjunction(elements: ?[*]const f64, n: u32, grav: i32, covariance: ?[*]const f64, model: ?[*]const u8, primary: ?[*]const u32, secondary: ?[*]const u32, jd: ?[*]const f64, fr: ?[*]const f64, window_min: ?[*]const f64, hbr_km: ?[*]const f64, m: u32, frame: i32, device: i32, record: ?[*]f64, states: ?[*]f64, state_covariance: ?[*]f64, status: ?[*]u8) i32;
+pub extern fn astroz_cuda_conjunction_device(d_elements: ?[*]const f64, n: u32, grav: i32, d_covariance: ?[*]const f64, d_model: ?[*]const u8, d_primary: ?[*]const u32, d_secondary: ?[*]const u32, d_jd: ?[*]const f64, d_fr: ?[*]const f64, d_window_min: ?[*]const f64, d_hbr_km: ?[*]const f64, m: u32, frame: i32, device: i32, d_record: ?[*]f64, d_states: ?[*]f64, d_state_covariance: ?[*]f64, d_status: ?[*]u8, stream: ?*anyopaque) i32;
 pub extern fn astroz_cuda_parse_tle(line1: [*:0]const u8, line2: [*:0]const u8, elements: ?[*]f64) i32;
 pub extern fn astroz_cuda_lambert(r1: ?[*]const f64, r2: ?[*]const f64, tof: ?[*]const f64, normal: ?[*]const f64, n: u32, mu: f64, max_revs: u32, device: i32, v1: ?[*]f64, v2: ?[*]f64, status: ?[*]u8, iterations: ?[*]u8) i32;
 pub extern fn astroz_cuda_lambert_device(d_r1: ?[*]const f64, d_r2: ?[*]const f64, d_tof: ?[*]const f64, d_normal: ?[*]const f64, n: u32, mu: f64, max_revs: u32, device: i32, d_v1: ?[*]f64, d_v2: ?[*]f64, d_status: ?[*]u8, d_iterations: ?[*]u8, stream: ?*anyopaque) i32;
