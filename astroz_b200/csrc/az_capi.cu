@@ -27,6 +27,7 @@
 
 #include "az_covariance.cuh"
 #include "az_conjunction.cuh"
+#include "az_correlate.cuh"
 #include "az_fit.cuh"
 #include "az_hostcopy.cuh"
 #include "az_ingest.cuh"
@@ -3214,6 +3215,186 @@ int32_t astroz_cuda_conjunction(const double *elements, uint32_t n, int32_t grav
     if (state_covariance)
         AZ_CUDA(cudaMemcpyAsync(state_covariance, a.sigma, (size_t)16 * az::kCovWords * m, cudaMemcpyDeviceToHost, st));
     AZ_CUDA(cudaMemcpyAsync(status, a.status, m, cudaMemcpyDeviceToHost, st));
+    AZ_CUDA(d.buf.release());
+    AZ_CUDA(cudaStreamSynchronize(st));
+    return ASTROZ_OK;
+}
+
+// ---- track correlation (K12, az_correlate.cu, az_correlate.cuh) -------------------------------------------------------
+static_assert(ASTROZ_CORR_OK == az::kCorrOk && ASTROZ_CORR_UNCORRELATED == az::kCorrUncorrelated &&
+                  ASTROZ_CORR_NO_ROW == az::kCorrNoRow && ASTROZ_CORR_BAD_TRACK == az::kCorrBadTrack &&
+                  ASTROZ_CORR_MAX_TRACK == az::kCorrMaxTrack && ASTROZ_CORR_MAX_BEST == az::kCorrMaxBest,
+              "correlation status bytes and limits");
+
+// Scalar checks of the correlation calls, before anything is read, written or allocated; a receives the scalars.
+static int32_t corr_check(uint32_t n, int32_t grav, uint32_t t, double gate_probability, uint32_t best,
+                          int32_t device, az::CorrArgs *a) {
+    if (device < 0) return value_error("track correlation runs on one device: pass its ordinal");
+    if (grav != ASTROZ_WGS72 && grav != ASTROZ_WGS84) return value_error("grav must be ASTROZ_WGS72 or ASTROZ_WGS84");
+    if (best < 1 || best > (uint32_t)az::kCorrMaxBest) return value_error("best must be in [1, ASTROZ_CORR_MAX_BEST]");
+    if (!(gate_probability > 0.0 && gate_probability < 1.0)) return value_error("gate_probability must be in (0, 1)");
+    a->n = n;
+    a->t = t;
+    a->grav = grav;
+    a->g = az::grav_consts(az::gravity(grav));
+    a->gateProbability = gate_probability;
+    a->best = best;
+    return ASTROZ_OK;
+}
+
+int32_t astroz_cuda_correlate_scratch_bytes(uint32_t n, uint32_t t, uint32_t best, uint64_t *bytes) {
+    if (!bytes) return ASTROZ_NULL_POINTER;
+    if (best < 1 || best > (uint32_t)az::kCorrMaxBest) return value_error("best must be in [1, ASTROZ_CORR_MAX_BEST]");
+    *bytes = az::corr_scratch_bytes(n, t, best);
+    return ASTROZ_OK;
+}
+
+int32_t astroz_cuda_chi2_quantile(uint32_t k, double p, double *x) {
+    if (!x) return ASTROZ_NULL_POINTER;
+    if (k == 0 || !(p > 0.0 && p < 1.0)) return value_error("the chi-square quantile needs k >= 1 and p in (0, 1)");
+    *x = az::corr_chi2_quantile(k, p);
+    return ASTROZ_OK;
+}
+
+static void corr_device_args(az::CorrArgs &a, const double *d_elements, const double *d_covariance,
+                             const uint8_t *d_model, const uint32_t *d_offsets, const double *d_jd, const double *d_fr,
+                             const uint8_t *d_kind, const double *d_value, const double *d_sigma,
+                             const uint32_t *d_station, const double *d_stations) {
+    a.elements = d_elements;
+    a.covariance = d_covariance;
+    a.model = d_model;
+    a.offsets = d_offsets;
+    a.jd = d_jd;
+    a.fr = d_fr;
+    a.kind = d_kind;
+    a.value = d_value;
+    a.sigma = d_sigma;
+    a.station = d_station;
+    a.stations = d_stations;
+}
+
+int32_t astroz_cuda_correlate_device(const double *d_elements, uint32_t n, int32_t grav, const double *d_covariance,
+                                     const uint8_t *d_model, const uint32_t *d_offsets, uint32_t t, const double *d_jd,
+                                     const double *d_fr, const uint8_t *d_kind, const double *d_value,
+                                     const double *d_sigma, const uint32_t *d_station, const double *d_stations,
+                                     double gate_probability, uint32_t best, int32_t device, void *d_scratch,
+                                     uint32_t *d_rows, double *d_d2, uint32_t *d_used, uint32_t *d_n_gate,
+                                     uint32_t *d_n_failed, uint8_t *d_status, uint8_t *d_row_status, void *stream) {
+    az::CorrArgs a{};
+    int32_t rc = corr_check(n, grav, t, gate_probability, best, device, &a);
+    if (rc != ASTROZ_OK) return rc;
+    if (n == 0 && t == 0) return ASTROZ_OK;
+    if ((n && (!d_elements || !d_row_status)) || !d_offsets || !d_scratch)
+        return ASTROZ_NULL_POINTER;
+    if (t && (!d_jd || !d_fr || !d_kind || !d_value || !d_sigma || !d_rows || !d_d2 || !d_used || !d_n_gate ||
+              !d_n_failed || !d_status))
+        return ASTROZ_NULL_POINTER;
+    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
+    AZ_CUDA(cudaSetDevice(device));
+    corr_device_args(a, d_elements, d_covariance, d_model, d_offsets, d_jd, d_fr, d_kind, d_value, d_sigma, d_station,
+                     d_stations);
+    a.scratch = d_scratch;
+    a.rows = d_rows;
+    a.d2 = d_d2;
+    a.used = d_used;
+    a.nGate = d_n_gate;
+    a.nFailed = d_n_failed;
+    a.status = d_status;
+    a.rowStatus = d_row_status;
+    AZ_CUDA(az::launch_correlate(a, static_cast<cudaStream_t>(stream)));
+    return ASTROZ_OK;
+}
+
+// Host buffers: as astroz_cuda_conjunction -- the inputs go up once (pageable through the pinned ring, pinned by direct
+// DMA), the launches run on the device's stream with the scratch in the same device block, and the results come back
+// by plain copies.
+int32_t astroz_cuda_correlate(const double *elements, uint32_t n, int32_t grav, const double *covariance,
+                              const uint8_t *model, const uint32_t *offsets, uint32_t t, const double *jd,
+                              const double *fr, const uint8_t *kind, const double *value, const double *sigma,
+                              const uint32_t *station, uint32_t m, const double *stations, uint32_t k,
+                              double gate_probability, uint32_t best, int32_t device, uint32_t *rows, double *d2,
+                              uint32_t *used, uint32_t *n_gate, uint32_t *n_failed, uint8_t *status,
+                              uint8_t *row_status) {
+    az::CorrArgs a{};
+    int32_t rc = corr_check(n, grav, t, gate_probability, best, device, &a);
+    if (rc != ASTROZ_OK) return rc;
+    if (!offsets) return ASTROZ_NULL_POINTER;
+    if (n && (!elements || !row_status)) return ASTROZ_NULL_POINTER;
+    if (t && (!rows || !d2 || !used || !n_gate || !n_failed || !status)) return ASTROZ_NULL_POINTER;
+    if (m && (!jd || !fr || !kind || !value || !sigma)) return ASTROZ_NULL_POINTER;
+    if (offsets[0] != 0) return value_error("offsets[0] must be 0");
+    for (uint32_t j = 0; j < t; ++j) {
+        if (offsets[j + 1] < offsets[j]) return value_error("offsets must be non-decreasing");
+        if (offsets[j + 1] == offsets[j]) return value_error("a track has no observation");
+        if (offsets[j + 1] - offsets[j] > az::kCorrMaxTrack)
+            return value_error("a track is longer than ASTROZ_CORR_MAX_TRACK observations");
+    }
+    if (offsets[t] != m) return value_error("offsets[t] must equal the observation count m");
+    if ((rc = obs_values_check(jd, fr, value, sigma, station, kind, m, stations, k)) != ASTROZ_OK) return rc;
+    {
+        const az::CorrObsArrays in{jd, fr, kind, value, sigma, station, stations};
+        for (uint32_t j = 0; j < t; ++j)
+            if (az::corr_used(in, offsets[j], offsets[j + 1]) == 0) return value_error("a track has no used residual");
+    }
+    if (!all_finite(elements, (size_t)8 * n)) return value_error("elements must be finite");
+    if (covariance && !all_finite(covariance, (size_t)az::kFitN * n))
+        return value_error("covariance words must be finite");
+    if (model)
+        for (uint32_t s = 0; s < n; ++s)
+            if (model[s] > 1) return value_error("a model byte is not 0 (near-earth) or 1 (deep space)");
+    if (n == 0 && t == 0) return ASTROZ_OK;
+    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
+    NumericalContext *c = nullptr;
+    if ((rc = numerical_context(device, &c)) != ASTROZ_OK) return rc;
+    std::lock_guard<std::mutex> lk(c->m);
+    AZ_CUDA(cudaSetDevice(device));
+    cudaStream_t st = c->stream;
+    // elements | covariance | model | offsets | jd | fr | kind | value | sigma | station | stations | scratch | rows |
+    // d2 | used | n_gate | n_failed | status | row_status
+    DeviceBlock d(st);
+    AZ_CUDA(d.alloc({(size_t)64 * n, covariance ? (size_t)8 * az::kFitN * n : 0, model ? (size_t)n : 0,
+                     (size_t)4 * (t + 1), (size_t)8 * m, (size_t)8 * m, (size_t)m, (size_t)48 * m, (size_t)48 * m,
+                     station ? (size_t)4 * m : 0, (size_t)24 * k, az::corr_scratch_bytes(n, t, best),
+                     (size_t)4 * best * t, (size_t)8 * best * t, (size_t)4 * t, (size_t)4 * t, (size_t)4 * t,
+                     (size_t)t, (size_t)n}));
+    auto up = [&](const void *src, void *dst, size_t elemBytes, size_t count) {
+        void *const dd[1] = {dst};
+        const void *const ss[1] = {src};
+        return c->pipe.ring.upload(az::is_pageable(src), 1, ss, dd, &elemBytes, count, st);
+    };
+    if (n) AZ_CUDA(up(elements, d.f64(0), 8, (size_t)8 * n));
+    if (n && covariance) AZ_CUDA(up(covariance, d.f64(1), 8 * az::kFitN, n));
+    if (n && model) AZ_CUDA(up(model, d.u8(2), 1, n));
+    AZ_CUDA(up(offsets, d.u32(3), 4, (size_t)t + 1));
+    if (m) {
+        AZ_CUDA(up(jd, d.f64(4), 8, m));
+        AZ_CUDA(up(fr, d.f64(5), 8, m));
+        AZ_CUDA(up(kind, d.u8(6), 1, m));
+        AZ_CUDA(up(value, d.f64(7), 48, m));
+        AZ_CUDA(up(sigma, d.f64(8), 48, m));
+        if (station) AZ_CUDA(up(station, d.u32(9), 4, m));
+    }
+    if (k) AZ_CUDA(up(stations, d.f64(10), 24, k));
+    corr_device_args(a, d.f64(0), covariance ? d.f64(1) : nullptr, model ? d.u8(2) : nullptr, d.u32(3), d.f64(4),
+                     d.f64(5), d.u8(6), d.f64(7), d.f64(8), station ? d.u32(9) : nullptr, k ? d.f64(10) : nullptr);
+    a.scratch = d.piece(11);
+    a.rows = d.u32(12);
+    a.d2 = d.f64(13);
+    a.used = d.u32(14);
+    a.nGate = d.u32(15);
+    a.nFailed = d.u32(16);
+    a.status = d.u8(17);
+    a.rowStatus = d.u8(18);
+    AZ_CUDA(az::launch_correlate(a, st));
+    if (t) {
+        AZ_CUDA(cudaMemcpyAsync(rows, a.rows, (size_t)4 * best * t, cudaMemcpyDeviceToHost, st));
+        AZ_CUDA(cudaMemcpyAsync(d2, a.d2, (size_t)8 * best * t, cudaMemcpyDeviceToHost, st));
+        AZ_CUDA(cudaMemcpyAsync(used, a.used, (size_t)4 * t, cudaMemcpyDeviceToHost, st));
+        AZ_CUDA(cudaMemcpyAsync(n_gate, a.nGate, (size_t)4 * t, cudaMemcpyDeviceToHost, st));
+        AZ_CUDA(cudaMemcpyAsync(n_failed, a.nFailed, (size_t)4 * t, cudaMemcpyDeviceToHost, st));
+        AZ_CUDA(cudaMemcpyAsync(status, a.status, t, cudaMemcpyDeviceToHost, st));
+    }
+    if (n) AZ_CUDA(cudaMemcpyAsync(row_status, a.rowStatus, n, cudaMemcpyDeviceToHost, st));
     AZ_CUDA(d.buf.release());
     AZ_CUDA(cudaStreamSynchronize(st));
     return ASTROZ_OK;

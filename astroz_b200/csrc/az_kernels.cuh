@@ -227,6 +227,33 @@ struct ConjArgs {
 // the pairs of two near-earth rows, then on the same stream every other pair
 cudaError_t launch_conjunction(const ConjArgs &a, cudaStream_t stream);
 
+// K12: sensor tracks correlated with catalogue rows (az_correlate.cu, az_correlate.cuh).  Device pointers.
+struct CorrArgs {
+    const double *elements = nullptr;    // [8][n]
+    const double *covariance = nullptr;  // [n][28], nullable (every P zero)
+    const uint8_t *model = nullptr;      // [n], nullable (all 0)
+    uint32_t n = 0;
+    const uint32_t *offsets = nullptr;   // [t + 1]: track j owns observations [offsets[j], offsets[j + 1])
+    uint32_t t = 0;
+    const double *jd = nullptr, *fr = nullptr;
+    const uint8_t *kind = nullptr;
+    const double *value = nullptr, *sigma = nullptr;   // [m][6]
+    const uint32_t *station = nullptr;
+    const double *stations = nullptr;
+    double gateProbability = 0.999;
+    uint32_t best = 4;
+    int grav = 1;
+    GravConsts g{};
+    void *scratch = nullptr;             // corr_scratch_bytes(n, t, best)
+    uint32_t *rows = nullptr;            // [t][best]
+    double *d2 = nullptr;                // [t][best]
+    uint32_t *used = nullptr, *nGate = nullptr, *nFailed = nullptr;   // [t]
+    uint8_t *status = nullptr;           // [t] ASTROZ_CORR_*
+    uint8_t *rowStatus = nullptr;        // [n] ASTROZ_COV_OK / ASTROZ_COV_INIT_FAILED
+};
+// the gates, the near-earth rows, the deep-space rows (when model is given) and the merge, on one stream
+cudaError_t launch_correlate(const CorrArgs &a, cudaStream_t stream);
+
 // DFMA throughput microbenchmark: returns achieved fp64 FLOP/s (FMA = 2).
 cudaError_t measure_fp64_peak(double *flops);
 // Arithmetic peak of the fp64 pipe: SMs x 64 lanes x 2 FLOP x the maximum SM clock.

@@ -139,9 +139,45 @@ AZ_HD void obs_frame(int kind, double jdFull, const double *llh, double &sg, dou
     else st = ObsStation{};
 }
 
-// fit_accumulate_model with the measurement layer: observation (kind, value[6], w[6] from obs_weights, frame) against
-// the model under set 0 and sets 1..nvar.  Components are summed in fit_accumulate_model's order, (0, 3), (1, 4),
-// (2, 5); pos2 and vel2 are formed only on the K8 path below.
+// One observation's weighted residual row and weighted Jacobian rows: observation (kind, value[6], w[6] from
+// obs_weights, frame) against the model under set 0 and sets 1..nvar (eval as fit_accumulate_model's).  r[c] =
+// (observed - model) w[c], the azimuth / right-ascension difference wrapped; J entry (j, c) at J[(j * 6 + c) * stride]
+// = the same difference between set 1 + j and set 0, times w[c] inv[1 + j].  obs receives the used observed values and
+// sc the nominal model's floor scales (obs_model).  The element fit's rows (fit_accumulate_obs) and K12's pair rows
+// (az_correlate.cuh) are these.  Returns false when a cell failed.
+template <typename EvalFn>
+AZ_HD bool obs_residual_rows(EvalFn eval, int nvar, const double *inv, double jdFull, double epochJd, int kind,
+                             const double *value, const double (&w)[6], double sg, double cg, const ObsStation &st,
+                             double (&obs)[6], double (&sc)[6], double (&r)[6], double *J, int stride) {
+    const double ts[1] = {mul_rn(sub_rn(jdFull, epochJd), 1440.0)};
+    bool ok = true;
+    const int wr = obs_wrapped(kind);
+    double f0[6], h0[6];
+    for (int c = 0; c < 6; ++c) obs[c] = w[c] != 0.0 ? value[c] : 0.0;
+    ok = eval(0, jdFull, ts, f0) && ok;
+    obs_model(kind, f0, sg, cg, st, h0, sc);
+    for (int c = 0; c < 6; ++c) {
+        const double d = c == wr ? obs_wrap(obs[c] - h0[c]) : obs[c] - h0[c];
+        r[c] = w[c] != 0.0 ? d * w[c] : 0.0;
+    }
+#ifdef __CUDA_ARCH__
+#pragma unroll 1
+#endif
+    for (int j = 0; j < nvar; ++j) {
+        double f[6], h[6], scj[6];
+        ok = eval(1 + j, jdFull, ts, f) && ok;
+        obs_model(kind, f, sg, cg, st, h, scj);
+        for (int c = 0; c < 6; ++c) {
+            const double d = c == wr ? obs_wrap(h[c] - h0[c]) : h[c] - h0[c];
+            J[(j * 6 + c) * stride] = w[c] != 0.0 ? d * w[c] * inv[1 + j] : 0.0;
+        }
+    }
+    return ok;
+}
+
+// fit_accumulate_model with the measurement layer: obs_residual_rows, then the cost, floor and normal sums.
+// Components are summed in fit_accumulate_model's order, (0, 3), (1, 4), (2, 5); pos2 and vel2 are formed only on the
+// K8 path below.
 template <typename EvalFn>
 AZ_HD bool fit_accumulate_obs(EvalFn eval, int nvar, const double *inv, double jdFull, double epochJd, int kind,
                               const double *value, const double (&w)[6], double sg, double cg, const ObsStation &st,
@@ -151,18 +187,9 @@ AZ_HD bool fit_accumulate_obs(EvalFn eval, int nvar, const double *inv, double j
     if (kind == kObsTemeState && w[0] != 0.0 && w[0] == w[1] && w[1] == w[2] && w[3] == w[4] && w[4] == w[5])
         return fit_accumulate_model(eval, nvar, inv, jdFull, epochJd, value, w[3] != 0.0 ? value + 3 : nullptr, w[0],
                                     w[3], J, acc, stride);
-    const double ts[1] = {mul_rn(sub_rn(jdFull, epochJd), 1440.0)};
-    bool ok = true;
-    const int wr = obs_wrapped(kind);
-    double obs[6], f0[6], h0[6], sc[6];
-    for (int c = 0; c < 6; ++c) obs[c] = w[c] != 0.0 ? value[c] : 0.0;
-    ok = eval(0, jdFull, ts, f0) && ok;
-    obs_model(kind, f0, sg, cg, st, h0, sc);
-    double r[6];
-    for (int c = 0; c < 6; ++c) {
-        const double d = c == wr ? obs_wrap(obs[c] - h0[c]) : obs[c] - h0[c];
-        r[c] = w[c] != 0.0 ? d * w[c] : 0.0;
-    }
+    double obs[6], sc[6], r[6];
+    const bool ok = obs_residual_rows(eval, nvar, inv, jdFull, epochJd, kind, value, w, sg, cg, st, obs, sc, r, J,
+                                      stride);
     {
         double F = acc[0], fl = acc[3 * stride];
         for (int c = 0; c < 3; ++c) {   // components in the order (0, 3), (1, 4), (2, 5): fit_accumulate_model's sums
@@ -176,18 +203,6 @@ AZ_HD bool fit_accumulate_obs(EvalFn eval, int nvar, const double *inv, double j
         }
         acc[0] = F;
         acc[3 * stride] = fl;
-    }
-#ifdef __CUDA_ARCH__
-#pragma unroll 1
-#endif
-    for (int j = 0; j < nvar; ++j) {
-        double f[6], h[6], scj[6];
-        ok = eval(1 + j, jdFull, ts, f) && ok;
-        obs_model(kind, f, sg, cg, st, h, scj);
-        for (int c = 0; c < 6; ++c) {
-            const double d = c == wr ? obs_wrap(h[c] - h0[c]) : h[c] - h0[c];
-            J[(j * 6 + c) * stride] = w[c] != 0.0 ? d * w[c] * inv[1 + j] : 0.0;
-        }
     }
     fit_accumulate_normal(nvar, r, J, acc, stride);
     return ok;

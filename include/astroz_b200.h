@@ -783,6 +783,64 @@ int32_t astroz_cuda_conjunction_device(const double *d_elements, uint32_t n, int
                                        const double *d_hbr_km, uint32_t m, int32_t frame, int32_t device,
                                        double *d_record, double *d_states, double *d_state_covariance,
                                        uint8_t *d_status, void *stream);
+/* ---- track correlation (K12): which catalogue rows predict a sensor track within their uncertainty ----------------------
+ * The catalogue is K10's: elements[8][n], covariance[n][28] in the fit's variables (NULL: every P zero, a plain TLE
+ * catalogue) and model[n] (NULL: all 0).  Track j is the observations [offsets[j], offsets[j + 1]) (offsets[0] = 0,
+ * offsets[t] = m) in the layout of astroz_cuda_fit_observations: jd[i] + fr[i], kind[i], value[i][6], sigma[i][6],
+ * station[i] into stations[k][3].  For each (track, row) pair, x the row's variables:
+ *   sets:      the row's nominal and stepped sets as K10 builds them (B* held when P's B* row is zero); when P is all zero
+ *              no stepped set is built or propagated;
+ *   rows:      per observation, the weighted residual z and weighted Jacobian rows G of the element fit (azimuth and
+ *              right ascension wrapped, scaled by the cosine of the observed elevation / declination), at K10's time;
+ *   distance:  d2 = z^T (I + G P G^T)^-1 z over the track's stacked residuals, evaluated as |z|^2 - b^T (I + P N)^-1 P b
+ *              with b = G^T z and N = G^T G summed in track order (a 7 x 7 solve, exact for any positive semi-definite
+ *              P), clamped at 0.  For one observation it is r^T (H Sigma H^T + R)^-1 r; for a track it accounts for the
+ *              element error its residuals share;
+ *   gate:      the chi-square quantile of k degrees of freedom at gate_probability, k = used[j] the track's used scalar
+ *              residuals (astroz_cuda_chi2_quantile);
+ *   failure:   a deep-space cell that fails, or sums that are not finite: the pair is skipped and counted.
+ * Outputs per track: rows[t][best] and d2[t][best] the best smallest (d2, row) over the evaluated pairs, by d2 and then
+ * row index, in or out of the gate (empty slots 0xFFFFFFFF / +inf); used[t] = k; n_gate[t] the rows with d2 <= gate;
+ * n_failed[t] the skipped pairs; status[t] (ASTROZ_CORR_*): OK at least one row in the gate, UNCORRELATED none,
+ * NO_ROW no pair evaluated, BAD_TRACK (device call only) an empty track, k = 0 or more than ASTROZ_CORR_MAX_TRACK
+ * observations (every other output of the track empty or zero).  Per row: row_status[n] ASTROZ_COV_OK, or
+ * ASTROZ_COV_INIT_FAILED when its sets cannot be built under its model (or, device call only, its model byte is > 1):
+ * such a row takes part in no pair.
+ * A track's bytes depend on its own observations and the catalogue alone: not on other tracks, their order, the batch
+ * split or the call form.  Every pair is scored: there is no pre-screen.
+ * ASTROZ_VALUE_ERROR, nothing written: device = -1, an unknown grav, best outside [1, ASTROZ_CORR_MAX_BEST],
+ * gate_probability outside (0, 1); and for the host call offsets that decrease or do not run from 0 to m, an empty
+ * track, a track of more than ASTROZ_CORR_MAX_TRACK observations or with no used residual, every observation check of
+ * astroz_cuda_fit_observations, a non-finite element, covariance word or time, a model byte > 1. */
+#define ASTROZ_CORR_OK           0
+#define ASTROZ_CORR_UNCORRELATED 1
+#define ASTROZ_CORR_NO_ROW       2
+#define ASTROZ_CORR_BAD_TRACK    3
+#define ASTROZ_CORR_MAX_TRACK    256
+#define ASTROZ_CORR_MAX_BEST     8
+/* HOST buffers: one upload (pageable through a pinned ring, pinned by direct DMA), the launches, plain copies back. */
+int32_t astroz_cuda_correlate(const double *elements, uint32_t n, int32_t grav, const double *covariance,
+                              const uint8_t *model, const uint32_t *offsets, uint32_t t, const double *jd,
+                              const double *fr, const uint8_t *kind, const double *value, const double *sigma,
+                              const uint32_t *station, uint32_t m, const double *stations, uint32_t k,
+                              double gate_probability, uint32_t best, int32_t device, uint32_t *rows, double *d2,
+                              uint32_t *used, uint32_t *n_gate, uint32_t *n_failed, uint8_t *status,
+                              uint8_t *row_status);
+/* DEVICE pointers on `device`: the launches on `stream`, no allocation, no synchronisation; only the scalar arguments
+ * are checked (kinds, stations and sigmas must be valid; a bad track gets BAD_TRACK).  d_scratch holds
+ * *bytes of astroz_cuda_correlate_scratch_bytes(n, t, best, bytes), 8-byte aligned, for the row chunks' partial lists. */
+int32_t astroz_cuda_correlate_device(const double *d_elements, uint32_t n, int32_t grav, const double *d_covariance,
+                                     const uint8_t *d_model, const uint32_t *d_offsets, uint32_t t, const double *d_jd,
+                                     const double *d_fr, const uint8_t *d_kind, const double *d_value,
+                                     const double *d_sigma, const uint32_t *d_station, const double *d_stations,
+                                     double gate_probability, uint32_t best, int32_t device, void *d_scratch,
+                                     uint32_t *d_rows, double *d_d2, uint32_t *d_used, uint32_t *d_n_gate,
+                                     uint32_t *d_n_failed, uint8_t *d_status, uint8_t *d_row_status, void *stream);
+int32_t astroz_cuda_correlate_scratch_bytes(uint32_t n, uint32_t t, uint32_t best, uint64_t *bytes);
+/* The gate: the quantile x of the chi-square distribution of k >= 1 degrees of freedom at probability p in (0, 1), by
+ * the function the kernels evaluate.  ASTROZ_VALUE_ERROR for k = 0 or p outside (0, 1). */
+int32_t astroz_cuda_chi2_quantile(uint32_t k, double p, double *x);
+
 /* One TLE line pair read by the library's own parser (src/Tle.zig:49-101) into the eight element columns above, the
  * numbers astroz_cuda_constellation_create would use.  ASTROZ_BAD_TLE_LENGTH when the pair cannot be read. */
 int32_t astroz_cuda_parse_tle(const char *line1, const char *line2, double *elements);
