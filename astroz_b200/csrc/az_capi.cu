@@ -31,6 +31,7 @@
 #include "az_fit.cuh"
 #include "az_hostcopy.cuh"
 #include "az_ingest.cuh"
+#include "az_iod.cuh"
 #include "az_kernels.cuh"
 #include "az_lambert.cuh"
 #include "az_numerical.cuh"
@@ -3395,6 +3396,181 @@ int32_t astroz_cuda_correlate(const double *elements, uint32_t n, int32_t grav, 
         AZ_CUDA(cudaMemcpyAsync(status, a.status, t, cudaMemcpyDeviceToHost, st));
     }
     if (n) AZ_CUDA(cudaMemcpyAsync(row_status, a.rowStatus, n, cudaMemcpyDeviceToHost, st));
+    AZ_CUDA(d.buf.release());
+    AZ_CUDA(cudaStreamSynchronize(st));
+    return ASTROZ_OK;
+}
+
+// ---- initial orbits (K13, az_iod.cu, az_iod.cuh) ----------------------------------------------------------------------
+static_assert(ASTROZ_IOD_OK == az::kIodOk && ASTROZ_IOD_TOO_FEW == az::kIodTooFew &&
+                  ASTROZ_IOD_NO_CANDIDATE == az::kIodNoCandidate &&
+                  ASTROZ_IOD_CONVERSION_FAILED == az::kIodConversionFailed &&
+                  ASTROZ_IOD_BAD_TRACK == az::kIodBadTrack && ASTROZ_IOD_MAX_TRACK == az::kIodMaxTrack &&
+                  ASTROZ_IOD_METHOD_STATE == az::kIodState && ASTROZ_IOD_METHOD_GIBBS == az::kIodGibbs &&
+                  ASTROZ_IOD_METHOD_HERRICK_GIBBS == az::kIodHerrickGibbs &&
+                  ASTROZ_IOD_METHOD_LAMBERT == az::kIodLambert && ASTROZ_IOD_METHOD_GAUSS == az::kIodGauss &&
+                  ASTROZ_IOD_METHOD_NONE == az::kIodNone,
+              "initial-orbit status and method bytes");
+
+// Scalar checks of the initial-orbit calls, before anything is read, written or allocated; a receives the scalars.
+static int32_t iod_check(uint32_t t, int32_t grav, int32_t device, az::IodArgs *a) {
+    if (device < 0) return value_error("initial orbit determination runs on one device: pass its ordinal");
+    if (grav != ASTROZ_WGS72 && grav != ASTROZ_WGS84) return value_error("grav must be ASTROZ_WGS72 or ASTROZ_WGS84");
+    a->t = t;
+    a->grav = grav;
+    a->g = az::grav_consts(az::gravity(grav));
+    return ASTROZ_OK;
+}
+
+int32_t astroz_cuda_initial_orbits_scratch_bytes(uint32_t t, uint64_t *bytes) {
+    if (!bytes) return ASTROZ_NULL_POINTER;
+    *bytes = az::iod_scratch_bytes(t);
+    return ASTROZ_OK;
+}
+
+static void iod_outputs(az::IodArgs &a, double *elements, double *state, double *wrms, uint8_t *method,
+                        uint32_t *candidates, double *conv, uint8_t *deep_space, uint8_t *status) {
+    a.elements = elements;
+    a.state = state;
+    a.wrms = wrms;
+    a.method = method;
+    a.candidates = candidates;
+    a.conv = conv;
+    a.deepSpace = deep_space;
+    a.status = status;
+}
+
+int32_t astroz_cuda_initial_orbits_device(const uint32_t *d_offsets, uint32_t t, const double *d_jd,
+                                          const double *d_fr, const uint8_t *d_kind, const double *d_value,
+                                          const double *d_sigma, const uint32_t *d_station, const double *d_stations,
+                                          const double *d_bstar, int32_t grav, int32_t device, void *d_scratch,
+                                          double *d_elements, double *d_state, double *d_wrms, uint8_t *d_method,
+                                          uint32_t *d_candidates, double *d_conv, uint8_t *d_deep_space,
+                                          uint8_t *d_status, void *stream) {
+    az::IodArgs a{};
+    int32_t rc = iod_check(t, grav, device, &a);
+    if (rc != ASTROZ_OK) return rc;
+    if (t == 0) return ASTROZ_OK;
+    if (!d_offsets || !d_jd || !d_fr || !d_kind || !d_value || !d_sigma || !d_scratch || !d_elements || !d_state ||
+        !d_wrms || !d_method || !d_candidates || !d_conv || !d_deep_space || !d_status)
+        return ASTROZ_NULL_POINTER;
+    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
+    AZ_CUDA(cudaSetDevice(device));
+    a.offsets = d_offsets;
+    a.jd = d_jd;
+    a.fr = d_fr;
+    a.kind = d_kind;
+    a.value = d_value;
+    a.sigma = d_sigma;
+    a.station = d_station;
+    a.stations = d_stations;
+    a.bstar = d_bstar;
+    a.scratch = d_scratch;
+    iod_outputs(a, d_elements, d_state, d_wrms, d_method, d_candidates, d_conv, d_deep_space, d_status);
+    AZ_CUDA(az::launch_iod(a, static_cast<cudaStream_t>(stream)));
+    return ASTROZ_OK;
+}
+
+// Host buffers: every check, then each track's observations sorted stably by jd + fr into host staging, which goes up
+// through the pinned ring (the caller's pinned arrays are not read by DMA: the staging copy is pageable), the launches
+// on the device's stream with the scratch in the same device block, and plain copies back.
+int32_t astroz_cuda_initial_orbits(const uint32_t *offsets, uint32_t t, const double *jd, const double *fr,
+                                   const uint8_t *kind, const double *value, const double *sigma,
+                                   const uint32_t *station, uint32_t m, const double *stations, uint32_t k,
+                                   const double *bstar, int32_t grav, int32_t device, double *elements, double *state,
+                                   double *wrms, uint8_t *method, uint32_t *candidates, double *conv,
+                                   uint8_t *deep_space, uint8_t *status) {
+    az::IodArgs a{};
+    int32_t rc = iod_check(t, grav, device, &a);
+    if (rc != ASTROZ_OK) return rc;
+    if (!offsets) return ASTROZ_NULL_POINTER;
+    if (t && (!elements || !state || !wrms || !method || !candidates || !conv || !deep_space || !status))
+        return ASTROZ_NULL_POINTER;
+    if (m && (!jd || !fr || !kind || !value || !sigma)) return ASTROZ_NULL_POINTER;
+    if (offsets[0] != 0) return value_error("offsets[0] must be 0");
+    for (uint32_t j = 0; j < t; ++j) {
+        if (offsets[j + 1] < offsets[j]) return value_error("offsets must be non-decreasing");
+        if (offsets[j + 1] == offsets[j]) return value_error("a track has no observation");
+        if (offsets[j + 1] - offsets[j] > az::kIodMaxTrack)
+            return value_error("a track is longer than ASTROZ_IOD_MAX_TRACK observations");
+    }
+    if (offsets[t] != m) return value_error("offsets[t] must equal the observation count m");
+    if ((rc = obs_values_check(jd, fr, value, sigma, station, kind, m, stations, k)) != ASTROZ_OK) return rc;
+    {
+        const az::CorrObsArrays in{jd, fr, kind, value, sigma, station, stations};
+        for (uint32_t j = 0; j < t; ++j)
+            if (az::corr_used(in, offsets[j], offsets[j + 1]) == 0) return value_error("a track has no used residual");
+    }
+    if (bstar && !all_finite(bstar, t)) return value_error("bstar must be finite");
+    if (t == 0) return ASTROZ_OK;
+    // each track in time order, stably
+    std::vector<uint32_t> order(m);
+    for (uint32_t i = 0; i < m; ++i) order[i] = i;
+    for (uint32_t j = 0; j < t; ++j)
+        std::stable_sort(order.begin() + offsets[j], order.begin() + offsets[j + 1], [&](uint32_t p, uint32_t q) {
+            return az::add_rn(jd[p], fr[p]) < az::add_rn(jd[q], fr[q]);
+        });
+    std::vector<double> sJd(m), sFr(m), sValue((size_t)6 * m), sSigma((size_t)6 * m);
+    std::vector<uint8_t> sKind(m);
+    std::vector<uint32_t> sStation(station ? m : 0);
+    for (uint32_t i = 0; i < m; ++i) {
+        const uint32_t p = order[i];
+        sJd[i] = jd[p];
+        sFr[i] = fr[p];
+        sKind[i] = kind[p];
+        std::memcpy(&sValue[(size_t)6 * i], value + (size_t)6 * p, 48);
+        std::memcpy(&sSigma[(size_t)6 * i], sigma + (size_t)6 * p, 48);
+        if (station) sStation[i] = station[p];
+    }
+    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
+    NumericalContext *c = nullptr;
+    if ((rc = numerical_context(device, &c)) != ASTROZ_OK) return rc;
+    std::lock_guard<std::mutex> lk(c->m);
+    AZ_CUDA(cudaSetDevice(device));
+    cudaStream_t st = c->stream;
+    // offsets | jd | fr | kind | value | sigma | station | stations | bstar | scratch | elements | state | wrms | method |
+    // candidates | conv | deep_space | status
+    DeviceBlock d(st);
+    AZ_CUDA(d.alloc({(size_t)4 * (t + 1), (size_t)8 * m, (size_t)8 * m, (size_t)m, (size_t)48 * m, (size_t)48 * m,
+                     station ? (size_t)4 * m : 0, (size_t)24 * k, bstar ? (size_t)8 * t : 0, az::iod_scratch_bytes(t),
+                     (size_t)64 * t, (size_t)48 * t, (size_t)8 * t, (size_t)t, (size_t)4 * t, (size_t)16 * t, (size_t)t,
+                     (size_t)t}));
+    auto up = [&](const void *src, void *dst, size_t elemBytes, size_t count) {
+        void *const dd[1] = {dst};
+        const void *const ss[1] = {src};
+        return c->pipe.ring.upload(az::is_pageable(src), 1, ss, dd, &elemBytes, count, st);
+    };
+    AZ_CUDA(up(offsets, d.u32(0), 4, (size_t)t + 1));
+    if (m) {
+        AZ_CUDA(up(sJd.data(), d.f64(1), 8, m));
+        AZ_CUDA(up(sFr.data(), d.f64(2), 8, m));
+        AZ_CUDA(up(sKind.data(), d.u8(3), 1, m));
+        AZ_CUDA(up(sValue.data(), d.f64(4), 48, m));
+        AZ_CUDA(up(sSigma.data(), d.f64(5), 48, m));
+        if (station) AZ_CUDA(up(sStation.data(), d.u32(6), 4, m));
+    }
+    if (k) AZ_CUDA(up(stations, d.f64(7), 24, k));
+    if (bstar) AZ_CUDA(up(bstar, d.f64(8), 8, t));
+    a.offsets = d.u32(0);
+    a.jd = d.f64(1);
+    a.fr = d.f64(2);
+    a.kind = d.u8(3);
+    a.value = d.f64(4);
+    a.sigma = d.f64(5);
+    a.station = station ? d.u32(6) : nullptr;
+    a.stations = k ? d.f64(7) : nullptr;
+    a.bstar = bstar ? d.f64(8) : nullptr;
+    a.scratch = d.piece(9);
+    iod_outputs(a, d.f64(10), d.f64(11), d.f64(12), d.u8(13), d.u32(14), d.f64(15), d.u8(16), d.u8(17));
+    AZ_CUDA(az::launch_iod(a, st));
+    AZ_CUDA(cudaMemcpyAsync(elements, a.elements, (size_t)64 * t, cudaMemcpyDeviceToHost, st));
+    AZ_CUDA(cudaMemcpyAsync(state, a.state, (size_t)48 * t, cudaMemcpyDeviceToHost, st));
+    AZ_CUDA(cudaMemcpyAsync(wrms, a.wrms, (size_t)8 * t, cudaMemcpyDeviceToHost, st));
+    AZ_CUDA(cudaMemcpyAsync(method, a.method, t, cudaMemcpyDeviceToHost, st));
+    AZ_CUDA(cudaMemcpyAsync(candidates, a.candidates, (size_t)4 * t, cudaMemcpyDeviceToHost, st));
+    AZ_CUDA(cudaMemcpyAsync(conv, a.conv, (size_t)16 * t, cudaMemcpyDeviceToHost, st));
+    AZ_CUDA(cudaMemcpyAsync(deep_space, a.deepSpace, t, cudaMemcpyDeviceToHost, st));
+    AZ_CUDA(cudaMemcpyAsync(status, a.status, t, cudaMemcpyDeviceToHost, st));
     AZ_CUDA(d.buf.release());
     AZ_CUDA(cudaStreamSynchronize(st));
     return ASTROZ_OK;

@@ -254,6 +254,32 @@ struct CorrArgs {
 // the gates, the near-earth rows, the deep-space rows (when model is given) and the merge, on one stream
 cudaError_t launch_correlate(const CorrArgs &a, cudaStream_t stream);
 
+// K13: initial orbits of tracks (az_iod.cu, az_iod.cuh).  Device pointers.
+struct IodArgs {
+    const uint32_t *offsets = nullptr;   // [t + 1]: track j owns observations [offsets[j], offsets[j + 1]), time-ordered
+    uint32_t t = 0;
+    const double *jd = nullptr, *fr = nullptr;
+    const uint8_t *kind = nullptr;
+    const double *value = nullptr, *sigma = nullptr;   // [m][6]
+    const uint32_t *station = nullptr;
+    const double *stations = nullptr;
+    const double *bstar = nullptr;       // [t], nullable (all 0)
+    int grav = 1;
+    GravConsts g{};
+    void *scratch = nullptr;             // iod_scratch_bytes(t)
+    double *elements = nullptr;          // [8][t] converted sets, epoch = the track's epoch
+    double *state = nullptr;             // [t][6] TEME state at the epoch
+    double *wrms = nullptr;              // [t]
+    uint8_t *method = nullptr;           // [t] ASTROZ_IOD_METHOD_*
+    uint32_t *candidates = nullptr;      // [t]
+    double *conv = nullptr;              // [t][2] conversion |dr| km, |dv| km/s
+    uint8_t *deepSpace = nullptr;        // [t]
+    uint8_t *status = nullptr;           // [t] ASTROZ_IOD_*
+};
+size_t iod_scratch_bytes(uint32_t t);
+// the IOD kernel, K8's near-earth and deep-space fits over one TEME state per track, and the finishing kernel
+cudaError_t launch_iod(const IodArgs &a, cudaStream_t stream);
+
 // DFMA throughput microbenchmark: returns achieved fp64 FLOP/s (FMA = 2).
 cudaError_t measure_fp64_peak(double *flops);
 // Arithmetic peak of the fp64 pipe: SMs x 64 lanes x 2 FLOP x the maximum SM clock.

@@ -840,6 +840,70 @@ int32_t astroz_cuda_correlate_scratch_bytes(uint32_t n, uint32_t t, uint32_t bes
 /* The gate: the quantile x of the chi-square distribution of k >= 1 degrees of freedom at probability p in (0, 1), by
  * the function the kernels evaluate.  ASTROZ_VALUE_ERROR for k = 0 or p outside (0, 1). */
 int32_t astroz_cuda_chi2_quantile(uint32_t k, double p, double *x);
+/* ---- initial orbits (K13): an element set for a track no catalogue row predicts ---------------------------------------
+ * New capability: the reference has no initial orbit determination, so these calls replace nothing in it.
+ * Track j is the observations [offsets[j], offsets[j + 1]) in the layout of astroz_cuda_correlate, in time order (the
+ * host call sorts each track stably by jd + fr; the device call reports a track out of order as BAD_TRACK).  Its epoch
+ * is the time of its middle observation, index floor(m_j / 2).  mu is the gravity model's (grav).
+ *   geometry:   the inverses of the measurement model: TEME and ECEF states give a TEME state, radar range / azimuth /
+ *               elevation a TEME position (range-rate is scored only), optical angles a TEME line of sight from the
+ *               station.  A method builds only from observations whose geometry components are all used: a TEME or
+ *               ECEF state without its velocity, for one, builds nothing (it is scored only), so a track of such
+ *               states alone is TOO_FEW;
+ *   candidates: every state observation; with >= 3 radar positions a Gibbs and a Herrick-Gibbs velocity for the middle
+ *               of every triplet of a fixed table of up to 30 (first, middle, last always among them); with exactly 2,
+ *               the zero-revolution Lambert transfer for the normals +z and -z; with >= 3 optical observations Gauss'
+ *               method on every triplet with |L1 . (L2 x L3)| >= 1e-12, every real root above 1 earth radius of its
+ *               8th-degree polynomial refined by universal-variable f and g (Curtis, Algorithm 5.6).  A candidate that
+ *               is not finite, has e >= 1 or a perigee radius below 1 earth radius is rejected;
+ *   score:      each candidate propagated two-body to every observation of the track and scored by the element fit's
+ *               residual rules: F = sum of squared weighted residuals.  The least (F, method, triplet, root) wins;
+ *   conversion: the winner two-body at the epoch -> osculating elements (n in rev/day, B* = bstar[j], 0 when bstar is
+ *               NULL) -> astroz_cuda_fit_elements_mixed's own fit to that one TEME state at the epoch with B* held.
+ * Outputs per track: elements[8][t] the converted set (epoch = the track's epoch), state[t][6] the TEME state at the
+ * epoch, wrms[t] = sqrt(F / used residuals), method[t] (ASTROZ_IOD_METHOD_*), candidates[t] the candidates scored,
+ * conv[t][2] the converted set's |dr| [km] and |dv| [km/s] from the state at the epoch, deep_space[t] 1 when the set
+ * is an SDP4 (period > 225 min) set, status[t] (ASTROZ_IOD_*): OK; TOO_FEW fewer usable observations than any method
+ * needs (1 state, 2 radar, 3 optical); NO_CANDIDATE every candidate rejected; CONVERSION_FAILED the fit did not
+ * converge or left |dr| > 1e-6 km or |dv| > 1e-9 km/s (the outputs are kept); BAD_TRACK (device call only) an empty
+ * track, more than ASTROZ_IOD_MAX_TRACK observations, no used residual or out of time order.  Except for
+ * CONVERSION_FAILED, a track that is not OK has zero elements, state, wrms and conv and method NONE.
+ * A track's bytes depend on that track alone: not on other tracks, their order, the batch split or the call form.
+ * ASTROZ_VALUE_ERROR, nothing written: device = -1, an unknown grav; and for the host call offsets that decrease or do
+ * not run from 0 to m, an empty track, a track longer than ASTROZ_IOD_MAX_TRACK or with no used residual, every
+ * observation check of astroz_cuda_fit_observations, a non-finite bstar. */
+#define ASTROZ_IOD_OK                0
+#define ASTROZ_IOD_TOO_FEW           1
+#define ASTROZ_IOD_NO_CANDIDATE      2
+#define ASTROZ_IOD_CONVERSION_FAILED 3
+#define ASTROZ_IOD_BAD_TRACK         4
+#define ASTROZ_IOD_MAX_TRACK         256
+#define ASTROZ_IOD_METHOD_STATE         0
+#define ASTROZ_IOD_METHOD_GIBBS         1
+#define ASTROZ_IOD_METHOD_HERRICK_GIBBS 2
+#define ASTROZ_IOD_METHOD_LAMBERT       3
+#define ASTROZ_IOD_METHOD_GAUSS         4
+#define ASTROZ_IOD_METHOD_NONE          255
+/* HOST buffers: each track's observations are first sorted into host staging, which goes up through the pinned ring
+ * whether the caller's arrays are pinned or not; then the launches and plain copies back. */
+int32_t astroz_cuda_initial_orbits(const uint32_t *offsets, uint32_t t, const double *jd, const double *fr,
+                                   const uint8_t *kind, const double *value, const double *sigma,
+                                   const uint32_t *station, uint32_t m, const double *stations, uint32_t k,
+                                   const double *bstar, int32_t grav, int32_t device, double *elements, double *state,
+                                   double *wrms, uint8_t *method, uint32_t *candidates, double *conv,
+                                   uint8_t *deep_space, uint8_t *status);
+/* DEVICE pointers on `device`: four launches on `stream` (the IOD kernel, the near-earth and deep-space conversion fits,
+ * the finishing kernel), no allocation, no synchronisation; only the scalar arguments are checked (kinds, stations and
+ * sigmas must be valid; a bad track gets BAD_TRACK).  d_scratch holds *bytes of
+ * astroz_cuda_initial_orbits_scratch_bytes(t, bytes), 8-byte aligned. */
+int32_t astroz_cuda_initial_orbits_device(const uint32_t *d_offsets, uint32_t t, const double *d_jd,
+                                          const double *d_fr, const uint8_t *d_kind, const double *d_value,
+                                          const double *d_sigma, const uint32_t *d_station, const double *d_stations,
+                                          const double *d_bstar, int32_t grav, int32_t device, void *d_scratch,
+                                          double *d_elements, double *d_state, double *d_wrms, uint8_t *d_method,
+                                          uint32_t *d_candidates, double *d_conv, uint8_t *d_deep_space,
+                                          uint8_t *d_status, void *stream);
+int32_t astroz_cuda_initial_orbits_scratch_bytes(uint32_t t, uint64_t *bytes);
 
 /* One TLE line pair read by the library's own parser (src/Tle.zig:49-101) into the eight element columns above, the
  * numbers astroz_cuda_constellation_create would use.  ASTROZ_BAD_TLE_LENGTH when the pair cannot be read. */
