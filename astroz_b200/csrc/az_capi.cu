@@ -2513,6 +2513,121 @@ int32_t astroz_cuda_propagate_maneuvers(const double *states, uint32_t n, double
                                });
 }
 
+// ---- whole-batch host calls: element fits, observe, covariance, conjunctions, correlation, initial orbits, Lambert --
+// Their input checks, each rule stated once, and their one staging path.  The checks run before anything is read on,
+// written to or allocated on the device, in the order scalars, null pointers, values, device lookup.
+
+static bool all_finite(const double *p, size_t count) {
+    for (size_t i = 0; i < count; ++i)
+        if (!std::isfinite(p[i])) return false;
+    return true;
+}
+
+static int32_t grav_check(int32_t grav) {
+    if (grav != ASTROZ_WGS72 && grav != ASTROZ_WGS84) return value_error("grav must be ASTROZ_WGS72 or ASTROZ_WGS84");
+    return ASTROZ_OK;
+}
+
+// Group g of `groups` owns items [offsets[g], offsets[g + 1]) of m: the offsets are non-decreasing and end at m
+// (`wrong_end` is the refusal when they do not).  As the call states, offsets[0] must also be 0 (zero_first), and with
+// max_track > 0 the groups are tracks of 1 to max_track observations (`too_long` is the refusal of a longer one).
+static int32_t offsets_check(const uint32_t *offsets, uint32_t groups, uint32_t m, const char *wrong_end,
+                             bool zero_first = false, uint32_t max_track = 0, const char *too_long = nullptr) {
+    if (zero_first && offsets[0] != 0) return value_error("offsets[0] must be 0");
+    for (uint32_t g = 0; g < groups; ++g) {
+        if (offsets[g + 1] < offsets[g]) return value_error("offsets must be non-decreasing");
+        if (max_track == 0) continue;
+        if (offsets[g + 1] == offsets[g]) return value_error("a track has no observation");
+        if (offsets[g + 1] - offsets[g] > max_track) return value_error(too_long);
+    }
+    if (offsets[groups] != m) return value_error(wrong_end);
+    return ASTROZ_OK;
+}
+
+// Catalogue rows: n element columns [8][n], and their covariance [n][28] when it is given.
+static int32_t rows_check(const double *elements, const double *covariance, uint32_t n) {
+    if (!all_finite(elements, (size_t)8 * n)) return value_error("elements must be finite");
+    if (covariance && !all_finite(covariance, (size_t)az::kFitN * n)) return value_error("covariance words must be finite");
+    return ASTROZ_OK;
+}
+
+// The rows' model bytes, when given.
+static int32_t model_bytes_check(const uint8_t *model, uint32_t n) {
+    if (model)
+        for (uint32_t s = 0; s < n; ++s)
+            if (model[s] > 1) return value_error("a model byte is not 0 (near-earth) or 1 (deep space)");
+    return ASTROZ_OK;
+}
+
+// Every one of t tracks has a residual the scoring uses.
+static int32_t used_residuals_check(const az::CorrObsArrays &in, const uint32_t *offsets, uint32_t t) {
+    for (uint32_t j = 0; j < t; ++j)
+        if (az::corr_used(in, offsets[j], offsets[j + 1]) == 0) return value_error("a track has no used residual");
+    return ASTROZ_OK;
+}
+
+// One piece of a whole-batch call's device block: `bytes` long, uploaded from host `in` before the launch or copied to
+// host `out` after it (neither: scratch, or an optional array the caller did not pass).
+struct BatchPiece {
+    size_t bytes;
+    const void *in;
+    void *out;
+};
+static BatchPiece upload(const void *src, size_t bytes) { return {bytes, src, nullptr}; }
+static BatchPiece result(void *dst, size_t bytes) { return {bytes, nullptr, dst}; }
+static BatchPiece scratch(size_t bytes) { return {bytes, nullptr, nullptr}; }
+
+// A stream-ordered device block cut into the 16-byte aligned pieces of a list, at least 16 bytes in all: every piece
+// has an address in the block, an empty one too.
+struct DeviceBlock {
+    StreamBuf buf;
+    std::vector<size_t> at;
+    explicit DeviceBlock(cudaStream_t s) : buf(s) {}
+    cudaError_t alloc(std::initializer_list<BatchPiece> pieces) {
+        size_t total = 0;
+        for (const BatchPiece &p : pieces) at.push_back(total), total += (p.bytes + 15) & ~size_t(15);
+        return buf.alloc(std::max<size_t>(total, 16));
+    }
+    char *piece(int k) const { return static_cast<char *>(buf.p) + at[k]; }
+    double *f64(int k) const { return reinterpret_cast<double *>(piece(k)); }
+    uint32_t *u32(int k) const { return reinterpret_cast<uint32_t *>(piece(k)); }
+    uint8_t *u8(int k) const { return reinterpret_cast<uint8_t *>(piece(k)); }
+};
+using BatchLaunch = std::function<cudaError_t(const DeviceBlock &d, cudaStream_t s)>;
+
+// The host form of every whole-batch call, after its checks.  These calls are compute-bound (a fit propagates each
+// observation some 8 x iterations times for its ~56 bytes, a Lambert slot runs some 5 iterations of fp64
+// transcendentals for 56 bytes in), so there is no chunk pipeline to overlap transfers with: the whole batch goes up at
+// once into one device block -- pageable sources through the device's pinned ring, pinned ones by direct DMA, decided
+// per array -- launch(d, stream) queues the kernels on the device's stream with d.piece(k) the device copy of
+// pieces[k], each result comes back by a plain copy, and the block is returned before the call returns.
+static int32_t whole_batch(int32_t device, std::initializer_list<BatchPiece> pieces, const BatchLaunch &launch) {
+    int32_t rc = check_device_ordinal(device);
+    if (rc != ASTROZ_OK) return rc;
+    NumericalContext *c = nullptr;
+    if ((rc = numerical_context(device, &c)) != ASTROZ_OK) return rc;
+    std::lock_guard<std::mutex> lk(c->m);
+    AZ_CUDA(cudaSetDevice(device));
+    cudaStream_t st = c->stream;
+    DeviceBlock d(st);
+    AZ_CUDA(d.alloc(pieces));
+    const size_t byteSize = 1;
+    int k = 0;
+    for (const BatchPiece &p : pieces) {
+        void *const dst[1] = {d.piece(k++)};
+        if (p.in && p.bytes) AZ_CUDA(c->pipe.ring.upload(az::is_pageable(p.in), 1, &p.in, dst, &byteSize, p.bytes, st));
+    }
+    AZ_CUDA(launch(d, st));
+    k = 0;
+    for (const BatchPiece &p : pieces) {
+        char *const src = d.piece(k++);
+        if (p.out && p.bytes) AZ_CUDA(cudaMemcpyAsync(p.out, src, p.bytes, cudaMemcpyDeviceToHost, st));
+    }
+    AZ_CUDA(d.buf.release());
+    AZ_CUDA(cudaStreamSynchronize(st));
+    return ASTROZ_OK;
+}
+
 // ---- element fits (K8, az_fit.cu) ------------------------------------------------------------------------------------
 static_assert(ASTROZ_FIT_CONVERGED == az::kFitConverged && ASTROZ_FIT_ITERATION_LIMIT == az::kFitIterLimit &&
                   ASTROZ_FIT_INIT_FAILED == az::kFitInitFailed && ASTROZ_FIT_DEEP_SPACE == az::kFitDeepSpace &&
@@ -2523,7 +2638,8 @@ static_assert(ASTROZ_FIT_CONVERGED == az::kFitConverged && ASTROZ_FIT_ITERATION_
 static int32_t fit_check(uint32_t n, int32_t grav, double pos_sigma, double vel_sigma, int32_t fit_bstar,
                          uint32_t max_iter, int32_t device, az::FitArgs *a) {
     if (device < 0) return value_error("an element fit runs on one device: pass its ordinal");
-    if (grav != ASTROZ_WGS72 && grav != ASTROZ_WGS84) return value_error("grav must be ASTROZ_WGS72 or ASTROZ_WGS84");
+    const int32_t rc = grav_check(grav);
+    if (rc != ASTROZ_OK) return rc;
     if (!std::isfinite(pos_sigma) || !(pos_sigma > 0.0) || !std::isfinite(vel_sigma) || !(vel_sigma > 0.0))
         return value_error("pos_sigma and vel_sigma must be finite and > 0");
     if (max_iter == 0) return value_error("max_iter must be at least 1");
@@ -2537,16 +2653,27 @@ static int32_t fit_check(uint32_t n, int32_t grav, double pos_sigma, double vel_
     return ASTROZ_OK;
 }
 
-static bool all_finite(const double *p, size_t count) {
-    for (size_t i = 0; i < count; ++i)
-        if (!std::isfinite(p[i])) return false;
-    return true;
-}
-
 // The kernels one fit call queues on its stream: launch_fit, or launch_fit_mixed below.
 using FitLaunch = cudaError_t (*)(const az::FitArgs &a, cudaStream_t stream);
 
-// The device-pointer calls: checks, then launch(a, stream) queues the kernels.
+// Both call forms: a holds fit_check's scalars, the arrays are on the device, launch(a, st) queues the kernels.
+static cudaError_t fit_run(az::FitArgs a, const double *elements, const uint32_t *offsets, const double *jd,
+                           const double *fr, const double *pos, const double *vel, double *fitted, double *rms,
+                           uint32_t *iterations, uint8_t *status, cudaStream_t st, FitLaunch launch) {
+    a.elements = elements;
+    a.offsets = offsets;
+    a.jd = jd;
+    a.fr = fr;
+    a.pos = pos;
+    a.vel = vel;
+    a.fitted = fitted;
+    a.rms = rms;
+    a.iterations = iterations;
+    a.status = status;
+    return launch(a, st);
+}
+
+// The device-pointer calls.
 static int32_t fit_device(const double *d_elements, uint32_t n, int32_t grav, const uint32_t *d_offsets,
                           const double *d_jd, const double *d_fr, const double *d_pos, const double *d_vel,
                           double pos_sigma, double vel_sigma, int32_t fit_bstar, uint32_t max_iter, int32_t device,
@@ -2560,17 +2687,8 @@ static int32_t fit_device(const double *d_elements, uint32_t n, int32_t grav, co
         return ASTROZ_NULL_POINTER;
     if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
     AZ_CUDA(cudaSetDevice(device));
-    a.elements = d_elements;
-    a.offsets = d_offsets;
-    a.jd = d_jd;
-    a.fr = d_fr;
-    a.pos = d_pos;
-    a.vel = d_vel;
-    a.fitted = d_fitted;
-    a.rms = d_rms;
-    a.iterations = d_iterations;
-    a.status = d_status;
-    AZ_CUDA(launch(a, static_cast<cudaStream_t>(stream)));
+    AZ_CUDA(fit_run(a, d_elements, d_offsets, d_jd, d_fr, d_pos, d_vel, d_fitted, d_rms, d_iterations, d_status,
+                    static_cast<cudaStream_t>(stream), launch));
     return ASTROZ_OK;
 }
 
@@ -2600,9 +2718,6 @@ int32_t astroz_cuda_fit_elements_mixed_device(const double *d_elements, uint32_t
                       max_iter, device, d_fitted, d_rms, d_iterations, d_status, stream, launch_fit_mixed);
 }
 
-// Host buffers: a fit is compute-bound (each observation is propagated some 8 x iterations times for its ~56 bytes),
-// so the whole batch goes up at once -- pageable arrays through the device's pinned ring, pinned ones by direct DMA --
-// and launch(a, stream) fits it.  The results (~90 bytes per satellite) come back by plain copies.
 static int32_t fit_host(const double *elements, uint32_t n, int32_t grav, const uint32_t *offsets, const double *jd,
                         const double *fr, const double *pos, const double *vel, uint32_t m, double pos_sigma,
                         double vel_sigma, int32_t fit_bstar, uint32_t max_iter, int32_t device, double *fitted,
@@ -2613,64 +2728,19 @@ static int32_t fit_host(const double *elements, uint32_t n, int32_t grav, const 
     if (n == 0) return ASTROZ_OK;
     if (!elements || !offsets || !fitted || !rms || !iterations || !status) return ASTROZ_NULL_POINTER;
     if (m && (!jd || !fr || !pos)) return ASTROZ_NULL_POINTER;
-    for (uint32_t s = 0; s < n; ++s)
-        if (offsets[s + 1] < offsets[s]) return value_error("offsets must be non-decreasing");
-    if (offsets[n] != m) return value_error("offsets[n] must equal the observation count m");
+    if ((rc = offsets_check(offsets, n, m, "offsets[n] must equal the observation count m")) != ASTROZ_OK) return rc;
     if (!all_finite(elements, (size_t)8 * n) || !all_finite(jd, m) || !all_finite(fr, m) ||
         !all_finite(pos, (size_t)3 * m) || (vel && !all_finite(vel, (size_t)3 * m)))
         return value_error("elements and observations must be finite");
-    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
-    NumericalContext *c = nullptr;
-    if ((rc = numerical_context(device, &c)) != ASTROZ_OK) return rc;
-    std::lock_guard<std::mutex> lk(c->m);
-    AZ_CUDA(cudaSetDevice(device));
-    cudaStream_t st = c->stream;
-    // one device block: elements | fitted | rms | jd | fr | pos | vel | offsets | iterations | status
-    const size_t nObs = std::max<uint32_t>(m, 1);
-    const size_t words[] = {(size_t)8 * n, (size_t)8 * n, (size_t)2 * n, nObs, nObs, 3 * nObs, vel ? 3 * nObs : 0};
-    size_t at[7], total = 0;
-    for (int k = 0; k < 7; ++k) at[k] = total, total += (words[k] * 8 + 15) & ~size_t(15);
-    const size_t offAt = total;
-    total += ((size_t)(n + 1) * 4 + 15) & ~size_t(15);
-    const size_t iterAt = total;
-    total += ((size_t)n * 4 + 15) & ~size_t(15);
-    const size_t statusAt = total;
-    total += n;
-    StreamBuf dBuf(st);
-    AZ_CUDA(dBuf.alloc(total));
-    char *base = static_cast<char *>(dBuf.p);
-    auto dp = [&](int k) { return reinterpret_cast<double *>(base + at[k]); };
-    auto up = [&](const void *src, void *dst, size_t elemBytes, size_t count) {
-        void *const d[1] = {dst};
-        const void *const s[1] = {src};
-        return c->pipe.ring.upload(az::is_pageable(src), 1, s, d, &elemBytes, count, st);
-    };
-    AZ_CUDA(up(elements, dp(0), 8, (size_t)8 * n));
-    AZ_CUDA(up(offsets, base + offAt, 4, (size_t)n + 1));
-    if (m) {
-        AZ_CUDA(up(jd, dp(3), 8, m));
-        AZ_CUDA(up(fr, dp(4), 8, m));
-        AZ_CUDA(up(pos, dp(5), 24, m));
-        if (vel) AZ_CUDA(up(vel, dp(6), 24, m));
-    }
-    a.elements = dp(0);
-    a.offsets = reinterpret_cast<const uint32_t *>(base + offAt);
-    a.jd = dp(3);
-    a.fr = dp(4);
-    a.pos = dp(5);
-    a.vel = vel ? dp(6) : nullptr;
-    a.fitted = dp(1);
-    a.rms = dp(2);
-    a.iterations = reinterpret_cast<uint32_t *>(base + iterAt);
-    a.status = reinterpret_cast<uint8_t *>(base + statusAt);
-    AZ_CUDA(launch(a, st));
-    AZ_CUDA(cudaMemcpyAsync(fitted, a.fitted, (size_t)8 * n * 8, cudaMemcpyDeviceToHost, st));
-    AZ_CUDA(cudaMemcpyAsync(rms, a.rms, (size_t)2 * n * 8, cudaMemcpyDeviceToHost, st));
-    AZ_CUDA(cudaMemcpyAsync(iterations, a.iterations, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
-    AZ_CUDA(cudaMemcpyAsync(status, a.status, n, cudaMemcpyDeviceToHost, st));
-    AZ_CUDA(dBuf.release());
-    AZ_CUDA(cudaStreamSynchronize(st));
-    return ASTROZ_OK;
+    return whole_batch(device,
+                       {upload(elements, (size_t)64 * n), upload(offsets, (size_t)4 * (n + 1)), upload(jd, (size_t)8 * m),
+                        upload(fr, (size_t)8 * m), upload(pos, (size_t)24 * m), upload(vel, vel ? (size_t)24 * m : 0),
+                        result(fitted, (size_t)64 * n), result(rms, (size_t)16 * n), result(iterations, (size_t)4 * n),
+                        result(status, n)},
+                       [&](const DeviceBlock &d, cudaStream_t st) {
+                           return fit_run(a, d.f64(0), d.u32(1), d.f64(2), d.f64(3), d.f64(4),
+                                          vel ? d.f64(5) : nullptr, d.f64(6), d.f64(7), d.u32(8), d.u8(9), st, launch);
+                       });
 }
 
 int32_t astroz_cuda_fit_elements(const double *elements, uint32_t n, int32_t grav, const uint32_t *offsets,
@@ -2700,7 +2770,8 @@ static_assert(ASTROZ_OBS_TEME_STATE == az::kObsTemeState && ASTROZ_OBS_ECEF_STAT
 static int32_t fit_obs_check(uint32_t n, int32_t grav, int32_t fit_bstar, uint32_t max_iter, int32_t device,
                              az::FitObsArgs *a) {
     if (device < 0) return value_error("an element fit runs on one device: pass its ordinal");
-    if (grav != ASTROZ_WGS72 && grav != ASTROZ_WGS84) return value_error("grav must be ASTROZ_WGS72 or ASTROZ_WGS84");
+    const int32_t rc = grav_check(grav);
+    if (rc != ASTROZ_OK) return rc;
     if (max_iter == 0) return value_error("max_iter must be at least 1");
     a->n = n;
     a->grav = grav;
@@ -2748,6 +2819,31 @@ static cudaError_t launch_fit_obs_mixed(const az::FitObsArgs &a, cudaStream_t st
 }
 using FitObsLaunch = cudaError_t (*)(const az::FitObsArgs &a, cudaStream_t stream);
 
+// Both call forms: a holds fit_obs_check's scalars, the arrays are on the device, launch(a, st) queues the kernels.
+static cudaError_t fit_obs_run(az::FitObsArgs a, const double *elements, const uint32_t *offsets, const double *jd,
+                               const double *fr, const double *value, const double *sigma, const uint32_t *station,
+                               const uint8_t *kind, const double *stations, double *fitted, double *wrms,
+                               uint32_t *n_residuals, double *covariance, uint32_t *iterations, uint8_t *status,
+                               uint8_t *model, cudaStream_t st, FitObsLaunch launch) {
+    a.elements = elements;
+    a.offsets = offsets;
+    a.jd = jd;
+    a.fr = fr;
+    a.value = value;
+    a.sigma = sigma;
+    a.station = station;
+    a.kind = kind;
+    a.stations = stations;
+    a.fitted = fitted;
+    a.wrms = wrms;
+    a.nResiduals = n_residuals;
+    a.covariance = covariance;
+    a.iterations = iterations;
+    a.status = status;
+    a.model = model;
+    return launch(a, st);
+}
+
 static int32_t fit_obs_device(const double *d_elements, uint32_t n, int32_t grav, const uint32_t *d_offsets,
                               const double *d_jd, const double *d_fr, const double *d_value, const double *d_sigma,
                               const uint32_t *d_station, const uint8_t *d_kind, const double *d_stations,
@@ -2763,44 +2859,12 @@ static int32_t fit_obs_device(const double *d_elements, uint32_t n, int32_t grav
         return ASTROZ_NULL_POINTER;
     if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
     AZ_CUDA(cudaSetDevice(device));
-    a.elements = d_elements;
-    a.offsets = d_offsets;
-    a.jd = d_jd;
-    a.fr = d_fr;
-    a.value = d_value;
-    a.sigma = d_sigma;
-    a.station = d_station;
-    a.kind = d_kind;
-    a.stations = d_stations;
-    a.fitted = d_fitted;
-    a.wrms = d_wrms;
-    a.nResiduals = d_n_residuals;
-    a.covariance = d_covariance;
-    a.iterations = d_iterations;
-    a.status = d_status;
-    a.model = d_model;
-    AZ_CUDA(launch(a, static_cast<cudaStream_t>(stream)));
+    AZ_CUDA(fit_obs_run(a, d_elements, d_offsets, d_jd, d_fr, d_value, d_sigma, d_station, d_kind, d_stations,
+                        d_fitted, d_wrms, d_n_residuals, d_covariance, d_iterations, d_status, d_model,
+                        static_cast<cudaStream_t>(stream), launch));
     return ASTROZ_OK;
 }
 
-// A stream-ordered device block cut into 16-byte aligned pieces of the given byte sizes.
-struct DeviceBlock {
-    StreamBuf buf;
-    std::vector<size_t> at;
-    explicit DeviceBlock(cudaStream_t s) : buf(s) {}
-    cudaError_t alloc(std::initializer_list<size_t> bytes) {
-        size_t total = 0;
-        for (size_t b : bytes) at.push_back(total), total += (b + 15) & ~size_t(15);
-        return buf.alloc(std::max<size_t>(total, 16));
-    }
-    char *piece(int k) { return static_cast<char *>(buf.p) + at[k]; }
-    double *f64(int k) { return reinterpret_cast<double *>(piece(k)); }
-    uint32_t *u32(int k) { return reinterpret_cast<uint32_t *>(piece(k)); }
-    uint8_t *u8(int k) { return reinterpret_cast<uint8_t *>(piece(k)); }
-};
-
-// Host buffers: as fit_host -- the inputs go up once (pageable through the pinned ring, pinned by direct DMA), the
-// launch fits the batch, and the results come back by plain copies.
 static int32_t fit_obs_host(const double *elements, uint32_t n, int32_t grav, const uint32_t *offsets,
                             const double *jd, const double *fr, const double *value, const double *sigma,
                             const uint32_t *station, const uint8_t *kind, uint32_t m, const double *stations,
@@ -2814,66 +2878,22 @@ static int32_t fit_obs_host(const double *elements, uint32_t n, int32_t grav, co
     if (!elements || !offsets || !fitted || !wrms || !n_residuals || !covariance || !iterations || !status || !model)
         return ASTROZ_NULL_POINTER;
     if (m && (!jd || !fr || !value || !sigma || !kind)) return ASTROZ_NULL_POINTER;
-    for (uint32_t s = 0; s < n; ++s)
-        if (offsets[s + 1] < offsets[s]) return value_error("offsets must be non-decreasing");
-    if (offsets[n] != m) return value_error("offsets[n] must equal the observation count m");
-    if (!all_finite(elements, (size_t)8 * n)) return value_error("elements must be finite");
+    if ((rc = offsets_check(offsets, n, m, "offsets[n] must equal the observation count m")) != ASTROZ_OK) return rc;
+    if ((rc = rows_check(elements, nullptr, n)) != ASTROZ_OK) return rc;
     if ((rc = obs_values_check(jd, fr, value, sigma, station, kind, m, stations, k)) != ASTROZ_OK) return rc;
-    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
-    NumericalContext *c = nullptr;
-    if ((rc = numerical_context(device, &c)) != ASTROZ_OK) return rc;
-    std::lock_guard<std::mutex> lk(c->m);
-    AZ_CUDA(cudaSetDevice(device));
-    cudaStream_t st = c->stream;
-    // elements | offsets | jd | fr | value | sigma | station | kind | stations | fitted | wrms | n_res | cov | iter |
-    // status | model
-    DeviceBlock d(st);
-    AZ_CUDA(d.alloc({(size_t)64 * n, (size_t)4 * (n + 1), (size_t)8 * m, (size_t)8 * m, (size_t)48 * m,
-                     (size_t)48 * m, station ? (size_t)4 * m : 0, (size_t)m, (size_t)24 * k, (size_t)64 * n,
-                     (size_t)8 * n, (size_t)4 * n, (size_t)8 * az::kFitN * n, (size_t)4 * n, (size_t)n, (size_t)n}));
-    auto up = [&](const void *src, void *dst, size_t elemBytes, size_t count) {
-        void *const dd[1] = {dst};
-        const void *const ss[1] = {src};
-        return c->pipe.ring.upload(az::is_pageable(src), 1, ss, dd, &elemBytes, count, st);
-    };
-    AZ_CUDA(up(elements, d.f64(0), 8, (size_t)8 * n));
-    AZ_CUDA(up(offsets, d.u32(1), 4, (size_t)n + 1));
-    if (m) {
-        AZ_CUDA(up(jd, d.f64(2), 8, m));
-        AZ_CUDA(up(fr, d.f64(3), 8, m));
-        AZ_CUDA(up(value, d.f64(4), 48, m));
-        AZ_CUDA(up(sigma, d.f64(5), 48, m));
-        if (station) AZ_CUDA(up(station, d.u32(6), 4, m));
-        AZ_CUDA(up(kind, d.u8(7), 1, m));
-    }
-    if (k) AZ_CUDA(up(stations, d.f64(8), 24, k));
-    a.elements = d.f64(0);
-    a.offsets = d.u32(1);
-    a.jd = d.f64(2);
-    a.fr = d.f64(3);
-    a.value = d.f64(4);
-    a.sigma = d.f64(5);
-    a.station = station ? d.u32(6) : nullptr;
-    a.kind = d.u8(7);
-    a.stations = k ? d.f64(8) : nullptr;
-    a.fitted = d.f64(9);
-    a.wrms = d.f64(10);
-    a.nResiduals = d.u32(11);
-    a.covariance = d.f64(12);
-    a.iterations = d.u32(13);
-    a.status = d.u8(14);
-    a.model = d.u8(15);
-    AZ_CUDA(launch(a, st));
-    AZ_CUDA(cudaMemcpyAsync(fitted, a.fitted, (size_t)64 * n, cudaMemcpyDeviceToHost, st));
-    AZ_CUDA(cudaMemcpyAsync(wrms, a.wrms, (size_t)8 * n, cudaMemcpyDeviceToHost, st));
-    AZ_CUDA(cudaMemcpyAsync(n_residuals, a.nResiduals, (size_t)4 * n, cudaMemcpyDeviceToHost, st));
-    AZ_CUDA(cudaMemcpyAsync(covariance, a.covariance, (size_t)8 * az::kFitN * n, cudaMemcpyDeviceToHost, st));
-    AZ_CUDA(cudaMemcpyAsync(iterations, a.iterations, (size_t)4 * n, cudaMemcpyDeviceToHost, st));
-    AZ_CUDA(cudaMemcpyAsync(status, a.status, n, cudaMemcpyDeviceToHost, st));
-    AZ_CUDA(cudaMemcpyAsync(model, a.model, n, cudaMemcpyDeviceToHost, st));
-    AZ_CUDA(d.buf.release());
-    AZ_CUDA(cudaStreamSynchronize(st));
-    return ASTROZ_OK;
+    return whole_batch(device,
+                       {upload(elements, (size_t)64 * n), upload(offsets, (size_t)4 * (n + 1)), upload(jd, (size_t)8 * m),
+                        upload(fr, (size_t)8 * m), upload(value, (size_t)48 * m), upload(sigma, (size_t)48 * m),
+                        upload(station, station ? (size_t)4 * m : 0), upload(kind, m), upload(stations, (size_t)24 * k),
+                        result(fitted, (size_t)64 * n), result(wrms, (size_t)8 * n), result(n_residuals, (size_t)4 * n),
+                        result(covariance, (size_t)8 * az::kFitN * n), result(iterations, (size_t)4 * n),
+                        result(status, n), result(model, n)},
+                       [&](const DeviceBlock &d, cudaStream_t st) {
+                           return fit_obs_run(a, d.f64(0), d.u32(1), d.f64(2), d.f64(3), d.f64(4), d.f64(5),
+                                              station ? d.u32(6) : nullptr, d.u8(7), k ? d.f64(8) : nullptr, d.f64(9),
+                                              d.f64(10), d.u32(11), d.f64(12), d.u32(13), d.u8(14), d.u8(15), st,
+                                              launch);
+                       });
 }
 
 int32_t astroz_cuda_fit_observations(const double *elements, uint32_t n, int32_t grav, const uint32_t *offsets,
@@ -2931,36 +2951,17 @@ int32_t astroz_cuda_observe(const double *states, const double *jd, const double
     if (device < 0) return value_error("observe runs on one device: pass its ordinal");
     if (m == 0) return ASTROZ_OK;
     if (!states || !jd || !fr || !kind || !values) return ASTROZ_NULL_POINTER;
-    int32_t rc = obs_values_check(jd, fr, nullptr, nullptr, station, kind, m, stations, k);
+    const int32_t rc = obs_values_check(jd, fr, nullptr, nullptr, station, kind, m, stations, k);
     if (rc != ASTROZ_OK) return rc;
-    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
-    NumericalContext *c = nullptr;
-    if ((rc = numerical_context(device, &c)) != ASTROZ_OK) return rc;
-    std::lock_guard<std::mutex> lk(c->m);
-    AZ_CUDA(cudaSetDevice(device));
-    cudaStream_t st = c->stream;
-    // states | jd | fr | kind | station | stations | values
-    DeviceBlock d(st);
-    AZ_CUDA(d.alloc({(size_t)48 * m, (size_t)8 * m, (size_t)8 * m, (size_t)m, station ? (size_t)4 * m : 0,
-                     (size_t)24 * k, (size_t)48 * m}));
-    auto up = [&](const void *src, void *dst, size_t elemBytes, size_t count) {
-        void *const dd[1] = {dst};
-        const void *const ss[1] = {src};
-        return c->pipe.ring.upload(az::is_pageable(src), 1, ss, dd, &elemBytes, count, st);
-    };
-    AZ_CUDA(up(states, d.f64(0), 48, m));
-    AZ_CUDA(up(jd, d.f64(1), 8, m));
-    AZ_CUDA(up(fr, d.f64(2), 8, m));
-    AZ_CUDA(up(kind, d.u8(3), 1, m));
-    if (station) AZ_CUDA(up(station, d.u32(4), 4, m));
-    if (k) AZ_CUDA(up(stations, d.f64(5), 24, k));
-    AZ_CUDA(az::launch_observe(d.f64(0), d.f64(1), d.f64(2), d.u8(3),
-                               station ? d.u32(4) : nullptr, k ? d.f64(5) : nullptr, m,
-                               d.f64(6), st));
-    AZ_CUDA(cudaMemcpyAsync(values, d.f64(6), (size_t)48 * m, cudaMemcpyDeviceToHost, st));
-    AZ_CUDA(d.buf.release());
-    AZ_CUDA(cudaStreamSynchronize(st));
-    return ASTROZ_OK;
+    return whole_batch(device,
+                       {upload(states, (size_t)48 * m), upload(jd, (size_t)8 * m), upload(fr, (size_t)8 * m),
+                        upload(kind, m), upload(station, station ? (size_t)4 * m : 0), upload(stations, (size_t)24 * k),
+                        result(values, (size_t)48 * m)},
+                       [&](const DeviceBlock &d, cudaStream_t st) {
+                           return az::launch_observe(d.f64(0), d.f64(1), d.f64(2), d.u8(3),
+                                                     station ? d.u32(4) : nullptr, k ? d.f64(5) : nullptr, m,
+                                                     d.f64(6), st);
+                       });
 }
 
 int32_t astroz_cuda_observe_device(const double *d_states, const double *d_jd, const double *d_fr,
@@ -2986,7 +2987,8 @@ static_assert(ASTROZ_COV_OK == az::kCovOk && ASTROZ_COV_INIT_FAILED == az::kCovI
 // Scalar checks of the covariance calls, before anything is read, written or allocated; a receives the scalars.
 static int32_t cov_check(uint32_t n, int32_t grav, uint32_t m, int32_t frame, int32_t device, az::CovArgs *a) {
     if (device < 0) return value_error("covariance propagation runs on one device: pass its ordinal");
-    if (grav != ASTROZ_WGS72 && grav != ASTROZ_WGS84) return value_error("grav must be ASTROZ_WGS72 or ASTROZ_WGS84");
+    const int32_t rc = grav_check(grav);
+    if (rc != ASTROZ_OK) return rc;
     if (frame != ASTROZ_COV_FRAME_TEME && frame != ASTROZ_COV_FRAME_RTN)
         return value_error("frame must be ASTROZ_COV_FRAME_TEME or ASTROZ_COV_FRAME_RTN");
     a->n = n;
@@ -2995,6 +2997,23 @@ static int32_t cov_check(uint32_t n, int32_t grav, uint32_t m, int32_t frame, in
     a->g = az::grav_consts(az::gravity(grav));
     a->frame = frame;
     return ASTROZ_OK;
+}
+
+// Both call forms: a holds cov_check's scalars, the arrays are on the device.
+static cudaError_t cov_run(az::CovArgs a, const double *elements, const double *covariance, const uint8_t *model,
+                           const uint32_t *offsets, const double *jd, const double *fr, double *state,
+                           double *state_covariance, double *jacobian, uint8_t *status, cudaStream_t st) {
+    a.elements = elements;
+    a.covariance = covariance;
+    a.model = model;
+    a.offsets = offsets;
+    a.jd = jd;
+    a.fr = fr;
+    a.state = state;
+    a.sigma = state_covariance;
+    a.jacobian = jacobian;
+    a.status = status;
+    return az::launch_covariance(a, st);
 }
 
 int32_t astroz_cuda_propagate_covariance_device(const double *d_elements, uint32_t n, int32_t grav,
@@ -3011,22 +3030,11 @@ int32_t astroz_cuda_propagate_covariance_device(const double *d_elements, uint32
         return ASTROZ_NULL_POINTER;
     if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
     AZ_CUDA(cudaSetDevice(device));
-    a.elements = d_elements;
-    a.covariance = d_covariance;
-    a.model = d_model;
-    a.offsets = d_offsets;
-    a.jd = d_jd;
-    a.fr = d_fr;
-    a.state = d_state;
-    a.sigma = d_state_covariance;
-    a.jacobian = d_jacobian;
-    a.status = d_status;
-    AZ_CUDA(az::launch_covariance(a, static_cast<cudaStream_t>(stream)));
+    AZ_CUDA(cov_run(a, d_elements, d_covariance, d_model, d_offsets, d_jd, d_fr, d_state, d_state_covariance,
+                    d_jacobian, d_status, static_cast<cudaStream_t>(stream)));
     return ASTROZ_OK;
 }
 
-// Host buffers: as fit_obs_host -- the inputs go up once (pageable through the pinned ring, pinned by direct DMA), the
-// two launches run on the device's stream, and the results come back by plain copies.
 int32_t astroz_cuda_propagate_covariance(const double *elements, uint32_t n, int32_t grav, const double *covariance,
                                          const uint8_t *model, const uint32_t *offsets, const double *jd,
                                          const double *fr, uint32_t m, int32_t frame, int32_t device, double *state,
@@ -3037,58 +3045,22 @@ int32_t astroz_cuda_propagate_covariance(const double *elements, uint32_t n, int
     if (!offsets) return ASTROZ_NULL_POINTER;
     if (n && (!elements || !covariance)) return ASTROZ_NULL_POINTER;
     if (m && (!jd || !fr || !state_covariance || !status)) return ASTROZ_NULL_POINTER;
-    if (offsets[0] != 0) return value_error("offsets[0] must be 0");
-    for (uint32_t s = 0; s < n; ++s)
-        if (offsets[s + 1] < offsets[s]) return value_error("offsets must be non-decreasing");
-    if (offsets[n] != m) return value_error("offsets[n] must equal the query count m");
-    if (!all_finite(elements, (size_t)8 * n)) return value_error("elements must be finite");
-    if (!all_finite(covariance, (size_t)az::kFitN * n)) return value_error("covariance words must be finite");
+    if ((rc = offsets_check(offsets, n, m, "offsets[n] must equal the query count m", true)) != ASTROZ_OK) return rc;
+    if ((rc = rows_check(elements, covariance, n)) != ASTROZ_OK) return rc;
     if (!all_finite(jd, m) || !all_finite(fr, m)) return value_error("query times must be finite");
-    if (model)
-        for (uint32_t s = 0; s < n; ++s)
-            if (model[s] > 1) return value_error("a model byte is not 0 (near-earth) or 1 (deep space)");
+    if ((rc = model_bytes_check(model, n)) != ASTROZ_OK) return rc;
     if (n == 0 || m == 0) return ASTROZ_OK;
-    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
-    NumericalContext *c = nullptr;
-    if ((rc = numerical_context(device, &c)) != ASTROZ_OK) return rc;
-    std::lock_guard<std::mutex> lk(c->m);
-    AZ_CUDA(cudaSetDevice(device));
-    cudaStream_t st = c->stream;
-    // elements | covariance | model | offsets | jd | fr | state | state_covariance | jacobian | status
-    DeviceBlock d(st);
-    AZ_CUDA(d.alloc({(size_t)64 * n, (size_t)8 * az::kFitN * n, model ? (size_t)n : 0, (size_t)4 * (n + 1),
-                     (size_t)8 * m, (size_t)8 * m, state ? (size_t)48 * m : 0, (size_t)8 * az::kCovWords * m,
-                     jacobian ? (size_t)8 * az::kCovJacWords * m : 0, (size_t)m}));
-    auto up = [&](const void *src, void *dst, size_t elemBytes, size_t count) {
-        void *const dd[1] = {dst};
-        const void *const ss[1] = {src};
-        return c->pipe.ring.upload(az::is_pageable(src), 1, ss, dd, &elemBytes, count, st);
-    };
-    AZ_CUDA(up(elements, d.f64(0), 8, (size_t)8 * n));
-    AZ_CUDA(up(covariance, d.f64(1), 8 * az::kFitN, n));
-    if (model) AZ_CUDA(up(model, d.u8(2), 1, n));
-    AZ_CUDA(up(offsets, d.u32(3), 4, (size_t)n + 1));
-    AZ_CUDA(up(jd, d.f64(4), 8, m));
-    AZ_CUDA(up(fr, d.f64(5), 8, m));
-    a.elements = d.f64(0);
-    a.covariance = d.f64(1);
-    a.model = model ? d.u8(2) : nullptr;
-    a.offsets = d.u32(3);
-    a.jd = d.f64(4);
-    a.fr = d.f64(5);
-    a.state = state ? d.f64(6) : nullptr;
-    a.sigma = d.f64(7);
-    a.jacobian = jacobian ? d.f64(8) : nullptr;
-    a.status = d.u8(9);
-    AZ_CUDA(az::launch_covariance(a, st));
-    if (state) AZ_CUDA(cudaMemcpyAsync(state, a.state, (size_t)48 * m, cudaMemcpyDeviceToHost, st));
-    AZ_CUDA(cudaMemcpyAsync(state_covariance, a.sigma, (size_t)8 * az::kCovWords * m, cudaMemcpyDeviceToHost, st));
-    if (jacobian)
-        AZ_CUDA(cudaMemcpyAsync(jacobian, a.jacobian, (size_t)8 * az::kCovJacWords * m, cudaMemcpyDeviceToHost, st));
-    AZ_CUDA(cudaMemcpyAsync(status, a.status, m, cudaMemcpyDeviceToHost, st));
-    AZ_CUDA(d.buf.release());
-    AZ_CUDA(cudaStreamSynchronize(st));
-    return ASTROZ_OK;
+    return whole_batch(device,
+                       {upload(elements, (size_t)64 * n), upload(covariance, (size_t)8 * az::kFitN * n),
+                        upload(model, model ? (size_t)n : 0), upload(offsets, (size_t)4 * (n + 1)),
+                        upload(jd, (size_t)8 * m), upload(fr, (size_t)8 * m), result(state, state ? (size_t)48 * m : 0),
+                        result(state_covariance, (size_t)8 * az::kCovWords * m),
+                        result(jacobian, jacobian ? (size_t)8 * az::kCovJacWords * m : 0), result(status, m)},
+                       [&](const DeviceBlock &d, cudaStream_t st) {
+                           return cov_run(a, d.f64(0), d.f64(1), model ? d.u8(2) : nullptr, d.u32(3), d.f64(4),
+                                          d.f64(5), state ? d.f64(6) : nullptr, d.f64(7),
+                                          jacobian ? d.f64(8) : nullptr, d.u8(9), st);
+                       });
 }
 
 // ---- conjunction assessment (K11, az_conjunction.cu, az_conjunction.cuh) -------------------------------------------
@@ -3101,7 +3073,8 @@ static_assert(ASTROZ_CONJ_OK == az::kConjOk && ASTROZ_CONJ_INIT_FAILED == az::kC
 // Scalar checks of the conjunction calls, before anything is read, written or allocated; a receives the scalars.
 static int32_t conj_check(uint32_t n, int32_t grav, uint32_t m, int32_t frame, int32_t device, az::ConjArgs *a) {
     if (device < 0) return value_error("conjunction assessment runs on one device: pass its ordinal");
-    if (grav != ASTROZ_WGS72 && grav != ASTROZ_WGS84) return value_error("grav must be ASTROZ_WGS72 or ASTROZ_WGS84");
+    const int32_t rc = grav_check(grav);
+    if (rc != ASTROZ_OK) return rc;
     if (frame != ASTROZ_COV_FRAME_TEME && frame != ASTROZ_COV_FRAME_RTN)
         return value_error("frame must be ASTROZ_COV_FRAME_TEME or ASTROZ_COV_FRAME_RTN");
     a->n = n;
@@ -3110,6 +3083,27 @@ static int32_t conj_check(uint32_t n, int32_t grav, uint32_t m, int32_t frame, i
     a->g = az::grav_consts(az::gravity(grav));
     a->frame = frame;
     return ASTROZ_OK;
+}
+
+// Both call forms: a holds conj_check's scalars, the arrays are on the device.
+static cudaError_t conj_run(az::ConjArgs a, const double *elements, const double *covariance, const uint8_t *model,
+                            const uint32_t *primary, const uint32_t *secondary, const double *jd, const double *fr,
+                            const double *window_min, const double *hbr_km, double *record, double *states,
+                            double *state_covariance, uint8_t *status, cudaStream_t st) {
+    a.elements = elements;
+    a.covariance = covariance;
+    a.model = model;
+    a.primary = primary;
+    a.secondary = secondary;
+    a.jd = jd;
+    a.fr = fr;
+    a.window = window_min;
+    a.hbr = hbr_km;
+    a.record = record;
+    a.states = states;
+    a.sigma = state_covariance;
+    a.status = status;
+    return az::launch_conjunction(a, st);
 }
 
 int32_t astroz_cuda_conjunction_device(const double *d_elements, uint32_t n, int32_t grav, const double *d_covariance,
@@ -3127,25 +3121,11 @@ int32_t astroz_cuda_conjunction_device(const double *d_elements, uint32_t n, int
         return ASTROZ_NULL_POINTER;
     if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
     AZ_CUDA(cudaSetDevice(device));
-    a.elements = d_elements;
-    a.covariance = d_covariance;
-    a.model = d_model;
-    a.primary = d_primary;
-    a.secondary = d_secondary;
-    a.jd = d_jd;
-    a.fr = d_fr;
-    a.window = d_window_min;
-    a.hbr = d_hbr_km;
-    a.record = d_record;
-    a.states = d_states;
-    a.sigma = d_state_covariance;
-    a.status = d_status;
-    AZ_CUDA(az::launch_conjunction(a, static_cast<cudaStream_t>(stream)));
+    AZ_CUDA(conj_run(a, d_elements, d_covariance, d_model, d_primary, d_secondary, d_jd, d_fr, d_window_min, d_hbr_km,
+                     d_record, d_states, d_state_covariance, d_status, static_cast<cudaStream_t>(stream)));
     return ASTROZ_OK;
 }
 
-// Host buffers: as astroz_cuda_propagate_covariance -- the inputs go up once (pageable through the pinned ring, pinned
-// by direct DMA), the two launches run on the device's stream, and the results come back by plain copies.
 int32_t astroz_cuda_conjunction(const double *elements, uint32_t n, int32_t grav, const double *covariance,
                                 const uint8_t *model, const uint32_t *primary, const uint32_t *secondary,
                                 const double *jd, const double *fr, const double *window_min, const double *hbr_km,
@@ -3165,60 +3145,25 @@ int32_t astroz_cuda_conjunction(const double *elements, uint32_t n, int32_t grav
         if (!(hbr_km[i] >= 0.0) || !std::isfinite(hbr_km[i]))
             return value_error("hard-body radii must be finite and >= 0 km");
     }
-    if (!all_finite(elements, (size_t)8 * n)) return value_error("elements must be finite");
-    if (!all_finite(covariance, (size_t)az::kFitN * n)) return value_error("covariance words must be finite");
+    if ((rc = rows_check(elements, covariance, n)) != ASTROZ_OK) return rc;
     if (!all_finite(jd, m) || !all_finite(fr, m)) return value_error("guess times must be finite");
-    if (model)
-        for (uint32_t s = 0; s < n; ++s)
-            if (model[s] > 1) return value_error("a model byte is not 0 (near-earth) or 1 (deep space)");
+    if ((rc = model_bytes_check(model, n)) != ASTROZ_OK) return rc;
     if (m == 0) return ASTROZ_OK;
-    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
-    NumericalContext *c = nullptr;
-    if ((rc = numerical_context(device, &c)) != ASTROZ_OK) return rc;
-    std::lock_guard<std::mutex> lk(c->m);
-    AZ_CUDA(cudaSetDevice(device));
-    cudaStream_t st = c->stream;
-    // elements | covariance | model | primary | secondary | jd | fr | window | hbr | record | states | sigma | status
-    DeviceBlock d(st);
-    AZ_CUDA(d.alloc({(size_t)64 * n, (size_t)8 * az::kFitN * n, model ? (size_t)n : 0, (size_t)4 * m, (size_t)4 * m,
-                     (size_t)8 * m, (size_t)8 * m, (size_t)8 * m, (size_t)8 * m, (size_t)8 * az::kConjRecordWords * m,
-                     states ? (size_t)96 * m : 0, state_covariance ? (size_t)16 * az::kCovWords * m : 0, (size_t)m}));
-    auto up = [&](const void *src, void *dst, size_t elemBytes, size_t count) {
-        void *const dd[1] = {dst};
-        const void *const ss[1] = {src};
-        return c->pipe.ring.upload(az::is_pageable(src), 1, ss, dd, &elemBytes, count, st);
-    };
-    AZ_CUDA(up(elements, d.f64(0), 8, (size_t)8 * n));
-    AZ_CUDA(up(covariance, d.f64(1), 8 * az::kFitN, n));
-    if (model) AZ_CUDA(up(model, d.u8(2), 1, n));
-    AZ_CUDA(up(primary, d.u32(3), 4, m));
-    AZ_CUDA(up(secondary, d.u32(4), 4, m));
-    AZ_CUDA(up(jd, d.f64(5), 8, m));
-    AZ_CUDA(up(fr, d.f64(6), 8, m));
-    AZ_CUDA(up(window_min, d.f64(7), 8, m));
-    AZ_CUDA(up(hbr_km, d.f64(8), 8, m));
-    a.elements = d.f64(0);
-    a.covariance = d.f64(1);
-    a.model = model ? d.u8(2) : nullptr;
-    a.primary = d.u32(3);
-    a.secondary = d.u32(4);
-    a.jd = d.f64(5);
-    a.fr = d.f64(6);
-    a.window = d.f64(7);
-    a.hbr = d.f64(8);
-    a.record = d.f64(9);
-    a.states = states ? d.f64(10) : nullptr;
-    a.sigma = state_covariance ? d.f64(11) : nullptr;
-    a.status = d.u8(12);
-    AZ_CUDA(az::launch_conjunction(a, st));
-    AZ_CUDA(cudaMemcpyAsync(record, a.record, (size_t)8 * az::kConjRecordWords * m, cudaMemcpyDeviceToHost, st));
-    if (states) AZ_CUDA(cudaMemcpyAsync(states, a.states, (size_t)96 * m, cudaMemcpyDeviceToHost, st));
-    if (state_covariance)
-        AZ_CUDA(cudaMemcpyAsync(state_covariance, a.sigma, (size_t)16 * az::kCovWords * m, cudaMemcpyDeviceToHost, st));
-    AZ_CUDA(cudaMemcpyAsync(status, a.status, m, cudaMemcpyDeviceToHost, st));
-    AZ_CUDA(d.buf.release());
-    AZ_CUDA(cudaStreamSynchronize(st));
-    return ASTROZ_OK;
+    return whole_batch(device,
+                       {upload(elements, (size_t)64 * n), upload(covariance, (size_t)8 * az::kFitN * n),
+                        upload(model, model ? (size_t)n : 0), upload(primary, (size_t)4 * m),
+                        upload(secondary, (size_t)4 * m), upload(jd, (size_t)8 * m), upload(fr, (size_t)8 * m),
+                        upload(window_min, (size_t)8 * m), upload(hbr_km, (size_t)8 * m),
+                        result(record, (size_t)8 * az::kConjRecordWords * m),
+                        result(states, states ? (size_t)96 * m : 0),
+                        result(state_covariance, state_covariance ? (size_t)16 * az::kCovWords * m : 0),
+                        result(status, m)},
+                       [&](const DeviceBlock &d, cudaStream_t st) {
+                           return conj_run(a, d.f64(0), d.f64(1), model ? d.u8(2) : nullptr, d.u32(3), d.u32(4),
+                                           d.f64(5), d.f64(6), d.f64(7), d.f64(8), d.f64(9),
+                                           states ? d.f64(10) : nullptr, state_covariance ? d.f64(11) : nullptr,
+                                           d.u8(12), st);
+                       });
 }
 
 // ---- track correlation (K12, az_correlate.cu, az_correlate.cuh) -------------------------------------------------------
@@ -3231,7 +3176,8 @@ static_assert(ASTROZ_CORR_OK == az::kCorrOk && ASTROZ_CORR_UNCORRELATED == az::k
 static int32_t corr_check(uint32_t n, int32_t grav, uint32_t t, double gate_probability, uint32_t best,
                           int32_t device, az::CorrArgs *a) {
     if (device < 0) return value_error("track correlation runs on one device: pass its ordinal");
-    if (grav != ASTROZ_WGS72 && grav != ASTROZ_WGS84) return value_error("grav must be ASTROZ_WGS72 or ASTROZ_WGS84");
+    const int32_t rc = grav_check(grav);
+    if (rc != ASTROZ_OK) return rc;
     if (best < 1 || best > (uint32_t)az::kCorrMaxBest) return value_error("best must be in [1, ASTROZ_CORR_MAX_BEST]");
     if (!(gate_probability > 0.0 && gate_probability < 1.0)) return value_error("gate_probability must be in (0, 1)");
     a->n = n;
@@ -3257,21 +3203,33 @@ int32_t astroz_cuda_chi2_quantile(uint32_t k, double p, double *x) {
     return ASTROZ_OK;
 }
 
-static void corr_device_args(az::CorrArgs &a, const double *d_elements, const double *d_covariance,
-                             const uint8_t *d_model, const uint32_t *d_offsets, const double *d_jd, const double *d_fr,
-                             const uint8_t *d_kind, const double *d_value, const double *d_sigma,
-                             const uint32_t *d_station, const double *d_stations) {
-    a.elements = d_elements;
-    a.covariance = d_covariance;
-    a.model = d_model;
-    a.offsets = d_offsets;
-    a.jd = d_jd;
-    a.fr = d_fr;
-    a.kind = d_kind;
-    a.value = d_value;
-    a.sigma = d_sigma;
-    a.station = d_station;
-    a.stations = d_stations;
+// Both call forms: a holds corr_check's scalars, the arrays and the scratch are on the device.
+static cudaError_t corr_run(az::CorrArgs a, const double *elements, const double *covariance, const uint8_t *model,
+                            const uint32_t *offsets, const double *jd, const double *fr, const uint8_t *kind,
+                            const double *value, const double *sigma, const uint32_t *station,
+                            const double *stations, void *scratch, uint32_t *rows, double *d2, uint32_t *used,
+                            uint32_t *n_gate, uint32_t *n_failed, uint8_t *status, uint8_t *row_status,
+                            cudaStream_t st) {
+    a.elements = elements;
+    a.covariance = covariance;
+    a.model = model;
+    a.offsets = offsets;
+    a.jd = jd;
+    a.fr = fr;
+    a.kind = kind;
+    a.value = value;
+    a.sigma = sigma;
+    a.station = station;
+    a.stations = stations;
+    a.scratch = scratch;
+    a.rows = rows;
+    a.d2 = d2;
+    a.used = used;
+    a.nGate = n_gate;
+    a.nFailed = n_failed;
+    a.status = status;
+    a.rowStatus = row_status;
+    return az::launch_correlate(a, st);
 }
 
 int32_t astroz_cuda_correlate_device(const double *d_elements, uint32_t n, int32_t grav, const double *d_covariance,
@@ -3292,23 +3250,12 @@ int32_t astroz_cuda_correlate_device(const double *d_elements, uint32_t n, int32
         return ASTROZ_NULL_POINTER;
     if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
     AZ_CUDA(cudaSetDevice(device));
-    corr_device_args(a, d_elements, d_covariance, d_model, d_offsets, d_jd, d_fr, d_kind, d_value, d_sigma, d_station,
-                     d_stations);
-    a.scratch = d_scratch;
-    a.rows = d_rows;
-    a.d2 = d_d2;
-    a.used = d_used;
-    a.nGate = d_n_gate;
-    a.nFailed = d_n_failed;
-    a.status = d_status;
-    a.rowStatus = d_row_status;
-    AZ_CUDA(az::launch_correlate(a, static_cast<cudaStream_t>(stream)));
+    AZ_CUDA(corr_run(a, d_elements, d_covariance, d_model, d_offsets, d_jd, d_fr, d_kind, d_value, d_sigma, d_station,
+                     d_stations, d_scratch, d_rows, d_d2, d_used, d_n_gate, d_n_failed, d_status, d_row_status,
+                     static_cast<cudaStream_t>(stream)));
     return ASTROZ_OK;
 }
 
-// Host buffers: as astroz_cuda_conjunction -- the inputs go up once (pageable through the pinned ring, pinned by direct
-// DMA), the launches run on the device's stream with the scratch in the same device block, and the results come back
-// by plain copies.
 int32_t astroz_cuda_correlate(const double *elements, uint32_t n, int32_t grav, const double *covariance,
                               const uint8_t *model, const uint32_t *offsets, uint32_t t, const double *jd,
                               const double *fr, const uint8_t *kind, const double *value, const double *sigma,
@@ -3323,82 +3270,32 @@ int32_t astroz_cuda_correlate(const double *elements, uint32_t n, int32_t grav, 
     if (n && (!elements || !row_status)) return ASTROZ_NULL_POINTER;
     if (t && (!rows || !d2 || !used || !n_gate || !n_failed || !status)) return ASTROZ_NULL_POINTER;
     if (m && (!jd || !fr || !kind || !value || !sigma)) return ASTROZ_NULL_POINTER;
-    if (offsets[0] != 0) return value_error("offsets[0] must be 0");
-    for (uint32_t j = 0; j < t; ++j) {
-        if (offsets[j + 1] < offsets[j]) return value_error("offsets must be non-decreasing");
-        if (offsets[j + 1] == offsets[j]) return value_error("a track has no observation");
-        if (offsets[j + 1] - offsets[j] > az::kCorrMaxTrack)
-            return value_error("a track is longer than ASTROZ_CORR_MAX_TRACK observations");
-    }
-    if (offsets[t] != m) return value_error("offsets[t] must equal the observation count m");
+    if ((rc = offsets_check(offsets, t, m, "offsets[t] must equal the observation count m", true, az::kCorrMaxTrack,
+                            "a track is longer than ASTROZ_CORR_MAX_TRACK observations")) != ASTROZ_OK)
+        return rc;
     if ((rc = obs_values_check(jd, fr, value, sigma, station, kind, m, stations, k)) != ASTROZ_OK) return rc;
-    {
-        const az::CorrObsArrays in{jd, fr, kind, value, sigma, station, stations};
-        for (uint32_t j = 0; j < t; ++j)
-            if (az::corr_used(in, offsets[j], offsets[j + 1]) == 0) return value_error("a track has no used residual");
-    }
-    if (!all_finite(elements, (size_t)8 * n)) return value_error("elements must be finite");
-    if (covariance && !all_finite(covariance, (size_t)az::kFitN * n))
-        return value_error("covariance words must be finite");
-    if (model)
-        for (uint32_t s = 0; s < n; ++s)
-            if (model[s] > 1) return value_error("a model byte is not 0 (near-earth) or 1 (deep space)");
+    if ((rc = used_residuals_check({jd, fr, kind, value, sigma, station, stations}, offsets, t)) != ASTROZ_OK)
+        return rc;
+    if ((rc = rows_check(elements, covariance, n)) != ASTROZ_OK) return rc;
+    if ((rc = model_bytes_check(model, n)) != ASTROZ_OK) return rc;
     if (n == 0 && t == 0) return ASTROZ_OK;
-    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
-    NumericalContext *c = nullptr;
-    if ((rc = numerical_context(device, &c)) != ASTROZ_OK) return rc;
-    std::lock_guard<std::mutex> lk(c->m);
-    AZ_CUDA(cudaSetDevice(device));
-    cudaStream_t st = c->stream;
-    // elements | covariance | model | offsets | jd | fr | kind | value | sigma | station | stations | scratch | rows |
-    // d2 | used | n_gate | n_failed | status | row_status
-    DeviceBlock d(st);
-    AZ_CUDA(d.alloc({(size_t)64 * n, covariance ? (size_t)8 * az::kFitN * n : 0, model ? (size_t)n : 0,
-                     (size_t)4 * (t + 1), (size_t)8 * m, (size_t)8 * m, (size_t)m, (size_t)48 * m, (size_t)48 * m,
-                     station ? (size_t)4 * m : 0, (size_t)24 * k, az::corr_scratch_bytes(n, t, best),
-                     (size_t)4 * best * t, (size_t)8 * best * t, (size_t)4 * t, (size_t)4 * t, (size_t)4 * t,
-                     (size_t)t, (size_t)n}));
-    auto up = [&](const void *src, void *dst, size_t elemBytes, size_t count) {
-        void *const dd[1] = {dst};
-        const void *const ss[1] = {src};
-        return c->pipe.ring.upload(az::is_pageable(src), 1, ss, dd, &elemBytes, count, st);
-    };
-    if (n) AZ_CUDA(up(elements, d.f64(0), 8, (size_t)8 * n));
-    if (n && covariance) AZ_CUDA(up(covariance, d.f64(1), 8 * az::kFitN, n));
-    if (n && model) AZ_CUDA(up(model, d.u8(2), 1, n));
-    AZ_CUDA(up(offsets, d.u32(3), 4, (size_t)t + 1));
-    if (m) {
-        AZ_CUDA(up(jd, d.f64(4), 8, m));
-        AZ_CUDA(up(fr, d.f64(5), 8, m));
-        AZ_CUDA(up(kind, d.u8(6), 1, m));
-        AZ_CUDA(up(value, d.f64(7), 48, m));
-        AZ_CUDA(up(sigma, d.f64(8), 48, m));
-        if (station) AZ_CUDA(up(station, d.u32(9), 4, m));
-    }
-    if (k) AZ_CUDA(up(stations, d.f64(10), 24, k));
-    corr_device_args(a, d.f64(0), covariance ? d.f64(1) : nullptr, model ? d.u8(2) : nullptr, d.u32(3), d.f64(4),
-                     d.f64(5), d.u8(6), d.f64(7), d.f64(8), station ? d.u32(9) : nullptr, k ? d.f64(10) : nullptr);
-    a.scratch = d.piece(11);
-    a.rows = d.u32(12);
-    a.d2 = d.f64(13);
-    a.used = d.u32(14);
-    a.nGate = d.u32(15);
-    a.nFailed = d.u32(16);
-    a.status = d.u8(17);
-    a.rowStatus = d.u8(18);
-    AZ_CUDA(az::launch_correlate(a, st));
-    if (t) {
-        AZ_CUDA(cudaMemcpyAsync(rows, a.rows, (size_t)4 * best * t, cudaMemcpyDeviceToHost, st));
-        AZ_CUDA(cudaMemcpyAsync(d2, a.d2, (size_t)8 * best * t, cudaMemcpyDeviceToHost, st));
-        AZ_CUDA(cudaMemcpyAsync(used, a.used, (size_t)4 * t, cudaMemcpyDeviceToHost, st));
-        AZ_CUDA(cudaMemcpyAsync(n_gate, a.nGate, (size_t)4 * t, cudaMemcpyDeviceToHost, st));
-        AZ_CUDA(cudaMemcpyAsync(n_failed, a.nFailed, (size_t)4 * t, cudaMemcpyDeviceToHost, st));
-        AZ_CUDA(cudaMemcpyAsync(status, a.status, t, cudaMemcpyDeviceToHost, st));
-    }
-    if (n) AZ_CUDA(cudaMemcpyAsync(row_status, a.rowStatus, n, cudaMemcpyDeviceToHost, st));
-    AZ_CUDA(d.buf.release());
-    AZ_CUDA(cudaStreamSynchronize(st));
-    return ASTROZ_OK;
+    return whole_batch(device,
+                       {upload(elements, (size_t)64 * n),
+                        upload(covariance, covariance ? (size_t)8 * az::kFitN * n : 0),
+                        upload(model, model ? (size_t)n : 0), upload(offsets, (size_t)4 * (t + 1)),
+                        upload(jd, (size_t)8 * m), upload(fr, (size_t)8 * m), upload(kind, m),
+                        upload(value, (size_t)48 * m), upload(sigma, (size_t)48 * m),
+                        upload(station, station ? (size_t)4 * m : 0), upload(stations, (size_t)24 * k),
+                        scratch(az::corr_scratch_bytes(n, t, best)), result(rows, (size_t)4 * best * t),
+                        result(d2, (size_t)8 * best * t), result(used, (size_t)4 * t), result(n_gate, (size_t)4 * t),
+                        result(n_failed, (size_t)4 * t), result(status, t), result(row_status, n)},
+                       [&](const DeviceBlock &d, cudaStream_t st) {
+                           return corr_run(a, d.f64(0), covariance ? d.f64(1) : nullptr, model ? d.u8(2) : nullptr,
+                                           d.u32(3), d.f64(4), d.f64(5), d.u8(6), d.f64(7), d.f64(8),
+                                           station ? d.u32(9) : nullptr, k ? d.f64(10) : nullptr, d.piece(11),
+                                           d.u32(12), d.f64(13), d.u32(14), d.u32(15), d.u32(16), d.u8(17), d.u8(18),
+                                           st);
+                       });
 }
 
 // ---- initial orbits (K13, az_iod.cu, az_iod.cuh) ----------------------------------------------------------------------
@@ -3415,7 +3312,8 @@ static_assert(ASTROZ_IOD_OK == az::kIodOk && ASTROZ_IOD_TOO_FEW == az::kIodTooFe
 // Scalar checks of the initial-orbit calls, before anything is read, written or allocated; a receives the scalars.
 static int32_t iod_check(uint32_t t, int32_t grav, int32_t device, az::IodArgs *a) {
     if (device < 0) return value_error("initial orbit determination runs on one device: pass its ordinal");
-    if (grav != ASTROZ_WGS72 && grav != ASTROZ_WGS84) return value_error("grav must be ASTROZ_WGS72 or ASTROZ_WGS84");
+    const int32_t rc = grav_check(grav);
+    if (rc != ASTROZ_OK) return rc;
     a->t = t;
     a->grav = grav;
     a->g = az::grav_consts(az::gravity(grav));
@@ -3428,8 +3326,22 @@ int32_t astroz_cuda_initial_orbits_scratch_bytes(uint32_t t, uint64_t *bytes) {
     return ASTROZ_OK;
 }
 
-static void iod_outputs(az::IodArgs &a, double *elements, double *state, double *wrms, uint8_t *method,
-                        uint32_t *candidates, double *conv, uint8_t *deep_space, uint8_t *status) {
+// Both call forms: a holds iod_check's scalars, the arrays and the scratch are on the device.
+static cudaError_t iod_run(az::IodArgs a, const uint32_t *offsets, const double *jd, const double *fr,
+                           const uint8_t *kind, const double *value, const double *sigma, const uint32_t *station,
+                           const double *stations, const double *bstar, void *scratch, double *elements,
+                           double *state, double *wrms, uint8_t *method, uint32_t *candidates, double *conv,
+                           uint8_t *deep_space, uint8_t *status, cudaStream_t st) {
+    a.offsets = offsets;
+    a.jd = jd;
+    a.fr = fr;
+    a.kind = kind;
+    a.value = value;
+    a.sigma = sigma;
+    a.station = station;
+    a.stations = stations;
+    a.bstar = bstar;
+    a.scratch = scratch;
     a.elements = elements;
     a.state = state;
     a.wrms = wrms;
@@ -3438,6 +3350,7 @@ static void iod_outputs(az::IodArgs &a, double *elements, double *state, double 
     a.conv = conv;
     a.deepSpace = deep_space;
     a.status = status;
+    return az::launch_iod(a, st);
 }
 
 int32_t astroz_cuda_initial_orbits_device(const uint32_t *d_offsets, uint32_t t, const double *d_jd,
@@ -3456,24 +3369,14 @@ int32_t astroz_cuda_initial_orbits_device(const uint32_t *d_offsets, uint32_t t,
         return ASTROZ_NULL_POINTER;
     if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
     AZ_CUDA(cudaSetDevice(device));
-    a.offsets = d_offsets;
-    a.jd = d_jd;
-    a.fr = d_fr;
-    a.kind = d_kind;
-    a.value = d_value;
-    a.sigma = d_sigma;
-    a.station = d_station;
-    a.stations = d_stations;
-    a.bstar = d_bstar;
-    a.scratch = d_scratch;
-    iod_outputs(a, d_elements, d_state, d_wrms, d_method, d_candidates, d_conv, d_deep_space, d_status);
-    AZ_CUDA(az::launch_iod(a, static_cast<cudaStream_t>(stream)));
+    AZ_CUDA(iod_run(a, d_offsets, d_jd, d_fr, d_kind, d_value, d_sigma, d_station, d_stations, d_bstar, d_scratch,
+                    d_elements, d_state, d_wrms, d_method, d_candidates, d_conv, d_deep_space, d_status,
+                    static_cast<cudaStream_t>(stream)));
     return ASTROZ_OK;
 }
 
-// Host buffers: every check, then each track's observations sorted stably by jd + fr into host staging, which goes up
-// through the pinned ring (the caller's pinned arrays are not read by DMA: the staging copy is pageable), the launches
-// on the device's stream with the scratch in the same device block, and plain copies back.
+// Every check, then each track's observations sorted stably by jd + fr into host staging, which is what goes up (the
+// caller's pinned arrays are not read by DMA: the staging copy is pageable).
 int32_t astroz_cuda_initial_orbits(const uint32_t *offsets, uint32_t t, const double *jd, const double *fr,
                                    const uint8_t *kind, const double *value, const double *sigma,
                                    const uint32_t *station, uint32_t m, const double *stations, uint32_t k,
@@ -3487,20 +3390,12 @@ int32_t astroz_cuda_initial_orbits(const uint32_t *offsets, uint32_t t, const do
     if (t && (!elements || !state || !wrms || !method || !candidates || !conv || !deep_space || !status))
         return ASTROZ_NULL_POINTER;
     if (m && (!jd || !fr || !kind || !value || !sigma)) return ASTROZ_NULL_POINTER;
-    if (offsets[0] != 0) return value_error("offsets[0] must be 0");
-    for (uint32_t j = 0; j < t; ++j) {
-        if (offsets[j + 1] < offsets[j]) return value_error("offsets must be non-decreasing");
-        if (offsets[j + 1] == offsets[j]) return value_error("a track has no observation");
-        if (offsets[j + 1] - offsets[j] > az::kIodMaxTrack)
-            return value_error("a track is longer than ASTROZ_IOD_MAX_TRACK observations");
-    }
-    if (offsets[t] != m) return value_error("offsets[t] must equal the observation count m");
+    if ((rc = offsets_check(offsets, t, m, "offsets[t] must equal the observation count m", true, az::kIodMaxTrack,
+                            "a track is longer than ASTROZ_IOD_MAX_TRACK observations")) != ASTROZ_OK)
+        return rc;
     if ((rc = obs_values_check(jd, fr, value, sigma, station, kind, m, stations, k)) != ASTROZ_OK) return rc;
-    {
-        const az::CorrObsArrays in{jd, fr, kind, value, sigma, station, stations};
-        for (uint32_t j = 0; j < t; ++j)
-            if (az::corr_used(in, offsets[j], offsets[j + 1]) == 0) return value_error("a track has no used residual");
-    }
+    if ((rc = used_residuals_check({jd, fr, kind, value, sigma, station, stations}, offsets, t)) != ASTROZ_OK)
+        return rc;
     if (bstar && !all_finite(bstar, t)) return value_error("bstar must be finite");
     if (t == 0) return ASTROZ_OK;
     // each track in time order, stably
@@ -3522,58 +3417,21 @@ int32_t astroz_cuda_initial_orbits(const uint32_t *offsets, uint32_t t, const do
         std::memcpy(&sSigma[(size_t)6 * i], sigma + (size_t)6 * p, 48);
         if (station) sStation[i] = station[p];
     }
-    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
-    NumericalContext *c = nullptr;
-    if ((rc = numerical_context(device, &c)) != ASTROZ_OK) return rc;
-    std::lock_guard<std::mutex> lk(c->m);
-    AZ_CUDA(cudaSetDevice(device));
-    cudaStream_t st = c->stream;
-    // offsets | jd | fr | kind | value | sigma | station | stations | bstar | scratch | elements | state | wrms | method |
-    // candidates | conv | deep_space | status
-    DeviceBlock d(st);
-    AZ_CUDA(d.alloc({(size_t)4 * (t + 1), (size_t)8 * m, (size_t)8 * m, (size_t)m, (size_t)48 * m, (size_t)48 * m,
-                     station ? (size_t)4 * m : 0, (size_t)24 * k, bstar ? (size_t)8 * t : 0, az::iod_scratch_bytes(t),
-                     (size_t)64 * t, (size_t)48 * t, (size_t)8 * t, (size_t)t, (size_t)4 * t, (size_t)16 * t, (size_t)t,
-                     (size_t)t}));
-    auto up = [&](const void *src, void *dst, size_t elemBytes, size_t count) {
-        void *const dd[1] = {dst};
-        const void *const ss[1] = {src};
-        return c->pipe.ring.upload(az::is_pageable(src), 1, ss, dd, &elemBytes, count, st);
-    };
-    AZ_CUDA(up(offsets, d.u32(0), 4, (size_t)t + 1));
-    if (m) {
-        AZ_CUDA(up(sJd.data(), d.f64(1), 8, m));
-        AZ_CUDA(up(sFr.data(), d.f64(2), 8, m));
-        AZ_CUDA(up(sKind.data(), d.u8(3), 1, m));
-        AZ_CUDA(up(sValue.data(), d.f64(4), 48, m));
-        AZ_CUDA(up(sSigma.data(), d.f64(5), 48, m));
-        if (station) AZ_CUDA(up(sStation.data(), d.u32(6), 4, m));
-    }
-    if (k) AZ_CUDA(up(stations, d.f64(7), 24, k));
-    if (bstar) AZ_CUDA(up(bstar, d.f64(8), 8, t));
-    a.offsets = d.u32(0);
-    a.jd = d.f64(1);
-    a.fr = d.f64(2);
-    a.kind = d.u8(3);
-    a.value = d.f64(4);
-    a.sigma = d.f64(5);
-    a.station = station ? d.u32(6) : nullptr;
-    a.stations = k ? d.f64(7) : nullptr;
-    a.bstar = bstar ? d.f64(8) : nullptr;
-    a.scratch = d.piece(9);
-    iod_outputs(a, d.f64(10), d.f64(11), d.f64(12), d.u8(13), d.u32(14), d.f64(15), d.u8(16), d.u8(17));
-    AZ_CUDA(az::launch_iod(a, st));
-    AZ_CUDA(cudaMemcpyAsync(elements, a.elements, (size_t)64 * t, cudaMemcpyDeviceToHost, st));
-    AZ_CUDA(cudaMemcpyAsync(state, a.state, (size_t)48 * t, cudaMemcpyDeviceToHost, st));
-    AZ_CUDA(cudaMemcpyAsync(wrms, a.wrms, (size_t)8 * t, cudaMemcpyDeviceToHost, st));
-    AZ_CUDA(cudaMemcpyAsync(method, a.method, t, cudaMemcpyDeviceToHost, st));
-    AZ_CUDA(cudaMemcpyAsync(candidates, a.candidates, (size_t)4 * t, cudaMemcpyDeviceToHost, st));
-    AZ_CUDA(cudaMemcpyAsync(conv, a.conv, (size_t)16 * t, cudaMemcpyDeviceToHost, st));
-    AZ_CUDA(cudaMemcpyAsync(deep_space, a.deepSpace, t, cudaMemcpyDeviceToHost, st));
-    AZ_CUDA(cudaMemcpyAsync(status, a.status, t, cudaMemcpyDeviceToHost, st));
-    AZ_CUDA(d.buf.release());
-    AZ_CUDA(cudaStreamSynchronize(st));
-    return ASTROZ_OK;
+    return whole_batch(device,
+                       {upload(offsets, (size_t)4 * (t + 1)), upload(sJd.data(), (size_t)8 * m),
+                        upload(sFr.data(), (size_t)8 * m), upload(sKind.data(), m),
+                        upload(sValue.data(), (size_t)48 * m), upload(sSigma.data(), (size_t)48 * m),
+                        upload(sStation.data(), station ? (size_t)4 * m : 0), upload(stations, (size_t)24 * k),
+                        upload(bstar, bstar ? (size_t)8 * t : 0), scratch(az::iod_scratch_bytes(t)),
+                        result(elements, (size_t)64 * t), result(state, (size_t)48 * t), result(wrms, (size_t)8 * t),
+                        result(method, t), result(candidates, (size_t)4 * t), result(conv, (size_t)16 * t),
+                        result(deep_space, t), result(status, t)},
+                       [&](const DeviceBlock &d, cudaStream_t st) {
+                           return iod_run(a, d.u32(0), d.f64(1), d.f64(2), d.u8(3), d.f64(4), d.f64(5),
+                                          station ? d.u32(6) : nullptr, k ? d.f64(7) : nullptr,
+                                          bstar ? d.f64(8) : nullptr, d.piece(9), d.f64(10), d.f64(11), d.f64(12),
+                                          d.u8(13), d.u32(14), d.f64(15), d.u8(16), d.u8(17), st);
+                       });
 }
 
 int32_t astroz_cuda_parse_tle(const char *line1, const char *line2, double *elements) {
@@ -3610,6 +3468,13 @@ static int32_t porkchop_check(uint32_t n_pairs, uint32_t n_dep, uint32_t n_arr, 
     return ASTROZ_OK;
 }
 
+// Both call forms, on device arrays.
+static cudaError_t lambert_run(const double *r1, const double *r2, const double *tof, const double *normal,
+                               uint32_t n, double mu, uint32_t max_revs, double *v1, double *v2, uint8_t *status,
+                               uint8_t *iterations, cudaStream_t st) {
+    return az::launch_lambert(az::LambertArgs{r1, r2, tof, normal, n, max_revs, mu, v1, v2, status, iterations}, st);
+}
+
 int32_t astroz_cuda_lambert_device(const double *d_r1, const double *d_r2, const double *d_tof, const double *d_normal,
                                    uint32_t n, double mu, uint32_t max_revs, int32_t device, double *d_v1,
                                    double *d_v2, uint8_t *d_status, uint8_t *d_iterations, void *stream) {
@@ -3619,60 +3484,32 @@ int32_t astroz_cuda_lambert_device(const double *d_r1, const double *d_r2, const
     if (!d_r1 || !d_r2 || !d_tof || !d_v1 || !d_v2 || !d_status) return ASTROZ_NULL_POINTER;
     if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
     AZ_CUDA(cudaSetDevice(device));
-    const az::LambertArgs a{d_r1, d_r2, d_tof, d_normal, n, max_revs, mu, d_v1, d_v2, d_status, d_iterations};
-    AZ_CUDA(az::launch_lambert(a, static_cast<cudaStream_t>(stream)));
+    AZ_CUDA(lambert_run(d_r1, d_r2, d_tof, d_normal, n, mu, max_revs, d_v1, d_v2, d_status, d_iterations,
+                        static_cast<cudaStream_t>(stream)));
     return ASTROZ_OK;
 }
 
-// Host buffers: a solve is compute-bound (some 5 iterations of fp64 transcendentals per slot for 56 bytes in), so the
-// batch goes up at once -- pageable arrays through the device's pinned ring, pinned ones by direct DMA -- one launch
-// solves it and the results come back by plain copies.
 int32_t astroz_cuda_lambert(const double *r1, const double *r2, const double *tof, const double *normal, uint32_t n,
                             double mu, uint32_t max_revs, int32_t device, double *v1, double *v2, uint8_t *status,
                             uint8_t *iterations) {
-    int32_t rc = lambert_check(mu, max_revs, device);
+    const int32_t rc = lambert_check(mu, max_revs, device);
     if (rc != ASTROZ_OK) return rc;
     if (n == 0) return ASTROZ_OK;
     if (!r1 || !r2 || !tof || !v1 || !v2 || !status) return ASTROZ_NULL_POINTER;
     if (!all_finite(r1, (size_t)3 * n) || !all_finite(r2, (size_t)3 * n) || !all_finite(tof, n) ||
         (normal && !all_finite(normal, (size_t)3 * n)))
         return value_error("r1, r2, tof and normal must be finite");
-    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
-    NumericalContext *c = nullptr;
-    if ((rc = numerical_context(device, &c)) != ASTROZ_OK) return rc;
-    std::lock_guard<std::mutex> lk(c->m);
-    AZ_CUDA(cudaSetDevice(device));
-    cudaStream_t st = c->stream;
     const size_t slots = (size_t)n * (2 * (size_t)max_revs + 1);
-    // one device block: r1 | r2 | normal | tof | v1 | v2 | status | iterations
-    const size_t bytes[] = {(size_t)24 * n, (size_t)24 * n, normal ? (size_t)24 * n : 0, (size_t)8 * n, 24 * slots,
-                            24 * slots, slots, iterations ? slots : 0};
-    size_t at[8], total = 0;
-    for (int k = 0; k < 8; ++k) at[k] = total, total += (bytes[k] + 15) & ~size_t(15);
-    StreamBuf dBuf(st);
-    AZ_CUDA(dBuf.alloc(total));
-    char *base = static_cast<char *>(dBuf.p);
-    auto up = [&](const void *src, int k, size_t elemBytes, size_t count) {
-        void *const d[1] = {base + at[k]};
-        const void *const s[1] = {src};
-        return c->pipe.ring.upload(az::is_pageable(src), 1, s, d, &elemBytes, count, st);
-    };
-    AZ_CUDA(up(r1, 0, 24, n));
-    AZ_CUDA(up(r2, 1, 24, n));
-    if (normal) AZ_CUDA(up(normal, 2, 24, n));
-    AZ_CUDA(up(tof, 3, 8, n));
-    auto dd = [&](int k) { return reinterpret_cast<double *>(base + at[k]); };
-    auto db = [&](int k) { return reinterpret_cast<uint8_t *>(base + at[k]); };
-    const az::LambertArgs a{dd(0), dd(1), dd(3), normal ? dd(2) : nullptr, n, max_revs, mu, dd(4), dd(5), db(6),
-                            iterations ? db(7) : nullptr};
-    AZ_CUDA(az::launch_lambert(a, st));
-    AZ_CUDA(cudaMemcpyAsync(v1, a.v1, 24 * slots, cudaMemcpyDeviceToHost, st));
-    AZ_CUDA(cudaMemcpyAsync(v2, a.v2, 24 * slots, cudaMemcpyDeviceToHost, st));
-    AZ_CUDA(cudaMemcpyAsync(status, a.status, slots, cudaMemcpyDeviceToHost, st));
-    if (iterations) AZ_CUDA(cudaMemcpyAsync(iterations, a.iterations, slots, cudaMemcpyDeviceToHost, st));
-    AZ_CUDA(dBuf.release());
-    AZ_CUDA(cudaStreamSynchronize(st));
-    return ASTROZ_OK;
+    return whole_batch(device,
+                       {upload(r1, (size_t)24 * n), upload(r2, (size_t)24 * n),
+                        upload(normal, normal ? (size_t)24 * n : 0), upload(tof, (size_t)8 * n),
+                        result(v1, 24 * slots), result(v2, 24 * slots), result(status, slots),
+                        result(iterations, iterations ? slots : 0)},
+                       [&](const DeviceBlock &d, cudaStream_t st) {
+                           return lambert_run(d.f64(0), d.f64(1), d.f64(3), normal ? d.f64(2) : nullptr, n, mu,
+                                              max_revs, d.f64(4), d.f64(5), d.u8(6), iterations ? d.u8(7) : nullptr,
+                                              st);
+                       });
 }
 
 int32_t astroz_cuda_lambert_porkchop_device(const double *d_dep, const uint8_t *d_dep_status, const double *d_arr,

@@ -24,8 +24,18 @@ card's name, power limit and maximum SM clock.
   device         astroz_cuda_constellation_propagate_device_f32 (near-earth catalogue) and
                  astroz_cuda_sdp4_propagate_into_device (the mixed catalogue's deep-space members), 1,440 epochs
 
-    python tools/host_pipeline_timing.py [--reps 3]
-    python tools/host_pipeline_timing.py --compare OTHER.so [--rounds 5]
+The whole-batch calls (one device block per call, no chunk pipeline), each at a workload of its family's timing tool:
+  fit_elements FT1     tools/fit_timing.py's FT1: the config-2 catalogue, 1,440 K1-grid states each, perturbed guesses
+  fit_observations OT1 tools/fit_obs_timing.py's OT1: the config-2 catalogue from radar tracks of six stations, B* held
+  observe OT1          astroz_cuda_observe of OT1's observations, from propagate_pairs states at their times
+  covariance CV2       tools/covariance_timing.py's CV2: one query per config-2 row at a common time, TEME
+  conjunction PC1      tools/conjunction_timing.py's PC1: 100,000 engineered LEO crossings
+  correlate CR1        tools/correlate_timing.py's CR1 at 1,000 radar tracks of 10 observations
+  initial_orbits       tools/iod_timing.py's 100,000-track mix (tests/fit_oracle/iod.py mixed_tracks)
+  lambert L1           tools/lambert_timing.py's L1 problem set (10^7 LEO-GEO problems, max_revs = 0), seed 1
+
+    python tools/host_pipeline_timing.py [--reps 3] [--calls all|chunked|whole_batch]
+    python tools/host_pipeline_timing.py --compare OTHER.so [--rounds 5] [--calls ...]
 
 --compare alternates processes on OTHER.so (through ASTROZ_B200_LIB) and on this tree's library, --rounds each, and
 reports per call the best time of each library, the spread of its runs (slowest minus fastest) and whether every run of
@@ -225,7 +235,107 @@ def sdp4_device_case(c, jd, fr, reps):
     return best_ms(call, reps), checksum([block.cpu().numpy()])
 
 
-def measure(reps: int) -> dict:
+class Out:
+    """An output argument of a whole-batch call: zero-filled, pinned or pageable like the inputs."""
+
+    def __init__(self, shape, dtype=np.float64):
+        self.shape, self.dtype = shape, dtype
+
+
+def whole_batch_case(name, args, pinned, reps):
+    from astroz_b200 import _lib
+
+    held = [like(np.zeros(a.shape, a.dtype), pinned) if isinstance(a, Out)
+            else like(np.ascontiguousarray(a), pinned) if isinstance(a, np.ndarray) else a for a in args]
+    outs = [h for a, h in zip(args, held) if isinstance(a, Out)]
+    fn = getattr(_lib.lib(), f"astroz_cuda_{name}")
+    values = [ptr(h) if isinstance(h, np.ndarray) else h for h in held]
+    ms = best_ms(lambda: _lib.check(fn(*values)), reps)
+    return ms, checksum(outs)
+
+
+def whole_batch_workloads():
+    """(record name, C function without its astroz_cuda_ prefix, arguments) of every whole-batch call"""
+    import conjunction_timing
+    import correlate_timing
+    import covariance_timing
+    import fit_obs_timing
+    import lambert_timing
+
+    from astroz_b200 import synth
+    from astroz_b200.constellation import Constellation, Layout
+    from tests import fit_oracle as R
+    from tests.fit_oracle import conjunction_cases as cc
+    from tests.fit_oracle import iod as I
+    from tests.fit_oracle import obs as O
+
+    u8, u32 = np.uint8, np.uint32
+    el = synth.elements_from_tles(synth.near_earth_catalog(13478))
+    n = el.shape[1]
+    c = Constellation.from_elements(*el)
+    jd, fr = synth.time_grid(1440)
+    pos, vel = c.propagate(jd, fr, layout=Layout.satelliteMajor)
+    m = n * 1440
+    yield "fit_elements_FT1", "fit_elements", [
+        R.perturbed(el, seed=3), n, 1, np.arange(n + 1, dtype=u32) * 1440, np.tile(jd, n), np.tile(fr, n),
+        np.array(pos).reshape(-1, 3), np.array(vel).reshape(-1, 3), m, 1.0, 1e-3, 1, 25, 0, Out((8, n)), Out((n, 2)),
+        Out(n, u32), Out(n, u8)]
+    del pos, vel
+
+    g = R.perturbed(el, seed=3)
+    g[7] = el[7]
+    fr2 = np.arange(1440) * 2.0 / 1440.0 + fr[0]
+    ojd, ofr, kind, value, sigma, station, off = O.concat(
+        fit_obs_timing._tracks(el, O.RADAR, O.RADAR_SITES, jd, fr2))
+    off, station, sites = off.astype(u32), station.astype(u32), np.ascontiguousarray(O.RADAR_SITES, np.float64)
+    m, k = len(ojd), len(sites)
+    yield "fit_observations_OT1", "fit_observations", [
+        g, n, 1, off, ojd, ofr, value, sigma, station, kind, m, sites, k, 0, 25, 0, Out((8, n)), Out(n), Out(n, u32),
+        Out((n, 28)), Out(n, u32), Out(n, u8), Out(n, u8)]
+    p, v, _ = c.propagate_pairs(np.repeat(np.arange(n), np.diff(off)), ojd, ofr)
+    states = np.concatenate([np.asarray(p), np.asarray(v)], axis=1)
+    yield "observe_OT1", "observe", [states, ojd, ofr, kind, station, m, sites, k, 0, Out((m, 6))]
+    c.deinit()
+    del states, value, sigma
+
+    _, el_c, model, sat, qjd, qfr = next(w for w in covariance_timing._workloads() if w[0] == "CV2")
+    m = len(sat)
+    yield "covariance_CV2", "propagate_covariance", [
+        el_c, n, 1, covariance_timing._covariances(n), model, np.searchsorted(sat, np.arange(n + 1)).astype(u32), qjd,
+        qfr, m, 0, 0, Out((m, 6)), Out((m, 21)), None, Out(m, u8)]
+
+    _, el_p, pr, se, cjd, cfr, w, deep = next(x for x in conjunction_timing._workloads() if x[0] == "PC1")
+    np_, m = el_p.shape[1], len(pr)
+    model = np.full(np_, deep, u8)
+    yield "conjunction_PC1", "conjunction", [
+        el_p, np_, 1, conjunction_timing._covariances(np_, model.astype(bool)), model, pr.astype(u32),
+        se.astype(u32), cjd, cfr, np.full(m, w), np.full(m, 0.02), m, 0, 0, Out((m, 13)), Out((m, 2, 6)),
+        Out((m, 2, 21)), Out(m, u8)]
+
+    el2 = synth.elements_from_tles(synth.near_earth_catalog(13478, 13478))
+    n2 = el2.shape[1]
+    ids, tjd, tfr, kind, value, sigma, station = correlate_timing._tracks(
+        el2, np.random.default_rng(1).integers(0, n2, 1000), O.RADAR, 10, 10.0, seed=1000)
+    t, m, best = 1000, len(ids), 4
+    yield "correlate_CR1", "correlate", [
+        el2, n2, 1, cc.P_words(n2, scale=0.3, seed=12), None, np.searchsorted(ids, np.arange(t + 1)).astype(u32), t,
+        tjd, tfr, kind, value, sigma, station.astype(u32), m, sites, k, 0.999, best, 0, Out((t, best), u32),
+        Out((t, best)), Out(t, u32), Out(t, u32), Out(t, u32), Out(t, u8), Out(n2, u8)]
+
+    tr = I.mixed_tracks(100_000, 31)
+    t = tr.t
+    yield "initial_orbits_100k", "initial_orbits", [
+        tr.offsets, t, tr.jd, tr.fr, tr.kind, tr.value, tr.sigma, tr.station, len(tr.jd), tr.stations,
+        len(tr.stations), None, 1, 0, Out((8, t)), Out((t, 6)), Out(t), Out(t, u8), Out(t, u32), Out((t, 2)),
+        Out(t, u8), Out(t, u8)]
+
+    n = 10_000_000
+    r1, r2, tof, normal = lambert_timing.problems(np.random.default_rng(1), n, 6600.0, 42164.0, 2 * 86400.0)
+    yield "lambert_L1", "lambert", [r1, r2, tof, normal, n, lambert_timing.MU, 0, 0, Out((n, 3)), Out((n, 3)),
+                                    Out(n, u8), Out(n, u8)]
+
+
+def measure(reps: int, calls: str = "all") -> dict:
     import astroz_b200
     from astroz_b200 import _lib, numerical, synth
     from astroz_b200.api import WGS72, Satrec
@@ -246,6 +356,12 @@ def measure(reps: int) -> dict:
 
     def one(name, case, *args):
         record(name, *case(*args, reps))
+
+    if calls in ("all", "whole_batch"):
+        for name, fn, args in whole_batch_workloads():
+            both(name, whole_batch_case, fn, args)
+    if calls == "whole_batch":
+        return res
 
     near = synth.near_earth_catalog()
     c = astroz_b200.Constellation(near)
@@ -298,7 +414,7 @@ def measure(reps: int) -> dict:
     return res
 
 
-def compare(other: str, rounds: int, reps: int) -> dict:
+def compare(other: str, rounds: int, reps: int, calls: str) -> dict:
     runs = {"other": [], "this": []}
     for r in range(rounds):
         for label in (("other", "this") if r % 2 == 0 else ("this", "other")):
@@ -307,7 +423,7 @@ def compare(other: str, rounds: int, reps: int) -> dict:
             if label == "other":
                 env["ASTROZ_B200_LIB"] = os.path.abspath(other)
             print(f"round {r}: {label}", file=sys.stderr, flush=True)
-            p = subprocess.run([sys.executable, os.path.abspath(__file__), "--reps", str(reps)], env=env,
+            p = subprocess.run([sys.executable, os.path.abspath(__file__), "--reps", str(reps), "--calls", calls], env=env,
                                stdout=subprocess.PIPE, text=True, check=True)
             runs[label].append(json.loads(p.stdout.strip().splitlines()[-1]))
     first = runs["this"][0]
@@ -328,8 +444,11 @@ def main():
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--compare", metavar="OTHER.so")
     ap.add_argument("--rounds", type=int, default=5)
+    ap.add_argument("--calls", choices=("all", "chunked", "whole_batch"), default="all",
+                    help="chunked: the calls above the whole-batch ones; whole_batch: those alone")
     a = ap.parse_args()
-    print(json.dumps(compare(a.compare, a.rounds, a.reps) if a.compare else measure(a.reps)), flush=True)
+    print(json.dumps(compare(a.compare, a.rounds, a.reps, a.calls) if a.compare else measure(a.reps, a.calls)),
+          flush=True)
 
 
 if __name__ == "__main__":
