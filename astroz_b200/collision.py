@@ -12,6 +12,12 @@ minimum of the range inside the window, each object's state covariance comes fro
 TCA, and Pc is the short-encounter 2-D integral over the combined hard-body disk in the encounter plane, with the two
 objects' errors taken as uncorrelated.  For slow encounters (GEO pairs) the short-encounter assumption fails and Pc is
 not the collision probability.
+
+`monte_carlo` (K14) makes no such assumption: it draws both objects' element sets from their covariances, finds each
+drawn pair's own TCA with the same search and counts the draws that come within the hard-body radius.
+
+    mc = monte_carlo(fit, primary, secondary, jd, fr, window_min=30.0, hbr_km=0.02, samples=10**7, seed=1)
+    mc.pc, mc.interval(), mc.hits, mc.failed
 """
 from __future__ import annotations
 
@@ -32,6 +38,45 @@ STATUS_NAMES = {OK: "ok", INIT_FAILED: "a set cannot be built under the row's mo
                 NO_PLANE: "zero relative velocity: no encounter plane", BAD_PAIR: "bad row pair"}
 _WORDS = D["ASTROZ_CONJ_RECORD_WORDS"]
 _SIG = D["ASTROZ_STATE_COVARIANCE_WORDS"]
+
+
+def _catalogue(source, covariance, model):
+    """(elements (8, n), covariance words (n, 28), model bytes (n,) or None) of a FitResult or an element array"""
+    if hasattr(source, "elements") and hasattr(source, "deep_space"):
+        el = np.ascontiguousarray(source.elements, dtype=np.float64)
+        covariance = source.covariance if covariance is None else covariance
+        model = source.deep_space if model is None else model
+        if covariance is None:
+            raise ValueError("this FitResult has no covariance (fit_observations returns one)")
+    else:
+        el = np.ascontiguousarray(source, dtype=np.float64)
+        if el.ndim != 2 or el.shape[0] != 8:
+            raise ValueError("source must be a FitResult or an (8, n) array of element columns")
+        if covariance is None:
+            raise ValueError("covariance= is required with an element array")
+    n = el.shape[1]
+    cov = _covariance_words(covariance, n)
+    md = None
+    if model is not None:
+        mm = np.asarray(model).reshape(-1)
+        if len(mm) != n or (mm.size and (mm.min() < 0 or mm.max() > 1)):
+            raise ValueError("model must hold n values, 0 (near-earth) or 1 (deep space)")
+        md = np.ascontiguousarray(mm.astype(np.uint8))
+    return el, cov, md
+
+
+def _rows(primary, secondary, n):
+    """the candidates' row indices as uint32 arrays, checked against n"""
+    rows = []
+    for name, a in (("primary", primary), ("secondary", secondary)):
+        a = np.asarray(a).reshape(-1)
+        if a.size and (not np.issubdtype(a.dtype, np.integer) or a.min() < 0 or a.max() >= n):
+            raise ValueError(f"{name} must hold row indices in [0, n)")
+        rows.append(np.ascontiguousarray(a.astype(np.uint32)))
+    pr, se = rows
+    if len(pr) != len(se):
+        raise ValueError("primary and secondary must have the same length")
+    return pr, se
 
 
 @dataclass
@@ -66,35 +111,9 @@ def conjunctions(source, primary, secondary, jd, fr, *, window_min, hbr_km, cova
     and model= (n,) 0 / 1 or bool.  Candidate i: rows primary[i] != secondary[i] around jd[i] + fr[i], half window
     window_min [min] and combined hard-body radius hbr_km [km] (jd, fr, window_min and hbr_km broadcast to primary).
     frame chooses TEME or each object's own RTN for state_covariance; states=True also returns both TEME states."""
-    if hasattr(source, "elements") and hasattr(source, "deep_space"):
-        el = np.ascontiguousarray(source.elements, dtype=np.float64)
-        covariance = source.covariance if covariance is None else covariance
-        model = source.deep_space if model is None else model
-        if covariance is None:
-            raise ValueError("this FitResult has no covariance (fit_observations returns one)")
-    else:
-        el = np.ascontiguousarray(source, dtype=np.float64)
-        if el.ndim != 2 or el.shape[0] != 8:
-            raise ValueError("source must be a FitResult or an (8, n) array of element columns")
-        if covariance is None:
-            raise ValueError("covariance= is required with an element array")
+    el, cov, md = _catalogue(source, covariance, model)
     n = el.shape[1]
-    cov = _covariance_words(covariance, n)
-    md = None
-    if model is not None:
-        mm = np.asarray(model).reshape(-1)
-        if len(mm) != n or (mm.size and (mm.min() < 0 or mm.max() > 1)):
-            raise ValueError("model must hold n values, 0 (near-earth) or 1 (deep space)")
-        md = np.ascontiguousarray(mm.astype(np.uint8))
-    rows = []
-    for name, a in (("primary", primary), ("secondary", secondary)):
-        a = np.asarray(a).reshape(-1)
-        if a.size and (not np.issubdtype(a.dtype, np.integer) or a.min() < 0 or a.max() >= n):
-            raise ValueError(f"{name} must hold row indices in [0, n)")
-        rows.append(np.ascontiguousarray(a.astype(np.uint32)))
-    pr, se = rows
-    if len(pr) != len(se):
-        raise ValueError("primary and secondary must have the same length")
+    pr, se = _rows(primary, secondary, n)
     m = len(pr)
     f64 = lambda a: np.ascontiguousarray(np.broadcast_to(np.asarray(a, dtype=np.float64), (m,)))  # noqa: E731
     jd_, fr_, w_, r_ = f64(jd), f64(fr), f64(window_min), f64(hbr_km)
@@ -138,3 +157,129 @@ def conjunctions_device(elements, covariance, model, primary, secondary, jd, fr,
         ptr(elements), n, int(grav), ptr(covariance), ptr(model), ptr(primary), ptr(secondary), ptr(jd), ptr(fr),
         ptr(window_min), ptr(hbr_km), m, int(frame), int(elements.device.index), ptr(record), ptr(states),
         ptr(state_covariance), ptr(status), C.c_void_p(stream) if stream else None))
+
+
+# ---- Monte Carlo from epoch (K14, astroz_b200/csrc/az_conjunction_mc.cu) ----------------------------------------------
+NOT_PSD = D["ASTROZ_CONJ_NOT_PSD"]
+STATUS_NAMES[NOT_PSD] = "a covariance is not positive semidefinite"
+_MC_COUNT = D["ASTROZ_CONJ_MC_COUNT_WORDS"]
+_MC_SAMPLE = D["ASTROZ_CONJ_MC_SAMPLE_WORDS"]
+
+
+@dataclass
+class MonteCarloResult:
+    hits: np.ndarray                  # (m,) uint64: samples whose miss at their TCA is below the radius
+    edge: np.ndarray                  # (m,) uint64: samples whose search ended at a window end (scored all the same)
+    failed: np.ndarray                # (m,) uint64: samples with a set that cannot be built or a failed cell
+    samples: np.ndarray               # (m,) uint64: samples drawn
+    status: np.ndarray                # (m,) uint8 ASTROZ_CONJ_*: OK, INIT_FAILED, NOT_PSD
+    sample_dt: np.ndarray | None      # (m, record) dt_tca [min] of samples first .. first + record - 1 (NaN: none)
+    sample_miss: np.ndarray | None    # (m, record) miss [km]
+
+    @property
+    def valid(self) -> np.ndarray:
+        """samples scored: samples - failed, 0 for a candidate that is not OK"""
+        v = self.samples.astype(np.float64) - self.failed.astype(np.float64)
+        return np.where(self.status == OK, v, 0.0)
+
+    @property
+    def pc(self) -> np.ndarray:
+        """hits / (samples - failed), NaN where no sample was scored"""
+        v = self.valid
+        with np.errstate(divide="ignore", invalid="ignore"):
+            return np.where(v > 0, self.hits.astype(np.float64) / v, np.nan)
+
+    def interval(self, z: float = 1.96) -> tuple[np.ndarray, np.ndarray]:
+        """The Wilson score interval (lo, hi) of Pc at z standard errors: sensible at 0 hits, NaN with no sample"""
+        n = self.valid
+        with np.errstate(divide="ignore", invalid="ignore"):
+            p = self.hits.astype(np.float64) / n
+            d = 1.0 + z * z / n
+            c = (p + z * z / (2.0 * n)) / d
+            h = z * np.sqrt(p * (1.0 - p) / n + z * z / (4.0 * n * n)) / d
+        bad = ~(n > 0)
+        return np.where(bad, np.nan, np.maximum(c - h, 0.0)), np.where(bad, np.nan, np.minimum(c + h, 1.0))
+
+
+def monte_carlo(source, primary, secondary, jd, fr, *, window_min, hbr_km, samples, seed=0, first=0, record: int = 0,
+                covariance=None, model=None, grav: int = WGS72, device: int = 0) -> MonteCarloResult:
+    """Monte Carlo collision probability of m candidate conjunctions (astroz_cuda_conjunction_mc).
+
+    source, primary, secondary, jd, fr, window_min, hbr_km, covariance and model are those of `conjunctions`.  Each
+    candidate draws samples k in [first, first + samples) of both objects' element sets from their covariances
+    (Philox4x32-10 keyed by seed), finds each drawn pair's TCA in the window and counts the draws whose miss is below
+    hbr_km.  samples, seed and first broadcast to primary.  record > 0 also returns the dt_tca and miss of the first
+    `record` samples.  The draws depend on (seed, k) alone, so counts over [0, 2N) are those over [0, N) plus those
+    over [N, 2N): extend a run by calling again with first = N and adding the counts (there is no adaptive stopping).
+    Equal seeds give equal draws; pass different seeds for independent estimates."""
+    el, cov, md = _catalogue(source, covariance, model)
+    n = el.shape[1]
+    pr, se = _rows(primary, secondary, n)
+    m = len(pr)
+    record = int(record)
+    if record < 0:
+        raise ValueError("record must be >= 0")
+    f64 = lambda a: np.ascontiguousarray(np.broadcast_to(np.asarray(a, dtype=np.float64), (m,)))  # noqa: E731
+
+    def u64(a, name):
+        a = np.asarray(a)
+        if a.size and (not np.issubdtype(a.dtype, np.integer) or a.min() < 0):
+            raise ValueError(f"{name} must hold integers >= 0")
+        return np.ascontiguousarray(np.broadcast_to(a.astype(np.uint64), (m,)))
+
+    jd_, fr_, w_, r_ = f64(jd), f64(fr), f64(window_min), f64(hbr_km)
+    ns, fi, sd = u64(samples, "samples"), u64(first, "first"), u64(seed, "seed")
+    counts, stat = np.zeros((m, _MC_COUNT), np.uint64), np.zeros(m, dtype=np.uint8)
+    out = np.zeros((m, record, _MC_SAMPLE)) if record else None
+    vp = lambda a: None if a is None or a.size == 0 else C.c_void_p(a.ctypes.data)  # noqa: E731
+    check(lib().astroz_cuda_conjunction_mc(vp(el), n, int(grav), vp(cov), vp(md), vp(pr), vp(se), vp(jd_), vp(fr_),
+                                           vp(w_), vp(r_), vp(ns), vp(fi), vp(sd), m, record, int(device),
+                                           vp(counts), vp(out), vp(stat)))
+    return MonteCarloResult(counts[:, 0], counts[:, 1], counts[:, 2], ns.copy(), stat,
+                            None if out is None else out[:, :, 0], None if out is None else out[:, :, 1])
+
+
+def monte_carlo_scratch_bytes(m: int) -> int:
+    """The scratch of monte_carlo_device for m candidates"""
+    b = C.c_uint64(0)
+    check(lib().astroz_cuda_conjunction_mc_scratch_bytes(int(m), C.byref(b)))
+    return int(b.value)
+
+
+def monte_carlo_device(elements, covariance, model, primary, secondary, jd, fr, window_min, hbr_km, samples, first,
+                       seed, counts, sample_out, status, scratch, *, grav: int = WGS72, stream: int = 0) -> None:
+    """`monte_carlo` with torch CUDA tensors on one device: elements (8, n) float64, covariance (n, 28) float64, model
+    (n,) uint8 or None, primary / secondary (m,) int32, jd / fr / window_min / hbr_km (m,) float64, samples (m,)
+    int64, first / seed (m,) int64 or None (0); counts (m, 3) int64 (hits, edge, failed), sample_out (m, record, 2)
+    float64 or None and status (m,) uint8 receive the results; scratch a uint8 tensor of at least
+    monte_carlo_scratch_bytes(m) bytes.  The launches go on `stream` (a raw cudaStream_t value, 0 = the default
+    stream).  Rows are not checked here: a bad pair gets status BAD_PAIR."""
+    import torch
+
+    n = int(elements.shape[1]) if elements.dim() == 2 and elements.shape[0] == 8 else -1
+    if n < 0 or elements.dtype != torch.float64 or not elements.is_cuda:
+        raise ValueError("elements must be a CUDA float64 tensor of shape (8, n)")
+    m = int(primary.numel())
+    record = int(sample_out.shape[1]) if sample_out is not None and sample_out.dim() == 3 else 0
+    tensors = [("elements", elements, 8 * n, torch.float64), ("covariance", covariance, 28 * n, torch.float64),
+               ("model", model, n, torch.uint8), ("primary", primary, m, torch.int32),
+               ("secondary", secondary, m, torch.int32), ("jd", jd, m, torch.float64), ("fr", fr, m, torch.float64),
+               ("window_min", window_min, m, torch.float64), ("hbr_km", hbr_km, m, torch.float64),
+               ("samples", samples, m, torch.int64), ("first", first, m, torch.int64), ("seed", seed, m, torch.int64),
+               ("counts", counts, _MC_COUNT * m, torch.int64),
+               ("sample_out", sample_out, _MC_SAMPLE * record * m, torch.float64), ("status", status, m, torch.uint8)]
+    for name, t, size, dtype in tensors:
+        if t is None and name in ("model", "first", "seed", "sample_out"):
+            continue
+        if not isinstance(t, torch.Tensor) or t.dtype != dtype or not t.is_contiguous() or int(t.numel()) != size \
+                or t.device != elements.device:
+            raise ValueError(f"{name} must be a contiguous {dtype} tensor of {size} elements on {elements.device}")
+    if not isinstance(scratch, torch.Tensor) or not scratch.is_contiguous() or scratch.device != elements.device \
+            or scratch.numel() * scratch.element_size() < monte_carlo_scratch_bytes(m):
+        raise ValueError(f"scratch must be a contiguous tensor of monte_carlo_scratch_bytes({m}) bytes on "
+                         f"{elements.device}")
+    ptr = lambda t: None if t is None else C.c_void_p(t.data_ptr())  # noqa: E731
+    check(lib().astroz_cuda_conjunction_mc_device(
+        ptr(elements), n, int(grav), ptr(covariance), ptr(model), ptr(primary), ptr(secondary), ptr(jd), ptr(fr),
+        ptr(window_min), ptr(hbr_km), ptr(samples), ptr(first), ptr(seed), m, record, int(elements.device.index),
+        ptr(counts), ptr(sample_out), ptr(status), ptr(scratch), C.c_void_p(stream) if stream else None))

@@ -22,9 +22,10 @@
 
 namespace az {
 
-// per-candidate status bytes (ASTROZ_CONJ_*); 1 and 2 mean what K10's do
+// per-candidate status bytes (ASTROZ_CONJ_*); 1 and 2 mean what K10's do; kConjNotPsd is K14's alone
 enum ConjStatus : uint8_t {
-    kConjOk = 0, kConjInitFailed = 1, kConjCellFailed = 2, kConjWindowEdge = 3, kConjNoPlane = 4, kConjBadPair = 5
+    kConjOk = 0, kConjInitFailed = 1, kConjCellFailed = 2, kConjWindowEdge = 3, kConjNoPlane = 4, kConjBadPair = 5,
+    kConjNotPsd = 6
 };
 
 // record words: dt_tca [min], miss [km], relative speed [km/s], (dr, dv) in the primary's RTN frame, C2 (xx, xy, yy)

@@ -227,6 +227,33 @@ struct ConjArgs {
 // the pairs of two near-earth rows, then on the same stream every other pair
 cudaError_t launch_conjunction(const ConjArgs &a, cudaStream_t stream);
 
+// K14: Monte Carlo collision probability of candidate conjunctions (az_conjunction_mc.cu, az_conjunction_mc.cuh).
+// Device pointers.
+struct ConjMcArgs {
+    const double *elements = nullptr;    // [8][n]
+    const double *covariance = nullptr;  // [n][28]
+    const uint8_t *model = nullptr;      // [n], nullable (all 0)
+    uint32_t n = 0;
+    const uint32_t *primary = nullptr, *secondary = nullptr;  // [m] rows
+    const double *jd = nullptr, *fr = nullptr;                 // [m] guess times
+    const double *window = nullptr;      // [m] half window [min]
+    const double *hbr = nullptr;         // [m] combined hard-body radius [km]
+    const uint64_t *samples = nullptr;   // [m]
+    const uint64_t *first = nullptr;     // [m], nullable (all 0)
+    const uint64_t *seed = nullptr;      // [m], nullable (all 0)
+    uint32_t m = 0;
+    uint32_t record = 0;                 // sample words kept per candidate
+    int grav = 1;
+    GravConsts g{};
+    void *scratch = nullptr;             // conj_mc_scratch_bytes(m)
+    uint64_t *counts = nullptr;          // [m][3] hits, edge, failed
+    double *sampleOut = nullptr;         // [m][record][2] dt_tca, miss; nullable when record = 0
+    uint8_t *status = nullptr;           // [m] ASTROZ_CONJ_*
+};
+cudaError_t conj_mc_scratch_bytes(uint32_t m, size_t *bytes);
+// the candidates' statuses and work items, their scan, the near-earth pairs' items, then every other pair's
+cudaError_t launch_conjunction_mc(const ConjMcArgs &a, cudaStream_t stream);
+
 // K12: sensor tracks correlated with catalogue rows (az_correlate.cu, az_correlate.cuh).  Device pointers.
 struct CorrArgs {
     const double *elements = nullptr;    // [8][n]

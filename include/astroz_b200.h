@@ -783,6 +783,55 @@ int32_t astroz_cuda_conjunction_device(const double *d_elements, uint32_t n, int
                                        const double *d_hbr_km, uint32_t m, int32_t frame, int32_t device,
                                        double *d_record, double *d_states, double *d_state_covariance,
                                        uint8_t *d_status, void *stream);
+/* ---- Monte Carlo collision probability (K14): draws of both element sets from their covariances ---------------------
+ * The catalogue and candidates are astroz_cuda_conjunction's; candidate i also has samples[i], first[i] (NULL: all 0)
+ * and seed[i] (NULL: all 0).  For each row o:
+ *   nominal:   x^ = the row's fit variables, over nvar = 7 or 6 (B* held when P's B* row is zero, as K10 and K11);
+ *   factor:    S = D^-1/2 P D^-1/2 (D = diag P; a zero-variance variable has a zero row and column) factored S = L L^T
+ *              by a semidefinite Cholesky: a pivot in [-1e-12, 1e-12] zeroes its column, one below -1e-12 or a
+ *              negative variance is NOT_PSD;
+ *   sample k:  x_k = x^ + D^1/2 L z, k in [first, first + samples), z from Philox4x32-10 under key (seed lo, seed hi):
+ *              block j = 0 .. 6 of counter (j, k lo, k hi, 0) gives words (a, b, c, d), uniforms u1 = ((a 2^21 +
+ *              (b >> 11)) + 0.5) 2^-53 and u2 likewise from (c, d), and Box-Muller normals 2j (r cos) and 2j + 1
+ *              (r sin), r = sqrt(-2 ln u1), angle 2 pi u2.  Normals 0 .. 6 go to the primary's variables in order,
+ *              7 .. 13 to the secondary's (the B* normal is drawn when B* is held).
+ * Per sample: both drawn sets under their rows' models, astroz_cuda_conjunction's TCA search over [-w, w] on them and
+ * the miss |dr| at that TCA.  A sample is FAILED when a drawn set cannot be built or a deep-space cell fails (it is
+ * then neither a hit nor a miss), an EDGE when the search ends at a window end (still scored), a HIT when miss < R.
+ * Pc = hits / (samples - failed).  The errors of the two objects are UNCORRELATED; no linear or short-encounter
+ * assumption is made.
+ * Outputs: counts[m][3] (hits, edge, failed); sample_out[m][record][2] (dt_tca [min from jd + fr], miss [km]) of
+ * samples first .. first + record - 1, NaN for a failed sample, an index past samples[i] and every sample of a failed
+ * candidate; status[m]: OK, INIT_FAILED (a nominal set cannot be built, or a model byte > 1 on the device call),
+ * NOT_PSD, BAD_PAIR (device call only); counts of a candidate that is not OK are zero.
+ * A sample's words depend on its candidate's inputs and its index k alone, and counts are integer sums: the bytes do
+ * not depend on the batch, the order, the split of [first, first + samples) or the call form.  Counts over [0, 2N)
+ * equal those over [0, N) plus those over [N, 2N): a run is extended by calling again with first = N.  Equal seeds
+ * give equal draws; pass different seeds for independent estimates.
+ * ASTROZ_VALUE_ERROR, nothing written: device = -1, an unknown grav; and for the host call every input check of
+ * astroz_cuda_conjunction, first + samples above 2^64 - 1, record > 0 with a NULL sample_out. */
+#define ASTROZ_CONJ_NOT_PSD              6
+#define ASTROZ_CONJ_MC_COUNT_WORDS       3
+#define ASTROZ_CONJ_MC_SAMPLE_WORDS      2
+/* HOST buffers: one upload (pageable through a pinned ring, pinned by direct DMA), the launches, plain copies back. */
+int32_t astroz_cuda_conjunction_mc(const double *elements, uint32_t n, int32_t grav, const double *covariance,
+                                   const uint8_t *model, const uint32_t *primary, const uint32_t *secondary,
+                                   const double *jd, const double *fr, const double *window_min, const double *hbr_km,
+                                   const uint64_t *samples, const uint64_t *first, const uint64_t *seed, uint32_t m,
+                                   uint32_t record, int32_t device, uint64_t *counts, double *sample_out,
+                                   uint8_t *status);
+/* DEVICE pointers on `device`: the launches on `stream`, no allocation, no synchronisation; only the scalar arguments
+ * are checked (a bad pair gets BAD_PAIR).  d_scratch holds *bytes of astroz_cuda_conjunction_mc_scratch_bytes(m,
+ * bytes), 16-byte aligned, for the work-item scan. */
+int32_t astroz_cuda_conjunction_mc_device(const double *d_elements, uint32_t n, int32_t grav,
+                                          const double *d_covariance, const uint8_t *d_model,
+                                          const uint32_t *d_primary, const uint32_t *d_secondary, const double *d_jd,
+                                          const double *d_fr, const double *d_window_min, const double *d_hbr_km,
+                                          const uint64_t *d_samples, const uint64_t *d_first, const uint64_t *d_seed,
+                                          uint32_t m, uint32_t record, int32_t device, uint64_t *d_counts,
+                                          double *d_sample_out, uint8_t *d_status, void *d_scratch, void *stream);
+/* The scratch of the device call for m candidates (the scan's size is the device's: ASTROZ_NO_DEVICE without one). */
+int32_t astroz_cuda_conjunction_mc_scratch_bytes(uint32_t m, uint64_t *bytes);
 /* ---- track correlation (K12): which catalogue rows predict a sensor track within their uncertainty ----------------------
  * The catalogue is K10's: elements[8][n], covariance[n][28] in the fit's variables (NULL: every P zero, a plain TLE
  * catalogue) and model[n] (NULL: all 0).  Track j is the observations [offsets[j], offsets[j + 1]) (offsets[0] = 0,

@@ -38,7 +38,9 @@ def zig_type(ctype: str, name: str) -> str:
         "const uint32_t *": "?[*]const u32",
         "uint32_t *": "?[*]u32",
         "int32_t *": "?[*]i32",
-        "uint64_t *": "?[*]u64" if name in ("steps", "d_steps", "n_samples", "d_n_samples") else "*u64",
+        "const uint64_t *": "?[*]const u64",
+        "uint64_t *": "?[*]u64" if name in ("steps", "d_steps", "n_samples", "d_n_samples", "counts", "d_counts")
+        else "*u64",
         "void *": "?*anyopaque",
         "void *const *": "?[*]const ?*anyopaque",
         "astroz_constellation_t": "Handle",
