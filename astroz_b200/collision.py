@@ -18,6 +18,12 @@ drawn pair's own TCA with the same search and counts the draws that come within 
 
     mc = monte_carlo(fit, primary, secondary, jd, fr, window_min=30.0, hbr_km=0.02, samples=10**7, seed=1)
     mc.pc, mc.interval(), mc.hits, mc.failed
+
+`importance_sampling` (K15) moves the same draws onto the linearised collision point and weights each by its exact
+likelihood ratio, which reaches the Pc values of 1e-5 to 1e-10 that plain sampling cannot afford.
+
+    r = importance_sampling(fit, primary, secondary, jd, fr, window_min=2.0, hbr_km=0.02, samples=10**6, seed=1)
+    r.pc, r.std_error, r.interval(), r.kind
 """
 from __future__ import annotations
 
@@ -283,3 +289,176 @@ def monte_carlo_device(elements, covariance, model, primary, secondary, jd, fr, 
         ptr(elements), n, int(grav), ptr(covariance), ptr(model), ptr(primary), ptr(secondary), ptr(jd), ptr(fr),
         ptr(window_min), ptr(hbr_km), ptr(samples), ptr(first), ptr(seed), m, record, int(elements.device.index),
         ptr(counts), ptr(sample_out), ptr(status), ptr(scratch), C.c_void_p(stream) if stream else None))
+
+
+# ---- importance sampling (K15, astroz_b200/csrc/az_conjunction_is.cu) --------------------------------------------------
+LINEAR, GIVEN, PLAIN = D["ASTROZ_CONJ_IS_LINEAR"], D["ASTROZ_CONJ_IS_GIVEN"], D["ASTROZ_CONJ_IS_PLAIN"]
+_IS_COUNT = D["ASTROZ_CONJ_IS_COUNT_WORDS"]
+_IS_PROPOSAL = D["ASTROZ_CONJ_IS_PROPOSAL_WORDS"]
+_IS_SAMPLE = D["ASTROZ_CONJ_IS_SAMPLE_WORDS"]
+
+
+def _u256(words) -> list[int]:
+    """(m, 4) uint64 words, least significant first -> m Python integers"""
+    w = np.asarray(words, dtype=np.uint64).reshape(-1, 4)
+    return [sum(int(x) << (64 * q) for q, x in enumerate(row)) for row in w]
+
+
+@dataclass
+class ImportanceResult:
+    counts: np.ndarray                # (m, 12) uint64: hits, edge, failed, overflow, V_hit[4], V2_hit[4]
+    samples: np.ndarray               # (m,) uint64: samples drawn
+    shift: np.ndarray                 # (m, 14) the shift c (primary's 7 normals, then the secondary's)
+    log_scale: np.ndarray             # (m,) l0 = -|c|^2 / 2
+    kind: np.ndarray                  # (m,) uint8 LINEAR, GIVEN or PLAIN
+    status: np.ndarray                # (m,) uint8 ASTROZ_CONJ_*: OK, INIT_FAILED, NOT_PSD
+    sample_dt: np.ndarray | None      # (m, record) dt_tca [min] (NaN: none)
+    sample_miss: np.ndarray | None    # (m, record) miss [km]
+    sample_log_weight: np.ndarray | None   # (m, record) log w
+
+    hits = property(lambda self: self.counts[:, 0])
+    edge = property(lambda self: self.counts[:, 1])
+    failed = property(lambda self: self.counts[:, 2])
+    overflow = property(lambda self: self.counts[:, 3])
+
+    def _sums(self):
+        """(e^l0 V_hit 2^-128 / N, e^2l0 V2_hit 2^-128 / N) per candidate from the words through Python integers"""
+        v, v2 = _u256(self.counts[:, 4:8]), _u256(self.counts[:, 8:12])
+        m1, m2 = np.zeros(len(v)), np.zeros(len(v))
+        for i, (a, b) in enumerate(zip(v, v2)):
+            n = int(self.samples[i])
+            if n == 0 or self.status[i] != OK:
+                m1[i] = m2[i] = np.nan
+                continue
+            l0 = float(self.log_scale[i])
+            m1[i] = np.exp(l0) * float(a) * 2.0 ** -128 / n
+            m2[i] = np.exp(2 * l0) * float(b) * 2.0 ** -128 / n
+        return m1, m2
+
+    @property
+    def pc(self) -> np.ndarray:
+        """(1 / N) sum over hits of w: unbiased for P(hit) (a failed draw counts as a non-hit); NaN with no sample"""
+        return self._sums()[0]
+
+    @property
+    def std_error(self) -> np.ndarray:
+        """the standard error of pc: sqrt((mean of w^2 over hits - pc^2) / (N - 1))"""
+        m1, m2 = self._sums()
+        n = self.samples.astype(np.float64)
+        with np.errstate(divide="ignore", invalid="ignore"):
+            return np.sqrt(np.maximum(m2 - m1 * m1, 0.0) / np.maximum(n - 1.0, 1.0))
+
+    def interval(self, z: float = 1.96) -> tuple[np.ndarray, np.ndarray]:
+        """The normal-approximation interval (lo, hi) of Pc at z standard errors, lo clipped at 0; NaN with no hit"""
+        p, s = self.pc, self.std_error
+        bad = ~(self.hits > 0) | np.isnan(p)
+        return np.where(bad, np.nan, np.maximum(p - z * s, 0.0)), np.where(bad, np.nan, p + z * s)
+
+    @property
+    def proposal_hit_fraction(self) -> np.ndarray:
+        """hits / N: the share of the proposal's draws that hit"""
+        n = self.samples.astype(np.float64)
+        with np.errstate(divide="ignore", invalid="ignore"):
+            return np.where(n > 0, self.hits.astype(np.float64) / n, np.nan)
+
+    def combine(self, other: "ImportanceResult") -> "ImportanceResult":
+        """The result over both runs' samples: the words added exactly.  Both must be the same candidates with the same
+        shift, drawn over disjoint sample ranges (first = N for the second run of N samples)."""
+        if self.counts.shape != other.counts.shape or not np.array_equal(self.shift, other.shift):
+            raise ValueError("combine needs the same candidates with the same shifts")
+        counts = self.counts.copy()
+        counts[:, :4] = self.counts[:, :4] + other.counts[:, :4]
+        for lo in (4, 8):
+            tot = [a + b for a, b in zip(_u256(self.counts[:, lo:lo + 4]), _u256(other.counts[:, lo:lo + 4]))]
+            counts[:, lo:lo + 4] = np.array([[(t >> (64 * q)) & (2 ** 64 - 1) for q in range(4)] for t in tot],
+                                            dtype=np.uint64).reshape(-1, 4)
+        return ImportanceResult(counts, self.samples + other.samples, self.shift.copy(), self.log_scale.copy(),
+                                self.kind.copy(), self.status.copy(), None, None, None)
+
+
+def importance_sampling(source, primary, secondary, jd, fr, *, window_min, hbr_km, samples, seed=0, first=0,
+                        record: int = 0, shift=None, covariance=None, model=None, grav: int = WGS72,
+                        device: int = 0) -> ImportanceResult:
+    """Importance-sampled collision probability of m candidate conjunctions (astroz_cuda_conjunction_is).
+
+    The arguments are those of `monte_carlo`, plus shift: None (the linear shift onto the collision point from the
+    nominal assessment) or (m, 14) / (14,) given shifts of the normals.  Each draw of `monte_carlo` is moved by the
+    shift and weighted by its exact likelihood ratio, so pc = (1 / N) sum over hits of w is unbiased whatever the shift;
+    a failed draw counts as a non-hit, so where draws fail pc estimates monte_carlo's pc times (1 - P(failed)).  Extend
+    a run with first = N and `combine`."""
+    el, cov, md = _catalogue(source, covariance, model)
+    n = el.shape[1]
+    pr, se = _rows(primary, secondary, n)
+    m = len(pr)
+    record = int(record)
+    if record < 0:
+        raise ValueError("record must be >= 0")
+    f64 = lambda a: np.ascontiguousarray(np.broadcast_to(np.asarray(a, dtype=np.float64), (m,)))  # noqa: E731
+
+    def u64(a, name):
+        a = np.asarray(a)
+        if a.size and (not np.issubdtype(a.dtype, np.integer) or a.min() < 0):
+            raise ValueError(f"{name} must hold integers >= 0")
+        return np.ascontiguousarray(np.broadcast_to(a.astype(np.uint64), (m,)))
+
+    jd_, fr_, w_, r_ = f64(jd), f64(fr), f64(window_min), f64(hbr_km)
+    ns, fi, sd = u64(samples, "samples"), u64(first, "first"), u64(seed, "seed")
+    sh = None if shift is None else np.ascontiguousarray(
+        np.broadcast_to(np.asarray(shift, dtype=np.float64), (m, _IS_PROPOSAL - 1)))
+    counts, stat = np.zeros((m, _IS_COUNT), np.uint64), np.zeros(m, dtype=np.uint8)
+    prop, kind = np.zeros((m, _IS_PROPOSAL)), np.zeros(m, dtype=np.uint8)
+    out = np.zeros((m, record, _IS_SAMPLE)) if record else None
+    vp = lambda a: None if a is None or a.size == 0 else C.c_void_p(a.ctypes.data)  # noqa: E731
+    check(lib().astroz_cuda_conjunction_is(vp(el), n, int(grav), vp(cov), vp(md), vp(pr), vp(se), vp(jd_), vp(fr_),
+                                           vp(w_), vp(r_), vp(ns), vp(fi), vp(sd), vp(sh), m, record, int(device),
+                                           vp(counts), vp(prop), vp(kind), vp(out), vp(stat)))
+    return ImportanceResult(counts, ns.copy(), prop[:, :-1], prop[:, -1], kind, stat,
+                            *((None,) * 3 if out is None else (out[:, :, 0], out[:, :, 1], out[:, :, 2])))
+
+
+def importance_sampling_scratch_bytes(m: int) -> int:
+    """The scratch of importance_sampling_device for m candidates"""
+    b = C.c_uint64(0)
+    check(lib().astroz_cuda_conjunction_is_scratch_bytes(int(m), C.byref(b)))
+    return int(b.value)
+
+
+def importance_sampling_device(elements, covariance, model, primary, secondary, jd, fr, window_min, hbr_km, samples,
+                               first, seed, shift, counts, proposal, proposal_kind, sample_out, status, scratch, *,
+                               grav: int = WGS72, stream: int = 0) -> None:
+    """`importance_sampling` with torch CUDA tensors on one device: the inputs of `monte_carlo_device`, shift (m, 14)
+    float64 or None (linear); counts (m, 12) int64, proposal (m, 15) float64 or None, proposal_kind (m,) uint8 or None,
+    sample_out (m, record, 3) float64 or None and status (m,) uint8 receive the results; scratch a uint8 tensor of at
+    least importance_sampling_scratch_bytes(m) bytes.  The launches go on `stream` (a raw cudaStream_t value, 0 = the
+    default stream).  Rows are not checked here: a bad pair gets status BAD_PAIR."""
+    import torch
+
+    n = int(elements.shape[1]) if elements.dim() == 2 and elements.shape[0] == 8 else -1
+    if n < 0 or elements.dtype != torch.float64 or not elements.is_cuda:
+        raise ValueError("elements must be a CUDA float64 tensor of shape (8, n)")
+    m = int(primary.numel())
+    record = int(sample_out.shape[1]) if sample_out is not None and sample_out.dim() == 3 else 0
+    tensors = [("elements", elements, 8 * n, torch.float64), ("covariance", covariance, 28 * n, torch.float64),
+               ("model", model, n, torch.uint8), ("primary", primary, m, torch.int32),
+               ("secondary", secondary, m, torch.int32), ("jd", jd, m, torch.float64), ("fr", fr, m, torch.float64),
+               ("window_min", window_min, m, torch.float64), ("hbr_km", hbr_km, m, torch.float64),
+               ("samples", samples, m, torch.int64), ("first", first, m, torch.int64), ("seed", seed, m, torch.int64),
+               ("shift", shift, (_IS_PROPOSAL - 1) * m, torch.float64), ("counts", counts, _IS_COUNT * m, torch.int64),
+               ("proposal", proposal, _IS_PROPOSAL * m, torch.float64), ("proposal_kind", proposal_kind, m, torch.uint8),
+               ("sample_out", sample_out, _IS_SAMPLE * record * m, torch.float64), ("status", status, m, torch.uint8)]
+    for name, t, size, dtype in tensors:
+        if t is None and name in ("model", "first", "seed", "shift", "proposal", "proposal_kind", "sample_out"):
+            continue
+        if not isinstance(t, torch.Tensor) or t.dtype != dtype or not t.is_contiguous() or int(t.numel()) != size \
+                or t.device != elements.device:
+            raise ValueError(f"{name} must be a contiguous {dtype} tensor of {size} elements on {elements.device}")
+    if not isinstance(scratch, torch.Tensor) or not scratch.is_contiguous() or scratch.device != elements.device \
+            or scratch.numel() * scratch.element_size() < importance_sampling_scratch_bytes(m):
+        raise ValueError(f"scratch must be a contiguous tensor of importance_sampling_scratch_bytes({m}) bytes on "
+                         f"{elements.device}")
+    ptr = lambda t: None if t is None else C.c_void_p(t.data_ptr())  # noqa: E731
+    check(lib().astroz_cuda_conjunction_is_device(
+        ptr(elements), n, int(grav), ptr(covariance), ptr(model), ptr(primary), ptr(secondary), ptr(jd), ptr(fr),
+        ptr(window_min), ptr(hbr_km), ptr(samples), ptr(first), ptr(seed), ptr(shift), m, record,
+        int(elements.device.index), ptr(counts), ptr(proposal), ptr(proposal_kind), ptr(sample_out), ptr(status),
+        ptr(scratch), C.c_void_p(stream) if stream else None))

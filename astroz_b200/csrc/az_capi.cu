@@ -27,7 +27,7 @@
 
 #include "az_covariance.cuh"
 #include "az_conjunction.cuh"
-#include "az_conjunction_mc.cuh"
+#include "az_conjunction_is.cuh"
 #include "az_correlate.cuh"
 #include "az_fit.cuh"
 #include "az_hostcopy.cuh"
@@ -3292,6 +3292,131 @@ int32_t astroz_cuda_conjunction_mc(const double *elements, uint32_t n, int32_t g
                                               seed ? reinterpret_cast<const uint64_t *>(d.piece(11)) : nullptr,
                                               d.piece(12), reinterpret_cast<uint64_t *>(d.piece(13)),
                                               record ? d.f64(14) : nullptr, d.u8(15), st);
+                       });
+}
+
+// ---- importance-sampled collision probability (K15, az_conjunction_is.cu, az_conjunction_is.cuh) ---------------------
+static_assert(ASTROZ_CONJ_IS_COUNT_WORDS == az::kIsCountWords && ASTROZ_CONJ_IS_PROPOSAL_WORDS == az::kIsProposalWords &&
+                  ASTROZ_CONJ_IS_SAMPLE_WORDS == az::kIsSampleWords && ASTROZ_CONJ_IS_LINEAR == az::kIsLinear &&
+                  ASTROZ_CONJ_IS_GIVEN == az::kIsGiven && ASTROZ_CONJ_IS_PLAIN == az::kIsPlain,
+              "importance-sampling layouts and proposal kinds");
+
+// Both call forms: a holds conj_mc_check's scalars, the arrays are on the device.
+static cudaError_t conj_is_run(az::ConjIsArgs a, const double *elements, const double *covariance,
+                               const uint8_t *model, const uint32_t *primary, const uint32_t *secondary,
+                               const double *jd, const double *fr, const double *window_min, const double *hbr_km,
+                               const uint64_t *samples, const uint64_t *first, const uint64_t *seed,
+                               const double *shift, void *scratch, uint64_t *counts, double *proposal,
+                               uint8_t *proposal_kind, double *sample_out, uint8_t *status, cudaStream_t st) {
+    a.elements = elements;
+    a.covariance = covariance;
+    a.model = model;
+    a.primary = primary;
+    a.secondary = secondary;
+    a.jd = jd;
+    a.fr = fr;
+    a.window = window_min;
+    a.hbr = hbr_km;
+    a.samples = samples;
+    a.first = first;
+    a.seed = seed;
+    a.shift = shift;
+    a.scratch = scratch;
+    a.counts = counts;
+    a.proposal = proposal;
+    a.kind = proposal_kind;
+    a.sampleOut = sample_out;
+    a.status = status;
+    return az::launch_conjunction_is(a, st);
+}
+
+int32_t astroz_cuda_conjunction_is_scratch_bytes(uint32_t m, uint64_t *bytes) {
+    if (!bytes) return ASTROZ_NULL_POINTER;
+    int count = 0;
+    const int32_t rc = check_device_present(&count, "no CUDA device available (the scan's scratch is the device's)");
+    if (rc != ASTROZ_OK) return rc;
+    size_t b = 0;
+    AZ_CUDA(az::conj_is_scratch_bytes(m, &b));
+    *bytes = b;
+    return ASTROZ_OK;
+}
+
+int32_t astroz_cuda_conjunction_is_device(const double *d_elements, uint32_t n, int32_t grav,
+                                          const double *d_covariance, const uint8_t *d_model,
+                                          const uint32_t *d_primary, const uint32_t *d_secondary, const double *d_jd,
+                                          const double *d_fr, const double *d_window_min, const double *d_hbr_km,
+                                          const uint64_t *d_samples, const uint64_t *d_first, const uint64_t *d_seed,
+                                          const double *d_shift, uint32_t m, uint32_t record, int32_t device,
+                                          uint64_t *d_counts, double *d_proposal, uint8_t *d_proposal_kind,
+                                          double *d_sample_out, uint8_t *d_status, void *d_scratch, void *stream) {
+    az::ConjIsArgs a{};
+    int32_t rc = conj_mc_check(n, grav, m, record, device, &a);
+    if (rc != ASTROZ_OK) return rc;
+    if (m == 0) return ASTROZ_OK;
+    if ((n && (!d_elements || !d_covariance)) || !d_primary || !d_secondary || !d_jd || !d_fr || !d_window_min ||
+        !d_hbr_km || !d_samples || !d_counts || !d_status || !d_scratch || (record && !d_sample_out))
+        return ASTROZ_NULL_POINTER;
+    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
+    AZ_CUDA(cudaSetDevice(device));
+    AZ_CUDA(conj_is_run(a, d_elements, d_covariance, d_model, d_primary, d_secondary, d_jd, d_fr, d_window_min,
+                        d_hbr_km, d_samples, d_first, d_seed, d_shift, d_scratch, d_counts, d_proposal,
+                        d_proposal_kind, d_sample_out, d_status, static_cast<cudaStream_t>(stream)));
+    return ASTROZ_OK;
+}
+
+int32_t astroz_cuda_conjunction_is(const double *elements, uint32_t n, int32_t grav, const double *covariance,
+                                   const uint8_t *model, const uint32_t *primary, const uint32_t *secondary,
+                                   const double *jd, const double *fr, const double *window_min, const double *hbr_km,
+                                   const uint64_t *samples, const uint64_t *first, const uint64_t *seed,
+                                   const double *shift, uint32_t m, uint32_t record, int32_t device, uint64_t *counts,
+                                   double *proposal, uint8_t *proposal_kind, double *sample_out, uint8_t *status) {
+    az::ConjIsArgs a{};
+    int32_t rc = conj_mc_check(n, grav, m, record, device, &a);
+    if (rc != ASTROZ_OK) return rc;
+    if (n && (!elements || !covariance)) return ASTROZ_NULL_POINTER;
+    if (m && (!primary || !secondary || !jd || !fr || !window_min || !hbr_km || !samples || !counts || !status))
+        return ASTROZ_NULL_POINTER;
+    if (m && record && !sample_out) return value_error("record > 0 needs sample_out");
+    for (uint32_t i = 0; i < m; ++i) {
+        if (primary[i] >= n || secondary[i] >= n) return value_error("a candidate's row is outside the catalogue");
+        if (primary[i] == secondary[i]) return value_error("a candidate pairs a row with itself");
+        if (!(window_min[i] > 0.0) || !std::isfinite(window_min[i]))
+            return value_error("half windows must be finite and > 0 minutes");
+        if (!(hbr_km[i] >= 0.0) || !std::isfinite(hbr_km[i]))
+            return value_error("hard-body radii must be finite and >= 0 km");
+        if (first && samples[i] > UINT64_MAX - first[i])
+            return value_error("first + samples must not exceed 2^64 - 1");
+    }
+    if ((rc = rows_check(elements, covariance, n)) != ASTROZ_OK) return rc;
+    if (!all_finite(jd, m) || !all_finite(fr, m)) return value_error("guess times must be finite");
+    if ((rc = model_bytes_check(model, n)) != ASTROZ_OK) return rc;
+    if (shift && !all_finite(shift, (size_t)az::kIsShift * m)) return value_error("shift words must be finite");
+    if (m == 0) return ASTROZ_OK;
+    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
+    size_t scratchBytes = 0;
+    AZ_CUDA(cudaSetDevice(device));
+    AZ_CUDA(az::conj_is_scratch_bytes(m, &scratchBytes));
+    return whole_batch(device,
+                       {upload(elements, (size_t)64 * n), upload(covariance, (size_t)8 * az::kFitN * n),
+                        upload(model, model ? (size_t)n : 0), upload(primary, (size_t)4 * m),
+                        upload(secondary, (size_t)4 * m), upload(jd, (size_t)8 * m), upload(fr, (size_t)8 * m),
+                        upload(window_min, (size_t)8 * m), upload(hbr_km, (size_t)8 * m),
+                        upload(samples, (size_t)8 * m), upload(first, first ? (size_t)8 * m : 0),
+                        upload(seed, seed ? (size_t)8 * m : 0), upload(shift, shift ? (size_t)8 * az::kIsShift * m : 0),
+                        scratch(scratchBytes), result(counts, (size_t)8 * az::kIsCountWords * m),
+                        result(proposal, proposal ? (size_t)8 * az::kIsProposalWords * m : 0),
+                        result(proposal_kind, proposal_kind ? (size_t)m : 0),
+                        result(sample_out, (size_t)8 * az::kIsSampleWords * record * m), result(status, m)},
+                       [&](const DeviceBlock &d, cudaStream_t st) {
+                           return conj_is_run(a, d.f64(0), d.f64(1), model ? d.u8(2) : nullptr, d.u32(3), d.u32(4),
+                                              d.f64(5), d.f64(6), d.f64(7), d.f64(8),
+                                              reinterpret_cast<const uint64_t *>(d.piece(9)),
+                                              first ? reinterpret_cast<const uint64_t *>(d.piece(10)) : nullptr,
+                                              seed ? reinterpret_cast<const uint64_t *>(d.piece(11)) : nullptr,
+                                              shift ? d.f64(12) : nullptr, d.piece(13),
+                                              reinterpret_cast<uint64_t *>(d.piece(14)),
+                                              proposal ? d.f64(15) : nullptr, proposal_kind ? d.u8(16) : nullptr,
+                                              record ? d.f64(17) : nullptr, d.u8(18), st);
                        });
 }
 

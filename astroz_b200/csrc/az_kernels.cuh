@@ -254,6 +254,20 @@ cudaError_t conj_mc_scratch_bytes(uint32_t m, size_t *bytes);
 // the candidates' statuses and work items, their scan, the near-earth pairs' items, then every other pair's
 cudaError_t launch_conjunction_mc(const ConjMcArgs &a, cudaStream_t stream);
 
+// K15: importance-sampled collision probability (az_conjunction_is.cu, az_conjunction_is.cuh).  Device pointers.  The
+// inherited fields are K14's, except counts [m][12] (hits, edge, failed, overflow, V_hit[4], V2_hit[4]), sampleOut
+// [m][record][3] (dt_tca, miss, log w) and scratch (conj_is_scratch_bytes(m)).
+struct ConjIsArgs : ConjMcArgs {
+    const double *shift = nullptr;       // [m][14] given shifts, nullable: the linear shift
+    double *proposal = nullptr;          // [m][15] c, l0; nullable
+    uint8_t *kind = nullptr;             // [m] ASTROZ_CONJ_IS_*, nullable
+    const double *prop = nullptr;        // set by launch_conjunction_is: the proposals in the scratch ...
+    const uint8_t *propKind = nullptr;   // ... and their kinds
+};
+cudaError_t conj_is_scratch_bytes(uint32_t m, size_t *bytes);
+// for linear shifts K11's assessment into the scratch and the proposal kernel; then K14's steps with the shift
+cudaError_t launch_conjunction_is(const ConjIsArgs &a, cudaStream_t stream);
+
 // K12: sensor tracks correlated with catalogue rows (az_correlate.cu, az_correlate.cuh).  Device pointers.
 struct CorrArgs {
     const double *elements = nullptr;    // [8][n]

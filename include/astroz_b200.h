@@ -832,6 +832,60 @@ int32_t astroz_cuda_conjunction_mc_device(const double *d_elements, uint32_t n, 
                                           double *d_sample_out, uint8_t *d_status, void *d_scratch, void *stream);
 /* The scratch of the device call for m candidates (the scan's size is the device's: ASTROZ_NO_DEVICE without one). */
 int32_t astroz_cuda_conjunction_mc_scratch_bytes(uint32_t m, uint64_t *bytes);
+/* ---- importance-sampled collision probability (K15): K14's draws shifted onto the collision point, weighted exactly --
+ * The catalogue, candidates, samples, first, seed, factor, status rules and normals are astroz_cuda_conjunction_mc's.
+ * u in R^14 are K14's normals of sample k (0 .. 6 the primary's, 7 .. 13 the secondary's) and c in R^14 the
+ * candidate's shift:
+ *   draw:      z = u + c, x_k = x^ + D^1/2 L z for each row; then K14's sets, TCA search, miss and FAILED / EDGE /
+ *              HIT rules;
+ *   weight:    log w_k = -u . c - |c|^2 / 2 = log phi(z) - log phi(z - c), exactly;
+ *   estimate:  Pc = (1 / N) sum over hits of w_k, N = samples[i]: unbiased for P(hit) whatever the shift.  A FAILED
+ *              draw counts as a non-hit, so where draws fail this estimates K14's hits / (N - failed) times
+ *              (1 - P(failed));
+ *   proposal:  shift NULL: LINEAR, from astroz_cuda_conjunction's assessment of the nominal pair (TEME): its TCA, plane
+ *              (x, y) and in-plane miss d = (dr . x, dr . y).  J_o is row o's forward-difference Jacobian of its TEME
+ *              position at the TCA (astroz_cuda_propagate_covariance's, B* held when P's B* row is zero), G = [-Pi J_p
+ *              D_p^1/2 L_p | Pi J_s D_s^1/2 L_s] (2 x 14, Pi the projection on x, y) and c = -G^T C+ d, the least-norm
+ *              shift with d + G c = 0 (C = G G^T, C+ by its 2 x 2 eigen-decomposition, an eigenvalue <= 1e-14 trace
+ *              counting as zero); |c|^2 = d^T C+ d.  A nominal WINDOW_EDGE is still LINEAR.  PLAIN (c = 0, K14's
+ *              draws): the nominal assessment is not OK or WINDOW_EDGE, a Jacobian cannot be formed, or C = 0.
+ *              shift non-NULL: GIVEN, c = shift[i][14];
+ *   sums:      each hit's v = exp(-u . c) and v^2 (v * v in fp64) rounded to multiples of 2^-128 and summed as unsigned
+ *              256-bit integers (four u64 words, least significant first); a hit with v >= 2^31 enters neither sum
+ *              and counts in overflow.  l0 = -|c|^2 / 2 is not accumulated: Pc = e^l0 V_hit 2^-128 / N.
+ * Outputs: counts[m][12] (hits, edge, failed, overflow, V_hit[4], V2_hit[4]); proposal[m][15] (nullable: c, l0);
+ * proposal_kind[m] (nullable: ASTROZ_CONJ_IS_*); sample_out[m][record][3] (dt_tca [min from jd + fr], miss [km], log
+ * w) of samples first .. first + record - 1, NaN where K14's are; status[m] as K14's.  A candidate that is not OK has
+ * zero counts and proposal words, PLAIN and NaN sample words.
+ * The counts are integer sums: the bytes do not depend on the batch, the order, the split of [first, first + samples)
+ * or the call form, and counts over [0, 2N) equal those over [0, N) plus those over [N, 2N).
+ * ASTROZ_VALUE_ERROR, nothing written: every refusal of astroz_cuda_conjunction_mc, and a non-finite shift word. */
+#define ASTROZ_CONJ_IS_COUNT_WORDS       12
+#define ASTROZ_CONJ_IS_PROPOSAL_WORDS    15
+#define ASTROZ_CONJ_IS_SAMPLE_WORDS      3
+#define ASTROZ_CONJ_IS_LINEAR            0
+#define ASTROZ_CONJ_IS_GIVEN             1
+#define ASTROZ_CONJ_IS_PLAIN             2
+/* HOST buffers: one upload (pageable through a pinned ring, pinned by direct DMA), the launches, plain copies back. */
+int32_t astroz_cuda_conjunction_is(const double *elements, uint32_t n, int32_t grav, const double *covariance,
+                                   const uint8_t *model, const uint32_t *primary, const uint32_t *secondary,
+                                   const double *jd, const double *fr, const double *window_min, const double *hbr_km,
+                                   const uint64_t *samples, const uint64_t *first, const uint64_t *seed,
+                                   const double *shift, uint32_t m, uint32_t record, int32_t device, uint64_t *counts,
+                                   double *proposal, uint8_t *proposal_kind, double *sample_out, uint8_t *status);
+/* DEVICE pointers on `device`: the launches on `stream`, no allocation, no synchronisation; only the scalar arguments
+ * are checked (a bad pair gets BAD_PAIR).  d_scratch holds *bytes of astroz_cuda_conjunction_is_scratch_bytes(m,
+ * bytes), 16-byte aligned: the work-item scan and the nominal assessment of linear shifts. */
+int32_t astroz_cuda_conjunction_is_device(const double *d_elements, uint32_t n, int32_t grav,
+                                          const double *d_covariance, const uint8_t *d_model,
+                                          const uint32_t *d_primary, const uint32_t *d_secondary, const double *d_jd,
+                                          const double *d_fr, const double *d_window_min, const double *d_hbr_km,
+                                          const uint64_t *d_samples, const uint64_t *d_first, const uint64_t *d_seed,
+                                          const double *d_shift, uint32_t m, uint32_t record, int32_t device,
+                                          uint64_t *d_counts, double *d_proposal, uint8_t *d_proposal_kind,
+                                          double *d_sample_out, uint8_t *d_status, void *d_scratch, void *stream);
+/* The scratch of the device call for m candidates (the scan's size is the device's: ASTROZ_NO_DEVICE without one). */
+int32_t astroz_cuda_conjunction_is_scratch_bytes(uint32_t m, uint64_t *bytes);
 /* ---- track correlation (K12): which catalogue rows predict a sensor track within their uncertainty ----------------------
  * The catalogue is K10's: elements[8][n], covariance[n][28] in the fit's variables (NULL: every P zero, a plain TLE
  * catalogue) and model[n] (NULL: all 0).  Track j is the observations [offsets[j], offsets[j + 1]) (offsets[0] = 0,
