@@ -462,3 +462,223 @@ def importance_sampling_device(elements, covariance, model, primary, secondary, 
         ptr(window_min), ptr(hbr_km), ptr(samples), ptr(first), ptr(seed), ptr(shift), m, record,
         int(elements.device.index), ptr(counts), ptr(proposal), ptr(proposal_kind), ptr(sample_out), ptr(status),
         ptr(scratch), C.c_void_p(stream) if stream else None))
+
+
+# ---- manoeuvre trials and the avoidance planner (K16, astroz_b200/csrc/az_avoid.cu) -----------------------------------
+CONVERSION_FAILED, BAD_TRIAL = D["ASTROZ_CONJ_CONVERSION_FAILED"], D["ASTROZ_CONJ_BAD_TRIAL"]
+STATUS_NAMES[CONVERSION_FAILED] = "the post-burn state could not be converted to an element set"
+STATUS_NAMES[BAD_TRIAL] = "bad trial: candidate index or burn not before the window"
+
+
+@dataclass
+class ManeuverResult(ConjunctionResult):
+    elements: np.ndarray = None          # (t, 8) the post-burn set (epoch, n, e, i, node, w, M, B*)
+    covariance: np.ndarray = None        # (t, 28) P' words in the fit's variables
+    residual: np.ndarray = None          # (t, 2) conversion residuals [km, km/s]
+    model: np.ndarray = None             # (t,) uint8 the primary's model byte
+
+    def catalogue_rows(self):
+        """(elements (8, t), covariance words (t, 28), model (t,)): the new rows, ready to append to the catalogue"""
+        return np.ascontiguousarray(self.elements.T), self.covariance.copy(), self.model.copy()
+
+
+def maneuver_trials(source, primary, secondary, jd, fr, *, window_min, hbr_km, candidate, burn_jd, burn_fr, dv_rtn,
+                    dv_sigma=None, covariance=None, model=None, grav: int = WGS72, device: int = 0) -> ManeuverResult:
+    """Reassess candidates after trial burns of their primary (astroz_cuda_conjunction_maneuver).
+
+    source, primary, secondary, jd, fr, window_min, hbr_km, covariance and model are those of `conjunctions`; the
+    primary is the object that burns.  Trial k burns candidate[k]'s primary at burn_jd[k] + burn_fr[k] (before the
+    window) by dv_rtn[k] (3,) [km/s] in its RTN frame, with execution sigmas dv_sigma[k] (3,) [km/s] or None; candidate,
+    burn_jd, burn_fr, dv_rtn and dv_sigma broadcast to the longest of them.  Each trial's post-burn set keeps the
+    primary's epoch; a zero burn copies the primary's row, so its record is conjunctions' record of the nominal pair.
+    The returned rows (catalogue_rows) are ordinary catalogue rows for every other call of this module.  P' inherits the
+    quantisation of the forward-difference B* columns of J and J' (about 1e-4 km per unit B* in LEO): on rows with B*
+    free and a large B* variance its phase entries are good to some 20 % of sqrt(P'_jj P'_kk) (a few cm along track at
+    the burn); rows with B* held are not affected (astroz_b200.h, K16)."""
+    el, cov, md = _catalogue(source, covariance, model)
+    n = el.shape[1]
+    pr, se = _rows(primary, secondary, n)
+    m = len(pr)
+    f64 = lambda a, k: np.ascontiguousarray(np.broadcast_to(np.asarray(a, dtype=np.float64), (k,)))  # noqa: E731
+    jd_, fr_, w_, r_ = f64(jd, m), f64(fr, m), f64(window_min, m), f64(hbr_km, m)
+    ca = np.asarray(candidate).reshape(-1) if np.ndim(candidate) else np.asarray([candidate])
+    if ca.size and (not np.issubdtype(ca.dtype, np.integer) or ca.min() < 0 or ca.max() >= m):
+        raise ValueError("candidate must hold candidate indices in [0, m)")
+    dv = np.asarray(dv_rtn, dtype=np.float64)
+    sg = None if dv_sigma is None else np.asarray(dv_sigma, dtype=np.float64)
+    t = max(len(ca), np.size(burn_jd), np.size(burn_fr), dv.size // 3 if dv.ndim > 1 else 1,
+            1 if sg is None or sg.ndim < 2 else len(sg))
+    ca = np.ascontiguousarray(np.broadcast_to(ca.astype(np.uint32), (t,)))
+    bj, bf = f64(burn_jd, t), f64(burn_fr, t)
+    dv = np.ascontiguousarray(np.broadcast_to(dv, (t, 3)))
+    sg = None if sg is None else np.ascontiguousarray(np.broadcast_to(sg, (t, 3)))
+    rec, stat = np.zeros((t, _WORDS)), np.zeros(t, dtype=np.uint8)
+    ne, nc, res = np.zeros((t, 8)), np.zeros((t, 28)), np.zeros((t, 2))
+    vp = lambda a: None if a is None or a.size == 0 else C.c_void_p(a.ctypes.data)  # noqa: E731
+    check(lib().astroz_cuda_conjunction_maneuver(vp(el), n, int(grav), vp(cov), vp(md), vp(pr), vp(se), vp(jd_),
+                                                 vp(fr_), vp(w_), vp(r_), m, vp(ca), vp(bj), vp(bf), vp(dv), vp(sg), t,
+                                                 int(device), vp(rec), vp(ne), vp(nc), vp(res), vp(stat)))
+    mdl = np.zeros(t, np.uint8) if md is None else md[pr[ca]]
+    return ManeuverResult(rec, jd_[ca], fr_[ca] + rec[:, 0] / 1440.0, None, None, stat, ne, nc, res, mdl)
+
+
+def maneuver_trials_scratch_bytes(t: int) -> int:
+    """The scratch of maneuver_trials_device for t trials"""
+    b = C.c_uint64(0)
+    check(lib().astroz_cuda_conjunction_maneuver_scratch_bytes(int(t), C.byref(b)))
+    return int(b.value)
+
+
+def maneuver_trials_device(elements, covariance, model, primary, secondary, jd, fr, window_min, hbr_km, candidate,
+                           burn_jd, burn_fr, dv_rtn, dv_sigma, record, new_elements, new_covariance, residual, status,
+                           scratch, *, grav: int = WGS72, stream: int = 0) -> None:
+    """`maneuver_trials` with torch CUDA tensors on one device: the catalogue and candidates of `conjunctions_device`,
+    candidate (t,) int32, burn_jd / burn_fr (t,) float64, dv_rtn (t, 3) float64, dv_sigma (t, 3) float64 or None;
+    record (t, 13) float64, new_elements (t, 8) / new_covariance (t, 28) / residual (t, 2) float64 or None and status
+    (t,) uint8 receive the results; scratch a uint8 tensor of at least maneuver_trials_scratch_bytes(t) bytes.  The
+    launches go on `stream` (a raw cudaStream_t value, 0 = the default stream).  Nothing is checked here: a bad
+    candidate index or burn time gets BAD_TRIAL, a bad pair BAD_PAIR."""
+    import torch
+
+    n = int(elements.shape[1]) if elements.dim() == 2 and elements.shape[0] == 8 else -1
+    if n < 0 or elements.dtype != torch.float64 or not elements.is_cuda:
+        raise ValueError("elements must be a CUDA float64 tensor of shape (8, n)")
+    m, t = int(primary.numel()), int(candidate.numel())
+    tensors = [("elements", elements, 8 * n, torch.float64), ("covariance", covariance, 28 * n, torch.float64),
+               ("model", model, n, torch.uint8), ("primary", primary, m, torch.int32),
+               ("secondary", secondary, m, torch.int32), ("jd", jd, m, torch.float64), ("fr", fr, m, torch.float64),
+               ("window_min", window_min, m, torch.float64), ("hbr_km", hbr_km, m, torch.float64),
+               ("candidate", candidate, t, torch.int32), ("burn_jd", burn_jd, t, torch.float64),
+               ("burn_fr", burn_fr, t, torch.float64), ("dv_rtn", dv_rtn, 3 * t, torch.float64),
+               ("dv_sigma", dv_sigma, 3 * t, torch.float64), ("record", record, _WORDS * t, torch.float64),
+               ("new_elements", new_elements, 8 * t, torch.float64),
+               ("new_covariance", new_covariance, 28 * t, torch.float64), ("residual", residual, 2 * t, torch.float64),
+               ("status", status, t, torch.uint8)]
+    for name, x, size, dtype in tensors:
+        if x is None and name in ("model", "dv_sigma", "new_elements", "new_covariance", "residual"):
+            continue
+        if not isinstance(x, torch.Tensor) or x.dtype != dtype or not x.is_contiguous() or int(x.numel()) != size \
+                or x.device != elements.device:
+            raise ValueError(f"{name} must be a contiguous {dtype} tensor of {size} elements on {elements.device}")
+    if not isinstance(scratch, torch.Tensor) or not scratch.is_contiguous() or scratch.device != elements.device \
+            or scratch.numel() * scratch.element_size() < maneuver_trials_scratch_bytes(t):
+        raise ValueError(f"scratch must be a contiguous tensor of maneuver_trials_scratch_bytes({t}) bytes on "
+                         f"{elements.device}")
+    ptr = lambda x: None if x is None else C.c_void_p(x.data_ptr())  # noqa: E731
+    check(lib().astroz_cuda_conjunction_maneuver_device(
+        ptr(elements), n, int(grav), ptr(covariance), ptr(model), ptr(primary), ptr(secondary), ptr(jd), ptr(fr),
+        ptr(window_min), ptr(hbr_km), m, ptr(candidate), ptr(burn_jd), ptr(burn_fr), ptr(dv_rtn), ptr(dv_sigma), t,
+        int(elements.device.index), ptr(record), ptr(new_elements), ptr(new_covariance), ptr(residual), ptr(status),
+        ptr(scratch), C.c_void_p(stream) if stream else None))
+
+
+NOT_FOUND = 255   # AvoidanceResult.status of a (candidate, lead, sign) where no step up to dv_max_kms is feasible
+
+
+@dataclass
+class AvoidanceResult:
+    dv_kms: np.ndarray         # (m, L, 2) the least |dv| found along -direction (0) and +direction (1); NaN: none
+    record: np.ndarray         # (m, L, 2, 13) the trial's record at that dv (zeros where NaN)
+    status: np.ndarray         # (m, L, 2) its status: OK, or NOT_FOUND where dv_kms is NaN
+    ladder_kms: np.ndarray     # (ladder,) the round-0 magnitudes
+    pc: np.ndarray             # (m, L, 2, ladder) round 0's Pc (NaN where the trial's status is not OK)
+    pc_nominal: np.ndarray     # (m,) the zero burn's Pc without execution error (NaN where it is not OK)
+    burn_jd: np.ndarray        # (m, L) the burn times: guess - lead, as jd ...
+    burn_fr: np.ndarray        # (m, L) ... and fr
+
+
+def _feasible(rec, st, pc_max):
+    """OK and Pc <= pc_max.  A WINDOW_EDGE record is taken at a window end, not at a TCA, so its Pc says nothing about
+    the encounter: a burn that moves the TCA out of the window is never feasible."""
+    return (st == OK) & (rec[..., 12] <= pc_max)
+
+
+def _avoidance(run, m, jd, fr, lead_min, direction, pc_max, dv_max_kms, ladder, rounds, dv_sigma):
+    """The planner over run(candidate, burn_jd, burn_fr, dv_rtn, dv_sigma (t, 3) or None) -> (record (t, 13),
+    status (t,))"""
+    lead = np.atleast_1d(np.asarray(lead_min, dtype=np.float64))
+    u = np.asarray(direction, dtype=np.float64).reshape(3)
+    if not np.isclose(np.linalg.norm(u), 1.0):
+        raise ValueError("direction must be a unit RTN vector")
+    if not (dv_max_kms > 0) or int(ladder) < 1 or int(rounds) < 0:
+        raise ValueError("dv_max_kms must be > 0, ladder >= 1 and rounds >= 0")
+    ladder, Lr = int(ladder), len(lead)
+    steps = dv_max_kms * 2.0 ** (np.arange(ladder) - (ladder - 1))   # geometric: dv_max / 2^(ladder-1) .. dv_max
+    bj = np.broadcast_to(jd[:, None], (m, Lr))
+    bf = fr[:, None] - lead[None, :] / 1440.0
+    sgn = np.array([-1.0, 1.0])
+    sg = None if dv_sigma is None else np.asarray(dv_sigma, dtype=np.float64).reshape(3)
+    sig = lambda t, zero=0: None if sg is None else np.r_[np.tile(sg, (t, 1)), np.zeros((zero, 3))]  # noqa: E731
+    # round 0: every (candidate, lead, sign, step), plus one zero burn per candidate without execution error
+    ci, li, si, ki = (a.reshape(-1) for a in np.meshgrid(np.arange(m), np.arange(Lr), np.arange(2), np.arange(ladder),
+                                                           indexing="ij"))
+    nt = len(ci)
+    cand = np.r_[ci, np.arange(m)]
+    bjd = np.r_[bj[ci, li], jd]
+    bfr = np.r_[bf[ci, li], fr - lead.max() / 1440.0]
+    dv = np.r_[(sgn[si] * steps[ki])[:, None] * u[None, :], np.zeros((m, 3))]
+    rec, st = run(cand, bjd, bfr, dv, sig(nt, m))
+    rec0, st0 = rec[:nt].reshape(m, Lr, 2, ladder, -1), st[:nt].reshape(m, Lr, 2, ladder)
+    pc_tab = np.where(st0 == OK, rec0[..., 12], np.nan)
+    feas = _feasible(rec0, st0, pc_max)
+    first = np.where(feas.any(-1), feas.argmax(-1), -1)
+    hi = np.where(first >= 0, steps[np.maximum(first, 0)], np.nan)
+    lo = np.where(first > 0, steps[np.maximum(first - 1, 0)], 0.0)
+    idx = np.maximum(first, 0)[..., None, None]
+    best_rec = np.where((first >= 0)[..., None], np.take_along_axis(rec0, idx, axis=3)[:, :, :, 0], 0.0)
+    best_st = np.where(first >= 0, np.take_along_axis(st0, idx[..., 0], axis=3)[..., 0], NOT_FOUND).astype(np.uint8)
+    # the nominal already meets the target: dv = 0 (no burn, so no execution error either)
+    zero_ok = _feasible(rec[nt:], st[nt:], pc_max)[:, None, None]
+    first = np.where(zero_ok, -1, first)
+    hi = np.where(zero_ok, 0.0, hi)
+    best_rec = np.where(zero_ok[..., None], rec[nt:][:, None, None], best_rec)
+    best_st = np.where(zero_ok, st[nt:][:, None, None], best_st).astype(np.uint8)
+    for _ in range(rounds):
+        open_ = np.argwhere(first >= 0)
+        if len(open_) == 0:
+            break
+        c, l, s = open_.T
+        mid = 0.5 * (lo[c, l, s] + hi[c, l, s])
+        r, q = run(c, bj[c, l], bf[c, l], (sgn[s] * mid)[:, None] * u[None, :], sig(len(c)))
+        ok = _feasible(r, q, pc_max)
+        hi[c[ok], l[ok], s[ok]] = mid[ok]
+        best_rec[c[ok], l[ok], s[ok]] = r[ok]
+        best_st[c[ok], l[ok], s[ok]] = q[ok]
+        lo[c[~ok], l[~ok], s[~ok]] = mid[~ok]
+    pc_nominal = np.where(st[nt:] == OK, rec[nt:, 12], np.nan)
+    return AvoidanceResult(hi, best_rec, best_st, steps, pc_tab, pc_nominal, np.array(bj), bf)
+
+
+def avoidance(source, primary, secondary, jd, fr, *, window_min, hbr_km, lead_min, direction=(0.0, 1.0, 0.0), pc_max,
+              dv_max_kms, ladder: int = 32, rounds: int = 20, dv_sigma=None, covariance=None, model=None,
+              grav: int = WGS72, device: int = 0) -> AvoidanceResult:
+    """The least |dv| along +-direction (a unit RTN vector) that brings each candidate's Pc to pc_max or below.
+
+    For each candidate, each lead in lead_min (burn = guess - lead minutes; each must come before the window) and
+    each sign, round 0 is one batched maneuver_trials call over a geometric ladder of `ladder` magnitudes up to
+    dv_max_kms (each step twice the one below it), plus the zero burn.  A trial is feasible when its status is OK and
+    its Pc <= pc_max.  WINDOW_EDGE is not feasible: its record is taken at a window end, not at a TCA, so a burn that
+    moves the encounter out of the window (along-track drift is about 3 dv t) is rejected however low that Pc is; give
+    window_min room for the shift the burns cause.  The first feasible step is bracketed against the step below it (or
+    0), and
+    `rounds` bisection rounds follow, each one batched call over all open brackets; the upper end always stays feasible,
+    so dv_kms meets the target and dv_kms (1 - 2 * 2^-rounds) of the bracket does not, to the ladder's resolution.
+    Pc(|dv|) need not be monotone: a burn can first move the miss towards the covariance's centre and raise Pc.  The
+    result is the least feasible dv at the ladder's resolution: a feasible interval narrower than one ladder step below
+    the first feasible step can be missed.  dv_kms is NaN where no step up to dv_max_kms works.  The whole round-0 table
+    is returned as pc (NaN where a trial is not OK).  pc_nominal is the zero burn's Pc, without execution error (no burn,
+    no execution error); where it already meets pc_max, dv_kms is 0 and the record is the nominal's.  dv_sigma (3,)
+    [km/s] is the execution error of every burn.  Where no step is feasible, dv_kms is NaN and status NOT_FOUND."""
+    el, cov, md = _catalogue(source, covariance, model)
+    n = el.shape[1]
+    pr, se = _rows(primary, secondary, n)
+    m = len(pr)
+    jd_ = np.ascontiguousarray(np.broadcast_to(np.asarray(jd, dtype=np.float64), (m,)))
+    fr_ = np.ascontiguousarray(np.broadcast_to(np.asarray(fr, dtype=np.float64), (m,)))
+
+    def run(cand, bjd, bfr, dv, sg):
+        r = maneuver_trials(el, pr, se, jd_, fr_, window_min=window_min, hbr_km=hbr_km, candidate=cand, burn_jd=bjd,
+                            burn_fr=bfr, dv_rtn=dv, dv_sigma=sg, covariance=cov, model=md, grav=grav, device=device)
+        return r.record, r.status
+
+    return _avoidance(run, m, jd_, fr_, lead_min, direction, pc_max, dv_max_kms, ladder, rounds, dv_sigma)

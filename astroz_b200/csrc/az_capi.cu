@@ -25,6 +25,7 @@
 #include <thread>
 #include <vector>
 
+#include "az_avoid.cuh"
 #include "az_covariance.cuh"
 #include "az_conjunction.cuh"
 #include "az_conjunction_is.cuh"
@@ -3107,6 +3108,24 @@ static cudaError_t conj_run(az::ConjArgs a, const double *elements, const double
     return az::launch_conjunction(a, st);
 }
 
+// The value checks of astroz_cuda_conjunction's host call on its catalogue and candidates (pointers already checked).
+static int32_t conj_inputs_check(const double *elements, uint32_t n, const double *covariance, const uint8_t *model,
+                                 const uint32_t *primary, const uint32_t *secondary, const double *jd, const double *fr,
+                                 const double *window_min, const double *hbr_km, uint32_t m) {
+    for (uint32_t i = 0; i < m; ++i) {
+        if (primary[i] >= n || secondary[i] >= n) return value_error("a candidate's row is outside the catalogue");
+        if (primary[i] == secondary[i]) return value_error("a candidate pairs a row with itself");
+        if (!(window_min[i] > 0.0) || !std::isfinite(window_min[i]))
+            return value_error("half windows must be finite and > 0 minutes");
+        if (!(hbr_km[i] >= 0.0) || !std::isfinite(hbr_km[i]))
+            return value_error("hard-body radii must be finite and >= 0 km");
+    }
+    int32_t rc = rows_check(elements, covariance, n);
+    if (rc != ASTROZ_OK) return rc;
+    if (!all_finite(jd, m) || !all_finite(fr, m)) return value_error("guess times must be finite");
+    return model_bytes_check(model, n);
+}
+
 int32_t astroz_cuda_conjunction_device(const double *d_elements, uint32_t n, int32_t grav, const double *d_covariance,
                                        const uint8_t *d_model, const uint32_t *d_primary, const uint32_t *d_secondary,
                                        const double *d_jd, const double *d_fr, const double *d_window_min,
@@ -3138,17 +3157,9 @@ int32_t astroz_cuda_conjunction(const double *elements, uint32_t n, int32_t grav
     if (n && (!elements || !covariance)) return ASTROZ_NULL_POINTER;
     if (m && (!primary || !secondary || !jd || !fr || !window_min || !hbr_km || !record || !status))
         return ASTROZ_NULL_POINTER;
-    for (uint32_t i = 0; i < m; ++i) {
-        if (primary[i] >= n || secondary[i] >= n) return value_error("a candidate's row is outside the catalogue");
-        if (primary[i] == secondary[i]) return value_error("a candidate pairs a row with itself");
-        if (!(window_min[i] > 0.0) || !std::isfinite(window_min[i]))
-            return value_error("half windows must be finite and > 0 minutes");
-        if (!(hbr_km[i] >= 0.0) || !std::isfinite(hbr_km[i]))
-            return value_error("hard-body radii must be finite and >= 0 km");
-    }
-    if ((rc = rows_check(elements, covariance, n)) != ASTROZ_OK) return rc;
-    if (!all_finite(jd, m) || !all_finite(fr, m)) return value_error("guess times must be finite");
-    if ((rc = model_bytes_check(model, n)) != ASTROZ_OK) return rc;
+    if ((rc = conj_inputs_check(elements, n, covariance, model, primary, secondary, jd, fr, window_min, hbr_km, m)) !=
+        ASTROZ_OK)
+        return rc;
     if (m == 0) return ASTROZ_OK;
     return whole_batch(device,
                        {upload(elements, (size_t)64 * n), upload(covariance, (size_t)8 * az::kFitN * n),
@@ -3417,6 +3428,139 @@ int32_t astroz_cuda_conjunction_is(const double *elements, uint32_t n, int32_t g
                                               reinterpret_cast<uint64_t *>(d.piece(14)),
                                               proposal ? d.f64(15) : nullptr, proposal_kind ? d.u8(16) : nullptr,
                                               record ? d.f64(17) : nullptr, d.u8(18), st);
+                       });
+}
+
+// ---- collision-avoidance manoeuvre trials (K16, az_avoid.cu, az_avoid.cuh) -------------------------------------------
+static_assert(ASTROZ_CONJ_CONVERSION_FAILED == az::kConjConversionFailed && ASTROZ_CONJ_BAD_TRIAL == az::kConjBadTrial,
+              "manoeuvre status bytes");
+
+// Scalar checks of the manoeuvre calls, before anything is read, written or allocated; a receives the scalars.
+static int32_t avoid_check(uint32_t n, int32_t grav, uint32_t m, uint32_t t, int32_t device, az::AvoidArgs *a) {
+    if (device < 0) return value_error("manoeuvre trials run on one device: pass its ordinal");
+    const int32_t rc = grav_check(grav);
+    if (rc != ASTROZ_OK) return rc;
+    if (t >= 0x80000000u) return value_error("t must be below 2^31 (the reassessment's catalogue has 2t rows)");
+    a->n = n;
+    a->m = m;
+    a->t = t;
+    a->grav = grav;
+    a->g = az::grav_consts(az::gravity(grav));
+    return ASTROZ_OK;
+}
+
+// Both call forms: a holds avoid_check's scalars, the arrays are on the device.
+static cudaError_t avoid_run(az::AvoidArgs a, const double *elements, const double *covariance, const uint8_t *model,
+                             const uint32_t *primary, const uint32_t *secondary, const double *jd, const double *fr,
+                             const double *window_min, const double *hbr_km, const uint32_t *candidate,
+                             const double *burn_jd, const double *burn_fr, const double *dv_rtn,
+                             const double *dv_sigma, void *scratch, double *record, double *new_elements,
+                             double *new_covariance, double *residual, uint8_t *status, cudaStream_t st) {
+    a.elements = elements;
+    a.covariance = covariance;
+    a.model = model;
+    a.primary = primary;
+    a.secondary = secondary;
+    a.jd = jd;
+    a.fr = fr;
+    a.window = window_min;
+    a.hbr = hbr_km;
+    a.candidate = candidate;
+    a.burnJd = burn_jd;
+    a.burnFr = burn_fr;
+    a.dv = dv_rtn;
+    a.dvSigma = dv_sigma;
+    a.scratch = scratch;
+    a.record = record;
+    a.newElements = new_elements;
+    a.newCovariance = new_covariance;
+    a.residual = residual;
+    a.status = status;
+    return az::launch_avoid(a, st);
+}
+
+int32_t astroz_cuda_conjunction_maneuver_scratch_bytes(uint32_t t, uint64_t *bytes) {
+    if (!bytes) return ASTROZ_NULL_POINTER;
+    *bytes = az::avoid_scratch_bytes(t);
+    return ASTROZ_OK;
+}
+
+int32_t astroz_cuda_conjunction_maneuver_device(const double *d_elements, uint32_t n, int32_t grav,
+                                                const double *d_covariance, const uint8_t *d_model,
+                                                const uint32_t *d_primary, const uint32_t *d_secondary,
+                                                const double *d_jd, const double *d_fr, const double *d_window_min,
+                                                const double *d_hbr_km, uint32_t m, const uint32_t *d_candidate,
+                                                const double *d_burn_jd, const double *d_burn_fr,
+                                                const double *d_dv_rtn, const double *d_dv_sigma, uint32_t t,
+                                                int32_t device, double *d_record, double *d_new_elements,
+                                                double *d_new_covariance, double *d_residual, uint8_t *d_status,
+                                                void *d_scratch, void *stream) {
+    az::AvoidArgs a{};
+    int32_t rc = avoid_check(n, grav, m, t, device, &a);
+    if (rc != ASTROZ_OK) return rc;
+    if (t == 0) return ASTROZ_OK;
+    if ((n && (!d_elements || !d_covariance)) || (m && (!d_primary || !d_secondary || !d_jd || !d_fr ||
+                                                        !d_window_min || !d_hbr_km)) ||
+        !d_candidate || !d_burn_jd || !d_burn_fr || !d_dv_rtn || !d_record || !d_status || !d_scratch)
+        return ASTROZ_NULL_POINTER;
+    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
+    AZ_CUDA(cudaSetDevice(device));
+    AZ_CUDA(avoid_run(a, d_elements, d_covariance, d_model, d_primary, d_secondary, d_jd, d_fr, d_window_min, d_hbr_km,
+                      d_candidate, d_burn_jd, d_burn_fr, d_dv_rtn, d_dv_sigma, d_scratch, d_record, d_new_elements,
+                      d_new_covariance, d_residual, d_status, static_cast<cudaStream_t>(stream)));
+    return ASTROZ_OK;
+}
+
+int32_t astroz_cuda_conjunction_maneuver(const double *elements, uint32_t n, int32_t grav, const double *covariance,
+                                         const uint8_t *model, const uint32_t *primary, const uint32_t *secondary,
+                                         const double *jd, const double *fr, const double *window_min,
+                                         const double *hbr_km, uint32_t m, const uint32_t *candidate,
+                                         const double *burn_jd, const double *burn_fr, const double *dv_rtn,
+                                         const double *dv_sigma, uint32_t t, int32_t device, double *record,
+                                         double *new_elements, double *new_covariance, double *residual,
+                                         uint8_t *status) {
+    az::AvoidArgs a{};
+    int32_t rc = avoid_check(n, grav, m, t, device, &a);
+    if (rc != ASTROZ_OK) return rc;
+    if (n && (!elements || !covariance)) return ASTROZ_NULL_POINTER;
+    if (m && (!primary || !secondary || !jd || !fr || !window_min || !hbr_km)) return ASTROZ_NULL_POINTER;
+    if (t && (!candidate || !burn_jd || !burn_fr || !dv_rtn || !record || !status)) return ASTROZ_NULL_POINTER;
+    if ((rc = conj_inputs_check(elements, n, covariance, model, primary, secondary, jd, fr, window_min, hbr_km, m)) !=
+        ASTROZ_OK)
+        return rc;
+    if (!all_finite(burn_jd, t) || !all_finite(burn_fr, t)) return value_error("burn times must be finite");
+    if (!all_finite(dv_rtn, (size_t)3 * t)) return value_error("dv words must be finite");
+    if (dv_sigma)
+        for (size_t q = 0; q < (size_t)3 * t; ++q)
+            if (!(dv_sigma[q] >= 0.0) || !std::isfinite(dv_sigma[q]))
+                return value_error("execution sigmas must be finite and >= 0 km/s");
+    for (uint32_t k = 0; k < t; ++k) {
+        const uint32_t c = candidate[k];
+        if (c >= m) return value_error("a trial's candidate index is not below m");
+        const double epoch = elements[primary[c]];
+        const double tsb = az::pairs_tsince_deep(az::add_rn(burn_jd[k], burn_fr[k]), epoch);
+        const double ts0 = az::pairs_tsince_deep(az::add_rn(jd[c], fr[c]), epoch);
+        if (!(tsb <= ts0 - window_min[c])) return value_error("a burn does not come before its candidate's window");
+    }
+    if (t == 0) return ASTROZ_OK;
+    return whole_batch(device,
+                       {upload(elements, (size_t)64 * n), upload(covariance, (size_t)8 * az::kFitN * n),
+                        upload(model, model ? (size_t)n : 0), upload(primary, (size_t)4 * m),
+                        upload(secondary, (size_t)4 * m), upload(jd, (size_t)8 * m), upload(fr, (size_t)8 * m),
+                        upload(window_min, (size_t)8 * m), upload(hbr_km, (size_t)8 * m),
+                        upload(candidate, (size_t)4 * t), upload(burn_jd, (size_t)8 * t),
+                        upload(burn_fr, (size_t)8 * t), upload(dv_rtn, (size_t)24 * t),
+                        upload(dv_sigma, dv_sigma ? (size_t)24 * t : 0), scratch(az::avoid_scratch_bytes(t)),
+                        result(record, (size_t)8 * az::kConjRecordWords * t),
+                        result(new_elements, new_elements ? (size_t)64 * t : 0),
+                        result(new_covariance, new_covariance ? (size_t)8 * az::kFitN * t : 0),
+                        result(residual, residual ? (size_t)16 * t : 0), result(status, t)},
+                       [&](const DeviceBlock &d, cudaStream_t st) {
+                           return avoid_run(a, d.f64(0), d.f64(1), model ? d.u8(2) : nullptr, d.u32(3), d.u32(4),
+                                            d.f64(5), d.f64(6), d.f64(7), d.f64(8), d.u32(9), d.f64(10), d.f64(11),
+                                            d.f64(12), dv_sigma ? d.f64(13) : nullptr, d.piece(14), d.f64(15),
+                                            new_elements ? d.f64(16) : nullptr, new_covariance ? d.f64(17) : nullptr,
+                                            residual ? d.f64(18) : nullptr, d.u8(19), st);
                        });
 }
 

@@ -321,6 +321,11 @@ size_t iod_scratch_bytes(uint32_t t);
 // the IOD kernel, K8's near-earth and deep-space fits over one TEME state per track, and the finishing kernel
 cudaError_t launch_iod(const IodArgs &a, cudaStream_t stream);
 
+// K16: collision-avoidance manoeuvre trials (az_avoid.cu, az_avoid.cuh; AvoidArgs and avoid_scratch_bytes are there).
+// K10 at the burn, the burn, K8's conversion, K10 on the new sets, the covariance transport, K11, the finishing kernel
+struct AvoidArgs;
+cudaError_t launch_avoid(const AvoidArgs &a, cudaStream_t stream);
+
 // DFMA throughput microbenchmark: returns achieved fp64 FLOP/s (FMA = 2).
 cudaError_t measure_fp64_peak(double *flops);
 // Arithmetic peak of the fp64 pipe: SMs x 64 lanes x 2 FLOP x the maximum SM clock.

@@ -886,6 +886,80 @@ int32_t astroz_cuda_conjunction_is_device(const double *d_elements, uint32_t n, 
                                           double *d_sample_out, uint8_t *d_status, void *d_scratch, void *stream);
 /* The scratch of the device call for m candidates (the scan's size is the device's: ASTROZ_NO_DEVICE without one). */
 int32_t astroz_cuda_conjunction_is_scratch_bytes(uint32_t m, uint64_t *bytes);
+/* ---- collision-avoidance manoeuvre trials (K16): burn the primary, refit it, carry its covariance, reassess -----------
+ * The catalogue and candidates are astroz_cuda_conjunction's.  The PRIMARY of a candidate is the object that burns: to
+ * plan a burn of the other object, swap the two.  Trial k takes candidate[k] < m, a burn time burn_jd[k] + burn_fr[k],
+ * an impulsive dv_rtn[k][3] [km/s] in the primary's RTN frame at the burn (R = r / |r|, N = r x v / |r x v|, T = N x R)
+ * and dv_sigma[k][3] (NULL: all 0), the 1-sigma execution error per RTN axis [km/s] (independent axes, uncorrelated with
+ * the orbit error).  Per trial:
+ *   burn:       ts_b = ((burn_jd + burn_fr) - epoch) * 1440, formed as astroz_cuda_propagate_covariance forms tsince,
+ *               must come before the window: ts_b <= ts0 - w (ts0 the candidate's guess tsince, w its half window).
+ *               x(t_b) and J (6 x 7, TEME) are astroz_cuda_propagate_covariance's nominal and Jacobian of the primary's
+ *               row at t_b (B* held when P's B* row is zero); the post-burn state is x(t_b) + [0; R dv];
+ *   conversion: the element fit (astroz_cuda_fit_elements_mixed's kernels, no other least squares) from the primary's
+ *               own set to the one TEME state at t_b, B* held at the primary's B*, pos_sigma 1 km, vel_sigma 1e-3
+ *               km/s, at most 50 iterations; the class follows the primary's set.  THE EPOCH STAYS THE PRIMARY'S
+ *               EPOCH: the new set meets the post-burn state at t_b and shares the nominal's drag history, where a set
+ *               re-epoched at the burn would restart SGP4's drag terms there and drift from the nominal even for a zero
+ *               burn.  CONVERSION_FAILED: the fit does not converge, its residuals exceed 1e-6 km / 1e-9 km/s, or the
+ *               new set cannot be built or propagated under the primary's model byte (a burn that moves the period
+ *               across 225 min);
+ *   zero burn:  dv = (0, 0, 0): the new row is the primary's set, copied (no fit), so with dv_sigma zero the trial's
+ *               record is astroz_cuda_conjunction's record of the nominal pair bit for bit;
+ *   covariance: J' = the Jacobian of the new set at t_b (same routine), J'6 its six orbital columns.  A (7 x 7): rows
+ *               0-5 J'6^-1 (J - J'(:, B*) e_B*^T), row 6 e_B*^T (B* carried over, a held B* stays held).  P' = A P A^T
+ *               + [J'6^-1 [0 0; 0 R diag(sigma^2) R^T] J'6^-T, 0; 0, 0].  J'6^-1 by LU with partial pivoting on J'6
+ *               equilibrated by rows, then columns, to a largest |entry| of 1: a pivot |u| <= 1e-12 is singular
+ *               (CONVERSION_FAILED);
+ *   reassess:   astroz_cuda_conjunction (TEME) on the pair (new row with P' and the primary's model byte, the
+ *               secondary's row) with the candidate's guess, window and radius.
+ * THE RETURNED ROW IS AN ORDINARY CATALOGUE ROW: appended to the catalogue (elements, P', the primary's model byte) it
+ * gives the trial's record bit for bit from astroz_cuda_conjunction, and it feeds the Monte Carlo, importance-sampling,
+ * pairs and screening calls unchanged, which is how a chosen burn is verified with K15 or the post-burn orbit screened.
+ * Outputs: record[T][13] astroz_cuda_conjunction's record (dt_tca from the candidate's guess); elements[T][8] (nullable)
+ * the new set; covariance[T][28] (nullable) P'; residual[T][2] (nullable) the conversion residuals [km, km/s], 0 for a
+ * zero burn; status[T], the first that applies: BAD_TRIAL / BAD_PAIR (device call only: candidate index >= m, burn not
+ * before the window / a bad row pair); INIT_FAILED (a model byte > 1 on the device call, or the primary's set cannot be
+ * built at t_b) / CELL_FAILED (its deep-space cell fails at t_b); CONVERSION_FAILED; then astroz_cuda_conjunction's
+ * statuses of the post-burn pair.  A trial that is not assessed (stopped before the reassessment, or INIT_FAILED /
+ * CELL_FAILED of the post-burn pair in it) has every output zero.
+ * Precision of P': J and J' are forward differences, and their B* columns are quantised at about ulp(|r|) / 1e-8 (1e-4
+ * km per unit B* in LEO).  A's B* column is the difference of two such columns mapped through J'6^-1, so on a row with
+ * B* free whose B* variance dwarfs its orbital ones, P''s phase (lambda) entries carry that noise: measured up to 0.21
+ * of sqrt(P'_jj P'_kk) on fitted LEO rows (an along-track error of a few cm at the burn), the same size in any build.
+ * Rows with B* held do not carry it.  The reassessment's C2 agrees between builds within 5e-3 of its trace.
+ * Limits: impulsive burns of one object, one burn per trial; the errors of the two objects are uncorrelated.
+ * A trial's bytes depend on its own inputs, its candidate and its two rows alone: not on the batch, its order or the
+ * call form.
+ * ASTROZ_VALUE_ERROR, nothing written: device = -1, an unknown grav, T >= 2^31; and for the host call every refusal of
+ * astroz_cuda_conjunction, a candidate index >= m, a burn not before its window, a non-finite burn time, dv or sigma
+ * word, a negative sigma. */
+#define ASTROZ_CONJ_CONVERSION_FAILED  7
+#define ASTROZ_CONJ_BAD_TRIAL          8
+/* HOST buffers: one upload (pageable through a pinned ring, pinned by direct DMA), the launches, plain copies back. */
+int32_t astroz_cuda_conjunction_maneuver(const double *elements, uint32_t n, int32_t grav, const double *covariance,
+                                         const uint8_t *model, const uint32_t *primary, const uint32_t *secondary,
+                                         const double *jd, const double *fr, const double *window_min,
+                                         const double *hbr_km, uint32_t m, const uint32_t *candidate,
+                                         const double *burn_jd, const double *burn_fr, const double *dv_rtn,
+                                         const double *dv_sigma, uint32_t t, int32_t device, double *record,
+                                         double *new_elements, double *new_covariance, double *residual,
+                                         uint8_t *status);
+/* DEVICE pointers on `device`: the launches on `stream`, no allocation, no synchronisation; only the scalar arguments
+ * are checked (a bad candidate index or burn time gets BAD_TRIAL, a bad pair BAD_PAIR).  d_scratch holds *bytes of
+ * astroz_cuda_conjunction_maneuver_scratch_bytes(t, bytes), 16-byte aligned. */
+int32_t astroz_cuda_conjunction_maneuver_device(const double *d_elements, uint32_t n, int32_t grav,
+                                                const double *d_covariance, const uint8_t *d_model,
+                                                const uint32_t *d_primary, const uint32_t *d_secondary,
+                                                const double *d_jd, const double *d_fr, const double *d_window_min,
+                                                const double *d_hbr_km, uint32_t m, const uint32_t *d_candidate,
+                                                const double *d_burn_jd, const double *d_burn_fr,
+                                                const double *d_dv_rtn, const double *d_dv_sigma, uint32_t t,
+                                                int32_t device, double *d_record, double *d_new_elements,
+                                                double *d_new_covariance, double *d_residual, uint8_t *d_status,
+                                                void *d_scratch, void *stream);
+/* The scratch of the device call for t trials. */
+int32_t astroz_cuda_conjunction_maneuver_scratch_bytes(uint32_t t, uint64_t *bytes);
 /* ---- track correlation (K12): which catalogue rows predict a sensor track within their uncertainty ----------------------
  * The catalogue is K10's: elements[8][n], covariance[n][28] in the fit's variables (NULL: every P zero, a plain TLE
  * catalogue) and model[n] (NULL: all 0).  Track j is the observations [offsets[j], offsets[j + 1]) (offsets[0] = 0,

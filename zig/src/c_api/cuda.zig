@@ -105,6 +105,9 @@ pub extern fn astroz_cuda_conjunction_mc_scratch_bytes(m: u32, bytes: *u64) i32;
 pub extern fn astroz_cuda_conjunction_is(elements: ?[*]const f64, n: u32, grav: i32, covariance: ?[*]const f64, model: ?[*]const u8, primary: ?[*]const u32, secondary: ?[*]const u32, jd: ?[*]const f64, fr: ?[*]const f64, window_min: ?[*]const f64, hbr_km: ?[*]const f64, samples: ?[*]const u64, first: ?[*]const u64, seed: ?[*]const u64, shift: ?[*]const f64, m: u32, record: u32, device: i32, counts: ?[*]u64, proposal: ?[*]f64, proposal_kind: ?[*]u8, sample_out: ?[*]f64, status: ?[*]u8) i32;
 pub extern fn astroz_cuda_conjunction_is_device(d_elements: ?[*]const f64, n: u32, grav: i32, d_covariance: ?[*]const f64, d_model: ?[*]const u8, d_primary: ?[*]const u32, d_secondary: ?[*]const u32, d_jd: ?[*]const f64, d_fr: ?[*]const f64, d_window_min: ?[*]const f64, d_hbr_km: ?[*]const f64, d_samples: ?[*]const u64, d_first: ?[*]const u64, d_seed: ?[*]const u64, d_shift: ?[*]const f64, m: u32, record: u32, device: i32, d_counts: ?[*]u64, d_proposal: ?[*]f64, d_proposal_kind: ?[*]u8, d_sample_out: ?[*]f64, d_status: ?[*]u8, d_scratch: ?*anyopaque, stream: ?*anyopaque) i32;
 pub extern fn astroz_cuda_conjunction_is_scratch_bytes(m: u32, bytes: *u64) i32;
+pub extern fn astroz_cuda_conjunction_maneuver(elements: ?[*]const f64, n: u32, grav: i32, covariance: ?[*]const f64, model: ?[*]const u8, primary: ?[*]const u32, secondary: ?[*]const u32, jd: ?[*]const f64, fr: ?[*]const f64, window_min: ?[*]const f64, hbr_km: ?[*]const f64, m: u32, candidate: ?[*]const u32, burn_jd: ?[*]const f64, burn_fr: ?[*]const f64, dv_rtn: ?[*]const f64, dv_sigma: ?[*]const f64, t: u32, device: i32, record: ?[*]f64, new_elements: ?[*]f64, new_covariance: ?[*]f64, residual: ?[*]f64, status: ?[*]u8) i32;
+pub extern fn astroz_cuda_conjunction_maneuver_device(d_elements: ?[*]const f64, n: u32, grav: i32, d_covariance: ?[*]const f64, d_model: ?[*]const u8, d_primary: ?[*]const u32, d_secondary: ?[*]const u32, d_jd: ?[*]const f64, d_fr: ?[*]const f64, d_window_min: ?[*]const f64, d_hbr_km: ?[*]const f64, m: u32, d_candidate: ?[*]const u32, d_burn_jd: ?[*]const f64, d_burn_fr: ?[*]const f64, d_dv_rtn: ?[*]const f64, d_dv_sigma: ?[*]const f64, t: u32, device: i32, d_record: ?[*]f64, d_new_elements: ?[*]f64, d_new_covariance: ?[*]f64, d_residual: ?[*]f64, d_status: ?[*]u8, d_scratch: ?*anyopaque, stream: ?*anyopaque) i32;
+pub extern fn astroz_cuda_conjunction_maneuver_scratch_bytes(t: u32, bytes: *u64) i32;
 pub extern fn astroz_cuda_correlate(elements: ?[*]const f64, n: u32, grav: i32, covariance: ?[*]const f64, model: ?[*]const u8, offsets: ?[*]const u32, t: u32, jd: ?[*]const f64, fr: ?[*]const f64, kind: ?[*]const u8, value: ?[*]const f64, sigma: ?[*]const f64, station: ?[*]const u32, m: u32, stations: ?[*]const f64, k: u32, gate_probability: f64, best: u32, device: i32, rows: ?[*]u32, d2: ?[*]f64, used: ?[*]u32, n_gate: ?[*]u32, n_failed: ?[*]u32, status: ?[*]u8, row_status: ?[*]u8) i32;
 pub extern fn astroz_cuda_correlate_device(d_elements: ?[*]const f64, n: u32, grav: i32, d_covariance: ?[*]const f64, d_model: ?[*]const u8, d_offsets: ?[*]const u32, t: u32, d_jd: ?[*]const f64, d_fr: ?[*]const f64, d_kind: ?[*]const u8, d_value: ?[*]const f64, d_sigma: ?[*]const f64, d_station: ?[*]const u32, d_stations: ?[*]const f64, gate_probability: f64, best: u32, device: i32, d_scratch: ?*anyopaque, d_rows: ?[*]u32, d_d2: ?[*]f64, d_used: ?[*]u32, d_n_gate: ?[*]u32, d_n_failed: ?[*]u32, d_status: ?[*]u8, d_row_status: ?[*]u8, stream: ?*anyopaque) i32;
 pub extern fn astroz_cuda_correlate_scratch_bytes(n: u32, t: u32, best: u32, bytes: *u64) i32;
