@@ -34,6 +34,7 @@
 #include "az_hostcopy.cuh"
 #include "az_ingest.cuh"
 #include "az_iod.cuh"
+#include "az_link.cuh"
 #include "az_kernels.cuh"
 #include "az_lambert.cuh"
 #include "az_numerical.cuh"
@@ -3773,6 +3774,41 @@ int32_t astroz_cuda_initial_orbits_device(const uint32_t *d_offsets, uint32_t t,
     return ASTROZ_OK;
 }
 
+// The observations of each track sorted stably by jd + fr, into host staging: what the track calls upload.
+struct SortedTracks {
+    std::vector<double> jd, fr, value, sigma;
+    std::vector<uint8_t> kind;
+    std::vector<uint32_t> station;
+};
+
+static SortedTracks sorted_tracks(const uint32_t *offsets, uint32_t t, const double *jd, const double *fr,
+                                  const uint8_t *kind, const double *value, const double *sigma,
+                                  const uint32_t *station, uint32_t m) {
+    std::vector<uint32_t> order(m);
+    for (uint32_t i = 0; i < m; ++i) order[i] = i;
+    for (uint32_t j = 0; j < t; ++j)
+        std::stable_sort(order.begin() + offsets[j], order.begin() + offsets[j + 1], [&](uint32_t p, uint32_t q) {
+            return az::add_rn(jd[p], fr[p]) < az::add_rn(jd[q], fr[q]);
+        });
+    SortedTracks s;
+    s.jd.resize(m);
+    s.fr.resize(m);
+    s.value.resize((size_t)6 * m);
+    s.sigma.resize((size_t)6 * m);
+    s.kind.resize(m);
+    s.station.resize(station ? m : 0);
+    for (uint32_t i = 0; i < m; ++i) {
+        const uint32_t p = order[i];
+        s.jd[i] = jd[p];
+        s.fr[i] = fr[p];
+        s.kind[i] = kind[p];
+        std::memcpy(&s.value[(size_t)6 * i], value + (size_t)6 * p, 48);
+        std::memcpy(&s.sigma[(size_t)6 * i], sigma + (size_t)6 * p, 48);
+        if (station) s.station[i] = station[p];
+    }
+    return s;
+}
+
 // Every check, then each track's observations sorted stably by jd + fr into host staging, which is what goes up (the
 // caller's pinned arrays are not read by DMA: the staging copy is pageable).
 int32_t astroz_cuda_initial_orbits(const uint32_t *offsets, uint32_t t, const double *jd, const double *fr,
@@ -3796,30 +3832,12 @@ int32_t astroz_cuda_initial_orbits(const uint32_t *offsets, uint32_t t, const do
         return rc;
     if (bstar && !all_finite(bstar, t)) return value_error("bstar must be finite");
     if (t == 0) return ASTROZ_OK;
-    // each track in time order, stably
-    std::vector<uint32_t> order(m);
-    for (uint32_t i = 0; i < m; ++i) order[i] = i;
-    for (uint32_t j = 0; j < t; ++j)
-        std::stable_sort(order.begin() + offsets[j], order.begin() + offsets[j + 1], [&](uint32_t p, uint32_t q) {
-            return az::add_rn(jd[p], fr[p]) < az::add_rn(jd[q], fr[q]);
-        });
-    std::vector<double> sJd(m), sFr(m), sValue((size_t)6 * m), sSigma((size_t)6 * m);
-    std::vector<uint8_t> sKind(m);
-    std::vector<uint32_t> sStation(station ? m : 0);
-    for (uint32_t i = 0; i < m; ++i) {
-        const uint32_t p = order[i];
-        sJd[i] = jd[p];
-        sFr[i] = fr[p];
-        sKind[i] = kind[p];
-        std::memcpy(&sValue[(size_t)6 * i], value + (size_t)6 * p, 48);
-        std::memcpy(&sSigma[(size_t)6 * i], sigma + (size_t)6 * p, 48);
-        if (station) sStation[i] = station[p];
-    }
+    const SortedTracks so = sorted_tracks(offsets, t, jd, fr, kind, value, sigma, station, m);
     return whole_batch(device,
-                       {upload(offsets, (size_t)4 * (t + 1)), upload(sJd.data(), (size_t)8 * m),
-                        upload(sFr.data(), (size_t)8 * m), upload(sKind.data(), m),
-                        upload(sValue.data(), (size_t)48 * m), upload(sSigma.data(), (size_t)48 * m),
-                        upload(sStation.data(), station ? (size_t)4 * m : 0), upload(stations, (size_t)24 * k),
+                       {upload(offsets, (size_t)4 * (t + 1)), upload(so.jd.data(), (size_t)8 * m),
+                        upload(so.fr.data(), (size_t)8 * m), upload(so.kind.data(), m),
+                        upload(so.value.data(), (size_t)48 * m), upload(so.sigma.data(), (size_t)48 * m),
+                        upload(so.station.data(), station ? (size_t)4 * m : 0), upload(stations, (size_t)24 * k),
                         upload(bstar, bstar ? (size_t)8 * t : 0), scratch(az::iod_scratch_bytes(t)),
                         result(elements, (size_t)64 * t), result(state, (size_t)48 * t), result(wrms, (size_t)8 * t),
                         result(method, t), result(candidates, (size_t)4 * t), result(conv, (size_t)16 * t),
@@ -3829,6 +3847,160 @@ int32_t astroz_cuda_initial_orbits(const uint32_t *offsets, uint32_t t, const do
                                           station ? d.u32(6) : nullptr, k ? d.f64(7) : nullptr,
                                           bstar ? d.f64(8) : nullptr, d.piece(9), d.f64(10), d.f64(11), d.f64(12),
                                           d.u8(13), d.u32(14), d.f64(15), d.u8(16), d.u8(17), st);
+                       });
+}
+
+// ---- track linking (K17, az_link.cu, az_link.cuh) ----------------------------------------------------------------------
+static_assert(ASTROZ_LINK_OK == az::kLinkOk && ASTROZ_LINK_TOO_FEW == az::kLinkTooFew &&
+                  ASTROZ_LINK_NO_CANDIDATE == az::kLinkNoCandidate &&
+                  ASTROZ_LINK_CONVERSION_FAILED == az::kLinkConversionFailed &&
+                  ASTROZ_LINK_BAD_TRACK == az::kLinkBadTrack && ASTROZ_LINK_BAD_PAIR == az::kLinkBadPair &&
+                  ASTROZ_LINK_RETROGRADE == az::kLinkRetrograde && ASTROZ_LINK_RIGHT_BRANCH == az::kLinkRightBranch &&
+                  ASTROZ_LINK_RANGES == az::kLinkRanges && ASTROZ_LINK_SEEDS == az::kLinkSeeds,
+              "track-link status, flag and size constants");
+
+// Scalar checks of the link calls, before anything is read, written or allocated; a receives the scalars.
+static int32_t link_check(uint32_t t, uint32_t p, double r_min, double r_max, uint32_t max_revs, int32_t grav,
+                          int32_t device, az::LinkArgs *a) {
+    if (device < 0) return value_error("track linking runs on one device: pass its ordinal");
+    const int32_t rc = grav_check(grav);
+    if (rc != ASTROZ_OK) return rc;
+    if (max_revs > az::kLamMaxRevs) return value_error("max_revs must be at most ASTROZ_LAMBERT_MAX_REVS");
+    if (!(r_min > 0.0) || !std::isfinite(r_min)) return value_error("r_min must be finite and positive");
+    if (!(r_max > r_min) || !std::isfinite(r_max)) return value_error("r_max must be finite and above r_min");
+    a->t = t;
+    a->p = p;
+    a->rMin = r_min;
+    a->rMax = r_max;
+    a->maxRevs = max_revs;
+    a->grav = grav;
+    a->g = az::grav_consts(az::gravity(grav));
+    return ASTROZ_OK;
+}
+
+int32_t astroz_cuda_link_tracks_scratch_bytes(uint32_t p, uint64_t *bytes) {
+    if (!bytes) return ASTROZ_NULL_POINTER;
+    *bytes = az::iod_scratch_bytes(p);
+    return ASTROZ_OK;
+}
+
+// Both call forms: a holds link_check's scalars, the arrays and the scratch are on the device.
+static cudaError_t link_run(az::LinkArgs a, const uint32_t *offsets, const double *jd, const double *fr,
+                            const uint8_t *kind, const double *value, const double *sigma, const uint32_t *station,
+                            const double *stations, const uint32_t *pairs, const double *bstar, void *scratch,
+                            double *elements, double *state, double *rho, uint8_t *revs, uint8_t *flags, double *wrms,
+                            uint32_t *used, uint32_t *hypotheses, double *conv, uint8_t *deep_space, uint8_t *status,
+                            cudaStream_t st) {
+    a.offsets = offsets;
+    a.jd = jd;
+    a.fr = fr;
+    a.kind = kind;
+    a.value = value;
+    a.sigma = sigma;
+    a.station = station;
+    a.stations = stations;
+    a.pairs = pairs;
+    a.bstar = bstar;
+    a.scratch = scratch;
+    a.elements = elements;
+    a.state = state;
+    a.rho = rho;
+    a.revs = revs;
+    a.flags = flags;
+    a.wrms = wrms;
+    a.used = used;
+    a.hypotheses = hypotheses;
+    a.conv = conv;
+    a.deepSpace = deep_space;
+    a.status = status;
+    return az::launch_link(a, st);
+}
+
+int32_t astroz_cuda_link_tracks_device(const uint32_t *d_offsets, uint32_t t, const double *d_jd, const double *d_fr,
+                                       const uint8_t *d_kind, const double *d_value, const double *d_sigma,
+                                       const uint32_t *d_station, const double *d_stations, const uint32_t *d_pairs,
+                                       uint32_t p, const double *d_bstar, double r_min, double r_max,
+                                       uint32_t max_revs, int32_t grav, int32_t device, void *d_scratch,
+                                       double *d_elements, double *d_state, double *d_rho, uint8_t *d_revs,
+                                       uint8_t *d_flags, double *d_wrms, uint32_t *d_used, uint32_t *d_hypotheses,
+                                       double *d_conv, uint8_t *d_deep_space, uint8_t *d_status, void *stream) {
+    az::LinkArgs a{};
+    int32_t rc = link_check(t, p, r_min, r_max, max_revs, grav, device, &a);
+    if (rc != ASTROZ_OK) return rc;
+    if (p == 0) return ASTROZ_OK;
+    if (!d_offsets || !d_jd || !d_fr || !d_kind || !d_value || !d_sigma || !d_pairs || !d_scratch || !d_elements ||
+        !d_state || !d_rho || !d_revs || !d_flags || !d_wrms || !d_used || !d_hypotheses || !d_conv ||
+        !d_deep_space || !d_status)
+        return ASTROZ_NULL_POINTER;
+    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
+    AZ_CUDA(cudaSetDevice(device));
+    AZ_CUDA(link_run(a, d_offsets, d_jd, d_fr, d_kind, d_value, d_sigma, d_station, d_stations, d_pairs, d_bstar,
+                     d_scratch, d_elements, d_state, d_rho, d_revs, d_flags, d_wrms, d_used, d_hypotheses, d_conv,
+                     d_deep_space, d_status, static_cast<cudaStream_t>(stream)));
+    return ASTROZ_OK;
+}
+
+// Every check of astroz_cuda_initial_orbits, then the pairs' and the range bounds'; the tracks go up sorted, as there.
+int32_t astroz_cuda_link_tracks(const uint32_t *offsets, uint32_t t, const double *jd, const double *fr,
+                                const uint8_t *kind, const double *value, const double *sigma, const uint32_t *station,
+                                uint32_t m, const double *stations, uint32_t k, const uint32_t *pairs, uint32_t p,
+                                const double *bstar, double r_min, double r_max, uint32_t max_revs, int32_t grav,
+                                int32_t device, double *elements, double *state, double *rho, uint8_t *revs,
+                                uint8_t *flags, double *wrms, uint32_t *used, uint32_t *hypotheses, double *conv,
+                                uint8_t *deep_space, uint8_t *status) {
+    az::LinkArgs a{};
+    int32_t rc = link_check(t, p, r_min, r_max, max_revs, grav, device, &a);
+    if (rc != ASTROZ_OK) return rc;
+    if (!offsets) return ASTROZ_NULL_POINTER;
+    if (p && (!pairs || !elements || !state || !rho || !revs || !flags || !wrms || !used || !hypotheses || !conv ||
+              !deep_space || !status))
+        return ASTROZ_NULL_POINTER;
+    if (m && (!jd || !fr || !kind || !value || !sigma)) return ASTROZ_NULL_POINTER;
+    if ((rc = offsets_check(offsets, t, m, "offsets[t] must equal the observation count m", true, az::kIodMaxTrack,
+                            "a track is longer than ASTROZ_IOD_MAX_TRACK observations")) != ASTROZ_OK)
+        return rc;
+    if ((rc = obs_values_check(jd, fr, value, sigma, station, kind, m, stations, k)) != ASTROZ_OK) return rc;
+    if ((rc = used_residuals_check({jd, fr, kind, value, sigma, station, stations}, offsets, t)) != ASTROZ_OK)
+        return rc;
+    if (bstar && !all_finite(bstar, p)) return value_error("bstar must be finite");
+    for (uint32_t q = 0; q < k; ++q) {
+        az::ObsStation st;
+        az::obs_station(stations + (size_t)3 * q, st);
+        if (!(r_min > std::sqrt(st.r[0] * st.r[0] + st.r[1] * st.r[1] + st.r[2] * st.r[2])))
+            return value_error("r_min must exceed every station's radius");
+    }
+    for (uint64_t q = 0; q < 2 * (uint64_t)p; ++q)
+        if (pairs[q] >= t) return value_error("a pair names a track index >= t");
+    if (p == 0) return ASTROZ_OK;
+    const SortedTracks so = sorted_tracks(offsets, t, jd, fr, kind, value, sigma, station, m);
+    const az::CorrObsArrays in{so.jd.data(), so.fr.data(), so.kind.data(), so.value.data(), so.sigma.data(),
+                               station ? so.station.data() : nullptr, stations};
+    std::vector<double> anchorT(t, NAN);
+    for (uint32_t j = 0; j < t; ++j) {
+        const uint32_t i = az::link_anchor_index(in, offsets[j], offsets[j + 1]);
+        if (i != offsets[j + 1]) anchorT[j] = az::add_rn(so.jd[i], so.fr[i]);
+    }
+    for (uint32_t q = 0; q < p; ++q) {
+        if (pairs[2 * q] == pairs[2 * q + 1]) return value_error("a pair names one track twice");
+        if (anchorT[pairs[2 * q]] == anchorT[pairs[2 * q + 1]])
+            return value_error("the two tracks of a pair have their anchors at the same time");
+    }
+    return whole_batch(device,
+                       {upload(offsets, (size_t)4 * (t + 1)), upload(so.jd.data(), (size_t)8 * m),
+                        upload(so.fr.data(), (size_t)8 * m), upload(so.kind.data(), m),
+                        upload(so.value.data(), (size_t)48 * m), upload(so.sigma.data(), (size_t)48 * m),
+                        upload(so.station.data(), station ? (size_t)4 * m : 0), upload(stations, (size_t)24 * k),
+                        upload(pairs, (size_t)8 * p), upload(bstar, bstar ? (size_t)8 * p : 0),
+                        scratch(az::iod_scratch_bytes(p)), result(elements, (size_t)64 * p),
+                        result(state, (size_t)48 * p), result(rho, (size_t)16 * p), result(revs, p), result(flags, p),
+                        result(wrms, (size_t)8 * p), result(used, (size_t)4 * p), result(hypotheses, (size_t)4 * p),
+                        result(conv, (size_t)16 * p), result(deep_space, p), result(status, p)},
+                       [&](const DeviceBlock &d, cudaStream_t st) {
+                           return link_run(a, d.u32(0), d.f64(1), d.f64(2), d.u8(3), d.f64(4), d.f64(5),
+                                           station ? d.u32(6) : nullptr, k ? d.f64(7) : nullptr, d.u32(8),
+                                           bstar ? d.f64(9) : nullptr, d.piece(10), d.f64(11), d.f64(12), d.f64(13),
+                                           d.u8(14), d.u8(15), d.f64(16), d.u32(17), d.u32(18), d.f64(19), d.u8(20),
+                                           d.u8(21), st);
                        });
 }
 

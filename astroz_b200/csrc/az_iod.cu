@@ -16,18 +16,7 @@ namespace az {
 
 constexpr int kIodWarps = 4;
 
-// The scratch of iod_scratch_bytes: the conversion batch and the fit's outputs
-struct IodScratch {
-    double *init;       // [8][t] osculating initial sets
-    double *jd, *fr;    // [t] the epoch observation's time
-    double *pos, *vel;  // [t][3] TEME state at the epoch
-    double *rms;        // [t][2]
-    uint32_t *offsets;  // [t + 1] = 0, 1, ..., t
-    uint32_t *iters;    // [t]
-    uint8_t *fitStatus, *iodStatus;   // [t]
-};
-
-static IodScratch iod_scratch(void *p, uint32_t t) {
+IodScratch iod_scratch(void *p, uint32_t t) {
     IodScratch s;
     s.init = static_cast<double *>(p);
     s.jd = s.init + (size_t)8 * t;
@@ -128,15 +117,11 @@ __global__ void __launch_bounds__(128) iod_finish_kernel(const IodArgs a, const 
         for (int c = 0; c < 8; ++c) a.elements[(size_t)c * a.t + j] = 0.0;
 }
 
-cudaError_t launch_iod(const IodArgs &a, cudaStream_t stream) {
-    if (a.t == 0) return cudaSuccess;
-    const IodScratch sc = iod_scratch(a.scratch, a.t);
-    iod_kernel<<<(a.t + kIodWarps - 1) / kIodWarps, kIodWarps * 32, 0, stream>>>(a, sc);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return e;
+cudaError_t launch_iod_conversion(const IodScratch &sc, uint32_t t, int grav, const GravConsts &g, double *elements,
+                                  cudaStream_t stream) {
     FitArgs f{};
     f.elements = sc.init;
-    f.n = a.t;
+    f.n = t;
     f.offsets = sc.offsets;
     f.jd = sc.jd;
     f.fr = sc.fr;
@@ -146,14 +131,24 @@ cudaError_t launch_iod(const IodArgs &a, cudaStream_t stream) {
     f.wv = 1.0 / kIodFitVelSigma;
     f.fitBstar = 0;
     f.maxIter = kIodFitIter;
-    f.grav = a.grav;
-    f.g = a.g;
-    f.fitted = a.elements;
+    f.grav = grav;
+    f.g = g;
+    f.fitted = elements;
     f.rms = sc.rms;
     f.iterations = sc.iters;
     f.status = sc.fitStatus;
-    if ((e = launch_fit(f, stream)) != cudaSuccess) return e;
-    if ((e = launch_fit_deep(f, stream)) != cudaSuccess) return e;
+    cudaError_t e = launch_fit(f, stream);
+    if (e != cudaSuccess) return e;
+    return launch_fit_deep(f, stream);
+}
+
+cudaError_t launch_iod(const IodArgs &a, cudaStream_t stream) {
+    if (a.t == 0) return cudaSuccess;
+    const IodScratch sc = iod_scratch(a.scratch, a.t);
+    iod_kernel<<<(a.t + kIodWarps - 1) / kIodWarps, kIodWarps * 32, 0, stream>>>(a, sc);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+    if ((e = launch_iod_conversion(sc, a.t, a.grav, a.g, a.elements, stream)) != cudaSuccess) return e;
     iod_finish_kernel<<<(a.t + 127) / 128, 128, 0, stream>>>(a, sc);
     return cudaGetLastError();
 }

@@ -320,6 +320,52 @@ struct IodArgs {
 size_t iod_scratch_bytes(uint32_t t);
 // the IOD kernel, K8's near-earth and deep-space fits over one TEME state per track, and the finishing kernel
 cudaError_t launch_iod(const IodArgs &a, cudaStream_t stream);
+// The scratch of iod_scratch_bytes(t): the conversion batch and the fit's outputs (K13's, and K17's per pair)
+struct IodScratch {
+    double *init;       // [8][t] osculating initial sets
+    double *jd, *fr;    // [t] the epoch observation's time
+    double *pos, *vel;  // [t][3] TEME state at the epoch
+    double *rms;        // [t][2]
+    uint32_t *offsets;  // [t + 1] = 0, 1, ..., t
+    uint32_t *iters;    // [t]
+    uint8_t *fitStatus, *iodStatus;   // [t]
+};
+IodScratch iod_scratch(void *p, uint32_t t);
+// K8's near-earth and deep-space fits of each initial set to its one TEME state, B* held, into elements[8][t]
+cudaError_t launch_iod_conversion(const IodScratch &sc, uint32_t t, int grav, const GravConsts &g, double *elements,
+                                  cudaStream_t stream);
+
+// K17: orbits from pairs of tracks (az_link.cu, az_link.cuh)
+struct LinkArgs {
+    const uint32_t *offsets = nullptr;   // [t + 1]: track j owns observations [offsets[j], offsets[j + 1]), time-ordered
+    uint32_t t = 0;
+    const double *jd = nullptr, *fr = nullptr;
+    const uint8_t *kind = nullptr;
+    const double *value = nullptr, *sigma = nullptr;   // [m][6]
+    const uint32_t *station = nullptr;
+    const double *stations = nullptr;
+    const uint32_t *pairs = nullptr;     // [p][2]
+    uint32_t p = 0;
+    const double *bstar = nullptr;       // [p], nullable (all 0)
+    double rMin = 0.0, rMax = 0.0;       // km
+    uint32_t maxRevs = 0;
+    int grav = 1;
+    GravConsts g{};
+    void *scratch = nullptr;             // iod_scratch_bytes(p)
+    double *elements = nullptr;          // [8][p] converted sets, epoch = the later anchor's time
+    double *state = nullptr;             // [p][6] TEME state at the epoch
+    double *rho = nullptr;               // [p][2] the winner's ranges, track 1 (earlier anchor) first
+    uint8_t *revs = nullptr;             // [p]
+    uint8_t *flags = nullptr;            // [p] ASTROZ_LINK_RETROGRADE | ASTROZ_LINK_RIGHT_BRANCH
+    double *wrms = nullptr;              // [p]
+    uint32_t *used = nullptr;            // [p] used residuals of both tracks
+    uint32_t *hypotheses = nullptr;      // [p] admissible states scored
+    double *conv = nullptr;              // [p][2] conversion |dr| km, |dv| km/s
+    uint8_t *deepSpace = nullptr;        // [p]
+    uint8_t *status = nullptr;           // [p] ASTROZ_LINK_*
+};
+// the link kernel, K13's conversion fits, and the finishing kernel
+cudaError_t launch_link(const LinkArgs &a, cudaStream_t stream);
 
 // K16: collision-avoidance manoeuvre trials (az_avoid.cu, az_avoid.cuh; AvoidArgs and avoid_scratch_bytes are there).
 // K10 at the burn, the burn, K8's conversion, K10 on the new sets, the covariance transport, K11, the finishing kernel

@@ -1082,6 +1082,67 @@ int32_t astroz_cuda_initial_orbits_device(const uint32_t *d_offsets, uint32_t t,
                                           uint8_t *d_status, void *stream);
 int32_t astroz_cuda_initial_orbits_scratch_bytes(uint32_t t, uint64_t *bytes);
 
+/* ---- track linking (K17): an element set from two tracks of one unknown object ---------------------------------------
+ * New capability: the reference has no track linking, so these calls replace nothing in it.
+ * Tracks as in astroz_cuda_initial_orbits; pairs[p][2] the track pairs to test.
+ *   anchor:     a track's middle observation among those that give a line of sight with every component used (both
+ *               optical angles; radar range, azimuth and elevation; the position of a TEME or ECEF state, from the
+ *               geocentre): a TEME origin R, unit vector L and range, known except for optical observations;
+ *   pair:       the track with the earlier anchor is track 1, so (a, b) and (b, a) give the same bytes; the epoch is
+ *               track 2's anchor time;
+ *   hypotheses: a known range is one; an unknown one ASTROZ_LINK_RANGES geometric points from the root of
+ *               |R + rho L| = r_min to the root of |R + rho L| = r_max (km; r_min above every station's radius);
+ *   transfers:  every (rho1, rho2) and normal +z, -z: Lambert (astroz_cuda_lambert's solver, 0 .. max_revs
+ *               revolutions, both branches) from R1 + rho1 L1 to R2 + rho2 L2, the state (r2, v2) at the epoch kept
+ *               when finite with e < 1 and perigee >= 1 earth radius;
+ *   score:      each state two-body against the first, anchor and last observation of each track (F_probe, the
+ *               element fit's residual rules); the ASTROZ_LINK_SEEDS least are refined by Levenberg-Marquardt on their
+ *               unknown ranges (revolutions, direction and branch fixed) over every observation of both tracks; the
+ *               least F wins;
+ *   conversion: astroz_cuda_initial_orbits' (the epoch state -> osculating elements, B* = bstar[p] or 0 -> the mixed
+ *               element fit to that one state, B* held) and its thresholds.
+ * Outputs per pair: elements[8][p], state[p][6] at the epoch, rho[p][2] the winner's ranges (track 1 first), revs[p],
+ * flags[p] (ASTROZ_LINK_RETROGRADE: normal -z; ASTROZ_LINK_RIGHT_BRANCH), wrms[p] = sqrt(F / used), used[p] the used
+ * residuals of both tracks, hypotheses[p] the admissible states scored, conv[p][2], deep_space[p], status[p]
+ * (ASTROZ_LINK_*): OK; TOO_FEW a track without an anchor; NO_CANDIDATE no admissible state; CONVERSION_FAILED as for
+ * initial orbits (outputs kept); BAD_TRACK (device call only) as for initial orbits; BAD_PAIR (device call only) a
+ * pair index >= t, a == b, or equal anchor times.  Except for CONVERSION_FAILED a pair that is not OK has zero
+ * elements, state, rho, revs, flags, wrms and conv; used and hypotheses are zero unless the pair was scored.
+ * A pair's bytes depend on its two tracks alone: not on other pairs, their order, the batch split or the call form.
+ * ASTROZ_VALUE_ERROR, nothing written: device = -1, an unknown grav, max_revs > ASTROZ_LAMBERT_MAX_REVS, r_min not
+ * finite or <= 0, r_max not finite or <= r_min; and for the host call every refusal of astroz_cuda_initial_orbits
+ * (bstar now per pair), a pair index >= t, a == b, equal anchor times and r_min <= the largest station radius. */
+#define ASTROZ_LINK_OK                0
+#define ASTROZ_LINK_TOO_FEW           1
+#define ASTROZ_LINK_NO_CANDIDATE      2
+#define ASTROZ_LINK_CONVERSION_FAILED 3
+#define ASTROZ_LINK_BAD_TRACK         4
+#define ASTROZ_LINK_BAD_PAIR          5
+#define ASTROZ_LINK_RETROGRADE        1
+#define ASTROZ_LINK_RIGHT_BRANCH      2
+#define ASTROZ_LINK_RANGES            32
+#define ASTROZ_LINK_SEEDS             4
+/* HOST buffers: each track's observations are first sorted into host staging, as for astroz_cuda_initial_orbits. */
+int32_t astroz_cuda_link_tracks(const uint32_t *offsets, uint32_t t, const double *jd, const double *fr,
+                                const uint8_t *kind, const double *value, const double *sigma, const uint32_t *station,
+                                uint32_t m, const double *stations, uint32_t k, const uint32_t *pairs, uint32_t p,
+                                const double *bstar, double r_min, double r_max, uint32_t max_revs, int32_t grav,
+                                int32_t device, double *elements, double *state, double *rho, uint8_t *revs,
+                                uint8_t *flags, double *wrms, uint32_t *used, uint32_t *hypotheses, double *conv,
+                                uint8_t *deep_space, uint8_t *status);
+/* DEVICE pointers on `device`: four launches on `stream` (the link kernel, the two conversion fits, the finishing
+ * kernel), no allocation, no synchronisation; only the scalar arguments are checked.  d_scratch holds *bytes of
+ * astroz_cuda_link_tracks_scratch_bytes(p, bytes), 8-byte aligned. */
+int32_t astroz_cuda_link_tracks_device(const uint32_t *d_offsets, uint32_t t, const double *d_jd, const double *d_fr,
+                                       const uint8_t *d_kind, const double *d_value, const double *d_sigma,
+                                       const uint32_t *d_station, const double *d_stations, const uint32_t *d_pairs,
+                                       uint32_t p, const double *d_bstar, double r_min, double r_max,
+                                       uint32_t max_revs, int32_t grav, int32_t device, void *d_scratch,
+                                       double *d_elements, double *d_state, double *d_rho, uint8_t *d_revs,
+                                       uint8_t *d_flags, double *d_wrms, uint32_t *d_used, uint32_t *d_hypotheses,
+                                       double *d_conv, uint8_t *d_deep_space, uint8_t *d_status, void *stream);
+int32_t astroz_cuda_link_tracks_scratch_bytes(uint32_t p, uint64_t *bytes);
+
 /* One TLE line pair read by the library's own parser (src/Tle.zig:49-101) into the eight element columns above, the
  * numbers astroz_cuda_constellation_create would use.  ASTROZ_BAD_TLE_LENGTH when the pair cannot be read. */
 int32_t astroz_cuda_parse_tle(const char *line1, const char *line2, double *elements);

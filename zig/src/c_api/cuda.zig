@@ -115,6 +115,9 @@ pub extern fn astroz_cuda_chi2_quantile(k: u32, p: f64, x: ?[*]f64) i32;
 pub extern fn astroz_cuda_initial_orbits(offsets: ?[*]const u32, t: u32, jd: ?[*]const f64, fr: ?[*]const f64, kind: ?[*]const u8, value: ?[*]const f64, sigma: ?[*]const f64, station: ?[*]const u32, m: u32, stations: ?[*]const f64, k: u32, bstar: ?[*]const f64, grav: i32, device: i32, elements: ?[*]f64, state: ?[*]f64, wrms: ?[*]f64, method: ?[*]u8, candidates: ?[*]u32, conv: ?[*]f64, deep_space: ?[*]u8, status: ?[*]u8) i32;
 pub extern fn astroz_cuda_initial_orbits_device(d_offsets: ?[*]const u32, t: u32, d_jd: ?[*]const f64, d_fr: ?[*]const f64, d_kind: ?[*]const u8, d_value: ?[*]const f64, d_sigma: ?[*]const f64, d_station: ?[*]const u32, d_stations: ?[*]const f64, d_bstar: ?[*]const f64, grav: i32, device: i32, d_scratch: ?*anyopaque, d_elements: ?[*]f64, d_state: ?[*]f64, d_wrms: ?[*]f64, d_method: ?[*]u8, d_candidates: ?[*]u32, d_conv: ?[*]f64, d_deep_space: ?[*]u8, d_status: ?[*]u8, stream: ?*anyopaque) i32;
 pub extern fn astroz_cuda_initial_orbits_scratch_bytes(t: u32, bytes: *u64) i32;
+pub extern fn astroz_cuda_link_tracks(offsets: ?[*]const u32, t: u32, jd: ?[*]const f64, fr: ?[*]const f64, kind: ?[*]const u8, value: ?[*]const f64, sigma: ?[*]const f64, station: ?[*]const u32, m: u32, stations: ?[*]const f64, k: u32, pairs: ?[*]const u32, p: u32, bstar: ?[*]const f64, r_min: f64, r_max: f64, max_revs: u32, grav: i32, device: i32, elements: ?[*]f64, state: ?[*]f64, rho: ?[*]f64, revs: ?[*]u8, flags: ?[*]u8, wrms: ?[*]f64, used: ?[*]u32, hypotheses: ?[*]u32, conv: ?[*]f64, deep_space: ?[*]u8, status: ?[*]u8) i32;
+pub extern fn astroz_cuda_link_tracks_device(d_offsets: ?[*]const u32, t: u32, d_jd: ?[*]const f64, d_fr: ?[*]const f64, d_kind: ?[*]const u8, d_value: ?[*]const f64, d_sigma: ?[*]const f64, d_station: ?[*]const u32, d_stations: ?[*]const f64, d_pairs: ?[*]const u32, p: u32, d_bstar: ?[*]const f64, r_min: f64, r_max: f64, max_revs: u32, grav: i32, device: i32, d_scratch: ?*anyopaque, d_elements: ?[*]f64, d_state: ?[*]f64, d_rho: ?[*]f64, d_revs: ?[*]u8, d_flags: ?[*]u8, d_wrms: ?[*]f64, d_used: ?[*]u32, d_hypotheses: ?[*]u32, d_conv: ?[*]f64, d_deep_space: ?[*]u8, d_status: ?[*]u8, stream: ?*anyopaque) i32;
+pub extern fn astroz_cuda_link_tracks_scratch_bytes(p: u32, bytes: *u64) i32;
 pub extern fn astroz_cuda_parse_tle(line1: [*:0]const u8, line2: [*:0]const u8, elements: ?[*]f64) i32;
 pub extern fn astroz_cuda_lambert(r1: ?[*]const f64, r2: ?[*]const f64, tof: ?[*]const f64, normal: ?[*]const f64, n: u32, mu: f64, max_revs: u32, device: i32, v1: ?[*]f64, v2: ?[*]f64, status: ?[*]u8, iterations: ?[*]u8) i32;
 pub extern fn astroz_cuda_lambert_device(d_r1: ?[*]const f64, d_r2: ?[*]const f64, d_tof: ?[*]const f64, d_normal: ?[*]const f64, n: u32, mu: f64, max_revs: u32, device: i32, d_v1: ?[*]f64, d_v2: ?[*]f64, d_status: ?[*]u8, d_iterations: ?[*]u8, stream: ?*anyopaque) i32;
