@@ -14,8 +14,8 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libastroz_b200.so")
-SOURCES = ["az_kernels.cu", "az_ingest.cu", "az_pairs.cu", "az_numerical.cu", "az_fit.cu", "az_fit_obs.cu", "az_covariance.cu", "az_conjunction.cu", "az_conjunction_mc.cu", "az_conjunction_is.cu", "az_avoid.cu", "az_correlate.cu", "az_iod.cu", "az_link.cu", "az_lambert.cu", "az_hostcopy.cu", "az_capi.cu"]
-HEADERS = ["az_math.cuh", "az_device.cuh", "az_kernels.cuh", "az_ingest.cuh", "az_pairs.cuh", "az_numerical.cuh", "az_fit.cuh", "az_obs.cuh", "az_covariance.cuh", "az_conjunction.cuh", "az_conjunction_mc.cuh", "az_conjunction_is.cuh", "az_conjunction_mc_warp.cuh", "az_avoid.cuh", "az_correlate.cuh", "az_iod.cuh", "az_link.cuh", "az_lambert.cuh", "az_hostcopy.cuh", "az_screen.cuh", "az_elements.hpp",
+SOURCES = ["az_kernels.cu", "az_ingest.cu", "az_pairs.cu", "az_numerical.cu", "az_fit.cu", "az_fit_obs.cu", "az_covariance.cu", "az_conjunction.cu", "az_conjunction_mc.cu", "az_conjunction_is.cu", "az_avoid.cu", "az_correlate.cu", "az_iod.cu", "az_link.cu", "az_tasking.cu", "az_lambert.cu", "az_hostcopy.cu", "az_capi.cu"]
+HEADERS = ["az_math.cuh", "az_device.cuh", "az_kernels.cuh", "az_ingest.cuh", "az_pairs.cuh", "az_numerical.cuh", "az_fit.cuh", "az_obs.cuh", "az_covariance.cuh", "az_conjunction.cuh", "az_conjunction_mc.cuh", "az_conjunction_is.cuh", "az_conjunction_mc_warp.cuh", "az_avoid.cuh", "az_correlate.cuh", "az_iod.cuh", "az_link.cuh", "az_tasking.cuh", "az_lambert.cuh", "az_hostcopy.cuh", "az_screen.cuh", "az_elements.hpp",
            "az_tables.hpp", os.path.join("..", "..", "include", "astroz_b200.h")]
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = [*GENCODE, "-O3", "-std=c++17", "-lineinfo",

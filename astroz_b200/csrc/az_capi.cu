@@ -30,6 +30,7 @@
 #include "az_conjunction.cuh"
 #include "az_conjunction_is.cuh"
 #include "az_correlate.cuh"
+#include "az_tasking.cuh"
 #include "az_fit.cuh"
 #include "az_hostcopy.cuh"
 #include "az_ingest.cuh"
@@ -3694,6 +3695,175 @@ int32_t astroz_cuda_correlate(const double *elements, uint32_t n, int32_t grav, 
                                            station ? d.u32(9) : nullptr, k ? d.f64(10) : nullptr, d.piece(11),
                                            d.u32(12), d.f64(13), d.u32(14), d.u32(15), d.u32(16), d.u8(17), d.u8(18),
                                            st);
+                       });
+}
+
+// ---- sensor tasking (K18, az_tasking.cu, az_tasking.cuh) --------------------------------------------------------------
+static_assert(ASTROZ_TASK_MAX_SENSORS == az::kTaskMaxSensors && ASTROZ_TASK_LIMIT_EL_MIN == az::kTaskElMin &&
+                  ASTROZ_TASK_LIMIT_RANGE_MAX == az::kTaskRangeMax &&
+                  ASTROZ_TASK_LIMIT_SUN_EL_MAX == az::kTaskSunElMax &&
+                  ASTROZ_TASK_LIMIT_EXCLUSION == az::kTaskExclusion,
+              "tasking limits");
+
+// Scalar checks of the tasking calls, before anything is read, written or allocated; a receives the scalars.
+static int32_t task_check(uint32_t n, int32_t grav, uint32_t s, uint32_t t, double gain_min, int32_t device,
+                          az::TaskArgs *a) {
+    if (device < 0) return value_error("sensor tasking runs on one device: pass its ordinal");
+    const int32_t rc = grav_check(grav);
+    if (rc != ASTROZ_OK) return rc;
+    if (s == 0 || s > (uint32_t)az::kTaskMaxSensors) return value_error("s must be in [1, ASTROZ_TASK_MAX_SENSORS]");
+    if (t == 0) return value_error("t must be at least 1");
+    if (!(gain_min >= 0.0 && gain_min < INFINITY)) return value_error("gain_min must be finite and >= 0");
+    a->n = n;
+    a->S = s;
+    a->T = t;
+    a->grav = grav;
+    a->g = az::grav_consts(az::gravity(grav));
+    a->gainMin = gain_min;
+    return ASTROZ_OK;
+}
+
+// The sensors, slots and Sun rows of the host call.
+static int32_t task_values_check(const uint8_t *kind, const uint32_t *station, const double *sigma,
+                                 const double *limits, uint32_t s, uint32_t k, const double *jd, const double *fr,
+                                 uint32_t t, const double *sun) {
+    bool optical = false;
+    for (uint32_t q = 0; q < s; ++q) {
+        if (kind[q] != az::kObsRadar && kind[q] != az::kObsOptical)
+            return value_error("a sensor kind is not ASTROZ_OBS_RADAR or ASTROZ_OBS_OPTICAL");
+        optical = optical || kind[q] == az::kObsOptical;
+        if (station[q] >= k) return value_error("a sensor's station index is not below the station count k");
+        int used = 0;
+        for (int c = 0; c < az::obs_count(kind[q]); ++c) {
+            const double sg = sigma[(size_t)q * 4 + c];
+            if (!(sg > 0.0)) return value_error("sensor sigma must be > 0 (+inf: component not measured)");
+            used += sg < INFINITY;
+        }
+        if (used == 0) return value_error("a sensor measures no component");
+        const double *lim = limits + (size_t)q * 4;
+        const double halfPi = 0.5 * az::kPi;
+        if (!(std::fabs(lim[az::kTaskElMin]) <= halfPi) || !(std::fabs(lim[az::kTaskSunElMax]) <= halfPi))
+            return value_error("an elevation limit is outside [-pi/2, pi/2]");
+        if (!(lim[az::kTaskRangeMax] > 0.0)) return value_error("range_max must be > 0 (+inf allowed)");
+        if (!(lim[az::kTaskExclusion] >= 0.0 && lim[az::kTaskExclusion] <= az::kPi))
+            return value_error("an exclusion angle is outside [0, pi]");
+    }
+    if (!all_finite(jd, t) || !all_finite(fr, t)) return value_error("slot times must be finite");
+    for (uint32_t i = 1; i < t; ++i)
+        if ((jd[i] - jd[i - 1]) + (fr[i] - fr[i - 1]) < 0.0) return value_error("slot times must be non-decreasing");
+    if (optical && !sun) return value_error("an optical sensor needs the Sun's direction at every slot");
+    if (sun)
+        for (uint32_t i = 0; i < t; ++i) {
+            const double *u = sun + (size_t)i * 3;
+            if (!all_finite(u, 3) || (u[0] == 0.0 && u[1] == 0.0 && u[2] == 0.0))
+                return value_error("a Sun direction is zero or not finite");
+        }
+    return ASTROZ_OK;
+}
+
+int32_t astroz_cuda_tasking_scratch_bytes(uint32_t n, uint32_t s, uint64_t *bytes) {
+    if (!bytes) return ASTROZ_NULL_POINTER;
+    if (s == 0 || s > (uint32_t)az::kTaskMaxSensors) return value_error("s must be in [1, ASTROZ_TASK_MAX_SENSORS]");
+    *bytes = az::task_scratch_bytes(n, s);
+    return ASTROZ_OK;
+}
+
+// Both call forms: a holds task_check's scalars, the arrays and the scratch are on the device.
+static cudaError_t tasking_run(az::TaskArgs a, const double *elements, const double *covariance, const uint8_t *model,
+                               const uint8_t *kind, const uint32_t *station, const double *sigma,
+                               const double *limits, const double *stations, const double *jd, const double *fr,
+                               const double *sun, void *scratch, uint32_t *task_row, double *task_gain,
+                               double *task_value, double *task_spread, uint32_t *n_candidates, double *posterior,
+                               uint32_t *n_tasks, uint32_t *n_visible, uint32_t *n_failed, uint8_t *row_status,
+                               cudaStream_t st) {
+    a.elements = elements;
+    a.covariance = covariance;
+    a.model = model;
+    a.kind = kind;
+    a.station = station;
+    a.sigma = sigma;
+    a.limits = limits;
+    a.stations = stations;
+    a.jd = jd;
+    a.fr = fr;
+    a.sun = sun;
+    a.scratch = scratch;
+    a.taskRow = task_row;
+    a.taskGain = task_gain;
+    a.taskValue = task_value;
+    a.taskSpread = task_spread;
+    a.nCandidates = n_candidates;
+    a.posterior = posterior;
+    a.nTasks = n_tasks;
+    a.nVisible = n_visible;
+    a.nFailed = n_failed;
+    a.rowStatus = row_status;
+    return az::launch_tasking(a, st);
+}
+
+int32_t astroz_cuda_tasking_device(const double *d_elements, uint32_t n, int32_t grav, const double *d_covariance,
+                                   const uint8_t *d_model, const uint8_t *d_kind, const uint32_t *d_station,
+                                   const double *d_sigma, const double *d_limits, uint32_t s, const double *d_stations,
+                                   const double *d_jd, const double *d_fr, uint32_t t, const double *d_sun,
+                                   double gain_min, int32_t device, void *d_scratch, uint32_t *d_task_row,
+                                   double *d_task_gain, double *d_task_value, double *d_task_spread,
+                                   uint32_t *d_n_candidates, double *d_posterior, uint32_t *d_n_tasks,
+                                   uint32_t *d_n_visible, uint32_t *d_n_failed, uint8_t *d_row_status, void *stream) {
+    az::TaskArgs a{};
+    int32_t rc = task_check(n, grav, s, t, gain_min, device, &a);
+    if (rc != ASTROZ_OK) return rc;
+    if (!d_kind || !d_station || !d_sigma || !d_limits || !d_stations || !d_jd || !d_fr || !d_scratch ||
+        !d_task_row || !d_task_gain || !d_task_value || !d_task_spread || !d_n_candidates)
+        return ASTROZ_NULL_POINTER;
+    if (n && (!d_elements || !d_posterior || !d_n_tasks || !d_n_visible || !d_n_failed || !d_row_status))
+        return ASTROZ_NULL_POINTER;
+    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
+    AZ_CUDA(cudaSetDevice(device));
+    AZ_CUDA(tasking_run(a, d_elements, d_covariance, d_model, d_kind, d_station, d_sigma, d_limits, d_stations, d_jd,
+                        d_fr, d_sun, d_scratch, d_task_row, d_task_gain, d_task_value, d_task_spread, d_n_candidates,
+                        d_posterior, d_n_tasks, d_n_visible, d_n_failed, d_row_status,
+                        static_cast<cudaStream_t>(stream)));
+    return ASTROZ_OK;
+}
+
+int32_t astroz_cuda_tasking(const double *elements, uint32_t n, int32_t grav, const double *covariance,
+                            const uint8_t *model, const uint8_t *kind, const uint32_t *station, const double *sigma,
+                            const double *limits, uint32_t s, const double *stations, uint32_t k, const double *jd,
+                            const double *fr, uint32_t t, const double *sun, double gain_min, int32_t device,
+                            uint32_t *task_row, double *task_gain, double *task_value, double *task_spread,
+                            uint32_t *n_candidates, double *posterior, uint32_t *n_tasks, uint32_t *n_visible,
+                            uint32_t *n_failed, uint8_t *row_status) {
+    az::TaskArgs a{};
+    int32_t rc = task_check(n, grav, s, t, gain_min, device, &a);
+    if (rc != ASTROZ_OK) return rc;
+    if (!kind || !station || !sigma || !limits || !stations || !jd || !fr || !task_row || !task_gain ||
+        !task_value || !task_spread || !n_candidates)
+        return ASTROZ_NULL_POINTER;
+    if (n && (!elements || !posterior || !n_tasks || !n_visible || !n_failed || !row_status))
+        return ASTROZ_NULL_POINTER;
+    if ((rc = obs_values_check(nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, stations, k)) != ASTROZ_OK)
+        return rc;
+    if ((rc = task_values_check(kind, station, sigma, limits, s, k, jd, fr, t, sun)) != ASTROZ_OK) return rc;
+    if ((rc = rows_check(elements, covariance, n)) != ASTROZ_OK) return rc;
+    if ((rc = model_bytes_check(model, n)) != ASTROZ_OK) return rc;
+    return whole_batch(device,
+                       {upload(elements, (size_t)64 * n),
+                        upload(covariance, covariance ? (size_t)8 * az::kFitN * n : 0),
+                        upload(model, model ? (size_t)n : 0), upload(kind, s), upload(station, (size_t)4 * s),
+                        upload(sigma, (size_t)32 * s), upload(limits, (size_t)32 * s),
+                        upload(stations, (size_t)24 * k), upload(jd, (size_t)8 * t), upload(fr, (size_t)8 * t),
+                        upload(sun, sun ? (size_t)24 * t : 0), scratch(az::task_scratch_bytes(n, s)),
+                        result(task_row, (size_t)4 * s * t), result(task_gain, (size_t)8 * s * t),
+                        result(task_value, (size_t)32 * s * t), result(task_spread, (size_t)32 * s * t),
+                        result(n_candidates, (size_t)4 * s * t), result(posterior, (size_t)8 * az::kFitN * n),
+                        result(n_tasks, (size_t)4 * n), result(n_visible, (size_t)4 * n),
+                        result(n_failed, (size_t)4 * n), result(row_status, n)},
+                       [&](const DeviceBlock &d, cudaStream_t st) {
+                           return tasking_run(a, d.f64(0), covariance ? d.f64(1) : nullptr,
+                                              model ? d.u8(2) : nullptr, d.u8(3), d.u32(4), d.f64(5), d.f64(6),
+                                              d.f64(7), d.f64(8), d.f64(9), sun ? d.f64(10) : nullptr, d.piece(11),
+                                              d.u32(12), d.f64(13), d.f64(14), d.f64(15), d.u32(16), d.f64(17),
+                                              d.u32(18), d.u32(19), d.u32(20), d.u8(21), st);
                        });
 }
 

@@ -367,6 +367,36 @@ struct LinkArgs {
 // the link kernel, K13's conversion fits, and the finishing kernel
 cudaError_t launch_link(const LinkArgs &a, cudaStream_t stream);
 
+// K18: sensor tasking (az_tasking.cu, az_tasking.cuh).  Device pointers.
+struct TaskArgs {
+    const double *elements = nullptr;    // [8][n]
+    const double *covariance = nullptr;  // [n][28], nullable (every P zero)
+    const uint8_t *model = nullptr;      // [n], nullable (all 0)
+    uint32_t n = 0;
+    const uint8_t *kind = nullptr;       // [S] ASTROZ_OBS_RADAR / ASTROZ_OBS_OPTICAL
+    const uint32_t *station = nullptr;   // [S] into stations
+    const double *sigma = nullptr;       // [S][4]
+    const double *limits = nullptr;      // [S][4] ASTROZ_TASK_LIMIT_*
+    uint32_t S = 0;
+    const double *stations = nullptr;    // [k][3]
+    const double *jd = nullptr, *fr = nullptr;   // [T]
+    uint32_t T = 0;
+    const double *sun = nullptr;         // [T][3], nullable when no sensor is optical
+    double gainMin = 0.0;
+    int grav = 1;
+    GravConsts g{};
+    void *scratch = nullptr;             // task_scratch_bytes(n, S)
+    uint32_t *taskRow = nullptr;         // [S][T]
+    double *taskGain = nullptr;          // [S][T]
+    double *taskValue = nullptr, *taskSpread = nullptr;   // [S][T][4]
+    uint32_t *nCandidates = nullptr;     // [S][T]
+    double *posterior = nullptr;         // [n][28]
+    uint32_t *nTasks = nullptr, *nVisible = nullptr, *nFailed = nullptr;   // [n]
+    uint8_t *rowStatus = nullptr;        // [n] ASTROZ_COV_OK / ASTROZ_COV_INIT_FAILED
+};
+// the build kernel, then per slot the near-earth and deep-space scoring kernels and the one-CTA select kernel
+cudaError_t launch_tasking(const TaskArgs &a, cudaStream_t stream);
+
 // K16: collision-avoidance manoeuvre trials (az_avoid.cu, az_avoid.cuh; AvoidArgs and avoid_scratch_bytes are there).
 // K10 at the burn, the burn, K8's conversion, K10 on the new sets, the covariance transport, K11, the finishing kernel
 struct AvoidArgs;

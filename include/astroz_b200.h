@@ -1017,6 +1017,66 @@ int32_t astroz_cuda_correlate_scratch_bytes(uint32_t n, uint32_t t, uint32_t bes
 /* The gate: the quantile x of the chi-square distribution of k >= 1 degrees of freedom at probability p in (0, 1), by
  * the function the kernels evaluate.  ASTROZ_VALUE_ERROR for k = 0 or p outside (0, 1). */
 int32_t astroz_cuda_chi2_quantile(uint32_t k, double p, double *x);
+/* ---- sensor tasking (K18): which catalogue row each sensor should observe at each slot --------------------------------
+ * New capability: the reference has no tasking, so these calls replace nothing in it.
+ * The catalogue is K10's: elements[8][n], covariance[n][28] in the fit's variables (NULL: every P zero) and model[n]
+ * (NULL: all 0).  Sensor k of s (1 <= s <= ASTROZ_TASK_MAX_SENSORS) is kind[k] (ASTROZ_OBS_RADAR or ASTROZ_OBS_OPTICAL),
+ * station[k] into stations[K][3] (lat deg, lon deg, h km on WGS84), sigma[k][4] (radar range km / azimuth rad /
+ * elevation rad / range-rate km/s, optical RA / Dec rad; +inf: not measured) and limits[k][4], indexed by
+ * ASTROZ_TASK_LIMIT_*: the minimum elevation (rad), the maximum range (km, +inf allowed), the maximum Sun elevation at
+ * the station (rad) and the minimum solar exclusion angle (rad), the last two for optical sensors only.  Slots are
+ * jd[t] + fr[t] (non-decreasing); sun[t][3] is the Sun's direction in TEME at each slot, of any length (required when a
+ * sensor is optical).  For each cell (row, sensor, slot), at K10's time:
+ *   visible:   the radar elevation of the nominal state above the station's geodetic horizon >= the minimum and the
+ *              range <= the maximum (no refraction); optical sensors also need the object sunlit under a cylindrical
+ *              shadow of radius 6378.137 km, the Sun's elevation at the station <= its limit and the angle between the
+ *              line of sight and the Sun >= the exclusion angle;
+ *   rows:      the predicted measurement h, and the weighted Jacobian rows G of the element fit with h as the
+ *              observation (azimuth / RA scaled by the cosine of the predicted elevation / declination), from the
+ *              row's nominal and stepped sets as K10 builds them (stepped sets propagated only where a sensor sees it);
+ *   gain:      g = 1/2 log det(I + G P G^T) nats, the information of one observation about the row's variables, formed
+ *              as 1/2 log det(I + L^T G^T G L) with P = L L^T (K12's semi-definite Cholesky): 0 exactly when P = 0;
+ *   spread:    sqrt((G P G^T)_cc) sigma_c, the predicted 1-sigma of each measured component (azimuth / RA as an arc);
+ *   failure:   a deep-space cell that fails (decay, eccentricity) is not visible and is counted.
+ * Schedule: slot by slot, sensor k = 0 .. s-1 takes the row of largest g (then lowest row index) among the rows visible
+ * to it with g > gain_min not taken by a lower sensor in the slot, or idles; each taken row's covariance becomes the
+ * Kalman posterior of that one observation, P+ = L (I + L^T G^T G L)^-1 L^T (symmetric, 28 words), before the next
+ * slot.  The elements are not changed; a held B* row stays zero.
+ * Outputs per (sensor, slot): task_row[s][t] (0xFFFFFFFF idle), task_gain[s][t], task_value[s][t][4] the pointing (the
+ * prediction h), task_spread[s][t][4], n_candidates[s][t] the rows that qualified when the sensor chose (idle: the
+ * gain, value and spread are 0).  Per row: posterior[n][28], n_tasks[n], n_visible[n] the visible (sensor, slot)
+ * cells, n_failed[n] the failed cells, row_status[n] ASTROZ_COV_OK or ASTROZ_COV_INIT_FAILED (such a row takes part in
+ * nothing).  No byte depends on the launch shape or the call form.
+ * ASTROZ_VALUE_ERROR, nothing written: device = -1, an unknown grav, s = 0 or s > ASTROZ_TASK_MAX_SENSORS, t = 0,
+ * gain_min negative or not finite; and for the host call an unknown sensor kind, a station index >= K, a sigma that is
+ * not positive or a sensor with no used component, a minimum elevation or maximum Sun elevation outside [-pi/2, pi/2],
+ * a maximum range not > 0, an exclusion angle outside [0, pi], non-finite or decreasing slot times, sun NULL with an
+ * optical sensor or a Sun row that is zero or not finite, a non-finite element or covariance word, a model byte > 1. */
+#define ASTROZ_TASK_MAX_SENSORS       32
+#define ASTROZ_TASK_LIMIT_EL_MIN      0
+#define ASTROZ_TASK_LIMIT_RANGE_MAX   1
+#define ASTROZ_TASK_LIMIT_SUN_EL_MAX  2
+#define ASTROZ_TASK_LIMIT_EXCLUSION   3
+/* HOST buffers: one upload (pageable through a pinned ring, pinned by direct DMA), the launches, plain copies back. */
+int32_t astroz_cuda_tasking(const double *elements, uint32_t n, int32_t grav, const double *covariance,
+                            const uint8_t *model, const uint8_t *kind, const uint32_t *station, const double *sigma,
+                            const double *limits, uint32_t s, const double *stations, uint32_t k, const double *jd,
+                            const double *fr, uint32_t t, const double *sun, double gain_min, int32_t device,
+                            uint32_t *task_row, double *task_gain, double *task_value, double *task_spread,
+                            uint32_t *n_candidates, double *posterior, uint32_t *n_tasks, uint32_t *n_visible,
+                            uint32_t *n_failed, uint8_t *row_status);
+/* DEVICE pointers on `device`: one build launch, then two launches per slot (three with model given) on `stream`, no
+ * allocation, no synchronisation; only the scalar arguments are checked (sensors, slots and Sun rows must be valid).
+ * d_scratch holds *bytes of astroz_cuda_tasking_scratch_bytes(n, s, bytes), 16-byte aligned. */
+int32_t astroz_cuda_tasking_device(const double *d_elements, uint32_t n, int32_t grav, const double *d_covariance,
+                                   const uint8_t *d_model, const uint8_t *d_kind, const uint32_t *d_station,
+                                   const double *d_sigma, const double *d_limits, uint32_t s, const double *d_stations,
+                                   const double *d_jd, const double *d_fr, uint32_t t, const double *d_sun,
+                                   double gain_min, int32_t device, void *d_scratch, uint32_t *d_task_row,
+                                   double *d_task_gain, double *d_task_value, double *d_task_spread,
+                                   uint32_t *d_n_candidates, double *d_posterior, uint32_t *d_n_tasks,
+                                   uint32_t *d_n_visible, uint32_t *d_n_failed, uint8_t *d_row_status, void *stream);
+int32_t astroz_cuda_tasking_scratch_bytes(uint32_t n, uint32_t s, uint64_t *bytes);
 /* ---- initial orbits (K13): an element set for a track no catalogue row predicts ---------------------------------------
  * New capability: the reference has no initial orbit determination, so these calls replace nothing in it.
  * Track j is the observations [offsets[j], offsets[j + 1]) in the layout of astroz_cuda_correlate, in time order (the

@@ -112,6 +112,9 @@ pub extern fn astroz_cuda_correlate(elements: ?[*]const f64, n: u32, grav: i32, 
 pub extern fn astroz_cuda_correlate_device(d_elements: ?[*]const f64, n: u32, grav: i32, d_covariance: ?[*]const f64, d_model: ?[*]const u8, d_offsets: ?[*]const u32, t: u32, d_jd: ?[*]const f64, d_fr: ?[*]const f64, d_kind: ?[*]const u8, d_value: ?[*]const f64, d_sigma: ?[*]const f64, d_station: ?[*]const u32, d_stations: ?[*]const f64, gate_probability: f64, best: u32, device: i32, d_scratch: ?*anyopaque, d_rows: ?[*]u32, d_d2: ?[*]f64, d_used: ?[*]u32, d_n_gate: ?[*]u32, d_n_failed: ?[*]u32, d_status: ?[*]u8, d_row_status: ?[*]u8, stream: ?*anyopaque) i32;
 pub extern fn astroz_cuda_correlate_scratch_bytes(n: u32, t: u32, best: u32, bytes: *u64) i32;
 pub extern fn astroz_cuda_chi2_quantile(k: u32, p: f64, x: ?[*]f64) i32;
+pub extern fn astroz_cuda_tasking(elements: ?[*]const f64, n: u32, grav: i32, covariance: ?[*]const f64, model: ?[*]const u8, kind: ?[*]const u8, station: ?[*]const u32, sigma: ?[*]const f64, limits: ?[*]const f64, s: u32, stations: ?[*]const f64, k: u32, jd: ?[*]const f64, fr: ?[*]const f64, t: u32, sun: ?[*]const f64, gain_min: f64, device: i32, task_row: ?[*]u32, task_gain: ?[*]f64, task_value: ?[*]f64, task_spread: ?[*]f64, n_candidates: ?[*]u32, posterior: ?[*]f64, n_tasks: ?[*]u32, n_visible: ?[*]u32, n_failed: ?[*]u32, row_status: ?[*]u8) i32;
+pub extern fn astroz_cuda_tasking_device(d_elements: ?[*]const f64, n: u32, grav: i32, d_covariance: ?[*]const f64, d_model: ?[*]const u8, d_kind: ?[*]const u8, d_station: ?[*]const u32, d_sigma: ?[*]const f64, d_limits: ?[*]const f64, s: u32, d_stations: ?[*]const f64, d_jd: ?[*]const f64, d_fr: ?[*]const f64, t: u32, d_sun: ?[*]const f64, gain_min: f64, device: i32, d_scratch: ?*anyopaque, d_task_row: ?[*]u32, d_task_gain: ?[*]f64, d_task_value: ?[*]f64, d_task_spread: ?[*]f64, d_n_candidates: ?[*]u32, d_posterior: ?[*]f64, d_n_tasks: ?[*]u32, d_n_visible: ?[*]u32, d_n_failed: ?[*]u32, d_row_status: ?[*]u8, stream: ?*anyopaque) i32;
+pub extern fn astroz_cuda_tasking_scratch_bytes(n: u32, s: u32, bytes: *u64) i32;
 pub extern fn astroz_cuda_initial_orbits(offsets: ?[*]const u32, t: u32, jd: ?[*]const f64, fr: ?[*]const f64, kind: ?[*]const u8, value: ?[*]const f64, sigma: ?[*]const f64, station: ?[*]const u32, m: u32, stations: ?[*]const f64, k: u32, bstar: ?[*]const f64, grav: i32, device: i32, elements: ?[*]f64, state: ?[*]f64, wrms: ?[*]f64, method: ?[*]u8, candidates: ?[*]u32, conv: ?[*]f64, deep_space: ?[*]u8, status: ?[*]u8) i32;
 pub extern fn astroz_cuda_initial_orbits_device(d_offsets: ?[*]const u32, t: u32, d_jd: ?[*]const f64, d_fr: ?[*]const f64, d_kind: ?[*]const u8, d_value: ?[*]const f64, d_sigma: ?[*]const f64, d_station: ?[*]const u32, d_stations: ?[*]const f64, d_bstar: ?[*]const f64, grav: i32, device: i32, d_scratch: ?*anyopaque, d_elements: ?[*]f64, d_state: ?[*]f64, d_wrms: ?[*]f64, d_method: ?[*]u8, d_candidates: ?[*]u32, d_conv: ?[*]f64, d_deep_space: ?[*]u8, d_status: ?[*]u8, stream: ?*anyopaque) i32;
 pub extern fn astroz_cuda_initial_orbits_scratch_bytes(t: u32, bytes: *u64) i32;
