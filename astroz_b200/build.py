@@ -14,8 +14,8 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libastroz_b200.so")
-SOURCES = ["az_kernels.cu", "az_ingest.cu", "az_pairs.cu", "az_numerical.cu", "az_fit.cu", "az_fit_obs.cu", "az_covariance.cu", "az_conjunction.cu", "az_conjunction_mc.cu", "az_conjunction_is.cu", "az_avoid.cu", "az_correlate.cu", "az_iod.cu", "az_link.cu", "az_tasking.cu", "az_lambert.cu", "az_hostcopy.cu", "az_capi.cu"]
-HEADERS = ["az_math.cuh", "az_device.cuh", "az_kernels.cuh", "az_ingest.cuh", "az_pairs.cuh", "az_numerical.cuh", "az_fit.cuh", "az_obs.cuh", "az_covariance.cuh", "az_conjunction.cuh", "az_conjunction_mc.cuh", "az_conjunction_is.cuh", "az_conjunction_mc_warp.cuh", "az_avoid.cuh", "az_correlate.cuh", "az_iod.cuh", "az_link.cuh", "az_tasking.cuh", "az_lambert.cuh", "az_hostcopy.cuh", "az_screen.cuh", "az_elements.hpp",
+SOURCES = ["az_kernels.cu", "az_ingest.cu", "az_pairs.cu", "az_numerical.cu", "az_fit.cu", "az_fit_obs.cu", "az_covariance.cu", "az_conjunction.cu", "az_conjunction_mc.cu", "az_conjunction_is.cu", "az_avoid.cu", "az_correlate.cu", "az_iod.cu", "az_link.cu", "az_tasking.cu", "az_reentry.cu", "az_lambert.cu", "az_hostcopy.cu", "az_capi.cu"]
+HEADERS = ["az_math.cuh", "az_device.cuh", "az_kernels.cuh", "az_ingest.cuh", "az_pairs.cuh", "az_numerical.cuh", "az_fit.cuh", "az_obs.cuh", "az_covariance.cuh", "az_conjunction.cuh", "az_conjunction_mc.cuh", "az_conjunction_is.cuh", "az_conjunction_mc_warp.cuh", "az_avoid.cuh", "az_correlate.cuh", "az_iod.cuh", "az_link.cuh", "az_tasking.cuh", "az_reentry.cuh", "az_lambert.cuh", "az_hostcopy.cuh", "az_screen.cuh", "az_elements.hpp",
            "az_tables.hpp", os.path.join("..", "..", "include", "astroz_b200.h")]
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = [*GENCODE, "-O3", "-std=c++17", "-lineinfo",
@@ -28,9 +28,9 @@ NVCC_FLAGS = [*GENCODE, "-O3", "-std=c++17", "-lineinfo",
 # K9 (Lambert) likewise: its host build equals a scalar statement of the solver wherever no transcendental differs.
 # K13 (initial orbits) too: whether a Gauss refinement meets its tolerance, and so which candidate wins, must not turn
 # on a contraction the host build does not make.  K17 (track linking) for the same reason: where a refinement stops
-# decides the winner.
+# decides the winner.  K19 (reentry) runs K7's integrator, so it follows K7: its host build then takes the same steps.
 SOURCE_FLAGS = {"az_ingest.cu": ["-fmad=false"], "az_numerical.cu": ["-fmad=false"], "az_lambert.cu": ["-fmad=false"],
-                "az_iod.cu": ["-fmad=false"], "az_link.cu": ["-fmad=false"]}
+                "az_iod.cu": ["-fmad=false"], "az_link.cu": ["-fmad=false"], "az_reentry.cu": ["-fmad=false"]}
 
 
 def _nvcc() -> str:

@@ -3308,6 +3308,134 @@ int32_t astroz_cuda_conjunction_mc(const double *elements, uint32_t n, int32_t g
                        });
 }
 
+// ---- reentry prediction (K19, az_reentry.cu, az_reentry.cuh) ---------------------------------------------------------
+// Scalar checks of the reentry calls, before anything is read, written or allocated; a receives the scalars.
+static int32_t reentry_check(uint32_t n, int32_t grav, uint32_t m, double h_i, double horizon_days, double step_s,
+                             double density_scale, double density_sigma, uint32_t record, int32_t device,
+                             az::ReentryArgs *a) {
+    if (device < 0) return value_error("reentry prediction runs on one device: pass its ordinal");
+    const int32_t rc = grav_check(grav);
+    if (rc != ASTROZ_OK) return rc;
+    if (!(h_i >= 60.0 && h_i <= 200.0)) return value_error("h_i must be in [60, 200] km");
+    if (!(horizon_days > 0.0 && horizon_days <= 3660.0)) return value_error("horizon_days must be in (0, 3660]");
+    if (!(step_s >= 1.0 && step_s <= 3600.0)) return value_error("step_s must be in [1, 3600] s");
+    if (!(density_sigma >= 0.0 && density_sigma <= 2.0)) return value_error("density_sigma must be in [0, 2]");
+    if (!(density_scale > 0.0) || !std::isfinite(density_scale))
+        return value_error("density_scale must be finite and > 0");
+    a->n = n;
+    a->m = m;
+    a->record = record;
+    const az::Gravity gr = az::gravity(grav);
+    a->call = {h_i, horizon_days * 86400.0, step_s, density_scale, density_sigma, 7.292115e-5, gr.mu, gr.radiusEarthKm,
+               gr.j2};
+    a->grav = grav;
+    a->g = az::grav_consts(gr);
+    return ASTROZ_OK;
+}
+
+// Both call forms: a holds reentry_check's scalars, the arrays are on the device.
+static cudaError_t reentry_run(az::ReentryArgs a, const double *elements, const double *covariance,
+                               const uint8_t *model, const uint32_t *rows, const double *ballistic,
+                               const uint64_t *samples, const uint64_t *first, const uint64_t *seed, void *scratch,
+                               double *record_out, double *states, uint8_t *nominal_status, uint64_t *counts,
+                               double *sample_out, uint8_t *status, cudaStream_t st) {
+    a.elements = elements;
+    a.covariance = covariance;
+    a.model = model;
+    a.rows = rows;
+    a.ballistic = ballistic;
+    a.samples = samples;
+    a.first = first;
+    a.seed = seed;
+    a.scratch = scratch;
+    a.out = record_out;
+    a.states = states;
+    a.nominalStatus = nominal_status;
+    a.counts = counts;
+    a.sampleOut = sample_out;
+    a.status = status;
+    return az::launch_reentry(a, st);
+}
+
+int32_t astroz_cuda_reentry_scratch_bytes(uint32_t m, uint64_t *bytes) {
+    if (!bytes) return ASTROZ_NULL_POINTER;
+    int count = 0;
+    const int32_t rc = check_device_present(&count, "no CUDA device available (the scan's scratch is the device's)");
+    if (rc != ASTROZ_OK) return rc;
+    size_t b = 0;
+    AZ_CUDA(az::reentry_scratch_bytes(m, &b));
+    *bytes = b;
+    return ASTROZ_OK;
+}
+
+int32_t astroz_cuda_reentry_device(const double *d_elements, uint32_t n, int32_t grav, const double *d_covariance,
+                                   const uint8_t *d_model, const uint32_t *d_rows, const double *d_ballistic,
+                                   const uint64_t *d_samples, const uint64_t *d_first, const uint64_t *d_seed,
+                                   uint32_t m, double h_i, double horizon_days, double step_s, double density_scale,
+                                   double density_sigma, uint32_t record, int32_t device, double *d_record_out,
+                                   double *d_states, uint8_t *d_nominal_status, uint64_t *d_counts,
+                                   double *d_sample_out, uint8_t *d_status, void *d_scratch, void *stream) {
+    az::ReentryArgs a{};
+    int32_t rc = reentry_check(n, grav, m, h_i, horizon_days, step_s, density_scale, density_sigma, record, device, &a);
+    if (rc != ASTROZ_OK) return rc;
+    if (m == 0) return ASTROZ_OK;
+    if ((n && (!d_elements || !d_covariance)) || !d_rows || !d_samples || !d_record_out || !d_nominal_status ||
+        !d_counts || !d_status || !d_scratch || (record && !d_sample_out))
+        return ASTROZ_NULL_POINTER;
+    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
+    AZ_CUDA(cudaSetDevice(device));
+    AZ_CUDA(reentry_run(a, d_elements, d_covariance, d_model, d_rows, d_ballistic, d_samples, d_first, d_seed,
+                        d_scratch, d_record_out, d_states, d_nominal_status, d_counts, d_sample_out, d_status,
+                        static_cast<cudaStream_t>(stream)));
+    return ASTROZ_OK;
+}
+
+int32_t astroz_cuda_reentry(const double *elements, uint32_t n, int32_t grav, const double *covariance,
+                            const uint8_t *model, const uint32_t *rows, const double *ballistic, const uint64_t *samples,
+                            const uint64_t *first, const uint64_t *seed, uint32_t m, double h_i, double horizon_days,
+                            double step_s, double density_scale, double density_sigma, uint32_t record, int32_t device,
+                            double *record_out, double *states, uint8_t *nominal_status, uint64_t *counts,
+                            double *sample_out, uint8_t *status) {
+    az::ReentryArgs a{};
+    int32_t rc = reentry_check(n, grav, m, h_i, horizon_days, step_s, density_scale, density_sigma, record, device, &a);
+    if (rc != ASTROZ_OK) return rc;
+    if (n && (!elements || !covariance)) return ASTROZ_NULL_POINTER;
+    if (m && (!rows || !samples || !record_out || !nominal_status || !counts || !status)) return ASTROZ_NULL_POINTER;
+    if (m && record && !sample_out) return value_error("record > 0 needs sample_out");
+    for (uint32_t i = 0; i < m; ++i) {
+        if (rows[i] >= n) return value_error("a request's row is outside the catalogue");
+        if (first && samples[i] > UINT64_MAX - first[i])
+            return value_error("first + samples must not exceed 2^64 - 1");
+    }
+    if (ballistic && !all_finite(ballistic, m)) return value_error("ballistic coefficients must be finite");
+    if ((rc = rows_check(elements, covariance, n)) != ASTROZ_OK) return rc;
+    if ((rc = model_bytes_check(model, n)) != ASTROZ_OK) return rc;
+    if (m == 0) return ASTROZ_OK;
+    if ((rc = check_device_ordinal(device)) != ASTROZ_OK) return rc;
+    size_t scratchBytes = 0;
+    AZ_CUDA(cudaSetDevice(device));
+    AZ_CUDA(az::reentry_scratch_bytes(m, &scratchBytes));
+    return whole_batch(device,
+                       {upload(elements, (size_t)64 * n), upload(covariance, (size_t)8 * az::kFitN * n),
+                        upload(model, model ? (size_t)n : 0), upload(rows, (size_t)4 * m),
+                        upload(ballistic, ballistic ? (size_t)8 * m : 0), upload(samples, (size_t)8 * m),
+                        upload(first, first ? (size_t)8 * m : 0), upload(seed, seed ? (size_t)8 * m : 0),
+                        scratch(scratchBytes), result(record_out, (size_t)8 * ASTROZ_REENTRY_RECORD_WORDS * m),
+                        result(states, states ? (size_t)8 * ASTROZ_REENTRY_STATE_WORDS * m : 0),
+                        result(nominal_status, m), result(counts, (size_t)8 * ASTROZ_REENTRY_COUNT_WORDS * m),
+                        result(sample_out, (size_t)8 * ASTROZ_REENTRY_SAMPLE_WORDS * record * m), result(status, m)},
+                       [&](const DeviceBlock &d, cudaStream_t st) {
+                           return reentry_run(a, d.f64(0), d.f64(1), model ? d.u8(2) : nullptr, d.u32(3),
+                                              ballistic ? d.f64(4) : nullptr,
+                                              reinterpret_cast<const uint64_t *>(d.piece(5)),
+                                              first ? reinterpret_cast<const uint64_t *>(d.piece(6)) : nullptr,
+                                              seed ? reinterpret_cast<const uint64_t *>(d.piece(7)) : nullptr,
+                                              d.piece(8), d.f64(9), states ? d.f64(10) : nullptr, d.u8(11),
+                                              reinterpret_cast<uint64_t *>(d.piece(12)), record ? d.f64(13) : nullptr,
+                                              d.u8(14), st);
+                       });
+}
+
 // ---- importance-sampled collision probability (K15, az_conjunction_is.cu, az_conjunction_is.cuh) ---------------------
 static_assert(ASTROZ_CONJ_IS_COUNT_WORDS == az::kIsCountWords && ASTROZ_CONJ_IS_PROPOSAL_WORDS == az::kIsProposalWords &&
                   ASTROZ_CONJ_IS_SAMPLE_WORDS == az::kIsSampleWords && ASTROZ_CONJ_IS_LINEAR == az::kIsLinear &&

@@ -397,6 +397,45 @@ struct TaskArgs {
 // the build kernel, then per slot the near-earth and deep-space scoring kernels and the one-CTA select kernel
 cudaError_t launch_tasking(const TaskArgs &a, cudaStream_t stream);
 
+// K19: reentry prediction (az_reentry.cu, az_reentry.cuh).  The call's scalars as the trajectories read them (from the
+// launch's parameters on the device) ...
+struct ReentryCall {
+    double hi;          // interface height [km]
+    double horizon;     // [s] after epoch
+    double step;        // output interval [s]
+    double scale;       // density_scale
+    double sigma;       // density_sigma
+    double omega;       // the atmosphere's rotation rate [rad/s]
+    double mu, rEq, j2; // the call's grav
+};
+// ... and the arrays, device pointers.
+struct ReentryArgs {
+    const double *elements = nullptr;    // [8][n]
+    const double *covariance = nullptr;  // [n][28]
+    const uint8_t *model = nullptr;      // [n], nullable (all 0)
+    uint32_t n = 0;
+    const uint32_t *rows = nullptr;      // [m] catalogue rows
+    const double *ballistic = nullptr;   // [m] B [m^2/kg], nullable (12.741621 B*)
+    const uint64_t *samples = nullptr;   // [m]
+    const uint64_t *first = nullptr;     // [m], nullable (all 0)
+    const uint64_t *seed = nullptr;      // [m], nullable (all 0)
+    uint32_t m = 0;
+    uint32_t record = 0;                 // sample words kept per request
+    ReentryCall call{};
+    int grav = 1;
+    GravConsts g{};
+    void *scratch = nullptr;             // reentry_scratch_bytes(m)
+    double *out = nullptr;               // [m][8] nominal records
+    double *states = nullptr;            // [m][6] TEME state at the nominal crossing, nullable
+    uint8_t *nominalStatus = nullptr;    // [m] ASTROZ_REENTRY_TRAJ_*
+    uint64_t *counts = nullptr;          // [m][3] reentered, above, failed
+    double *sampleOut = nullptr;         // [m][record][4]; nullable when record = 0
+    uint8_t *status = nullptr;           // [m] ASTROZ_REENTRY_*
+};
+cudaError_t reentry_scratch_bytes(uint32_t m, size_t *bytes);
+// the build kernel, the work-item scan, the near-earth items, then the deep-space items
+cudaError_t launch_reentry(const ReentryArgs &a, cudaStream_t stream);
+
 // K16: collision-avoidance manoeuvre trials (az_avoid.cu, az_avoid.cuh; AvoidArgs and avoid_scratch_bytes are there).
 // K10 at the burn, the burn, K8's conversion, K10 on the new sets, the covariance transport, K11, the finishing kernel
 struct AvoidArgs;

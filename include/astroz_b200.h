@@ -1277,6 +1277,79 @@ int32_t astroz_cuda_constellation_porkchop(astroz_constellation_t h, const uint3
                                            const double *arr_jd, const double *arr_fr, uint32_t n_arr, double mu,
                                            uint32_t max_revs, double *dv, uint8_t *slot, uint8_t *status);
 
+/* ---- reentry prediction (K19): catalogue rows and their covariance draws carried down to the interface -------------
+ * Request i names catalogue row rows[i] (element columns, covariance words, model byte, as astroz_cuda_conjunction_mc)
+ * with samples[i], first[i] (NULL: all 0) and seed[i] (NULL: all 0).  A trajectory starts at the row's epoch from the
+ * TEME state (tsince 0) of a set built under the row's model with grav: the row's own set for the NOMINAL, a drawn set
+ * for SAMPLE k.  It is integrated by astroz_cuda_propagate_numerical's Dormand-Prince 8(7) (rtol 1e-9, atol 1e-12,
+ * its step control and stop rules) over intervals of step_s seconds until the first crossing of the interface height
+ * h_i [km] or horizon_days after epoch.
+ *   force:     two-body + the textbook J2 acceleration (mu, equatorial radius and J2 of grav), and drag quadratic in the
+ *              speed relative to a co-rotating atmosphere: a = -1/2 B f rho(h) |v_rel| v_rel 1e3 km/s^2, v_rel = v -
+ *              w x r, w = 7.292115e-5 rad/s about TEME z.  h is the WGS-84 geodetic height of the TEME position (the
+ *              height of the ECEF output mode's conversion; no GMST is needed for it).  rho(h) = density_scale x the
+ *              piecewise-exponential atmosphere of Vallado, Fundamentals of Astrodynamics and Applications, Table 8-4:
+ *              rho0 exp(-(h - h0) / H) in the band with the largest h0 <= h, the last band above 1000 km.  None of the
+ *              numerical propagator's own force models is used or changed;
+ *   B:         B_row = ballistic[i] [m^2/kg], or 12.741621 B* when ballistic is NULL (B* = B rho0 / 2, rho0 =
+ *              0.15696615 kg m^-2 ER^-1).  A sample's B_k = B_row + 12.741621 (B*_k - B*_row) (B_row when B* is held).
+ *              B <= 0 or non-finite: the trajectory is NONPHYSICAL;
+ *   draws:     astroz_cuda_conjunction_mc's factor and draws of the PRIMARY under the request's seed: sample k's set is
+ *              that call's primary set of sample k.  Normal 7 (block 3's second normal) gives the density factor
+ *              f_k = exp(density_sigma z_7); the nominal has f = 1 (the median density);
+ *   crossing:  after each interval, the cubic Hermite of position over it from its end states.  A crossing when the
+ *              end height is <= h_i, or when the radial velocity goes from - to + inside the interval and the
+ *              Hermite's minimum height (golden-section search to 1e-9 of the interval) is <= h_i (a perigee dip).  The crossing time is the root of the
+ *              Hermite's height - h_i, by bisection to 2^-30 of the interval; the state there is the Hermite and its
+ *              derivative.  A start at or below h_i crosses at dt = 0.
+ * Outputs: record[m][8] of the nominal (dt [min from epoch, +inf when still above at the horizon], geodetic latitude
+ * and east longitude [deg] by the ECEF mode's GMST, inertial speed [km/s], inertial flight-path angle [deg], B used,
+ * accepted and rejected DP87 attempts; NaN where not defined); states[m][6] (nullable: TEME state at the nominal
+ * crossing, NaN unless REENTERED); nominal_status[m] (ASTROZ_REENTRY_TRAJ_*); counts[m][3] (reentered, above, failed:
+ * INIT_FAILED, NONPHYSICAL or STOPPED samples); sample_out[m][record][4] (dt, latitude, longitude, attempts) of samples
+ * first .. first + record - 1, NaN past samples[i] and for every sample of a request that is not OK; status[m]: OK,
+ * INIT_FAILED (the row's set cannot be built, or a model byte > 1 on the device call), NOT_PSD, BAD_ROW (device call
+ * only).  A request that is not OK runs nothing: its counts are zero and its nominal is INIT_FAILED.
+ * A sample's words depend on its row's inputs, the call's scalars, the seed and k alone, and counts are integer sums:
+ * the bytes do not depend on the batch, the order, the split of [first, first + samples) or the call form.
+ * Lunisolar and higher zonal terms are not modelled: transfer-orbit predictions are indicative only.
+ * ASTROZ_VALUE_ERROR, nothing written: device = -1, an unknown grav, h_i outside [60, 200] km, horizon_days outside
+ * (0, 3660], step_s outside [1, 3600], density_sigma outside [0, 2], density_scale <= 0 or non-finite; and for the host
+ * call a row outside the catalogue, non-finite elements or covariance words, a model byte > 1, a non-finite ballistic,
+ * first + samples above 2^64 - 1, record > 0 with a NULL sample_out. */
+#define ASTROZ_REENTRY_RECORD_WORDS        8
+#define ASTROZ_REENTRY_SAMPLE_WORDS        4
+#define ASTROZ_REENTRY_COUNT_WORDS         3
+#define ASTROZ_REENTRY_STATE_WORDS         6
+#define ASTROZ_REENTRY_OK                  0
+#define ASTROZ_REENTRY_INIT_FAILED         1
+#define ASTROZ_REENTRY_NOT_PSD             2
+#define ASTROZ_REENTRY_BAD_ROW             3
+#define ASTROZ_REENTRY_TRAJ_REENTERED      0
+#define ASTROZ_REENTRY_TRAJ_ABOVE          1
+#define ASTROZ_REENTRY_TRAJ_INIT_FAILED    2   /* the set cannot be built, or its epoch state fails */
+#define ASTROZ_REENTRY_TRAJ_NONPHYSICAL    3   /* B <= 0 or non-finite */
+#define ASTROZ_REENTRY_TRAJ_STOPPED        4   /* the integrator's stop rule or substep limit, or a non-finite state */
+/* HOST buffers: one upload (pageable through a pinned ring, pinned by direct DMA), the launches, plain copies back. */
+int32_t astroz_cuda_reentry(const double *elements, uint32_t n, int32_t grav, const double *covariance,
+                            const uint8_t *model, const uint32_t *rows, const double *ballistic, const uint64_t *samples,
+                            const uint64_t *first, const uint64_t *seed, uint32_t m, double h_i, double horizon_days,
+                            double step_s, double density_scale, double density_sigma, uint32_t record, int32_t device,
+                            double *record_out, double *states, uint8_t *nominal_status, uint64_t *counts,
+                            double *sample_out, uint8_t *status);
+/* DEVICE pointers on `device`: the launches on `stream`, no allocation, no synchronisation; only the scalar arguments
+ * are checked (a row outside the catalogue gets BAD_ROW).  d_scratch holds *bytes of
+ * astroz_cuda_reentry_scratch_bytes(m, bytes), 256-byte aligned. */
+int32_t astroz_cuda_reentry_device(const double *d_elements, uint32_t n, int32_t grav, const double *d_covariance,
+                                   const uint8_t *d_model, const uint32_t *d_rows, const double *d_ballistic,
+                                   const uint64_t *d_samples, const uint64_t *d_first, const uint64_t *d_seed,
+                                   uint32_t m, double h_i, double horizon_days, double step_s, double density_scale,
+                                   double density_sigma, uint32_t record, int32_t device, double *d_record_out,
+                                   double *d_states, uint8_t *d_nominal_status, uint64_t *d_counts,
+                                   double *d_sample_out, uint8_t *d_status, void *d_scratch, void *stream);
+/* The scratch of the device call for m requests (the scan's size is the device's: ASTROZ_NO_DEVICE without one). */
+int32_t astroz_cuda_reentry_scratch_bytes(uint32_t m, uint64_t *bytes);
+
 /* ---- measurement helpers --------------------------------------------------------------------- */
 /* DFMA microbenchmark on `device`: achieved fp64 TFLOP/s (FMA = 2) -- the measured roofline denominator */
 int32_t astroz_cuda_fp64_peak(int32_t device, double *tflops);

@@ -126,6 +126,9 @@ pub extern fn astroz_cuda_lambert(r1: ?[*]const f64, r2: ?[*]const f64, tof: ?[*
 pub extern fn astroz_cuda_lambert_device(d_r1: ?[*]const f64, d_r2: ?[*]const f64, d_tof: ?[*]const f64, d_normal: ?[*]const f64, n: u32, mu: f64, max_revs: u32, device: i32, d_v1: ?[*]f64, d_v2: ?[*]f64, d_status: ?[*]u8, d_iterations: ?[*]u8, stream: ?*anyopaque) i32;
 pub extern fn astroz_cuda_lambert_porkchop_device(d_dep: ?[*]const f64, d_dep_status: ?[*]const u8, d_arr: ?[*]const f64, d_arr_status: ?[*]const u8, n_pairs: u32, d_dep_jd: ?[*]const f64, d_dep_fr: ?[*]const f64, n_dep: u32, d_arr_jd: ?[*]const f64, d_arr_fr: ?[*]const f64, n_arr: u32, mu: f64, max_revs: u32, device: i32, d_dv: ?[*]f64, d_slot: ?[*]u8, d_status: ?[*]u8, stream: ?*anyopaque) i32;
 pub extern fn astroz_cuda_constellation_porkchop(h: Handle, chaser: ?[*]const u32, target: ?[*]const u32, n_pairs: u32, dep_jd: ?[*]const f64, dep_fr: ?[*]const f64, n_dep: u32, arr_jd: ?[*]const f64, arr_fr: ?[*]const f64, n_arr: u32, mu: f64, max_revs: u32, dv: ?[*]f64, slot: ?[*]u8, status: ?[*]u8) i32;
+pub extern fn astroz_cuda_reentry(elements: ?[*]const f64, n: u32, grav: i32, covariance: ?[*]const f64, model: ?[*]const u8, rows: ?[*]const u32, ballistic: ?[*]const f64, samples: ?[*]const u64, first: ?[*]const u64, seed: ?[*]const u64, m: u32, h_i: f64, horizon_days: f64, step_s: f64, density_scale: f64, density_sigma: f64, record: u32, device: i32, record_out: ?[*]f64, states: ?[*]f64, nominal_status: ?[*]u8, counts: ?[*]u64, sample_out: ?[*]f64, status: ?[*]u8) i32;
+pub extern fn astroz_cuda_reentry_device(d_elements: ?[*]const f64, n: u32, grav: i32, d_covariance: ?[*]const f64, d_model: ?[*]const u8, d_rows: ?[*]const u32, d_ballistic: ?[*]const f64, d_samples: ?[*]const u64, d_first: ?[*]const u64, d_seed: ?[*]const u64, m: u32, h_i: f64, horizon_days: f64, step_s: f64, density_scale: f64, density_sigma: f64, record: u32, device: i32, d_record_out: ?[*]f64, d_states: ?[*]f64, d_nominal_status: ?[*]u8, d_counts: ?[*]u64, d_sample_out: ?[*]f64, d_status: ?[*]u8, d_scratch: ?*anyopaque, stream: ?*anyopaque) i32;
+pub extern fn astroz_cuda_reentry_scratch_bytes(m: u32, bytes: *u64) i32;
 pub extern fn astroz_cuda_fp64_peak(device: i32, tflops: ?[*]f64) i32;
 pub extern fn astroz_cuda_fp64_pipe_peak(device: i32, tflops: ?[*]f64) i32;
 
